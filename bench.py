@@ -3,17 +3,19 @@
 
   python bench.py --gpus N --steps K --warmup W            # CUDA path (this repo), config C2 (the metric's config)
   python bench.py --impl reference --gpus N ...            # the reference's own CPU path on the host cores
-  python bench.py --config C4|C5 ...                       # the other BASELINE configs (not the driver's bench line)
+  python bench.py --config C4|C5 ...                       # the other BASELINE configs (C2 is the headline workload)
   torchrun ... bench.py --gpus N ...                       # N > 1: one rank per GPU
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/<name>.npy
 
 A *step* is one scan: the full iterated update (esekfom.hpp:495-721; max_iteration 3 => up to 4 measurement passes,
 k-NN on the first pass and after a converged step) of the 3-LiDAR 100k-point merged scan against the 1M-point map
 (BASELINE configs[1], "C2"; with --gpus N > 1 the same scan point-sharded over N ranks: configs[2]).  Synthetic, seeded
 inputs (malio_b200/synth.py).  The map is a LIVE reference ikd-Tree (the real ikd_Tree.cpp, oracle/_ref: Build + the
 scripted churn of SURVEY.md §8d — 2 % Add_Points with down-sampling, a no-down-sampling batch, one Delete_Point_Boxes —
-so lazy flags and rebuilt subtrees exist); where oracle/_ref is not built the product's static builder stands in and the
-line says so.  The tree is INPUT here, exactly what a MA-LIO checkout holds on its host; nothing under oracle/ computes
-any part of the measured result.
+so lazy flags and rebuilt subtrees exist); where oracle/_ref is not built a static balanced tree stands in and the line
+says so: the product's builder, whose snapshot the CPU baseline then searches too; the --impl reference arm, which never
+loads the product library, uses the oracle's numpy restatement of that builder.  The tree is INPUT here, exactly what a
+MA-LIO checkout holds on its host; nothing under oracle/ computes any part of the measured result.
 
 `value`   scans/sec with every input already resident in HBM when the timed region starts (the per-scan state is
           re-armed on the device; sort, k-NN, plane fit, gate, reduction, D2H of the 3.5 KB system and the host 35x35
@@ -27,7 +29,13 @@ any part of the measured result.
           (include/malio_flatten.hpp, OpenMP over the host threads; `flatten_ms`) + compact snapshot upload (20 B per node);
           `e2e.snapshot_only` is that step with the flatten left out (the round-1 definition), for comparison.
 L2 is flushed (256 MiB write) between timed steps; each step is bracketed by CUDA events and the per-step times are
-summed (max over ranks).  Only the cpu_baseline / --impl reference legs time anything under oracle/.
+summed (max over ranks).  Every GPU timed loop runs --steps steps; the CPU arms honour --steps within a 150 s budget
+(the line reports the steps they ran).  Only the cpu_baseline / --impl reference legs time anything under oracle/.
+
+--dump-outputs DIR writes, after the timed steps, what the headline loop returned in its last step (rank 0): the updated
+state and covariance, the update report and the per-point side outputs of the last pass (C2/C4), or the neighbour lists
+of a fixed seeded sample of the queries (C5).  Inputs are seeded, so two builds run with the same arguments can be
+compared output for output.
 """
 from __future__ import annotations
 
@@ -55,8 +63,9 @@ WORKLOADS = {
     "C4": "C4: dense urban 300k-pt merged scan vs 5M-pt map, max_iteration=5",
     "C5": "C5: k-NN microbench, 1M queries vs 10M-pt tree, k=5",
 }
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu captures (profiles/), C2 only
-NCU_DRAM_BYTES = {"knn": 8.26e6, "pass": 10.1e6, "knn_c5": 535.6e6}   # profiles/r02_keys_pass_raw.csv (knn_keys_kernel, pass_kernel), r02_knn_direct_c5_raw.csv
+HBM_PEAK_GBS = 3350.0     # H100 SXM data sheet (HBM3); MEASURED_PEAKS.json, where present, takes precedence
+DUMP_LIMIT_BYTES = 64 << 20
+C5_DUMP_QUERIES = 200_000
 SYNC_THREADS = 16          # host threads of the per-scan voxel read-back (include/malio_mapsync.hpp)
 REF_CPU_BUDGET_S = 150.0   # bound of the CPU arms' total run time (both thread counts together)
 
@@ -71,7 +80,35 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sort", action="store_true")
     ap.add_argument("--static-map", action="store_true", help="static balanced snapshot instead of the live ikd-Tree")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32/float64, <= 64 MB in all)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    return args
+
+
+def dump_outputs(outdir, arrays):
+    """Write {name: array} as outdir/<name>.npy; integers become float64 (exact below 2**53), the rest keeps float32/64."""
+    os.makedirs(outdir, exist_ok=True)
+    out = {}
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        if a.dtype != np.float32 and a.dtype != np.float64:
+            a = a.astype(np.float64)
+        out[name] = np.ascontiguousarray(a)
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT_BYTES}-byte limit")
+    for name, a in out.items():
+        np.save(os.path.join(outdir, name + ".npy"), a)
+
+
+def hbm_peak():
+    try:
+        return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
+    except Exception:
+        return HBM_PEAK_GBS, f"H100 SXM data sheet, {HBM_PEAK_GBS:.0f} GB/s"
 
 
 # ------------------------------------------------------------------ clocks sampler (recipe's nvidia-smi line)
@@ -176,7 +213,7 @@ def live_tree(case, seed=7):
 
 
 # ------------------------------------------------------------------ reference / CPU arm
-def cpu_reference_run(case, tree, steps: int, warmup: int, threads: int):
+def cpu_reference_run(case, tree, steps: int, warmup: int, threads: int, static=None):
     """The reference's CPU path: real ikd_Tree.cpp (oracle/_ref) for the k-NN when it was compiled here, else the
     restated search; restated h_share_model + update_iterated_dyn_share_modified (oracle/), with esekfom.hpp:622-635
     evaluated the optimised way (orc_reduce_fast).  Returns a dict."""
@@ -188,9 +225,8 @@ def cpu_reference_run(case, tree, steps: int, warmup: int, threads: int):
         orc.set_knn_ref(tree)
         kind = "reference-knn+port"
     else:
-        from malio_b200 import plugin
-        snap = plugin.build_static_snapshot(case.map_xyz, case.map_normal_y)
-        orc.set_map_snapshot(snap.nodes, snap.node_cov)
+        nodes, cov, _ = static if static is not None else po.static_snapshot(case.map_xyz, case.map_normal_y)
+        orc.set_map_snapshot(nodes, cov)
         kind = "port"
     times, passes = [], 0
     for i in range(warmup + steps):
@@ -214,7 +250,7 @@ def cpu_reference_run(case, tree, steps: int, warmup: int, threads: int):
                                   "A_ieskf_rest": 1e3 * tA / npass}}
 
 
-def cpu_arms(case, tree, steps, warmup):
+def cpu_arms(case, tree, steps, warmup, static=None):
     """Both thread counts the survey asks for: 3 (what the reference ships, CMakeLists.txt:23-25) and all host threads.
     Steps are honoured up to a wall-clock budget (a full C2 scan is 0.2-0.7 s of CPU)."""
     th_all = host_threads()
@@ -223,12 +259,16 @@ def cpu_arms(case, tree, steps, warmup):
     # next to a large idle OpenMP team, so the best count lies between 3 and all: measured, not assumed
     counts = sorted({t for t in (3, 8, 16, 32, th_all) if t <= th_all})
     budget = REF_CPU_BUDGET_S / len(counts)
+    if tree is None and static is None:
+        sys.path.insert(0, os.path.join(ROOT, "oracle"))
+        import pyoracle as po
+        static = po.static_snapshot(case.map_xyz, case.map_normal_y)
     for th in counts:
-        probe = cpu_reference_run(case, tree, 1, 1, th)       # also the first warm-up
+        probe = cpu_reference_run(case, tree, 1, 1, th, static)       # also the first warm-up
         est = 1.0 / probe["scans_per_s"]
         k = int(max(1, min(steps, budget / est - warmup)))
         w = int(max(0, min(warmup - 1, budget / est - k)))
-        runs.append(cpu_reference_run(case, tree, k, w, th))
+        runs.append(cpu_reference_run(case, tree, k, w, th, static))
         runs[-1]["warmup"] = w + 2
     best = max(runs, key=lambda r: r["scans_per_s"])
     return best, runs
@@ -263,7 +303,7 @@ def run_reference(args, rank):
         "scaling": "strong", "vs_baseline": None, "dtype": "f64/f32", "data": "synthetic (seeded, malio_b200/synth.py)",
         "config": {"workload": WORKLOADS[args.config], "passes_per_scan": best["passes_per_scan"], "host_threads": host_threads(),
                    "steps_requested": args.steps, "warmup_requested": args.warmup,
-                   "map": ("live reference ikd-Tree: " + CHURN_NOTE) if tree is not None else "static snapshot (restated search)"},
+                   "map": ("live reference ikd-Tree: " + CHURN_NOTE) if tree is not None else "static balanced snapshot (the oracle's numpy builder; restated search)"},
         "cpu_baseline": cpu_baseline_obj(best, runs, f"{best['steps']} full {args.config} scans per thread count (steps bounded by a "
                                                          f"{REF_CPU_BUDGET_S:.0f} s CPU budget)"),
         "e2e": {"value": sps, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -328,7 +368,7 @@ def run_ours_c5(args, rank, world):
         sampler.start()
     for _ in range(max(args.warmup, 3)):
         m.Nearest_Search(q)
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     c0 = m.counters()
     dev_ms, e2e_ms = [], []
     tw0 = time.time()
@@ -353,13 +393,13 @@ def run_ours_c5(args, rank, world):
         if world > 1:
             dist.destroy_process_group()
         return
+    if args.dump_outputs:
+        # rank 0's shard of the caller-order lists; a fixed seeded sample keeps the dump small
+        pick = np.sort(np.random.default_rng(0).choice(idx.shape[0], min(C5_DUMP_QUERIES, idx.shape[0]), replace=False))
+        dump_outputs(args.dump_outputs, {"knn_query_index": pick + lo, "knn_idx": idx[pick], "knn_sqdist": d2[pick]})
     Q = q_all.shape[0]
     dev_s, e2e_s = t[0].item() * 1e-3 / steps, t[1].item() * 1e-3 / steps
-    peak, peak_src = 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
-    try:
-        peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]); peak_src = "MEASURED_PEAKS.json hbm_gbs"
-    except Exception:
-        pass
+    peak, peak_src = hbm_peak()
     cand = float(c1.knn_candidates - c0.knn_candidates) / float((c1.knn_queries - c0.knn_queries) or 1)
     bytes_per_launch = (hi - lo) * (12 + 9 * 8 + cand * 16 + 40)
     cpu = None
@@ -376,7 +416,7 @@ def run_ours_c5(args, rank, world):
                     "ms_per_step": e2e_s * 1e3, "what": "malio_knn: host queries -> sort -> search -> caller-order lists on the host"},
             "gpu_launches": int(c1.kernel_launches - c0.kernel_launches),
             "roofline": {"bound": "hbm", "kernel": "knn_direct_kernel (+ knn_list_kernel)", "achieved": bytes_per_launch / dev_s / 1e9,
-                         "peak": peak, "unit": "GB/s", "frac": bytes_per_launch / dev_s / 1e9 / peak, "traffic": NCU_DRAM_BYTES["knn_c5"] if world == 1 else None,
+                         "peak": peak, "unit": "GB/s", "frac": bytes_per_launch / dev_s / 1e9 / peak,
                          "algorithmic_bytes_per_launch": bytes_per_launch, "us_per_launch": dev_s * 1e6, "candidates_per_query": cand,
                          "fallback_queries_per_search": float(c1.knn_fallback_queries - c0.knn_fallback_queries) / steps,
                          "ring2_queries_per_search": float(c1.knn_ring2_queries - c0.knn_ring2_queries) / steps, "peak_source": peak_src,
@@ -447,7 +487,7 @@ def run_ours(args, rank, world):
     def step_resident():
         model.rearm_scan()
         x, P = case.x_prop.copy(), case.P_prop.copy()
-        return model.update_iterated_dyn_share_modified(x, P, case.max_iter), x
+        return model.update_iterated_dyn_share_modified(x, P, case.max_iter), x, P
 
     # root box of the map = the ikd-Tree root's node_range_* (node 0's point + its two children's boxes)
     n0 = snap.nodes[0]
@@ -625,13 +665,22 @@ def run_ours(args, rank, world):
     model.set_timing(False)       # no per-pass event records inside the measured loops
     tot_ms, reps, c0, c1, out, (tw0, tw1) = timed(step_resident, args.steps, args.warmup)
     x_res = out[1]
+    if args.dump_outputs and rank == 0:
+        rep = out[0]
+        dump = {"state": synth.state_to_vec(x_res, case.n_lidar), "covariance": out[2],
+                "report": np.array([rep.passes, rep.searches, rep.n_eff_last, rep.last_status], np.float64),
+                "dx_last": np.array(rep.dx_last[: case.n_dof], np.float64)}
+        a = model.aux()      # per-point outputs of the last pass of that step (this rank's block of the scan)
+        for k in ("world", "nn_idx", "nn_sqdist", "selected", "normal_y"):
+            dump["aux_" + k] = a[k]
+        dump_outputs(args.dump_outputs, dump)
     passes = sum(r.passes for r in reps)
     searches = sum(r.searches for r in reps)
     launches = int(c1.kernel_launches - c0.kernel_launches)
     host_ms = float(np.sum([r.ms_host_solve for r in reps]))
     value = args.steps / (tot_ms * 1e-3)
 
-    e_steps = max(3, min(args.steps, 10))
+    e_steps = args.steps
     e_ms, e_reps, ec0, ec1, e_out, _ = timed(step_e2e, e_steps, min(args.warmup, 3))
     flatten_ms = 1e3 * flat["s"] / max(flat["n"], 1) if tree is not None else None
     h2d = int(ec1.h2d_bytes - ec0.h2d_bytes) // e_steps
@@ -667,7 +716,7 @@ def run_ours(args, rank, world):
 
     # separate short loop with per-kernel CUDA events on (same steps, L2 flushed): kernel times for the rooflines
     model.set_timing(True)
-    r_steps = max(3, min(args.steps, 10))
+    r_steps = args.steps
     _, r_reps, rc0, rc1, _, (_, tw_end) = timed(step_resident, r_steps, 1)
     clocks = sampler.stop(tw0, tw_end) if rank == 0 else None
     knn_launches = int(rc1.knn_launches - rc0.knn_launches)
@@ -705,11 +754,7 @@ def run_ours(args, rank, world):
             dist.destroy_process_group()
         return
 
-    peak, peak_src = 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
-    try:
-        peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]); peak_src = "MEASURED_PEAKS.json hbm_gbs (burst copy)"
-    except Exception:
-        pass
+    peak, peak_src = hbm_peak()
     q_per_launch = (hi - lo)
     cand = int(rc1.knn_candidates - rc0.knn_candidates)
     roofs = []
@@ -719,19 +764,18 @@ def run_ours(args, rank, world):
         t_launch = knn_ms * 1e-3 / knn_launches
         achieved = bytes_per_launch / t_launch / 1e9
         n_q = case.pts.shape[0] // max(world, 1)
-        knn_name = ("knn_keys_kernel, 4 lanes per query" if n_q <= 256 * 148 else
-                    "knn_keys_kernel, 2 lanes per query" if n_q <= 1280 * 148 else "knn_direct_kernel, thread per query")
+        n_sm = torch.cuda.get_device_properties(local_rank).multi_processor_count   # the library's pick_group thresholds
+        knn_name = ("knn_keys_kernel, 4 lanes per query" if n_q <= 256 * n_sm else
+                    "knn_keys_kernel, 2 lanes per query" if n_q <= 1280 * n_sm else "knn_direct_kernel, thread per query")
         roofs.append({"bound": "hbm", "kernel": f"k-NN search: {knn_name} (+ knn_list_kernel)",
                       "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                      "traffic": NCU_DRAM_BYTES["knn"] if (world == 1 and args.config == "C2") else None,
                       "algorithmic_bytes_per_launch": bytes_per_launch, "us_per_launch": t_launch * 1e6,
                       "us_per_step": knn_ms * 1e3 / r_steps, "launches_timed": knn_launches, "candidates_per_query": cbar,
                       "fallback_queries_per_search": float(rc1.knn_fallback_queries - rc0.knn_fallback_queries) / knn_launches,
                       "ring2_queries_per_search": float(rc1.knn_ring2_queries - rc0.knn_ring2_queries) / knn_launches,
                       "peak_source": peak_src,
                       "note": "bytes = Q*(16 + 72 + C*16 + 57), C = candidates scanned per query (device counter); the cell-sorted point "
-                              "array and the scan are L2-resident at C2, so DRAM traffic is far below the algorithmic bytes; ncu: issue active 44 %, "
-                              "17 of 32 lanes, 0.59 waves (782 blocks): bound by divergence and latency at a grid that does not fill the machine"})
+                              "array and the scan fit in L2 at C2, so DRAM traffic can be far below the algorithmic bytes"})
     if pass_launches:
         # per point and pass: in 16 (scan point) + 16 (plane) + 8 (plane cov) + 16 (traces) + 1 (selected);
         # out 16 (world) + 4 (residual) + 8 (trace) + 4 (normal_y) + 96 (Jacobian row kept for the degenerate branch) + 1 + 1;
@@ -742,12 +786,12 @@ def run_ours(args, rank, world):
         t_launch = pass_ms * 1e-3 / pass_launches
         achieved = bytes_per_launch / t_launch / 1e9
         roofs.append({"bound": "hbm", "kernel": "pass_kernel (plane fit on search passes + gate + Jacobian rows + H^T R^-1 [H|h] + fold)",
-                      "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": NCU_DRAM_BYTES["pass"],
+                      "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                       "algorithmic_bytes_per_launch": bytes_per_launch, "us_per_launch": t_launch * 1e6,
                       "us_per_step": pass_ms * 1e3 / r_steps, "launches_timed": pass_launches, "search_pass_fraction": fit_frac,
                       "peak_source": peak_src,
-                      "note": "bytes/point = 57 in + 130 out (+144 on search passes); everything is L2-resident at C2: the kernel is "
-                              "bound by FP64 dependent-chain latency and two grid barriers, not by HBM (see profiles/)"})
+                      "note": "bytes/point = 57 in + 130 out (+144 on search passes); the working set fits in L2 at C2, so the kernel "
+                              "is bound by FP64 dependent-chain latency and two grid barriers rather than by HBM"})
     roofs.sort(key=lambda r: -r["us_per_step"])
     roof = roofs[0] if roofs else None
     roof2 = roofs[1] if len(roofs) > 1 else None
@@ -756,7 +800,7 @@ def run_ours(args, rank, world):
     if not args.no_cpu_baseline and world == 1:
         try:
             with c_stdout_to_stderr():
-                best, runs = cpu_arms(case, tree, 3, 1)
+                best, runs = cpu_arms(case, tree, 3, 1, None if tree is not None else (snap.nodes, snap.node_cov, snap.max_depth))
             cpu = cpu_baseline_obj(best, runs, f"3 full {args.config} scans after warm-up per thread count, same live ikd-Tree as the GPU arm")
         except Exception as e:   # the checker is optional for the product line
             cpu = {"value": None, "unit": UNIT, "cores": 0, "kind": "unavailable", "sample": repr(e)}

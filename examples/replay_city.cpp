@@ -14,12 +14,11 @@
 // There is no IMU stream in this example: the spline's control points are a constant pose (no motion inside the scan) and the
 // uncertainty lists hold two entries of a small constant covariance, so the numbers it prints are those of a static sensor.
 // The point is the call sequence and that it compiles and links against the header, the library and the reference's tree.
-// Status: compiled, linked and its --host-only part run in the CPU container; the device part was written after the round's GPU
-// budget was spent and has NOT been executed on a B200 yet (every call it makes is covered by tests/ through the ctypes mirror).
+// Tests: tests/test_examples_cpu.py runs its --host-only part, tests/test_gpu_more.py the whole program on the GPU.
 //
-// Build (tests/test_examples_cpu.py does this when /root/reference is present; running it needs a B200):
-//   g++ -O2 -std=c++14 -fopenmp -pthread -w -Ioracle/pcl_shim -I/root/reference/MA_LIO/include/ikd-Tree -Iinclude \
-//       examples/replay_city.cpp -Lma-lio_b200/malio_b200 -lmalio_b200 -o build/replay_city
+// Build (build() does this through oracle/Makefile when the reference checkout is present; running it needs an H100):
+//   g++ -O2 -std=c++14 -fopenmp -pthread -w -Ioracle/pcl_shim -I<reference>/MA_LIO/include/ikd-Tree -Iinclude \
+//       examples/replay_city.cpp -Lma-lio_b200/malio_b200 -lmalio_b200 -o oracle/_ref/replay_city
 //   ./replay_city ouster.bin avia.bin tele.bin      (no arguments: one synthetic scan per LiDAR)
 #include <cmath>
 #include <cstdint>
@@ -82,7 +81,7 @@ static std::vector<malio_raw_pt> load_raw(const char* path, bool ouster, unsigne
 }
 
 // --host-only: the host-side pieces alone (pose table, spline pose, the reference tree + the delta read-back), no device:
-// what tests/test_examples_cpu.py runs in the GPU-less container
+// what tests/test_examples_cpu.py runs without a GPU
 static int host_only() {
   const double q_id[4] = {1, 0, 0, 0}, t0[3] = {0, 0, 0}, t1[3] = {0.3, 0.1, -0.05};
   double cov6[36];

@@ -1,5 +1,5 @@
 /*
- * malio_b200.h — C-ABI of the B200-native MA-LIO measurement hot path.
+ * malio_b200.h — C-ABI of the H100-native (sm_90a) MA-LIO measurement hot path.
  *
  * Drop-in boundary (SURVEY.md §8b).  The reference's plug-in point is the IKFoM
  * measurement-model callback

@@ -1,6 +1,6 @@
-// malio_b200.cu — sm_100a kernels + device-side state of libmalio_b200.so.
+// malio_b200.cu — sm_90a kernels + device-side state of libmalio_b200.so.
 //
-// Hot path of MA-LIO's measurement update, B200-native (DESIGN.md has the data layout and rooflines):
+// Hot path of MA-LIO's measurement update, H100-native (DESIGN.md has the data layout and rooflines):
 //   K1 knn_kernel      KD_TREE::Nearest_Search / Search   (ikd_Tree.cpp:426-461, 1073-1255)
 //   K2 fit/tau/gate    h_share_model S1 + esti_plane (once per search) + evalPointUncertainty (once per scan)
 //                      (laserMapping.cpp:559-612, 725-743; common_lib.h:144-190; associate_uct.hpp:153-175)
@@ -2688,8 +2688,8 @@ static int pick_group(uint32_t n, int sm_count) {
   static const int forced = [] { const char* e = getenv("MALIO_KNN_GROUP"); return e ? atoi(e) : 0; }();
   if (forced == 1 || forced == 2 || forced == 4) return forced;
   const uint64_t per_sm = (uint64_t)n / (uint64_t)(sm_count > 0 ? sm_count : 1);
-  if (per_sm <= 256) return 4;        // <= ~38k queries on 148 SMs
-  if (per_sm <= 1280) return 2;       // <= ~190k
+  if (per_sm <= 256) return 4;        // <= ~34k queries on 132 SMs
+  if (per_sm <= 1280) return 2;       // <= ~169k
   return 1;                           // knn_direct_kernel
 }
 

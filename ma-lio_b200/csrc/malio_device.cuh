@@ -115,7 +115,7 @@ constexpr int MAIL_PARITY_BYTES = MAIL_MAX_WORLD * (MAIL_MIN_BYTES + MAIL_SUM_BY
 constexpr int MAIL_BYTES = 2 * MAIL_PARITY_BYTES;
 struct DeviceState {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;            // box rebuild of the compact upload runs beside the scan's first kernels
   cudaStream_t stream3 = nullptr;            // copy stream for the map-side weights of the compact upload

@@ -121,7 +121,7 @@ void sym3_singular_values(const double S[6], double sv[3]) { malio_manifold::sym
 // =================================================================== C-ABI
 extern "C" {
 
-const char* malio_version(void) { return "malio_b200 0.1 (sm_100a)"; }
+const char* malio_version(void) { return "malio_b200 0.1 (sm_90a)"; }
 
 void malio_default_params(malio_params* p, int n_lidar) {
   if (!p) return;

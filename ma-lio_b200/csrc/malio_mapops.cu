@@ -1,5 +1,5 @@
 // malio_mapops.cu — SURVEY.md §8f N1: the map as a device-resident point set kept in step with the host's ikd-Tree by
-// deltas (host side and reasoning: include/malio_mapsync.hpp), sm_100a.
+// deltas (host side and reasoning: include/malio_mapsync.hpp), sm_90a.
 //
 // Reference calls mirrored (paths relative to /root/reference/MA_LIO/include/ikd-Tree):
 //   KD_TREE::Build                ikd_Tree.cpp:370-424     -> build()

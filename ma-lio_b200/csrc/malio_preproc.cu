@@ -1,4 +1,4 @@
-// malio_preproc.cu — the two stages immediately before the hot path (SURVEY.md §8f), sm_100a:
+// malio_preproc.cu — the two stages immediately before the hot path (SURVEY.md §8f), sm_90a:
 //   N2  ImuProcess::UndistortPcl's per-raw-point loop        src/IMU_Processing.hpp:468-508
 //       BsplineSE3::get_pose                                  src/BsplineSE3.cpp:84-118, quat_ops.h:150-257
 //   N3  pcl::VoxelGrid down-sampling + merge into the scan    src/laserMapping.cpp:968-983

@@ -1,4 +1,4 @@
-// malio_solve.cu — the IESKF step on the device (sm_100a): esekf::update_iterated_dyn_share_modified's per-pass algebra
+// malio_solve.cu — the IESKF step on the device (sm_90a): esekf::update_iterated_dyn_share_modified's per-pass algebra
 // (esekfom.hpp:521-718) as a one-block kernel that runs after every measurement pass, so that a whole iterated update is ONE
 // enqueued kernel sequence without a host round trip per pass.
 //

@@ -283,6 +283,54 @@ def knn_snapshot(nodes, cov, q, k=5, nthreads=1):
     return ids, d2, found, int(visits.value)
 
 
+def static_snapshot(xyz, normal_y=0.001):
+    """Balanced k-d tree over xyz in snapshot form, built without the product library (so that CPU-only callers such as
+    bench.py's reference arm never map it): median split on the longest axis (ikd_Tree.cpp:696-735), DFS pre-order, child
+    boxes = the children's point AABBs — the layout of malio_build_static_snapshot.  Points with equal coordinates on the
+    split axis may land on other sides of a split than there (std::nth_element leaves their order unspecified); every
+    snapshot this builds is a valid balanced tree for the restated search.  All nodes of one tree level are split together
+    (one sort per level).  Returns (nodes capi.MAP_NODE[M], node_cov float32[M], max_depth)."""
+    xyz = np.ascontiguousarray(xyz, np.float32)
+    n = xyz.shape[0]
+    nodes = np.zeros(n, capi.MAP_NODE)
+    order = np.arange(n, dtype=np.int64)
+    slot_pt = np.zeros(n, np.int64)
+    link = np.zeros(n, np.uint32)
+    box = np.zeros((n, 6), np.float32)            # AABB of the subtree rooted at each slot
+    lo, hi, slot = (np.zeros(1, np.int64), np.full(1, n - 1, np.int64), np.zeros(1, np.int64)) if n else (np.zeros(0, np.int64),) * 3
+    depth = 0
+    while lo.size:
+        depth += 1
+        cnt = hi - lo + 1
+        starts = np.cumsum(cnt) - cnt
+        seg = np.repeat(np.arange(lo.size, dtype=np.int64), cnt)
+        pos = np.repeat(lo - starts, cnt) + np.arange(int(cnt.sum()), dtype=np.int64)   # this level's positions, by segment
+        p = xyz[order[pos]]
+        mn, mx = np.minimum.reduceat(p, starts, axis=0), np.maximum.reduceat(p, starts, axis=0)
+        axis = np.argmax(mx - mn, axis=1)         # first longest axis, like the strict '>' of the C++ builder
+        key = np.ascontiguousarray(p[np.arange(p.shape[0]), axis[seg]]).view(np.uint32)
+        key = key ^ np.where(key >> 31 == 1, np.uint32(0xFFFFFFFF), np.uint32(0x80000000))   # float order as unsigned order
+        o = np.argsort((seg.astype(np.uint64) << np.uint64(32)) | key.astype(np.uint64))        # sorted within each segment
+        order[pos] = order[pos[o]]
+        mid = (lo + hi) >> 1
+        slot_pt[slot] = order[mid]
+        box[slot, 0::2], box[slot, 1::2] = mn, mx
+        nl, nr = mid - lo, hi - mid
+        link[slot] = np.where(nl > 0, capi.LINK_HAS_LEFT, 0) | np.where(nr > 0, capi.LINK_HAS_RIGHT | (slot + 1 + nl), 0)
+        L, R = nl > 0, nr > 0
+        lo, hi, slot = (np.concatenate([lo[L], mid[R] + 1]), np.concatenate([mid[L] - 1, hi[R]]),
+                        np.concatenate([slot[L] + 1, (slot + 1 + nl)[R]]))
+    nodes["xyz"] = xyz[slot_pt]
+    nodes["link"] = link
+    idx = np.arange(n)
+    hl = (link & capi.LINK_HAS_LEFT) != 0
+    hr = (link & capi.LINK_HAS_RIGHT) != 0
+    nodes["lbox"][hl] = box[idx[hl] + 1]
+    nodes["rbox"][hr] = box[(link[hr] & capi.LINK_INDEX_MASK).astype(np.int64)]
+    cov = np.full(n, normal_y, np.float32) if np.isscalar(normal_y) else np.asarray(normal_y, np.float32)[slot_pt]
+    return nodes, np.ascontiguousarray(cov), depth
+
+
 class Oracle:
     """Restated h_share_model + update_iterated_dyn_share_modified on the CPU."""
 

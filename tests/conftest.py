@@ -10,7 +10,7 @@ for p in (os.path.join(ROOT, "ma-lio_b200"), os.path.join(ROOT, "oracle"), ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a)")
 
 
 @pytest.fixture(scope="session", autouse=True)

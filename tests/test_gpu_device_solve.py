@@ -12,7 +12,7 @@ pytestmark = pytest.mark.gpu
 
 
 def _pair(case, snap, monkeypatch):
-    monkeypatch.setenv("MALIO_DEVICE_SOLVE", "1")     # opt-in (measured slower than the host loop on B200, see DESIGN.md)
+    monkeypatch.setenv("MALIO_DEVICE_SOLVE", "1")     # opt-in experiment, see DESIGN.md
     dev = H.make_model(case, snap)
     monkeypatch.setenv("MALIO_DEVICE_SOLVE", "0")
     host = H.make_model(case, snap)

@@ -280,3 +280,21 @@ def test_map_incremental_decision_matches_oracle():
                 assert np.array_equal(w_g, w_o)
         assert len(set(cls_g.tolist())) >= 1
         model.close()
+
+
+EXAMPLE = os.path.join(ROOT, "oracle", "_ref", "replay_city")
+
+
+@pytest.mark.skipif(not os.path.exists(EXAMPLE), reason="oracle/_ref/replay_city not built (needs the reference's ikd_Tree.cpp)")
+def test_cpp_example_full_program_on_the_gpu():
+    """examples/replay_city.cpp end to end on the device: undistortion + voxel grid of three synthetic LiDARs, merged scan,
+    iterated update against the device-resident map, map_incremental and the map deltas; the device's live point count must
+    equal the reference tree's valid count afterwards (the program's exit code says so)."""
+    r = subprocess.run([EXAMPLE], capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0, (r.returncode, r.stdout[-1500:], r.stderr[-1500:])
+    lines = r.stdout.splitlines()
+    assert lines[0].startswith("malio_b200") and sum(l.startswith("LiDAR ") for l in lines) == 3
+    upd = [l for l in lines if l.startswith("update:")][0].split()
+    passes, n_eff = int(upd[1]), int(upd[upd.index("N_eff") + 1].rstrip(","))
+    assert 1 <= passes <= 4 and n_eff > 0
+    assert any(l.startswith("map: tree holds") for l in lines)

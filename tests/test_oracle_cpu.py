@@ -146,6 +146,17 @@ def test_static_snapshot_builder_invariants():
     assert np.all(ri > np.arange(n)[hr])
 
 
+@pytest.mark.parametrize("n", [1, 2, 3, 7, 20000])
+def test_oracle_static_snapshot_equals_the_product_builder(n):
+    """pyoracle.static_snapshot (what bench.py's reference arm builds its map with, without mapping the product library)
+    lays out the same tree as malio_build_static_snapshot when no two points share a coordinate on a split axis."""
+    xyz = synth.make_world(20000, seed=5)[:n]
+    ny = np.linspace(0.001, 0.01, n, dtype=np.float32)
+    nodes, cov, depth = po.static_snapshot(xyz, ny)
+    snap = plugin.build_static_snapshot(xyz, ny)
+    assert nodes.tobytes() == snap.nodes.tobytes() and np.array_equal(cov, snap.node_cov) and depth == snap.max_depth
+
+
 # ------------------------------------------------------------------ P / U / algebra vs numpy
 def test_esti_plane_vs_scipy_qr():
     L = po.oracle_lib()

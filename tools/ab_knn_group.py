@@ -35,7 +35,7 @@ if len(sys.argv) > 1 and sys.argv[1] == "child":
     print("keys", os.environ.get("MALIO_KNN_KEYS", "1"), "group", os.environ.get("MALIO_KNN_GROUP", "auto"), "knn us:", "  ".join(out), flush=True)
 else:
     # "old" = knn_direct_kernel; 2 / 4 = the key scan with that many lanes per query (4 lanes also preload the rows' first candidates).
-    # The sweep of profiles/r02_knn_variants_sweep.log also varied the preload and tried 1 and 8 lanes: those instantiations were
+    # An earlier sweep also varied the preload and tried 1 and 8 lanes: those instantiations were
     # removed from the library afterwards (MALIO_KNN_GROUP accepts 1, 2, 4).
     for g in ("old", "2", "4", "auto"):
         env = dict(os.environ)

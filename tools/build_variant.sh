@@ -1,5 +1,5 @@
 #!/bin/bash
-# Build a kernel-parameter variant of libmalio_b200.so under build/variants/<name>/ (git-ignored, shipped to the GPU box).
+# Build a kernel-parameter variant of libmalio_b200.so under build/variants/<name>/ (git-ignored).
 #   tools/build_variant.sh t1b6 "-DMALIO_PASS_TILES=1 -DMALIO_PASS_MINB=6"
 # Use it with MALIO_LIB_PATH=build/variants/<name>/libmalio_b200.so
 set -e
@@ -8,13 +8,14 @@ root=$(cd "$(dirname "$0")/.." && pwd)
 out=$root/build/variants/$name
 mkdir -p $out
 cd $root/ma-lio_b200/csrc
-NV="/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -fmad=false -Xcompiler -fPIC -ccbin /usr/bin/g++ -I../../include -I. $extra"
+NVCC=${NVCC:-nvcc}
+NV="$NVCC -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -fmad=false -Xcompiler -fPIC -ccbin /usr/bin/g++ -I../../include -I. $extra"
 for f in malio_b200 malio_preproc malio_mapops malio_solve; do
   $NV -Xptxas -v -c $f.cu -o $out/$f.o 2> $out/ptxas_$f.log &
 done
 /usr/bin/g++ -O3 -std=c++17 -fPIC -fopenmp -Wall -I../../include -I. -c malio_host.cpp -o $out/malio_host.o
 /usr/bin/g++ -O3 -std=c++17 -fPIC -fopenmp -Wall -ffp-contract=off -I../../include -I. -c malio_dataset.cpp -o $out/malio_dataset.o
 wait
-/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -shared -ccbin /usr/bin/g++ -Xcompiler -fPIC $out/*.o -o $out/libmalio_b200.so -lgomp -ldl
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -ccbin /usr/bin/g++ -Xcompiler -fPIC $out/*.o -o $out/libmalio_b200.so -lgomp -ldl
 grep -A2 "pass_kernel" $out/ptxas_malio_b200.log | grep -E "registers|spill" | head -8
 echo "built $out/libmalio_b200.so"

@@ -1,8 +1,7 @@
-"""Timing of the stages before the hot path (SURVEY.md §8f N2, N3, N4) on the GPU box: malio_undistort / malio_voxel_grid /
+"""Timing of the stages before the hot path (SURVEY.md §8f N2, N3, N4) on the GPU: malio_undistort / malio_voxel_grid /
 malio_upload_scan_device through the C-ABI with HOST buffers (copies inside the timed region) next to the CPU oracle
 (oracle/oracle_undistort.cpp, one thread: UndistortPcl's point loop and pcl::VoxelGrid are serial in the reference), and
-the .bin reader (host code) on a synthetic City-format file.  Prints one JSON line per stage.  Not a bench value: context
-for profiles/r02_preproc.md."""
+the .bin reader (host code) on a synthetic City-format file.  Prints one JSON line per stage.  Not a bench value: context for DESIGN.md."""
 import json
 import os
 import sys
