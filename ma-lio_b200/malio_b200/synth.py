@@ -6,7 +6,7 @@ the CUDA path and to the CPU oracle.  Extrinsics are the reference's /root/refer
 """
 from __future__ import annotations
 
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 
 import numpy as np
 
@@ -216,14 +216,26 @@ def init_P(n: int) -> np.ndarray:
     return P
 
 
-def make_tables(L: int, T: int, rng):
-    """pose_unc[l][j]: small SE(3) (<= 2 cm, <= 0.2 deg) and covariance growing with j (seed 45 stream)."""
-    table = np.zeros(L * T, dtype=capi.POSE_ENTRY)
+def table_sizes(L: int, T) -> np.ndarray:
+    """Per-LiDAR pose-table lengths: one length for all LiDARs, or one per LiDAR (real scans: pose_unc[l] has one entry per
+    IMU sample of LiDAR l, laserMapping.cpp:1028-1045).  upload_scan needs at least 2 per LiDAR."""
+    sizes = np.full(L, T, dtype=np.int64) if np.isscalar(T) else np.asarray(T, dtype=np.int64)
+    assert sizes.shape == (L,) and sizes.min() >= 2, sizes
+    return sizes
+
+
+def make_tables(L: int, T, rng):
+    """pose_unc[l][j]: small SE(3) (<= 2 cm, <= 0.2 deg) and covariance growing with j (seed 45 stream).  T: one table
+    length for every LiDAR or a sequence of L lengths; table_off is their cumulative sum."""
+    sizes = table_sizes(L, T)
+    table_off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.uint32)
+    table = np.zeros(int(table_off[-1]), dtype=capi.POSE_ENTRY)
     for l in range(L):
         axis = rand_unit(rng)
         tdir = rand_unit(rng)
-        for j in range(T):
-            f = (j + 1) / T
+        Tl = int(sizes[l])
+        for j in range(Tl):
+            f = (j + 1) / Tl
             q = q_exp(axis * np.deg2rad(0.2) * f)
             Tm = np.eye(4)
             Tm[:3, :3] = q_to_R(q)
@@ -231,16 +243,53 @@ def make_tables(L: int, T: int, rng):
             d = np.linspace(1e-8, 1e-6, 6) * (0.2 + f)
             A = rng.normal(size=(6, 6)) * 1e-4 * np.sqrt(f)
             cov = np.diag(d) + A @ A.T * 0.05
-            table[l * T + j]["T"] = Tm
-            table[l * T + j]["cov"] = cov
-    table_off = np.arange(L + 1, dtype=np.uint32) * T
+            table[table_off[l] + j]["T"] = Tm
+            table[table_off[l] + j]["cov"] = cov
     return table, table_off
+
+
+def draw_table_idx(mode: str, lidar: np.ndarray, T, rng) -> np.ndarray:
+    """Pose-table index of each scan point.
+      in_range  uniform in [0, T_l) of the point's LiDAR;
+      edges     T_l - 2, T_l - 1, T_l, T_l + 1 of the point's LiDAR (the two clamps, laserMapping.cpp:694-696 and 737-739);
+      raw       what a merged scan carries when the index is the point's intensity (laserMapping.cpp:972-977) and the
+                undistortion left that intensity as the raw reflectivity: uniform in 0..255 with ~1 % at 65535."""
+    N = lidar.shape[0]
+    if mode == "in_range" and np.isscalar(T):
+        return rng.integers(0, T, size=N).astype(np.uint16)   # the original draw: default cases stay byte-identical
+    sizes = table_sizes(int(lidar.max(initial=0)) + 1, T) if np.isscalar(T) else np.asarray(T, dtype=np.int64)
+    if mode == "in_range":
+        return rng.integers(0, sizes[lidar]).astype(np.uint16)
+    if mode == "edges":
+        return (sizes[lidar] + rng.integers(-2, 2, size=N)).astype(np.uint16)
+    if mode == "raw":
+        idx = rng.integers(0, 256, size=N)
+        idx[rng.random(N) < 0.01] = 65535
+        return idx.astype(np.uint16)
+    raise ValueError(f"table_idx mode {mode!r}")
+
+
+def world_to_sensor(pw: np.ndarray, lidar: np.ndarray, pos, rot, extq, extt, tcomp) -> np.ndarray:
+    """World points -> the frame of the LiDAR that saw them (float64): the inverse of pointBodyToWorld with the temporal
+    compensation of LiDARs 1.. (laserMapping.cpp:134-147)."""
+    p_imu = (pw - pos) @ q_to_R(rot)      # R^T (p - pos), row-vector form
+    xyz = np.zeros((pw.shape[0], 3))
+    for l in range(len(extq)):
+        m = lidar == l
+        v = p_imu[m]
+        if l != 0:
+            Rc = q_to_R(tcomp[l - 1]["q"])
+            v = (v - tcomp[l - 1]["t"]) @ Rc          # qC^T (p - tC)
+        Re = q_to_R(extq[l])
+        xyz[m] = (v - extt[l]) @ Re                   # qE^T (. - tE)
+    return xyz
 
 
 def make_case(name: str, N: int, M: int, n_lidar: int, max_iter: int, *, varied_map_cov: bool = False,
               seed_world: int = 42, seed_scan: int = 43, seed_state: int = 44, seed_tables: int = 45,
-              det_range: float = 100.0, table_T: int = 10, map_xyz: np.ndarray | None = None,
-              pos_err: float = 0.10, rot_err_deg: float = 0.5) -> Case:
+              det_range: float = 100.0, table_T=10, map_xyz: np.ndarray | None = None,
+              pos_err: float = 0.10, rot_err_deg: float = 0.5, table_idx: str = "in_range") -> Case:
+    """table_T: pose-table length of every LiDAR, or one length per LiDAR; table_idx: see draw_table_idx."""
     L = n_lidar
     if map_xyz is None:
         map_xyz = make_world(M, seed_world)
@@ -266,26 +315,15 @@ def make_case(name: str, N: int, M: int, n_lidar: int, max_iter: int, *, varied_
 
     pw = sample_surfaces(N, pos_true[:2], min(det_range, half), half, rng)
     pw += rng.normal(0, 0.02, size=pw.shape)
-    Rt = q_to_R(rot_true)
-    p_imu = (pw - pos_true) @ Rt          # R^T (p - pos), row-vector form
     split = np.array(LIDAR_SPLIT[:L], dtype=np.float64)
     split = split / split.sum()
     counts = np.floor(split * N).astype(int)
     counts[0] += N - counts.sum()
     lidar = np.repeat(np.arange(L), counts)
     pts = np.zeros(N, dtype=capi.SCAN_PT)
-    xyz = np.zeros((N, 3))
-    for l in range(L):
-        m = lidar == l
-        v = p_imu[m]
-        if l != 0:
-            Rc = q_to_R(tcomp[l - 1]["q"])
-            v = (v - tcomp[l - 1]["t"]) @ Rc          # qC^T (p - tC)
-        Re = q_to_R(extq[l])
-        xyz[m] = (v - extt[l]) @ Re                   # qE^T (. - tE)
-    pts["xyz"] = xyz.astype(np.float32)
+    pts["xyz"] = world_to_sensor(pw, lidar, pos_true, rot_true, extq, extt, tcomp).astype(np.float32)
     pts["lidar"] = lidar.astype(np.uint16)
-    pts["table_idx"] = rng.integers(0, table_T, size=N).astype(np.uint16)
+    pts["table_idx"] = draw_table_idx(table_idx, lidar, table_T, rng)
 
     rs = np.random.default_rng(seed_state)
     x_true = make_state(pos_true, rot_true, extq, extt, vel=rs.normal(0, 0.5, 3), bg=rs.normal(0, 1e-3, 3),
@@ -298,6 +336,141 @@ def make_case(name: str, N: int, M: int, n_lidar: int, max_iter: int, *, varied_
     prm = capi.default_params(L)
     return Case(name, L, max_iter, map_xyz, map_ny, pts, table, table_off, tcomp if L > 1 else None, x_true, x_prop,
                 init_P(17 + 6 * L), prm, meta=dict(N=N, M=M, half=half))
+
+
+# ------------------------------------------------------------------ scenes derived from a case
+def _sensor_points(case: Case, pw: np.ndarray, rng) -> np.ndarray:
+    """World points as scan points of `case` (seen from its true state), LiDARs assigned round-robin, table index in range."""
+    n = pw.shape[0]
+    lidar = np.arange(n) % case.n_lidar
+    s = case.x_true
+    extq = [np.array(s.ext[l].q[:]) for l in range(case.n_lidar)]
+    extt = [np.array(s.ext[l].t[:]) for l in range(case.n_lidar)]
+    pts = np.zeros(n, dtype=capi.SCAN_PT)
+    pts["xyz"] = world_to_sensor(pw, lidar, np.array(s.pos[:]), np.array(s.rot[:]), extq, extt,
+                                 case.temporal_comp).astype(np.float32)
+    pts["lidar"] = lidar.astype(np.uint16)
+    sizes = np.diff(case.table_off.astype(np.int64))
+    pts["table_idx"] = rng.integers(0, sizes[lidar]).astype(np.uint16)
+    return pts
+
+
+def with_scan(case: Case, pw: np.ndarray, *, keep: int = 0, seed: int = 0, name: str | None = None, **changes) -> Case:
+    """A copy of `case` whose scan is its first `keep` points followed by the world points `pw` (seen from the true state);
+    other fields may be replaced through `changes` (e.g. map_xyz, map_normal_y)."""
+    pts = np.concatenate([case.pts[:keep], _sensor_points(case, np.asarray(pw, np.float64).reshape(-1, 3),
+                                                            np.random.default_rng(seed))])
+    meta = dict(case.meta, N=int(pts.shape[0]))
+    return replace(case, name=name or case.name, pts=pts, meta=meta, **changes)
+
+
+def translated(case: Case, offset) -> Case:
+    """The same scene moved by `offset` (metres): map points (rounded to float32 again) and both states' positions.  The
+    scan is in sensor frames and does not change."""
+    off = np.asarray(offset, np.float64)
+    xt, xp = case.x_true.copy(), case.x_prop.copy()
+    xt.pos[:] = list(np.array(xt.pos[:]) + off)
+    xp.pos[:] = list(np.array(xp.pos[:]) + off)
+    return replace(case, name=f"{case.name} +{off.tolist()}", x_true=xt, x_prop=xp,
+                   map_xyz=np.ascontiguousarray((case.map_xyz.astype(np.float64) + off).astype(np.float32)))
+
+
+def surface_scan_points(case: Case, n_ground: int, n_xwall: int, n_ywall: int, seed: int = 0) -> np.ndarray:
+    """World points on the ground (z = 0) and on the two walls of the street grid closest to the true position (the wall
+    along x at y = c and the one along y at x = c), with the scan's 2 cm noise.  The mix sets the spread of plane normals
+    and so the ratio of the singular values behind the localization weight (laserMapping.cpp:745-756): ground only
+    gives sigma3/sigma1 ~ 0, a box room with equal shares ~ 1."""
+    rng = np.random.default_rng(seed)
+    px, py = case.x_true.pos[0], case.x_true.pos[1]
+    lines = _wall_lines(case.meta["half"])
+    cy = lines[np.argmin(np.abs(lines - py))]
+    cx = lines[np.argmin(np.abs(lines - px))]
+    r = np.sqrt(rng.uniform(0, 1, n_ground)) * 15.0
+    a = rng.uniform(-np.pi, np.pi, n_ground)
+    ground = np.stack([px + r * np.cos(a), py + r * np.sin(a), np.zeros(n_ground)], axis=1)
+    xwall = np.stack([px + rng.uniform(-15, 15, n_xwall), np.full(n_xwall, cy), rng.uniform(0.5, 15, n_xwall)], axis=1)
+    ywall = np.stack([np.full(n_ywall, cx), py + rng.uniform(-15, 15, n_ywall), rng.uniform(0.5, 15, n_ywall)], axis=1)
+    pw = np.concatenate([ground, xwall, ywall])
+    return pw + rng.normal(0, 0.02, size=pw.shape)
+
+
+# Degenerate plane-fit neighbourhoods (esti_plane, common_lib.h:144-190) planted into a map around known scan points:
+#   duplicates     6 copies of one point (A has rank 1; x == y at the site, so two column norms tie exactly)
+#   pole           a vertical line at 5 cm spacing (rank 2; again x == y)
+#   floor_z0       a patch exactly at z = 0 (a zero column; the plane holds the world origin)
+#   origin_plane   a vertical plane through the world origin (A n = -1 has no exact solution)
+#   cluster        6 points within 1e-4 m
+#   zero_weight    a plane patch whose map weights are all <= 1e-5 (the W(0,0) gate: plane_cov = 0, weight 1)
+#   cov_threshold  a plane patch whose map weights all equal cov_threshold (cov_sum = 0: esti_plane computes 0/0)
+DEGENERATE_KINDS = ("duplicates", "pole", "floor_z0", "origin_plane", "cluster", "zero_weight", "cov_threshold")
+
+
+def degenerate_sites(kinds, per_kind: int, half: float):
+    """Site centres on a 10 m grid, >= 5 m from every wall and, in the air, >= 5 m above the ground; the two kinds that
+    need x == y take diagonal cells.  Returns [(kind, (x, y, z))]."""
+    g = np.arange(-half + 5.0, half - 4.0, 10.0)
+    diag = [(v, v) for v in g if v != 0.0]
+    off = [(x, y) for x in g for y in g if x != y and not (x == 0.0 and y == 0.0)]
+    out, nd, no = [], 0, 0
+    for k in kinds:
+        for i in range(per_kind):
+            if k in ("duplicates", "pole"):
+                x, y = diag[nd]; nd += 1
+            else:
+                x, y = off[no]; no += 1
+            z = 0.0 if k == "floor_z0" else 5.0 + 5.0 * (i % 3)
+            out.append((k, (float(x), float(y), z)))
+    return out
+
+
+def plant_degenerate(map_xyz: np.ndarray, map_ny: np.ndarray, sites, cov_threshold: float = 0.5, seed: int = 0):
+    """Clear the map within 4 m of every site and plant the site's structure there.  Returns (map_xyz, map_ny, scan_world
+    [n,3], scan_site [n]): three scan points per site, each with its 5 nearest map points inside the structure."""
+    rng = np.random.default_rng(seed)
+    keep = np.ones(map_xyz.shape[0], bool)
+    for _, c in sites:
+        keep &= np.sum((map_xyz.astype(np.float64) - c) ** 2, axis=1) > 16.0
+    xyz, ny = [map_xyz[keep].astype(np.float64)], [map_ny[keep]]
+    scan, owner = [], []
+    for s, (kind, c) in enumerate(sites):
+        c = np.asarray(c, np.float64)
+        uv = np.arange(-1.5, 1.5001, 0.25)
+        U, V = np.meshgrid(uv, uv, indexing="ij")
+        U, V = U.ravel(), V.ravel()
+        w = np.full(U.size, 0.001, np.float32)
+        near = np.array([[0.03, -0.02, 0.04], [-0.04, 0.05, 0.02], [0.02, 0.03, -0.05]])
+        if kind == "duplicates":
+            p = np.repeat(c[None], 6, axis=0)
+            w = np.full(6, 0.001, np.float32)
+        elif kind == "pole":
+            p = c + np.outer(np.arange(-6, 7) * 0.05, [0.0, 0.0, 1.0])
+            w = np.full(p.shape[0], 0.001, np.float32)
+            near = np.array([[0.04, 0.07, 0.012], [-0.03, 0.02, 0.11], [0.05, -0.04, -0.09]])
+        elif kind == "floor_z0":
+            p = np.stack([c[0] + U, c[1] + V, np.zeros(U.size)], axis=1)
+            near = np.array([[0.1, -0.07, 0.03], [-0.12, 0.05, 0.02], [0.06, 0.11, -0.02]])
+        elif kind == "origin_plane":
+            d = np.array([c[0], c[1], 0.0]) / np.hypot(c[0], c[1])   # in-plane horizontal direction: the plane holds 0
+            nrm = np.array([-d[1], d[0], 0.0])
+            p = c + np.outer(U, d) + np.outer(V, [0.0, 0.0, 1.0])
+            near = np.array([0.1 * d + 0.03 * nrm, -0.08 * d + [0, 0, 0.1] - 0.02 * nrm, 0.05 * d - [0, 0, 0.07] + 0.04 * nrm])
+        elif kind == "cluster":
+            p = c + rng.uniform(-1e-4, 1e-4, size=(6, 3))
+            w = np.full(6, 0.001, np.float32)
+            near = np.array([[0.01, 0.005, -0.008], [-0.006, 0.01, 0.004], [0.003, -0.009, 0.01]])
+        elif kind in ("zero_weight", "cov_threshold"):
+            p = np.stack([c[0] + U, c[1] + V, np.full(U.size, c[2])], axis=1)
+            if kind == "zero_weight":
+                w = np.array([0.0, 1e-6, 1e-5], np.float32)[np.arange(U.size) % 3]
+            else:
+                w = np.full(U.size, cov_threshold, np.float32)
+            near = np.array([[0.1, -0.07, 0.03], [-0.12, 0.05, 0.02], [0.06, 0.11, -0.02]])
+        else:
+            raise ValueError(kind)
+        xyz.append(p); ny.append(w)
+        scan.append(c + near); owner += [s] * near.shape[0]
+    return (np.ascontiguousarray(np.concatenate(xyz).astype(np.float32)), np.ascontiguousarray(np.concatenate(ny).astype(np.float32)),
+            np.concatenate(scan), np.array(owner))
 
 
 # BASELINE.json configs

@@ -97,6 +97,39 @@ def test_product_host_ieskf_reproduces_the_oracle_update(stub, L, max_iter):
     assert np.allclose(Pp, Pp.T, rtol=1e-9, atol=1e-15)
 
 
+@pytest.mark.parametrize("L,tables,mode", [(3, (2, 7, 40), "raw"), (3, (2, 7, 40), "edges"), (1, 5, "raw")])
+@pytest.mark.parametrize("ext_en", [0, 1])
+def test_product_host_ieskf_frozen_extrinsics_and_uneven_tables(stub, L, tables, mode, ext_en):
+    """extrinsic_est_en = 0: the extrinsic columns of every reduced system are exactly zero, so the information block the
+    host algebra inverts is rank-deficient there and only the prior holds those states; pose tables of different lengths
+    per LiDAR with table indices at and beyond their ends."""
+    case = synth.make_case(f"hf{L}", 3000, 40000, L, 3, varied_map_cov=True, table_T=tables, table_idx=mode)
+    case.params.extrinsic_est_en = ext_en
+    snap = plugin.build_static_snapshot(case.map_xyz, case.map_normal_y)
+    orc = H.make_oracle(case, snap)
+    assert orc.h_share_model(case.x_prop, True, 2)
+    HTH, HTh = orc.reduce()
+    ext = np.arange(6, 6 * (L + 1))
+    st = orc.stats()
+    if ext_en:
+        assert np.abs(HTH[np.ix_(ext, ext)]).max() > 0 and st.tau_max > st.tau_min
+    else:
+        assert not HTH[ext].any() and not HTH[:, ext].any() and not HTh[ext].any()
+        assert (st.tau_min, st.tau_max) == (9999.0, 0.0)
+    rc, rep, xp, Pp, rco, rep_o, xo, Po, log = _run(stub, case, snap, 3)
+    assert rc == capi.OK and rco == 0
+    assert rep.passes == rep_o.passes and rep.searches == rep_o.searches and rep.converged_count == rep_o.converged_count
+    n = case.n_dof
+    assert np.abs(synth.state_to_vec(xp, L) - synth.state_to_vec(xo, L)).max() < 1e-9
+    assert np.abs(np.array(rep.dx_last[:n]) - np.array(rep_o.dx_last[:n])).max() < 1e-9
+    assert H.rel_err(Pp, Po) < 1e-7
+    if not ext_en:   # nothing observes the extrinsics: they keep their prior value, their covariance its prior block
+        e = slice(6, 6 + 6 * L)
+        v0, v1 = synth.state_to_vec(case.x_prop, L), synth.state_to_vec(xp, L)
+        assert np.abs(v1[7:7 + 7 * L] - v0[7:7 + 7 * L]).max() < 1e-12
+        assert H.rel_err(Pp[e, e], case.P_prop[e, e]) < 1e-12
+
+
 def test_product_host_degenerate_and_invalid_branches(stub):
     base = synth.make_case("hb", 3000, 40000, 3, 3, varied_map_cov=True)
     snap = plugin.build_static_snapshot(base.map_xyz, base.map_normal_y)
