@@ -301,7 +301,11 @@ int malio_bspline_get_pose(const double* ctrl_t, const double* ctrl_T, uint32_t 
  * result is x, y, z and the averaged `intensity` (the table index, moved to normal_x at :975).
  * in == NULL: take the device-resident output of the last malio_undistort(h, lidar, ...) (x, y, z, intensity = idx,
  * curvature; points the undistortion left untouched keep intensity 0).  in != NULL: n x 5 floats
- * {x, y, z, intensity, curvature} from the host.  Outputs (may be NULL): out n_out x 5 floats, same layout; *n_out.
+ * {x, y, z, intensity, curvature} from the host.  Outputs (may be NULL): out n_out x 5 floats, same layout, at most out_cap
+ * of them; *n_out = the full count.  Non-finite points are skipped; a cloud without a finite point gives n_out = 0.
+ * MALIO_ERR_CAPACITY (nothing computed) when the grid has more than 2^28 voxels, more than 2^24 voxels along one axis, or
+ * a voxel index floor(x / leaf) outside int.  PCL accepts up to 2^31 voxels, but its per-axis index is a float
+ * subtraction that can round up to the axis' size above 2^24 voxels; such leaf sizes are refused here instead.
  * The down-sampled cloud also stays on the device as LiDAR `lidar`'s part of the next scan (malio_upload_scan_device). */
 int malio_voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap,
                      uint32_t* n_out);

@@ -655,11 +655,22 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
   c.il = 1.0f / leaf;
   int maxb[3];
   for (int k = 0; k < 3; ++k) {
-    c.minb[k] = (int)std::floor(fkey_inv(S->h_small[k]) * c.il);
-    maxb[k] = (int)std::floor(fkey_inv(S->h_small[3 + k]) * c.il);
+    const float lo = std::floor(fkey_inv(S->h_small[k]) * c.il), hi = std::floor(fkey_inv(S->h_small[3 + k]) * c.il);
+    if (!(lo >= -2147483648.f && hi < 2147483648.f)) {   // x / leaf outside int (or infinite): PCL's int cast is undefined there
+      h->err = "voxel_grid: leaf size too small for the cloud's coordinates (voxel index outside int)";
+      return MALIO_ERR_CAPACITY;
+    }
+    c.minb[k] = (int)lo;
+    maxb[k] = (int)hi;
   }
   const long long dx = (long long)maxb[0] - c.minb[0] + 1, dy = (long long)maxb[1] - c.minb[1] + 1, dz = (long long)maxb[2] - c.minb[2] + 1;
   const long long cells = dx * dy * dz;
+  // PCL's per-axis index floor(x / leaf) - (float)min_b is a float subtraction: exact up to 2^24 voxels per axis, above that
+  // it can round up to the axis' size and the point would be counted one cell past the grid
+  if (dx > (1ll << 24) || dy > (1ll << 24) || dz > (1ll << 24)) {
+    h->err = "voxel_grid: leaf size too small for the cloud's extent (more than 2^24 voxels along an axis)";
+    return MALIO_ERR_CAPACITY;
+  }
   if (cells <= 0 || cells > (1ll << 28)) {   // PCL gives up (returns the input) above INT_MAX voxels; the dense index here stops at 2^28
     h->err = "voxel_grid: leaf size too small for the cloud's extent (more than 2^28 voxels)";
     return MALIO_ERR_CAPACITY;

@@ -506,39 +506,111 @@ def _se3(q, t):
     return T
 
 
+#   generic       the default: ~0.7 rad heading plus ~0.6 rad/s about a random axis (every pair turns by ~6e-3 rad)
+#   stationary    every control pose equal (log_se3's zero-rotation branch, exp_se3's small-angle branch)
+#   straight      20 m/s along the heading with yaw increments per 10 ms pair cycling through 5e-8, 1e-4, 2e-4, 3e-4 and
+#                 3.3e-4 rad: most pairs are under log_so3's Taylor threshold (~3.16e-4 rad), some just above it, and the
+#                 5e-8 pairs reach exp_se3's small-angle branch with a 0.2 m translation.  All turns share the body z axis.
+#   heading_x/y/z base rotations 2.2 rad about x, 2.7 rad about y, pi - 1e-3 about z: the rotation matrices have trace <= 0,
+#                 so Eigen's matrix->quaternion takes its else branch with i = 0, 1, 2; plus a 0.3 rad/s turn
+#   heading_wrap  yaw about z from ~pi - 0.08 to ~pi + 0.08 across the scan: the heading crosses +-pi mid-scan
+#   fast          ~10 rad/s about a random axis
+UNDISTORT_MOTIONS = ("generic", "stationary", "straight", "heading_x", "heading_y", "heading_z", "heading_wrap", "fast")
+STRAIGHT_YAW_STEPS = (5e-8, 1e-4, 2e-4, 3e-4, 3.3e-4)
+# covariance-list / control-point layouts:
+#   default     the list from before the scan start to past its end, cov_pointer as IMU_Processing.hpp:455-466 leaves it
+#   empty_cov   n_cov = 0, cov_pointer = -1
+#   last_cov    cov_pointer = n_cov - 1 (every entry may be popped)
+#   max         n_ctrl = MALIO_MAX_CTRL and n_cov = MALIO_MAX_COV (512 each), the scan at the end of both lists
+UNDISTORT_LISTS = ("default", "empty_cov", "last_cov", "max")
+MAX_CTRL = 512
+MAX_COV = 512
+
+
 def undistort_case(n: int = 60000, lidar: int = 0, seed: int = 51, scan_ms: float = 100.0, imu_hz: float = 200.0,
-                   sorted_times: bool = True):
+                   sorted_times: bool = True, *, motion: str = "generic", ties: bool = False, lists: str = "default"):
     """One LiDAR's raw scan for UndistortPcl's point loop: n points with time offsets (`curvature`, ms) over one scan, a
     cubic-spline control-point set at the reference's fixed 10 ms spacing (BsplineSE3.cpp:34) covering the scan with two
-    control points of margin on both sides (a smooth vehicle motion: ~8 m/s, ~0.6 rad/s), the IMU-covariance time list at
-    imu_hz, and cov_pointer as IMU_Processing.hpp:455-466 leaves it.  Returns a dict of plain arrays."""
+    control points of margin on both sides (by default a smooth vehicle motion: ~8 m/s, ~0.6 rad/s), the IMU-covariance
+    time list at imu_hz, and cov_pointer as IMU_Processing.hpp:455-466 leaves it.  Returns a dict of plain arrays.
+
+    motion: one of UNDISTORT_MOTIONS; lists: one of UNDISTORT_LISTS.  ties: control-point and covariance stamps are built
+    as float64(ms_f32) / 1000 + beg_time, the expression of IMU_Processing.hpp:474, and some points carry exactly those
+    ms values, so their times equal a control-point or a covariance stamp bit for bit; every 7th covariance stamp is
+    duplicated.  With the defaults the output is the same, byte for byte, as before these options existed."""
+    if motion not in UNDISTORT_MOTIONS or lists not in UNDISTORT_LISTS:
+        raise ValueError(f"motion {motion!r} / lists {lists!r}")
     rng = np.random.default_rng(seed)
     t0 = 1000.0 + 0.0137          # lidar_beg_time
     end_time = t0 + scan_ms * 1e-3
-    ctrl_t = t0 - 0.031 + 0.01 * np.arange(int(scan_ms / 10) + 8)
+    n_ctrl = int(scan_ms / 10) + 8
+    k_ctrl = np.arange(n_ctrl) if lists != "max" else np.arange(MAX_CTRL) - (MAX_CTRL - n_ctrl)
+    if ties:
+        ctrl_ms = (-31.0 + 10.0 * k_ctrl).astype(np.float32)
+        ctrl_t = ctrl_ms.astype(np.float64) / 1000.0 + t0
+    else:
+        ctrl_t = t0 - 0.031 + 0.01 * k_ctrl
     axis = rand_unit(rng)
-    w = axis * 0.6
+    w = axis * {"fast": 10.0}.get(motion, 0.6)
     v = np.array([8.0, 0.5, -0.1])
     acc = rng.normal(0, 1.0, 3)
+    q_base = q_exp([0.1, -0.05, 0.7])
+    p_base = np.array([3.0, -2.0, 1.5])
+    if motion == "straight":
+        steps = np.array(STRAIGHT_YAW_STEPS)[np.arange(ctrl_t.shape[0]) % len(STRAIGHT_YAW_STEPS)]
+        yaw = np.concatenate([[0.0], np.cumsum(steps[:-1])])
+    heading = {"heading_x": [2.2, 0, 0], "heading_y": [0, 2.7, 0], "heading_z": [0, 0, np.pi - 1e-3]}
     ctrl_T = np.zeros((ctrl_t.shape[0], 4, 4))
     for k, tk in enumerate(ctrl_t):
         dt = tk - t0
-        q = q_mul(q_exp([0.1, -0.05, 0.7]), q_exp(w * dt + 0.5 * rng.normal(0, 0.01, 3) * dt * dt))
-        ctrl_T[k] = _se3(q, np.array([3.0, -2.0, 1.5]) + v * dt + 0.5 * acc * dt * dt)
+        noise = rng.normal(0, 0.01, 3)
+        p = p_base + v * dt + 0.5 * acc * dt * dt
+        if motion in ("generic", "fast"):
+            q = q_mul(q_base, q_exp(w * dt + 0.5 * noise * dt * dt))
+        elif motion == "stationary":
+            q, p = q_base, p_base
+        elif motion == "straight":
+            q = q_mul(q_base, q_exp([0.0, 0.0, yaw[k]]))
+            p = p_base + q_to_R(q_base) @ np.array([20.0 * dt, 0.0, 0.0])
+        elif motion in heading:
+            q = q_mul(q_exp(heading[motion]), q_exp(axis * 0.3 * dt))
+        else:   # heading_wrap
+            q = q_mul(q_exp([0.02, -0.01, 0.0]), q_exp([0.0, 0.0, np.pi + 1.0 * (dt - 0.5 * scan_ms * 1e-3)]))
+        ctrl_T[k] = _se3(q, p)
     pts = np.zeros(n, dtype=capi.RAW_PT)
     rad = rng.uniform(1.0, 80.0, n)
     az = rng.uniform(-np.pi, np.pi, n)
     el = rng.uniform(-0.4, 0.4, n)
     pts["xyz"] = np.stack([rad * np.cos(el) * np.cos(az), rad * np.cos(el) * np.sin(az), rad * np.sin(el)], axis=1).astype(np.float32)
     curv = rng.uniform(0.0, scan_ms, n).astype(np.float32)
-    pts["curvature"] = np.sort(curv) if sorted_times else curv
     # imu_cov: forward-propagation stamps from before the scan start to past its end (IMU_Processing.hpp:327-360)
-    cov_t = t0 - 0.004 + np.arange(int((scan_ms * 1e-3 + 0.02) * imu_hz)) / imu_hz
-    cp = cov_t.shape[0] - 1
-    while cov_t[cp] > end_time:   # :455-466
-        cp -= 1
-    cp += 1
-    cp = min(cp, cov_t.shape[0] - 1)
+    n_cov = int((scan_ms * 1e-3 + 0.02) * imu_hz)
+    k_cov = np.arange(n_cov) if lists != "max" else np.arange(MAX_COV) - (MAX_COV - n_cov)
+    if ties:
+        cov_ms = (-4.0 + 1000.0 * k_cov / imu_hz).astype(np.float32)
+        cov_t = cov_ms.astype(np.float64) / 1000.0 + t0
+        cov_t = np.repeat(cov_t, np.where(np.arange(cov_t.shape[0]) % 7 == 3, 2, 1))
+        if lists == "max":   # still MAX_COV entries: the oldest ones make room for the duplicates
+            cov_t = cov_t[-MAX_COV:]
+        # points at control-point and covariance stamps inside the scan, two at each
+        in_scan = lambda ms: ms[(ms >= 0) & (ms <= scan_ms)]
+        tie_ms = np.repeat(np.concatenate([in_scan(ctrl_ms), in_scan(cov_ms)]), 2)
+        at = np.random.default_rng(seed + 1).choice(n, size=min(n, tie_ms.shape[0]), replace=False)
+        curv[at] = tie_ms[: at.shape[0]]
+    else:
+        cov_t = t0 - 0.004 + k_cov / imu_hz
+    pts["curvature"] = np.sort(curv) if sorted_times else curv
+    if lists == "empty_cov":
+        cov_t = cov_t[:0]
+        cp = -1
+    else:
+        cp = cov_t.shape[0] - 1
+        while cov_t[cp] > end_time:   # :455-466
+            cp -= 1
+        cp += 1
+        cp = min(cp, cov_t.shape[0] - 1)
+        if lists == "last_cov":
+            cp = cov_t.shape[0] - 1
     ext = (q_normalize(EXTRINSICS[lidar][0]), np.array(EXTRINSICS[lidar][1]))
     return dict(pts=pts, beg_time=t0, end_time=end_time, ctrl_t=ctrl_t, ctrl_T=ctrl_T.reshape(-1, 16), imu_cov_t=cov_t,
                 cov_pointer=int(cp), extrinsic=ext)

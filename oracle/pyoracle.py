@@ -461,6 +461,30 @@ class Oracle:
 
 
 # ------------------------------------------------------------------ N2 / N3 restatements (oracle_undistort.cpp)
+def log_se3(T):
+    """ov_core::log_se3 (quat_ops.h:223-243): 4x4 -> (w, u)."""
+    T = np.ascontiguousarray(T, np.float64).reshape(16)
+    v = np.zeros(6)
+    oracle_lib().orc_log_se3(ptr(T), ptr(v))
+    return v
+
+
+def exp_se3(v):
+    """ov_core::exp_se3 (quat_ops.h:190-220): (w, u) -> 4x4."""
+    v = np.ascontiguousarray(v, np.float64).reshape(6)
+    T = np.zeros(16)
+    oracle_lib().orc_exp_se3(ptr(v), ptr(T))
+    return T.reshape(4, 4)
+
+
+def quat_from_R(R):
+    """Eigen's rotation matrix -> quaternion (w, x, y, z)."""
+    R = np.ascontiguousarray(R, np.float64).reshape(9)
+    q = np.zeros(4)
+    oracle_lib().orc_quat_from_R(ptr(R), ptr(q))
+    return q
+
+
 def bspline_get_pose(ctrl_t, ctrl_T, timestamp):
     L = oracle_lib()
     ct = np.ascontiguousarray(ctrl_t, np.float64)
