@@ -355,7 +355,13 @@ int malio_preprocess_ouster(const malio_ouster_pt* pts, uint32_t n, int point_fi
  * neighbour list and every distance is the reference's, except for exact distance ties, which the reference breaks by
  * traversal order — those queries are counted (malio_counters.knn_tie_queries) and broken by slot index.
  * nn_idx of malio_download_aux / malio_knn are SLOT indices in this mode; malio_map_download gives slot -> id.
- * A later malio_upload_map* call switches the handle back to snapshot mode.
+ * A map without a live point (built empty, or everything deleted) answers like a snapshot of 0 nodes: every index
+ * 0xFFFFFFFF, every distance +inf, nothing selected (MALIO_ERR_NO_EFFECTIVE_POINTS from malio_measure), whatever its history.
+ * A later malio_upload_map* call switches the handle back to snapshot mode: malio_map_add_points / _delete_boxes /
+ * _sync_voxels / _info / _download then return MALIO_ERR_STATE until the next malio_map_build (malio_map_commit is a no-op).
+ * ids == NULL: malio_map_build numbers the points 0..n-1; malio_map_add_points and malio_map_sync_voxels give each point the
+ * slot index it is appended at (the number of slots at that moment; a compaction renumbers the slots, not the ids).
+ * Pinned by tests/test_gpu_mapops_edges.py against a numpy mirror and a brute-force k-NN (tests/test_mapops_edges_cpu.py).
  * Host arrays are consumed when a call returns.  Per-scan-sized batches (<= 65536 points, <= 16384 boxes) pass through a pinned
  * bounce buffer and the call returns WITHOUT waiting for the device; n_deleted (may be NULL) costs a device round trip when asked. */
 int malio_map_build(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids /* may be NULL: 0..n-1 */, uint32_t n);

@@ -2768,7 +2768,8 @@ int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pt
                                                                      D->d_fb_list, D->d_gstats + 2, D->d_nn_idx, D->d_nn_d2, sel, D->d_gstats + 3, ctl);
     D->ctr.kernel_launches += 2;
   } else {
-    if (D->tree_free) { h->err = "device-resident map: the cell-list index is required (map extent too large for it?)"; return MALIO_ERR_STATE; }
+    // device-resident map without a live point: n_nodes = 0, the traversal below answers with empty lists as for an empty snapshot
+    if (D->tree_free && D->n_nodes > 0) { h->err = "device-resident map: the cell-list index is required (map extent too large for it?)"; return MALIO_ERR_STATE; }
     if (int rc = need_boxes()) return rc;
     const int lanes = pick_lanes(n, D->sm_count);
     if (smem_stack)
@@ -2948,6 +2949,7 @@ static int ensure_map_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
   if (int rc = ensure(h, D->d_parent, (size_t)cap)) return rc;
   if (int rc = ensure(h, D->d_arrived, (size_t)cap)) return rc;
   D->cap_nodes = cap;
+  D->cap_slots = 0;        // d_mpts / d_cov now hold the snapshot: the next malio_map_build re-creates the slot storage (grow_slots)
   return MALIO_OK;
 }
 
@@ -3002,6 +3004,7 @@ int upload_map(malio_handle* h, const malio_map_node* nodes, const float* cov, u
   if (D->refit_pending) { CUDA_TRY(cudaStreamSynchronize(D->stream2)); D->refit_pending = false; }
   if (int rc = ensure_map_buffers(h, D, n)) return rc;
   D->tree_free = false;
+  malio_map::leave(h);
   CUDA_TRY(cudaMemcpyAsync(D->d_nodes, nodes, (size_t)n * sizeof(malio_map_node), cudaMemcpyHostToDevice, D->stream));
   CUDA_TRY(cudaMemcpyAsync(D->d_cov, cov, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, D->stream));
   if (n) {
@@ -3020,6 +3023,7 @@ int upload_map_compact(malio_handle* h, const malio_map_point* pts, const float*
   if (D->refit_pending) { CUDA_TRY(cudaStreamSynchronize(D->stream2)); D->refit_pending = false; }
   if (int rc = ensure_map_buffers(h, D, n)) return rc;
   D->tree_free = false;
+  malio_map::leave(h);
   static_assert(sizeof(malio_map_point) == sizeof(float4), "compact record is one float4");
   CUDA_TRY(cudaMemcpyAsync(D->d_mpts, pts, (size_t)n * sizeof(malio_map_point), cudaMemcpyHostToDevice, D->stream));
   CUDA_TRY(cudaEventRecord(D->ev_h2d, D->stream));

@@ -70,6 +70,7 @@ int launch_solve(malio_handle* h, cudaStream_t st, malio_devstate::ScanCtl* d_ct
 namespace malio_map {
 void destroy(malio_handle* h);
 int commit(malio_handle* h);   // pending deltas -> compaction (when worth it) + cell-list index; no-op when clean
+void leave(malio_handle* h);   // a snapshot upload took the handle: back to snapshot mode, the map_* calls refuse until the next build
 int build(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n);
 int add_points(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n);
 int delete_boxes(malio_handle* h, const float* boxes, uint32_t nb, uint32_t* n_deleted);

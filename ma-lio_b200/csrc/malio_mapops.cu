@@ -293,6 +293,7 @@ int append(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const f
   if (n == 0) return MALIO_OK;
   if ((uint64_t)M->n_slots + n > MALIO_LINK_INDEX_MASK) { h->err = "device-resident map: too many slots"; return MALIO_ERR_CAPACITY; }
   if (int rc = malio_dev::grow_slots(h, M->n_slots + n, M->n_slots)) return rc;
+  if (M->n_slots + n > D->cap_slots) { h->err = "device-resident map: slot storage smaller than its recorded use"; return MALIO_ERR_CAPACITY; }
   const float *d_xyz, *d_ny;
   const int32_t* d_ids;
   bool need_sync = true;
@@ -324,6 +325,14 @@ void destroy(malio_handle* h) {
   if (M->ev_bounce_box) cudaEventDestroy(M->ev_bounce_box);
   delete M;
   h->mapst = nullptr;
+}
+
+void leave(malio_handle* h) {
+  MapOps* M = (MapOps*)h->mapst;
+  if (!M) return;
+  M->active = false;
+  M->n_slots = 0; M->n_live = 0;
+  M->dirty = false; M->appended = false;
 }
 
 int commit(malio_handle* h) {
@@ -363,14 +372,16 @@ int commit(malio_handle* h) {
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(st));
     std::swap(D->d_mpts, M->d_mpts2); std::swap(D->d_cov, M->d_cov2); std::swap(D->d_ids, M->d_ids2);
-    M->cap2 = D->cap_slots;      // the buffers that were the live ones hold cap_slots entries; the new live ones hold at least as many
+    std::swap(D->cap_slots, M->cap2);   // each pair of buffers takes its own capacity along
     M->n_slots = M->n_live;
     D->ctr.kernel_launches += 3;
     D->ctr.map_compactions += 1;
   }
   float box[6] = {0, 0, 0, 0, 0, 0};
   if (M->n_live) for (int k = 0; k < 6; ++k) box[k] = fkey_inv(M->h_small[k]);
-  const int rc = malio_dev::index_from_slots(h, M->n_slots, box);
+  // no live point, whether built empty, compacted to nothing or with dead slots left: the index is empty and the search answers
+  // like a snapshot of 0 nodes (empty lists, nothing selected), whatever the history
+  const int rc = malio_dev::index_from_slots(h, M->n_live ? M->n_slots : 0, box);
   if (rc != MALIO_OK) return rc;
   M->dirty = false;
   M->appended = false;
