@@ -316,6 +316,48 @@ int malio_voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, fl
 int malio_upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uint32_t* table_off,
                              const malio_rigid* temporal_comp, uint32_t* n_total);
 
+/* ---- after the update (SURVEY.md §3.1): publish_frame_world and the saved map (laserMapping.cpp:448-489, :1076-1077) --------
+ * RGBpointBodyToWorld (:149-163) per point, on the device, with the state AFTER the update (pass a malio_pass_state built from
+ * the updated malio_state, as for malio_map_incremental; extrinsics from the state, extrinsic_update :291-308) and the temporal
+ * compensation of the last malio_upload_scan* (identity before the first):
+ *   lid = int(intensity); p_w = rot (q_E[0] p + t_E[0]) + pos                                   (lid == 0)
+ *                         p_w = rot (q_C[lid-1] (q_E[lid] p + t_E[lid]) + t_C[lid-1]) + pos     (otherwise)
+ * in double, stored as float, and intensity_out = the input point's normal_y.  The xyz are bit-identical to
+ * malio_map_incremental's world output (pointBodyToWorld, :134-147, is the same expression).  The output cloud is n x 4 floats
+ * {x, y, z, intensity}; as PointXYZINormal its normal_x/y/z and curvature are 0.  The two clouds of :452:
+ *   MALIO_WORLD_DOWNSAMPLED  feats_down_body: the handle's scan in caller order (lid = its `lidar` field), intensity = normal_y of
+ *                            the last pass (what malio_download_aux returns).  MALIO_ERR_STATE before a malio_measure /
+ *                            malio_ieskf_update on the current scan.
+ *   MALIO_WORLD_DENSE        feats_undistort (:977-981): the device-resident results of the last malio_undistort of slots
+ *                            0..L-1, concatenated in slot order, each in its own buffer order, point 0 and the points the
+ *                            spline could not reach included as they are (lid = slot).  intensity = the raw points' normal_y,
+ *                            which sync_packages sets to the cloud's position in lidar_buffer (:321-322) — not the slot in
+ *                            general (feats_undistort_vec[num] = lidar_multi[lid_num-num-1], IMU_Processing.hpp:231) — given
+ *                            per slot in slot_tag[L].  MALIO_ERR_STATE until malio_undistort has run on every slot 0..L-1
+ *                            (0 points is a valid, empty slot).
+ * With a communicator attached every rank registers what it holds (its block of the scan, its own slots); nothing is gathered.
+ * Neither call changes what any other entry point returns. */
+#define MALIO_WORLD_DOWNSAMPLED 0
+#define MALIO_WORLD_DENSE 1
+/* publish_frame_world's cloud (scan_pub_en, dense_pub_en selects the source): at most cap points to out (n x 4 floats; out may
+ * be NULL when cap == 0, to ask the size), *n_out = the full count.  slot_tag: L floats, dense only (may be NULL otherwise). */
+int malio_world_register(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out, uint32_t cap,
+                         uint32_t* n_out);
+/* pcd_save_en: pcl_wait_save += the registered DENSE cloud (:468-475), kept on the device (16 B per point, no copy to the host).
+ * The buffer starts at 65536 points and at least doubles whenever it grows (device-side copy); a failed allocation returns
+ * MALIO_ERR_CUDA and leaves the accumulated cloud intact.  n_total (may be NULL) = points accumulated since the last clear. */
+int malio_world_accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, uint64_t* n_total);
+/* pcd_writer.writeBinary(path, *pcl_wait_save) (:484, :1090), copied out in chunks through a pinned buffer and written by the
+ * same code as malio_write_pcd_binary; clear != 0 then empties the cloud (pcl_wait_save->clear(), :485).  MALIO_ERR_STATE on an
+ * empty cloud, MALIO_ERR_INVALID_ARG when the file cannot be opened or written; no file is left behind on any error.  The
+ * scan_wait_num / pcd_save_interval bookkeeping and the file names (scans_<k>.pcd, result.pcd) stay with the caller. */
+int malio_world_save_pcd(malio_handle* h, const char* path, int clear);
+/* Host: the same PCD file from n > 0 host points (n x 4 floats {x, y, z, intensity}): the header of PCDWriter::writeBinary for
+ * PointXYZINormal (FIELDS x y z intensity normal_x normal_y normal_z curvature, WIDTH = POINTS = n, HEIGHT 1, DATA binary) and
+ * n packed 32-byte records with normal_x/y/z = curvature = 0.  MALIO_ERR_INVALID_ARG for n == 0, a NULL argument or a file
+ * that cannot be opened or written (no file is left behind). */
+int malio_write_pcd_binary(const char* path, const float* xyzi, uint64_t n);
+
 /* ---- next to the path (SURVEY.md §8f N4): City dataset .bin scans without ROS -------------------------------------
  * One file = one scan of packed records as the reference's file player reads them (file_player/src/ROSThread.cpp:776-795
  * Livox, :952-967 Ouster), followed by the per-sensor conversion of MA_LIO/src/preprocess.cpp to the time-stamped raw

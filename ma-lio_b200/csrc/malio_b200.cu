@@ -2453,7 +2453,7 @@ __global__ void reset_scan_kernel(uint32_t cap, uint8_t* __restrict__ sel, float
 // ------------------------------------------------------------------ next to the path: map_incremental's decision
 // laserMapping.cpp:398-446 per point, from device-resident data: normal_y and Nearest_Points (indices into the snapshot)
 // of the last pass, the scan point and the state after the update.  pointBodyToWorld (:134-147) has its own operation
-// order (no detour through the LiDAR-0 frame), restated here exactly.  Outputs in caller order.
+// order (no detour through the LiDAR-0 frame), restated exactly by body_to_world (malio_device.cuh).  Outputs in caller order.
 __global__ void map_incr_kernel(const malio_scan_pt* __restrict__ pts, const uint32_t* __restrict__ perm, uint32_t N,
                                 PassConst pc, const float4* __restrict__ mpts, const uint32_t* __restrict__ nn_idx,
                                 const float* __restrict__ normal_y, double cov_threshold, double fs, int ekf_inited,
@@ -2465,18 +2465,7 @@ __global__ void map_incr_kernel(const malio_scan_pt* __restrict__ pts, const uin
   float w[3] = {0.f, 0.f, 0.f};
   if (!((double)normal_y[p] > cov_threshold)) {                                                 // :406
     const malio_scan_pt pt = pts[p];
-    const int lid = pt.lidar;
-    const double pb[3] = {(double)pt.x, (double)pt.y, (double)pt.z};
-    double a[3], g[3];
-    q_rot(pc.eq[lid], pb, a);
-    a[0] += pc.et[lid][0]; a[1] += pc.et[lid][1]; a[2] += pc.et[lid][2];
-    if (lid != 0) {                                                                             // :142
-      double b[3];
-      q_rot(pc.cq[lid], a, b);
-      a[0] = b[0] + pc.ct[lid][0]; a[1] = b[1] + pc.ct[lid][1]; a[2] = b[2] + pc.ct[lid][2];
-    }
-    q_rot(pc.rot, a, g);
-    w[0] = (float)(g[0] + pc.pos[0]); w[1] = (float)(g[1] + pc.pos[1]); w[2] = (float)(g[2] + pc.pos[2]);
+    body_to_world(pc, pt.lidar, pt.x, pt.y, pt.z, w);                                           // :134-147
     uint32_t id[MALIO_K];
     int cnt = 0;
 #pragma unroll

@@ -50,6 +50,36 @@ struct PassConst {
   double RcT[MALIO_MAX_LIDAR][9];      // R(temporal_comp_l)^T  (entry 0 unused)
 };
 
+// Quaternion * vector as Eigen's _transformVector: v + w*uv + qv x uv, uv = 2 (qv x v); q = (w,x,y,z).  The same operations,
+// in the same order, as malio_b200.cu's q_rot.
+__device__ __forceinline__ void eigen_q_rot(const double q[4], const double v[3], double o[3]) {
+  const double uv0 = q[2] * v[2] - q[3] * v[1], uv1 = q[3] * v[0] - q[1] * v[2], uv2 = q[1] * v[1] - q[2] * v[0];
+  const double u[3] = {uv0 + uv0, uv1 + uv1, uv2 + uv2};
+  const double c0 = q[2] * u[2] - q[3] * u[1], c1 = q[3] * u[0] - q[1] * u[2], c2 = q[1] * u[1] - q[2] * u[0];
+  o[0] = v[0] + q[0] * u[0] + c0;
+  o[1] = v[1] + q[0] * u[1] + c1;
+  o[2] = v[2] + q[0] * u[2] + c2;
+}
+
+// pointBodyToWorld / RGBpointBodyToWorld (laserMapping.cpp:134-163) in the reference's own operation order (no detour through
+// the LiDAR-0 frame), in double, rounded to float at the end:
+//   lid == 0:  p_w = rot (q_E[0] p + t_E[0]) + pos
+//   lid != 0:  p_w = rot (q_C[lid-1] (q_E[lid] p + t_E[lid]) + t_C[lid-1]) + pos      (PassConst keeps q_C[lid-1] at cq[lid])
+// One function for map_incr_kernel and world_kernel, so that both give the same bits.
+__device__ __forceinline__ void body_to_world(const PassConst& pc, int lid, float x, float y, float z, float w[3]) {
+  const double pb[3] = {(double)x, (double)y, (double)z};
+  double a[3], g[3];
+  eigen_q_rot(pc.eq[lid], pb, a);
+  a[0] += pc.et[lid][0]; a[1] += pc.et[lid][1]; a[2] += pc.et[lid][2];
+  if (lid != 0) {                                                                               // :142, :157
+    double b[3];
+    eigen_q_rot(pc.cq[lid], a, b);
+    a[0] = b[0] + pc.ct[lid][0]; a[1] = b[1] + pc.ct[lid][1]; a[2] = b[2] + pc.ct[lid][2];
+  }
+  eigen_q_rot(pc.rot, a, g);
+  w[0] = (float)(g[0] + pc.pos[0]); w[1] = (float)(g[1] + pc.pos[1]); w[2] = (float)(g[2] + pc.pos[2]);
+}
+
 struct ParamConst {
   float plane_th, knn_max_sqdist;
   double cov_threshold, point_cov_max, point_cov_min, plane_cov_max, plane_cov_min, range_min, range_max;

@@ -3,6 +3,7 @@
 #define MALIO_INTERNAL_H_
 
 #include <cstdint>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -89,6 +90,16 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
 int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uint32_t* table_off, const malio_rigid* tcomp,
                        uint32_t* n_total);
 }  // namespace malio_pre
+
+// malio_pcd.cpp — pcl::PCDWriter::writeBinary for PointXYZINormal (host)
+namespace malio_pcd {
+constexpr uint32_t CHUNK = 1u << 18;   // points per fetch
+// fetch(first, count, &xyzi) points *xyzi at count x {x, y, z, intensity} floats of points [first, first + count)
+using Fetch = std::function<int(uint64_t first, uint64_t count, const float** xyzi)>;
+std::string header(uint64_t n);
+// n > 0 points; on any failure the file is removed and a malio_status returned (err says why)
+int write_binary(const char* path, uint64_t n, const Fetch& fetch, std::string& err);
+}  // namespace malio_pcd
 
 // host math shared by measure() (localization weight) and the IESKF
 namespace malio_host {

@@ -2,6 +2,8 @@
 //   N2  ImuProcess::UndistortPcl's per-raw-point loop        src/IMU_Processing.hpp:468-508
 //       BsplineSE3::get_pose                                  src/BsplineSE3.cpp:84-118, quat_ops.h:150-257
 //   N3  pcl::VoxelGrid down-sampling + merge into the scan    src/laserMapping.cpp:968-983
+// and the one after the update that reads their clouds again:
+//       publish_frame_world + the saved map (pcl_wait_save)   src/laserMapping.cpp:448-489, 1083-1091
 // Compiled with -fmad=false like the rest of the library: every double expression is evaluated with the IEEE operations
 // the reference's x86-64 build uses, in its order.
 //
@@ -34,6 +36,7 @@ struct PreLidar {
   int32_t* d_idx = nullptr;
   uint8_t* d_ok = nullptr;
   double* d_pose = nullptr;           // n x 7, only when asked for
+  bool ud_valid = false;              // d_ud holds the result of a completed malio_undistort (possibly of 0 points)
   // voxel grid
   uint32_t n_ds = 0, cap_ds = 0;
   float* d_ds = nullptr;              // n_ds x 5
@@ -51,6 +54,10 @@ struct PreState {
   uint32_t *d_ctot = nullptr, *d_cbase = nullptr;     // chunk totals / bases of the two cell scans (2 x 65536)
   uint32_t* d_bounds = nullptr;       // 6 order-preserving keys + out count
   uint32_t* h_small = nullptr;        // pinned: 8 words
+  // publish_frame_world / pcd_save (world registration): {x, y, z, intensity} per point
+  float4* d_wstage = nullptr; uint64_t cap_wstage = 0;   // malio_world_register's result before its one D2H copy
+  float4* d_acc = nullptr; uint64_t n_acc = 0, cap_acc = 0;   // pcl_wait_save (laserMapping.cpp:475), device-resident
+  float4* h_bounce = nullptr;         // pinned, malio_pcd::CHUNK points: malio_world_save_pcd's D2H staging
 };
 
 template <class T>
@@ -535,6 +542,84 @@ __global__ void merge_scan_kernel(const float* __restrict__ ds, uint32_t n, uint
   dst[i] = o;
 }
 
+// ------------------------------------------------------------------ publish_frame_world: RGBpointBodyToWorld per point
+// laserMapping.cpp:149-163 over one of publish_frame_world's two clouds (:452), output {x, y, z, intensity} (16 B) per point:
+//   ud != NULL  dense (feats_undistort, :977-981): n x 5 undistorted records of LiDAR slot `slot`; lid = slot (:979),
+//               intensity = the raw points' normal_y, one value per slot (`tag`, set by sync_packages, :321-322)
+//   ud == NULL  down-sampled (feats_down_body): the scan in the library's position order; lid = its lidar field (:976),
+//               intensity = normal_y of the last pass (:699, :730, :741); written in caller order through perm
+__global__ void world_kernel(const float* __restrict__ ud, int slot, float tag, const malio_scan_pt* __restrict__ pts,
+                             const uint32_t* __restrict__ perm, const float* __restrict__ normal_y, uint32_t n, PassConst pc,
+                             float4* __restrict__ out) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  float w[3];
+  if (ud) {
+    const float* r = ud + 5 * (size_t)p;
+    body_to_world(pc, slot, r[0], r[1], r[2], w);
+    out[p] = make_float4(w[0], w[1], w[2], tag);
+  } else {
+    const malio_scan_pt pt = pts[p];
+    body_to_world(pc, pt.lidar, pt.x, pt.y, pt.z, w);
+    out[perm ? perm[p] : p] = make_float4(w[0], w[1], w[2], normal_y[p]);
+  }
+}
+
+constexpr uint64_t WORLD_ACC_MIN = 1u << 16;   // first capacity of the accumulated cloud (points); it doubles from there
+
+// the constants body_to_world reads: the updated state and, for LiDARs 1.., the scan's temporal compensation
+PassConst world_const(const malio_pass_state* s, const DeviceState* D) {
+  PassConst pc{};
+  std::memcpy(pc.rot, s->rot, sizeof(pc.rot));
+  std::memcpy(pc.pos, s->pos, sizeof(pc.pos));
+  for (int l = 0; l < MALIO_MAX_LIDAR; ++l) {
+    std::memcpy(pc.eq[l], s->ext[l].q, sizeof(pc.eq[l]));
+    std::memcpy(pc.et[l], s->ext[l].t, sizeof(pc.et[l]));
+    std::memcpy(pc.cq[l], D->tcomp[l].q, sizeof(pc.cq[l]));
+    std::memcpy(pc.ct[l], D->tcomp[l].t, sizeof(pc.ct[l]));
+  }
+  return pc;
+}
+
+// size of the cloud `source` registers, or a state error when it is not on the device
+int world_count(malio_handle* h, PreState* S, DeviceState* D, int source, uint64_t& n) {
+  n = 0;
+  if (source == MALIO_WORLD_DENSE) {
+    for (int l = 0; l < h->cfg.params.n_lidar; ++l) {
+      if (!S->lid[l].ud_valid) { h->err = "world registration (dense): malio_undistort has not run on every LiDAR slot 0..L-1"; return MALIO_ERR_STATE; }
+      n += S->lid[l].n;
+    }
+    return MALIO_OK;
+  }
+  if (!D->pass_done) { h->err = "world registration (down-sampled): no measurement pass on the current scan"; return MALIO_ERR_STATE; }
+  n = D->N;
+  return MALIO_OK;
+}
+
+// enqueue the registration of `source` into dst[0 .. n) on the handle's stream
+int world_launch(malio_handle* h, PreState* S, DeviceState* D, const malio_pass_state* s, int source, const float* slot_tag,
+                 float4* dst) {
+  const PassConst pc = world_const(s, D);
+  if (source == MALIO_WORLD_DENSE) {
+    uint64_t at = 0;
+    for (int l = 0; l < h->cfg.params.n_lidar; ++l) {
+      const uint32_t m = S->lid[l].n;
+      if (m) {
+        world_kernel<<<(m + 255) / 256, 256, 0, S->stream>>>(S->lid[l].d_ud, l, slot_tag[l], nullptr, nullptr, nullptr, m, pc, dst + at);
+        D->ctr.kernel_launches += 1;
+      }
+      at += m;
+    }
+  } else if (D->N) {
+    const bool sorted = h->cfg.sort_queries && D->perm_valid;
+    world_kernel<<<(D->N + 255) / 256, 256, 0, S->stream>>>(nullptr, 0, 0.f, sorted ? D->d_pts_sorted : D->d_pts,
+                                                           sorted ? D->d_perm : nullptr, D->d_normal_y, D->N, pc, dst);
+    D->ctr.kernel_launches += 1;
+  }
+  CUDA_TRY(cudaGetLastError());
+  return MALIO_OK;
+}
+
 }  // namespace
 
 namespace malio_pre {
@@ -547,9 +632,10 @@ void destroy(malio_handle* h) {
     for (void* q : p) if (q) cudaFree(q);
   }
   void* p[] = {S->d_ct, S->d_cT, S->d_seglog, S->d_covt, S->d_pop, S->d_vin, S->d_vidx, S->d_vtmp, S->d_vorder, S->d_vcnt, S->d_voff,
-               S->d_vocc, S->d_vcur, S->d_ctot, S->d_cbase, S->d_bounds};
+               S->d_vocc, S->d_vcur, S->d_ctot, S->d_cbase, S->d_bounds, S->d_wstage, S->d_acc};
   for (void* q : p) if (q) cudaFree(q);
   if (S->h_small) cudaFreeHost(S->h_small);
+  if (S->h_bounce) cudaFreeHost(S->h_bounce);
   delete S;
   h->pre = nullptr;
 }
@@ -567,6 +653,7 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   if (a->cov_pointer < -1 || a->cov_pointer >= (int32_t)a->n_cov) { h->err = "cov_pointer outside the list"; return MALIO_ERR_INVALID_ARG; }
   PreLidar& L = S->lid[lidar];
   cudaStream_t st = S->stream;
+  L.ud_valid = false;
   if (n > L.cap) {
     const uint32_t cap = n + n / 8 + 1024;
     if (int rc = grow(h, L.d_raw, cap)) return rc;
@@ -580,7 +667,7 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   if (pose && !L.d_pose) { if (int rc = grow(h, L.d_pose, (size_t)L.cap * 7)) return rc; }
   L.n = n;
   L.ds_valid = false;
-  if (n == 0) { if (n_pops) *n_pops = 0; return MALIO_OK; }
+  if (n == 0) { if (n_pops) *n_pops = 0; L.ud_valid = true; return MALIO_OK; }
   CUDA_TRY(cudaMemcpyAsync(L.d_raw, pts, (size_t)n * sizeof(malio_raw_pt), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(S->d_ct, a->ctrl_t, a->n_ctrl * sizeof(double), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(S->d_cT, a->ctrl_T, (size_t)a->n_ctrl * 16 * sizeof(double), cudaMemcpyHostToDevice, st));
@@ -611,6 +698,7 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   if (pop_point) std::memcpy(pop_point, pops.data(), a->n_cov * sizeof(int32_t));
   if (n_pops) *n_pops = (uint32_t)pops[a->n_cov];
   D->ctr.d2h_bytes += (uint64_t)n * ((xyz ? 20 : 0) + (idx ? 4 : 0) + (ok ? 1 : 0) + (pose ? 56 : 0));
+  L.ud_valid = true;
   return MALIO_OK;
 }
 
@@ -741,6 +829,88 @@ int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uin
   return MALIO_OK;
 }
 
+int world_register(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out, uint32_t cap,
+                   uint32_t* n_out) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  uint64_t n = 0;
+  if (int rc = world_count(h, S, D, source, n)) return rc;
+  if (n > 0xFFFFFFFFull) { h->err = "world registration: more than 2^32-1 points"; return MALIO_ERR_CAPACITY; }
+  *n_out = (uint32_t)n;
+  const uint64_t k = n < cap ? n : cap;
+  if (!out || k == 0) return MALIO_OK;
+  if (n > S->cap_wstage) {
+    const uint64_t c = n + n / 8 + 1024;
+    if (int rc = grow(h, S->d_wstage, c)) { S->cap_wstage = 0; return rc; }
+    S->cap_wstage = c;
+  }
+  if (int rc = world_launch(h, S, D, s, source, slot_tag, S->d_wstage)) return rc;
+  CUDA_TRY(cudaMemcpyAsync(out, S->d_wstage, (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, S->stream));
+  CUDA_TRY(cudaStreamSynchronize(S->stream));
+  D->ctr.d2h_bytes += k * sizeof(float4);
+  return MALIO_OK;
+}
+
+int world_accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, uint64_t* n_total) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  uint64_t n = 0;
+  if (int rc = world_count(h, S, D, MALIO_WORLD_DENSE, n)) return rc;
+  const uint64_t need = S->n_acc + n;
+  if (need > S->cap_acc) {
+    // geometric growth: a larger buffer, the old content copied over on the device, then the old one freed.  A failed
+    // allocation leaves the accumulated cloud as it was.
+    uint64_t c = S->cap_acc * 2;
+    if (c < need) c = need;
+    if (c < WORLD_ACC_MIN) c = WORLD_ACC_MIN;
+    float4* p = nullptr;
+    const cudaError_t e = cudaMalloc((void**)&p, c * sizeof(float4));
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      h->err = std::string("world accumulate: cannot grow the cloud to ") + std::to_string(c) + " points: " + cudaGetErrorString(e);
+      return MALIO_ERR_CUDA;
+    }
+    if (S->n_acc) {
+      const cudaError_t ec = cudaMemcpyAsync(p, S->d_acc, S->n_acc * sizeof(float4), cudaMemcpyDeviceToDevice, S->stream);
+      const cudaError_t es = ec == cudaSuccess ? cudaStreamSynchronize(S->stream) : ec;
+      if (es != cudaSuccess) { cudaFree(p); h->err = std::string("world accumulate: copy on growth: ") + cudaGetErrorString(es); return MALIO_ERR_CUDA; }
+    }
+    if (S->d_acc) cudaFree(S->d_acc);
+    S->d_acc = p;
+    S->cap_acc = c;
+  }
+  if (n) {
+    if (int rc = world_launch(h, S, D, s, MALIO_WORLD_DENSE, slot_tag, S->d_acc + S->n_acc)) return rc;
+    CUDA_TRY(cudaStreamSynchronize(S->stream));
+  }
+  S->n_acc = need;
+  if (n_total) *n_total = S->n_acc;
+  return MALIO_OK;
+}
+
+int world_save_pcd(malio_handle* h, const char* path, int clear) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (S->n_acc == 0) { h->err = "world save: the accumulated cloud is empty (nothing is written)"; return MALIO_ERR_STATE; }
+  if (!S->h_bounce) CUDA_TRY(cudaHostAlloc((void**)&S->h_bounce, (size_t)malio_pcd::CHUNK * sizeof(float4), cudaHostAllocDefault));
+  const int rc = malio_pcd::write_binary(path, S->n_acc, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
+    if (cudaMemcpyAsync(S->h_bounce, S->d_acc + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
+        cudaStreamSynchronize(S->stream) != cudaSuccess)
+      return (int)MALIO_ERR_CUDA;
+    D->ctr.d2h_bytes += cnt * sizeof(float4);
+    *xyzi = (const float*)S->h_bounce;
+    return (int)MALIO_OK;
+  }, h->err);
+  if (rc == MALIO_OK && clear) S->n_acc = 0;   // pcl_wait_save->clear() (:485); the buffer is kept
+  return rc;
+}
+
 }  // namespace malio_pre
 
 // host-side spline pose (same code as the device's, compiled for the host)
@@ -756,4 +926,22 @@ extern "C" int malio_bspline_get_pose(const double* ctrl_t, const double* ctrl_T
     log_se3(rel, seglog.data() + 6 * (size_t)k);
   }
   return spline_pose(ctrl_t, ctrl_T, seglog.data(), (int)n_ctrl, timestamp, q, p) ? 1 : 0;
+}
+
+// publish_frame_world / pcd_save (laserMapping.cpp:448-489)
+extern "C" int malio_world_register(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out,
+                                    uint32_t cap, uint32_t* n_out) {
+  if (!h || !s || !n_out || (cap && !out)) return MALIO_ERR_INVALID_ARG;
+  if (source != MALIO_WORLD_DOWNSAMPLED && source != MALIO_WORLD_DENSE) { h->err = "world register: unknown source"; return MALIO_ERR_INVALID_ARG; }
+  if (source == MALIO_WORLD_DENSE && !slot_tag) { h->err = "world register: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
+  return malio_pre::world_register(h, s, source, slot_tag, out, cap, n_out);
+}
+extern "C" int malio_world_accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, uint64_t* n_total) {
+  if (!h || !s) return MALIO_ERR_INVALID_ARG;
+  if (!slot_tag) { h->err = "world accumulate: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
+  return malio_pre::world_accumulate(h, s, slot_tag, n_total);
+}
+extern "C" int malio_world_save_pcd(malio_handle* h, const char* path, int clear) {
+  if (!h || !path) return MALIO_ERR_INVALID_ARG;
+  return malio_pre::world_save_pcd(h, path, clear);
 }

@@ -23,6 +23,7 @@ LINK_HAS_RIGHT = 0x40000000
 LINK_POINT_DELETED = 0x20000000
 LINK_INDEX_MASK = 0x0FFFFFFF
 MAP_SKIP, MAP_ADD, MAP_ADD_NO_DOWNSAMPLE, MAP_DROP = 0, 1, 2, 3
+WORLD_DOWNSAMPLED, WORLD_DENSE = 0, 1
 
 # numpy views of the C structs
 MAP_NODE = np.dtype([("xyz", "<f4", 3), ("link", "<u4"), ("lbox", "<f4", 6), ("rbox", "<f4", 6)])
@@ -120,6 +121,7 @@ EXPORTS = [
     "malio_map_download", "malio_read_livox_bin", "malio_read_ouster_bin", "malio_preprocess_livox", "malio_preprocess_ouster",
     "malio_undistort", "malio_bspline_get_pose", "malio_voxel_grid", "malio_upload_scan_device",
     "malio_pose_initial", "malio_compound_pose_with_cov", "malio_compound_inv_pose_with_cov", "malio_build_pose_unc",
+    "malio_world_register", "malio_world_accumulate", "malio_world_save_pcd", "malio_write_pcd_binary",
 ]
 
 
@@ -176,6 +178,10 @@ def load() -> C.CDLL:
     lib.malio_bspline_get_pose.argtypes = [vp, vp, u32, C.c_double, vp, vp]
     lib.malio_voxel_grid.argtypes = [vp, i32, vp, u32, C.c_float, vp, u32, C.POINTER(u32)]
     lib.malio_upload_scan_device.argtypes = [vp, vp, vp, vp, C.POINTER(u32)]
+    lib.malio_world_register.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, u32, C.POINTER(u32)]
+    lib.malio_world_accumulate.argtypes = [vp, C.POINTER(PassState), vp, C.POINTER(C.c_uint64)]
+    lib.malio_world_save_pcd.argtypes = [vp, C.c_char_p, i32]
+    lib.malio_write_pcd_binary.argtypes = [C.c_char_p, vp, C.c_uint64]
     lib.malio_measure.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, C.POINTER(PassStats)]
     lib.malio_download_rows.argtypes = [vp, vp, vp, u32, C.POINTER(u32)]
     lib.malio_download_aux.argtypes = [vp, vp, vp, vp, vp, vp]

@@ -9,6 +9,7 @@ Everything heavy happens inside libmalio_b200.so on the GPU; this file is marsha
 from __future__ import annotations
 
 import ctypes as C
+import os
 from dataclasses import dataclass
 
 import numpy as np
@@ -84,6 +85,46 @@ def bspline_get_pose(ctrl_t: np.ndarray, ctrl_T: np.ndarray, timestamp: float):
     q, p = np.zeros(4), np.zeros(3)
     ok = capi.load().malio_bspline_get_pose(capi.ptr(ct), capi.ptr(cT), ct.shape[0], float(timestamp), capi.ptr(q), capi.ptr(p))
     return bool(ok), q, p
+
+
+def write_pcd_binary(path: str, xyzi: np.ndarray):
+    """pcl::PCDWriter::writeBinary of PointXYZINormal points {x, y, z, intensity} (the other fields 0), host code."""
+    a = np.ascontiguousarray(xyzi, np.float32).reshape(-1, 4)
+    rc = capi.load().malio_write_pcd_binary(os.fsencode(path), capi.ptr(a), a.shape[0])
+    if rc != capi.OK:
+        raise capi.MalioError(rc, f"malio_write_pcd_binary({path!r})")
+
+
+class PcdSaver:
+    """The pcd_save_en branch of publish_frame_world (laserMapping.cpp:466-488) and the map save at shutdown (:1083-1091) over
+    a MeasurementModel: the library keeps pcl_wait_save on the device; the scan counter and the file names live here."""
+
+    def __init__(self, model: "MeasurementModel", directory: str, pcd_save_interval: int):
+        self.model, self.directory, self.interval = model, directory, int(pcd_save_interval)
+        self.scan_wait_num = 0
+        self.pcd_index = 0
+        self.n_wait_save = 0
+
+    def after_update(self, s, slot_tag) -> str | None:
+        """Once per scan after the update.  Returns the path written, if any."""
+        self.n_wait_save = self.model.pcd_accumulate(s, slot_tag)                          # :475
+        self.scan_wait_num += 1
+        if self.n_wait_save > 0 and self.interval > 0 and self.scan_wait_num > self.interval:   # :478
+            self.pcd_index += 1
+            path = os.path.join(self.directory, f"scans_{self.pcd_index}.pcd")
+            self.model.pcd_save(path, clear=True)                                          # :484-485
+            self.n_wait_save = 0
+            self.scan_wait_num = 0
+            return path
+        return None
+
+    def finish(self) -> str | None:
+        """At shutdown: result.pcd with whatever is still waiting (:1083-1091); nothing when the cloud is empty."""
+        if self.n_wait_save == 0:
+            return None
+        path = os.path.join(self.directory, "result.pcd")
+        self.model.pcd_save(path, clear=False)
+        return path
 
 
 class MeasurementModel:
@@ -268,6 +309,33 @@ class MeasurementModel:
         self._check(self.lib.malio_upload_scan_device(self._h, capi.ptr(table), capi.ptr(table_off), capi.ptr(tc), C.byref(n)))
         self.n_points = int(n.value)
         return self.n_points
+
+    # ---- after the update: publish_frame_world and the saved map (laserMapping.cpp:448-489)
+    def publish_frame_world(self, s: capi.PassState | capi.State, dense: bool, slot_tag=None) -> np.ndarray:
+        """The registered cloud of publish_frame_world (scan_pub_en) with the updated state: float32[n,4] {x, y, z, intensity}.
+        dense=True: the undistorted clouds of slots 0..L-1 (feats_undistort), slot_tag[l] = the raw points' normal_y of slot l;
+        dense=False: the down-sampled scan in caller order, intensity = normal_y of the last pass."""
+        ps = s.pass_state() if isinstance(s, capi.State) else s
+        src = capi.WORLD_DENSE if dense else capi.WORLD_DOWNSAMPLED
+        tag = None if slot_tag is None else np.ascontiguousarray(slot_tag, np.float32)
+        n = C.c_uint32(0)
+        self._check(self.lib.malio_world_register(self._h, C.byref(ps), src, capi.ptr(tag), None, 0, C.byref(n)))
+        out = np.zeros((n.value, 4), np.float32)
+        if n.value:
+            self._check(self.lib.malio_world_register(self._h, C.byref(ps), src, capi.ptr(tag), capi.ptr(out), n.value, C.byref(n)))
+        return out
+
+    def pcd_accumulate(self, s: capi.PassState | capi.State, slot_tag) -> int:
+        """pcl_wait_save += the registered dense cloud (laserMapping.cpp:468-475), kept on the device.  Returns its size."""
+        ps = s.pass_state() if isinstance(s, capi.State) else s
+        tag = np.ascontiguousarray(slot_tag, np.float32)
+        n = C.c_uint64(0)
+        self._check(self.lib.malio_world_accumulate(self._h, C.byref(ps), capi.ptr(tag), C.byref(n)))
+        return int(n.value)
+
+    def pcd_save(self, path: str, clear: bool):
+        """pcd_writer.writeBinary(path, *pcl_wait_save) (:484, :1090); clear=True also empties the cloud (:485)."""
+        self._check(self.lib.malio_world_save_pcd(self._h, os.fsencode(path), 1 if clear else 0))
 
     def rearm_scan(self):
         """Reset the per-scan state of the scan already resident on the device (no host copy)."""
