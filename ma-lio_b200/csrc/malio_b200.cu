@@ -2594,12 +2594,19 @@ uint32_t knn_blocks(uint32_t n, int lanes) {
   return (warps + KNN_THREADS / 32 - 1) / (KNN_THREADS / 32);
 }
 
+// blocks in one wave of the fused pass's FAST variant: its co-resident blocks, capped at the slots for the per-block
+// systems (red_grid).  measure(), update_on_device() and the sort's LiDAR-major switch derive the launch from it.
+static uint32_t fast_wave(const DeviceState* D) {
+  return (D->pass_max_blocks > 0 && (uint32_t)D->pass_max_blocks < D->red_grid) ? (uint32_t)D->pass_max_blocks : D->red_grid;
+}
+
 // keys + counting sort of n queries into D->d_perm (MODE 0: scan points through pc, MODE 1: D->d_queries)
 template <int MODE>
 int sort_queries(malio_handle* h, DeviceState* D, uint32_t n, const PassConst& pc) {
   cudaStream_t st = D->stream;
   CUDA_TRY(cudaMemsetAsync(D->d_hist, 0, SORT_BINS * sizeof(uint32_t), st));
-  const int lid_major = (MODE == 0 && (uint64_t)n > (uint64_t)PASS_FAST_TILES * RED_THREADS * (uint64_t)(D->pass_max_blocks > 0 ? D->pass_max_blocks : 1)) ? 1 : 0;
+  // LiDAR-major keys exactly where the fused pass leaves its FAST variant (more than PASS_FAST_TILES tiles per block)
+  const int lid_major = (MODE == 0 && (uint64_t)n > (uint64_t)PASS_FAST_TILES * RED_THREADS * (uint64_t)fast_wave(D)) ? 1 : 0;
   count_kernel<MODE><<<(n + 255) / 256, 256, 0, st>>>(D->d_pts, D->d_queries, n, pc, lid_major, D->d_keys16, D->d_hist);
   scan_kernel<<<SCAN_BLOCKS, SCAN_THREADS, 0, st>>>(D->d_hist, D->d_offs, D->d_cursor, D->d_btot);
   // d_fb_list (the k-NN hand-over list, filled only later in the pass) doubles as the arrival-slot array of the sort
@@ -3286,7 +3293,7 @@ int measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* Ht
   const uint32_t n_tiles = (N + RED_THREADS - 1) / RED_THREADS;
   // one resident wave, every block the same number of tiles (+-1): no straggler blocks
   const bool fused_now = D->fused && (!D->comm || D->p2p);
-  uint32_t wave = (fused_now && (uint32_t)D->pass_max_blocks < D->red_grid) ? (uint32_t)D->pass_max_blocks : D->red_grid;
+  uint32_t wave = fused_now ? fast_wave(D) : D->red_grid;
   uint32_t per_block = n_tiles ? (n_tiles + wave - 1) / wave : 1;
   if (fused_now && per_block > (uint32_t)PASS_FAST_TILES) {   // rows through global memory: that variant's own co-residency limit
     wave = (uint32_t)D->pass_max_blocks_generic < D->red_grid ? (uint32_t)D->pass_max_blocks_generic : D->red_grid;
@@ -3571,7 +3578,7 @@ int update_on_device(malio_handle* h, malio_state* x, double* P, int max_iter, m
   }
   // ---- the passes: k-NN (runs only where the control block says the search is repeated), pass kernel, solve kernel
   const uint32_t n_tiles = (N + RED_THREADS - 1) / RED_THREADS;
-  uint32_t wave = (uint32_t)D->pass_max_blocks < D->red_grid ? (uint32_t)D->pass_max_blocks : D->red_grid;
+  uint32_t wave = fast_wave(D);
   uint32_t per_block = (n_tiles + wave - 1) / wave;
   if (per_block > (uint32_t)PASS_FAST_TILES) {
     wave = (uint32_t)D->pass_max_blocks_generic < D->red_grid ? (uint32_t)D->pass_max_blocks_generic : D->red_grid;
