@@ -287,7 +287,8 @@ typedef struct malio_undistort_args {
 /* lidar = slot (0..L-1) whose device-resident result malio_voxel_grid(.., NULL input) picks up.  Host outputs (any may be
  * NULL): xyz n x 3 float; idx n (the value the reference writes to `intensity`, MALIO_IDX_UNTOUCHED where it writes nothing);
  * ok n (spline_flag); pop_point[k] = index of the point at which the k-th table entry is pushed (:487-494), n_pops their
- * number (the host builds those <= n_cov entries with malio_bspline_get_pose + malio_compound_*); pose n x 7 (q wxyz, p). */
+ * number (malio_scan_uncertainty builds the table entries from them on the device); pose n x 7 (q wxyz, p).  The handle keeps
+ * the slot's pop points, spline poses, cov_pointer, lt_imu_frame and n_cov for malio_scan_uncertainty. */
 int malio_undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, const malio_undistort_args* a,
                     float* xyz, int32_t* idx, uint8_t* ok, int32_t* pop_point, uint32_t* n_pops, double* pose);
 
@@ -315,6 +316,37 @@ int malio_voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, fl
  * a host bounce; then as malio_upload_scan.  n_total (optional) receives the merged size. */
 int malio_upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uint32_t* table_off,
                              const malio_rigid* temporal_comp, uint32_t* n_total);
+
+/* ---- next to the path (SURVEY.md §8f N2, second half): the scan's pose-uncertainty table from its undistortion ----------
+ * The rest of UndistortPcl (IMU_Processing.hpp:474-523) and the pose_unc loop of laserMapping.cpp:1028-1048, on the device,
+ * after malio_undistort has run on every slot 0..L-1 of the scan.  For the k-th pop point of slot num (pop_point[k]):
+ *   uncertainty[num][k] = inv(extrinsic[num]) * inv(lt_lidar_frame[num]) * (PoseInitial(spline pose, imu_cov[c0 - k]) * extrinsic[num])
+ * with the reference's three compoundings (:487-492) and the spline pose undistort_kernel compensated that point with, bit for
+ * bit; c0 = that slot's cov_pointer, lt_lidar_frame[0] = PoseInitial(lt_imu_frame[0], getUncertainty()) (:450) and
+ * lt_lidar_frame[num] = PoseInitial(lt_imu_frame[num], imu_cov[c0]) (:471).  temporal_comp[num-1] = lt_lidar_frame[0]^-1
+ * lt_lidar_frame[num] (:518).  pose_unc[num] = all but the last entry of uncertainty[num] (:1035, :1040), LiDARs >= 1 moved into
+ * LiDAR 0's frame by the compoundings of :1042-1044 (outputs aliasing the second input).  A slot with 0 or 1 pops gets no entry.
+ * A pop point the spline cannot reach: the reference reads an uninitialised quaternion there (get_pose, BsplineSE3.cpp:91-96,
+ * sets the translation to zero and a local rotation matrix to the identity, but never the quaternion); this library uses the
+ * identity rotation with zero translation (DESIGN.md, quirk 8c of §8(a)).
+ * extrinsic is the same struct Pose for both sources: the state's extrinsic and getExtrinsicUncertainty(num) are unchanged by
+ * the prediction between laserMapping.cpp:952 and IMU_Processing.hpp:448.
+ * Matrices are row-major.  Eigen's M6D (Matrix<double,6,6>) is column-major: pass kf.getUncertainty() and every imu_cov[k]
+ * through Eigen::Map<Eigen::Matrix<double,6,6,Eigen::RowMajor>> (or transpose), and build malio_pose.cov the same way. */
+typedef struct malio_scan_unc_args {
+  const double* imu_cov;        /* n_cov x 36: imu_cov[k].first.second, the list (same order) whose times malio_undistort got */
+  uint32_t n_cov;               /* must equal the n_cov of every malio_undistort call of the scan */
+  const malio_pose* extrinsic;  /* L: PoseInitial(extrinsic[num], t, q, kf.getExtrinsicUncertainty(num)) (:444-448) */
+  const double* uncertainty;    /* 36: kf.getUncertainty() (:450) */
+} malio_scan_unc_args;
+/* Outputs, copied from the device in one transfer: table / table_off (L + 1) as malio_upload_scan and malio_upload_scan_device
+ * take them; temporal_comp L - 1 poses (may be NULL when L == 1; malio_rigid = its q and t); lidar_unc (may be NULL) the lists
+ * kf.lidar_uncertainty back to back in slot order, sum of the slots' n_pops entries; lidar_unc_counts (may be NULL) their L sizes.
+ * MALIO_ERR_STATE when a slot 0..L-1 has not been undistorted; MALIO_ERR_INVALID_ARG for a NULL argument, an n_cov other than
+ * the undistort calls saw, or a slot >= 1 whose cov_pointer is -1; MALIO_ERR_CAPACITY when the table needs more than table_cap
+ * entries (the needed number is in table_off[L]).  No kernel runs on any error. */
+int malio_scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_entry* table, uint32_t table_cap,
+                           uint32_t* table_off, malio_pose* temporal_comp, malio_pose* lidar_unc, uint32_t* lidar_unc_counts);
 
 /* ---- after the update (SURVEY.md §3.1): publish_frame_world and the saved map (laserMapping.cpp:448-489, :1076-1077) --------
  * RGBpointBodyToWorld (:149-163) per point, on the device, with the state AFTER the update (pass a malio_pass_state built from

@@ -20,8 +20,10 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <string>
 #include <vector>
 
+#include "malio_compound.h"
 #include "malio_device.cuh"
 
 using namespace malio_devstate;
@@ -35,8 +37,13 @@ struct PreLidar {
   int32_t* d_need = nullptr;
   int32_t* d_idx = nullptr;
   uint8_t* d_ok = nullptr;
-  double* d_pose = nullptr;           // n x 7, only when asked for
+  double* d_pose = nullptr;           // n x 7: the spline pose of every point (zeros where get_pose failed, and at point 0)
+  int32_t* d_pop = nullptr;           // MALIO_MAX_COV + 1: pop points of the last malio_undistort (last = count)
   bool ud_valid = false;              // d_ud holds the result of a completed malio_undistort (possibly of 0 points)
+  // what malio_scan_uncertainty needs of that call besides the device buffers
+  uint32_t n_cov = 0, n_pops = 0;
+  int32_t cov_pointer = -1;
+  malio_rigid lt_imu_frame{};
   // voxel grid
   uint32_t n_ds = 0, cap_ds = 0;
   float* d_ds = nullptr;              // n_ds x 5
@@ -46,7 +53,9 @@ struct PreState {
   cudaStream_t stream = nullptr;
   PreLidar lid[MALIO_MAX_LIDAR];
   double *d_ct = nullptr, *d_cT = nullptr, *d_seglog = nullptr, *d_covt = nullptr;
-  int32_t* d_pop = nullptr;           // MALIO_MAX_COV + 1 (last = count)
+  // malio_scan_uncertainty: imu_cov (MALIO_MAX_COV x 36) and its one output buffer (table | temporal_comp | lidar_uncertainty)
+  double* d_ucov = nullptr;
+  char* d_uout = nullptr;
   // voxel scratch
   float* d_vin = nullptr; uint32_t cap_vin = 0;       // host-provided input staged on the device
   uint32_t *d_vidx = nullptr, *d_vtmp = nullptr, *d_vorder = nullptr; uint32_t cap_vpts = 0;
@@ -79,7 +88,6 @@ int get_state(malio_handle* h, PreState*& S) {
   CUDA_TRY(cudaMalloc((void**)&S->d_cT, (size_t)MALIO_MAX_CTRL * 16 * sizeof(double)));
   CUDA_TRY(cudaMalloc((void**)&S->d_seglog, (size_t)MALIO_MAX_CTRL * 6 * sizeof(double)));
   CUDA_TRY(cudaMalloc((void**)&S->d_covt, MALIO_MAX_COV * sizeof(double)));
-  CUDA_TRY(cudaMalloc((void**)&S->d_pop, (MALIO_MAX_COV + 1) * sizeof(int32_t)));
   CUDA_TRY(cudaMalloc((void**)&S->d_bounds, 8 * sizeof(uint32_t)));
   CUDA_TRY(cudaMalloc((void**)&S->d_ctot, 2 * 65536 * sizeof(uint32_t)));
   CUDA_TRY(cudaMalloc((void**)&S->d_cbase, 2 * 65536 * sizeof(uint32_t)));
@@ -620,6 +628,56 @@ int world_launch(malio_handle* h, PreState* S, DeviceState* D, const malio_pass_
   return MALIO_OK;
 }
 
+// ------------------------------------------------------------------ N2, second half: the scan's pose-uncertainty lists
+// IMU_Processing.hpp:474-523 and laserMapping.cpp:1028-1048 after malio_undistort has run on every slot.  One thread per
+// (slot, pop k): uncertainty[num][k] from the spline pose undistort_kernel computed for the k-th pop point (:483, :487-492),
+// then, unless it is the slot's last entry (:1035, :1040), its pose_unc entry.  Every slot has at least one thread; the
+// slot's first thread writes temporal_comp[num - 1] (:518), which each thread of the slot computes for itself: the same code
+// on the same inputs, so the same bits, and no second launch.
+struct UncConst {
+  malio_pose ext[MALIO_MAX_LIDAR];    // extrinsic[num] (:448)
+  malio_pose ltl[MALIO_MAX_LIDAR];    // lt_lidar_frame[num] (:450, :471)
+  const int32_t* pop[MALIO_MAX_LIDAR];
+  const double* pose[MALIO_MAX_LIDAR];
+  const uint8_t* ok[MALIO_MAX_LIDAR];
+  int32_t cov_pointer[MALIO_MAX_LIDAR], n_pops[MALIO_MAX_LIDAR];
+  uint32_t first[MALIO_MAX_LIDAR + 1];  // slot s owns threads [first[s], first[s + 1])
+  uint32_t unc_off[MALIO_MAX_LIDAR], tab_off[MALIO_MAX_LIDAR];
+  int L;
+};
+constexpr int UNC_THREADS = 64;
+__global__ void __launch_bounds__(UNC_THREADS)
+scan_unc_kernel(const UncConst c, const double* __restrict__ imu_cov, malio_pose_entry* __restrict__ tab, malio_pose* __restrict__ tc_out,
+                malio_pose* __restrict__ unc) {
+  using namespace malio_compound;
+  const uint32_t g = blockIdx.x * UNC_THREADS + threadIdx.x;
+  if (g >= c.first[c.L]) return;
+  int num = 0;
+  while (g >= c.first[num + 1]) ++num;
+  const int k = (int)(g - c.first[num]);
+  malio_pose tcomp{};
+  if (num != 0) {
+    compound_inv_pose_with_cov(&c.ltl[0], c.ltl[0].cov, &c.ltl[num], c.ltl[num].cov, &tcomp, tcomp.cov);   // :518
+    if (k == 0) tc_out[num - 1] = tcomp;
+  }
+  if (k >= c.n_pops[num]) return;
+  // the pose that compensated the pop point; where get_pose failed, the identity it sets up (BsplineSE3.cpp:93-95)
+  const int32_t i = c.pop[num][k];
+  double q[4] = {1.0, 0.0, 0.0, 0.0}, t[3] = {0.0, 0.0, 0.0};
+  if (c.ok[num][i]) {
+    const double* o = c.pose[num] + 7 * (size_t)i;
+    for (int j = 0; j < 4; ++j) q[j] = o[j];
+    for (int j = 0; j < 3; ++j) t[j] = o[4 + j];
+  }
+  malio_pose pt, pc{};
+  pose_initial(&pt, t, q, imu_cov + 36 * (size_t)(c.cov_pointer[num] - k));                                   // :488
+  compound_pose_with_cov(&pt, pt.cov, &c.ext[num], c.ext[num].cov, &pc, pc.cov);                              // :489
+  compound_inv_pose_with_cov(&c.ltl[num], c.ltl[num].cov, &pc, pc.cov, &pc, pc.cov);                          // :490
+  compound_inv_pose_with_cov(&c.ext[num], c.ext[num].cov, &pc, pc.cov, &pc, pc.cov);                          // :491
+  unc[c.unc_off[num] + k] = pc;
+  if (k < c.n_pops[num] - 1) pose_unc_entry(num, c.ext, &tcomp, &pc, &tab[c.tab_off[num] + k]);
+}
+
 }  // namespace
 
 namespace malio_pre {
@@ -628,10 +686,10 @@ void destroy(malio_handle* h) {
   PreState* S = (PreState*)h->pre;
   if (!S) return;
   for (auto& L : S->lid) {
-    void* p[] = {L.d_raw, L.d_ud, L.d_need, L.d_idx, L.d_ok, L.d_pose, L.d_ds};
+    void* p[] = {L.d_raw, L.d_ud, L.d_need, L.d_idx, L.d_ok, L.d_pose, L.d_pop, L.d_ds};
     for (void* q : p) if (q) cudaFree(q);
   }
-  void* p[] = {S->d_ct, S->d_cT, S->d_seglog, S->d_covt, S->d_pop, S->d_vin, S->d_vidx, S->d_vtmp, S->d_vorder, S->d_vcnt, S->d_voff,
+  void* p[] = {S->d_ct, S->d_cT, S->d_seglog, S->d_covt, S->d_ucov, S->d_uout, S->d_vin, S->d_vidx, S->d_vtmp, S->d_vorder, S->d_vcnt, S->d_voff,
                S->d_vocc, S->d_vcur, S->d_ctot, S->d_cbase, S->d_bounds, S->d_wstage, S->d_acc};
   for (void* q : p) if (q) cudaFree(q);
   if (S->h_small) cudaFreeHost(S->h_small);
@@ -661,12 +719,16 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
     if (int rc = grow(h, L.d_need, cap)) return rc;
     if (int rc = grow(h, L.d_idx, cap)) return rc;
     if (int rc = grow(h, L.d_ok, cap)) return rc;
-    if (L.d_pose) { cudaFree(L.d_pose); L.d_pose = nullptr; }
+    if (int rc = grow(h, L.d_pose, (size_t)cap * 7)) return rc;
     L.cap = cap;
   }
-  if (pose && !L.d_pose) { if (int rc = grow(h, L.d_pose, (size_t)L.cap * 7)) return rc; }
+  if (!L.d_pop) { if (int rc = grow(h, L.d_pop, MALIO_MAX_COV + 1)) return rc; }
   L.n = n;
   L.ds_valid = false;
+  L.n_cov = a->n_cov;
+  L.cov_pointer = a->cov_pointer;
+  L.lt_imu_frame = a->lt_imu_frame;
+  L.n_pops = 0;
   if (n == 0) { if (n_pops) *n_pops = 0; L.ud_valid = true; return MALIO_OK; }
   CUDA_TRY(cudaMemcpyAsync(L.d_raw, pts, (size_t)n * sizeof(malio_raw_pt), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(S->d_ct, a->ctrl_t, a->n_ctrl * sizeof(double), cudaMemcpyHostToDevice, st));
@@ -680,8 +742,8 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   if (a->n_ctrl > 1) seglog_kernel<<<(a->n_ctrl + 63) / 64, 64, 0, st>>>(S->d_cT, (int)a->n_ctrl, S->d_seglog);
   const size_t smem = (size_t)(a->n_ctrl + a->n_cov) * sizeof(double);
   undistort_kernel<<<(n + UD_THREADS - 1) / UD_THREADS, UD_THREADS, smem, st>>>(L.d_raw, n, c, S->d_ct, S->d_cT, S->d_seglog, S->d_covt,
-                                                                                  L.d_ud, L.d_need, L.d_ok, pose ? L.d_pose : nullptr);
-  idx_scan_kernel<<<1, SCAN_T, 0, st>>>(L.d_need, L.d_ok, n, L.d_ud, L.d_idx, S->d_pop, (int)a->n_cov);
+                                                                                  L.d_ud, L.d_need, L.d_ok, L.d_pose);
+  idx_scan_kernel<<<1, SCAN_T, 0, st>>>(L.d_need, L.d_ok, n, L.d_ud, L.d_idx, L.d_pop, (int)a->n_cov);
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 3;
   D->ctr.h2d_bytes += (uint64_t)n * sizeof(malio_raw_pt) + (uint64_t)a->n_ctrl * 17 * 8 + (uint64_t)a->n_cov * 8;
@@ -692,11 +754,12 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   if (idx) CUDA_TRY(cudaMemcpyAsync(idx, L.d_idx, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   if (ok) CUDA_TRY(cudaMemcpyAsync(ok, L.d_ok, (size_t)n, cudaMemcpyDeviceToHost, st));
   if (pose) CUDA_TRY(cudaMemcpyAsync(pose, L.d_pose, (size_t)n * 7 * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(pops.data(), S->d_pop, (a->n_cov + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(pops.data(), L.d_pop, (a->n_cov + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   if (xyz) for (uint32_t i = 0; i < n; ++i) { xyz[3 * (size_t)i] = ud_host[5 * (size_t)i]; xyz[3 * (size_t)i + 1] = ud_host[5 * (size_t)i + 1]; xyz[3 * (size_t)i + 2] = ud_host[5 * (size_t)i + 2]; }
   if (pop_point) std::memcpy(pop_point, pops.data(), a->n_cov * sizeof(int32_t));
   if (n_pops) *n_pops = (uint32_t)pops[a->n_cov];
+  L.n_pops = (uint32_t)pops[a->n_cov];
   D->ctr.d2h_bytes += (uint64_t)n * ((xyz ? 20 : 0) + (idx ? 4 : 0) + (ok ? 1 : 0) + (pose ? 56 : 0));
   L.ud_valid = true;
   return MALIO_OK;
@@ -911,6 +974,71 @@ int world_save_pcd(malio_handle* h, const char* path, int clear) {
   return rc;
 }
 
+int scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_entry* table, uint32_t table_cap, uint32_t* table_off,
+                     malio_pose* temporal_comp, malio_pose* lidar_unc, uint32_t* lidar_unc_counts) {
+  PreState* S = (PreState*)h->pre;
+  const int Ln = h->cfg.params.n_lidar;
+  UncConst c{};
+  c.L = Ln;
+  uint32_t n_unc = 0, n_tab = 0, n_thr = 0;
+  for (int l = 0; l < Ln; ++l) {
+    if (!S || !S->lid[l].ud_valid) { h->err = "scan_uncertainty: malio_undistort has not run on every LiDAR slot 0..L-1"; return MALIO_ERR_STATE; }
+    const PreLidar& P = S->lid[l];
+    if (P.n_cov != a->n_cov) { h->err = "scan_uncertainty: n_cov differs from the one malio_undistort of a slot saw"; return MALIO_ERR_INVALID_ARG; }
+    if (l != 0 && P.cov_pointer < 0) { h->err = "scan_uncertainty: lt_lidar_frame of LiDAR >= 1 needs imu_cov[cov_pointer] (:471), cov_pointer is -1"; return MALIO_ERR_INVALID_ARG; }
+    c.pop[l] = P.d_pop; c.pose[l] = P.d_pose; c.ok[l] = P.d_ok;
+    c.cov_pointer[l] = P.cov_pointer;
+    c.n_pops[l] = (int32_t)P.n_pops;
+    c.first[l] = n_thr;
+    c.unc_off[l] = n_unc;
+    c.tab_off[l] = n_tab;
+    table_off[l] = n_tab;
+    n_thr += P.n_pops > 0 ? P.n_pops : 1;
+    n_unc += P.n_pops;
+    n_tab += P.n_pops > 1 ? P.n_pops - 1 : 0;                               // (int)size() - 1 entries, laserMapping.cpp:1035, :1040
+  }
+  c.first[Ln] = n_thr;
+  table_off[Ln] = n_tab;
+  if (n_tab > table_cap) {
+    h->err = "scan_uncertainty: the table needs " + std::to_string(n_tab) + " entries (table_off[L]), table_cap is " + std::to_string(table_cap);
+    return MALIO_ERR_CAPACITY;
+  }
+  for (int l = 0; l < Ln; ++l) {
+    const PreLidar& P = S->lid[l];
+    c.ext[l] = a->extrinsic[l];
+    const double* cov = l == 0 ? a->uncertainty : a->imu_cov + 36 * (size_t)P.cov_pointer;   // :450 / :471
+    malio_compound::pose_initial(&c.ltl[l], P.lt_imu_frame.t, P.lt_imu_frame.q, cov);
+  }
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  cudaStream_t st = S->stream;
+  const size_t tab_bytes = (size_t)n_tab * sizeof(malio_pose_entry);
+  const size_t out_bytes = tab_bytes + (size_t)(Ln - 1 + (lidar_unc ? n_unc : 0)) * sizeof(malio_pose);
+  if (!S->d_ucov) {   // sized for the largest lists: L x MALIO_MAX_COV pops, L - 1 compensations
+    if (int rc = grow(h, S->d_ucov, (size_t)MALIO_MAX_COV * 36)) return rc;
+    if (int rc = grow(h, S->d_uout, (size_t)MALIO_MAX_LIDAR * MALIO_MAX_COV * (sizeof(malio_pose_entry) + sizeof(malio_pose)) +
+                                        MALIO_MAX_LIDAR * sizeof(malio_pose)))
+      return rc;
+  }
+  if (a->n_cov) CUDA_TRY(cudaMemcpyAsync(S->d_ucov, a->imu_cov, (size_t)a->n_cov * 36 * sizeof(double), cudaMemcpyHostToDevice, st));
+  malio_pose_entry* d_tab = (malio_pose_entry*)S->d_uout;
+  malio_pose* d_tc = (malio_pose*)(S->d_uout + tab_bytes);
+  malio_pose* d_unc = d_tc + (Ln - 1);
+  scan_unc_kernel<<<(n_thr + UNC_THREADS - 1) / UNC_THREADS, UNC_THREADS, 0, st>>>(c, S->d_ucov, d_tab, d_tc, d_unc);
+  CUDA_TRY(cudaGetLastError());
+  std::vector<char> out(out_bytes);
+  CUDA_TRY(cudaMemcpyAsync(out.data(), S->d_uout, out_bytes, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  D->ctr.kernel_launches += 1;
+  D->ctr.h2d_bytes += (uint64_t)a->n_cov * 36 * 8;
+  D->ctr.d2h_bytes += out_bytes;
+  std::memcpy(table, out.data(), tab_bytes);
+  if (Ln > 1) std::memcpy(temporal_comp, out.data() + tab_bytes, (size_t)(Ln - 1) * sizeof(malio_pose));
+  if (lidar_unc) std::memcpy(lidar_unc, out.data() + tab_bytes + (size_t)(Ln - 1) * sizeof(malio_pose), (size_t)n_unc * sizeof(malio_pose));
+  if (lidar_unc_counts) for (int l = 0; l < Ln; ++l) lidar_unc_counts[l] = (uint32_t)c.n_pops[l];
+  return MALIO_OK;
+}
+
 }  // namespace malio_pre
 
 // host-side spline pose (same code as the device's, compiled for the host)
@@ -926,6 +1054,14 @@ extern "C" int malio_bspline_get_pose(const double* ctrl_t, const double* ctrl_T
     log_se3(rel, seglog.data() + 6 * (size_t)k);
   }
   return spline_pose(ctrl_t, ctrl_T, seglog.data(), (int)n_ctrl, timestamp, q, p) ? 1 : 0;
+}
+
+// the scan's pose-uncertainty table (IMU_Processing.hpp:474-523, laserMapping.cpp:1028-1048)
+extern "C" int malio_scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_entry* table, uint32_t table_cap,
+                                      uint32_t* table_off, malio_pose* temporal_comp, malio_pose* lidar_unc, uint32_t* lidar_unc_counts) {
+  if (!h || !a || !table || !table_off || !a->extrinsic || !a->uncertainty || (a->n_cov && !a->imu_cov)) return MALIO_ERR_INVALID_ARG;
+  if (h->cfg.params.n_lidar > 1 && !temporal_comp) { h->err = "scan_uncertainty: temporal_comp required for L > 1"; return MALIO_ERR_INVALID_ARG; }
+  return malio_pre::scan_uncertainty(h, a, table, table_cap, table_off, temporal_comp, lidar_unc, lidar_unc_counts);
 }
 
 // publish_frame_world / pcd_save (laserMapping.cpp:448-489)

@@ -13,6 +13,7 @@ import numpy as np
 MAX_LIDAR = 3
 K = 5
 MAX_DOF = 17 + 6 * MAX_LIDAR
+MAX_COV = 512   # MALIO_MAX_COV
 NCCL_UNIQUE_ID_BYTES = 128
 
 OK = 0
@@ -47,6 +48,10 @@ class UndistortArgs(C.Structure):
     _fields_ = [("beg_time", C.c_double), ("extrinsic", Rigid), ("lt_imu_frame", Rigid), ("ctrl_t", C.c_void_p),
                 ("ctrl_T", C.c_void_p), ("n_ctrl", C.c_uint32), ("imu_cov_t", C.c_void_p), ("n_cov", C.c_uint32),
                 ("cov_pointer", C.c_int32)]
+
+
+class ScanUncArgs(C.Structure):
+    _fields_ = [("imu_cov", C.c_void_p), ("n_cov", C.c_uint32), ("extrinsic", C.c_void_p), ("uncertainty", C.c_void_p)]
 
 
 class PassState(C.Structure):
@@ -119,7 +124,7 @@ EXPORTS = [
     "malio_rearm_scan", "malio_get_counters", "malio_set_timing", "malio_upload_map_compact", "malio_download_map_nodes", "malio_map_incremental",
     "malio_map_build", "malio_map_add_points", "malio_map_delete_boxes", "malio_map_sync_voxels", "malio_map_commit", "malio_map_info",
     "malio_map_download", "malio_read_livox_bin", "malio_read_ouster_bin", "malio_preprocess_livox", "malio_preprocess_ouster",
-    "malio_undistort", "malio_bspline_get_pose", "malio_voxel_grid", "malio_upload_scan_device",
+    "malio_undistort", "malio_bspline_get_pose", "malio_voxel_grid", "malio_upload_scan_device", "malio_scan_uncertainty",
     "malio_pose_initial", "malio_compound_pose_with_cov", "malio_compound_inv_pose_with_cov", "malio_build_pose_unc",
     "malio_world_register", "malio_world_accumulate", "malio_world_save_pcd", "malio_write_pcd_binary",
 ]
@@ -178,6 +183,7 @@ def load() -> C.CDLL:
     lib.malio_bspline_get_pose.argtypes = [vp, vp, u32, C.c_double, vp, vp]
     lib.malio_voxel_grid.argtypes = [vp, i32, vp, u32, C.c_float, vp, u32, C.POINTER(u32)]
     lib.malio_upload_scan_device.argtypes = [vp, vp, vp, vp, C.POINTER(u32)]
+    lib.malio_scan_uncertainty.argtypes = [vp, C.POINTER(ScanUncArgs), vp, u32, vp, vp, vp, vp]
     lib.malio_world_register.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, u32, C.POINTER(u32)]
     lib.malio_world_accumulate.argtypes = [vp, C.POINTER(PassState), vp, C.POINTER(C.c_uint64)]
     lib.malio_world_save_pcd.argtypes = [vp, C.c_char_p, i32]

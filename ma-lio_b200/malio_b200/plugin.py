@@ -310,6 +310,40 @@ class MeasurementModel:
         self.n_points = int(n.value)
         return self.n_points
 
+    def scan_uncertainty(self, imu_cov: np.ndarray, extrinsic: np.ndarray, uncertainty: np.ndarray, want_lists: bool = False):
+        """The scan's pose-uncertainty lists, temporal compensation and pose_unc table (IMU_Processing.hpp:474-523,
+        laserMapping.cpp:1028-1048) on the device, after undistort() has run on every slot 0..L-1.  imu_cov: float64[n_cov,6,6]
+        (imu_cov[k].first.second, the list whose times undistort() got); extrinsic: capi.POSE[L] with the extrinsic
+        uncertainty; uncertainty: float64[6,6] (kf.getUncertainty()).  Returns dict(table, table_off, temporal_comp capi.POSE[L-1],
+        temporal_comp_rigid capi.RIGID[L-1] or None (what upload_scan* take), lidar_unc: list of capi.POSE arrays or None)."""
+        L = self.n_lidar
+        cov = np.ascontiguousarray(imu_cov, np.float64).reshape(-1, 36)
+        ext = np.ascontiguousarray(extrinsic, dtype=capi.POSE)
+        unc0 = np.ascontiguousarray(uncertainty, np.float64).reshape(36)
+        a = capi.ScanUncArgs()
+        a.imu_cov = cov.ctypes.data if cov.shape[0] else None
+        a.n_cov = cov.shape[0]
+        a.extrinsic = ext.ctypes.data
+        a.uncertainty = unc0.ctypes.data
+        cap = L * capi.MAX_COV
+        table = np.zeros(cap, dtype=capi.POSE_ENTRY)
+        off = np.zeros(L + 1, np.uint32)
+        tc = np.zeros(max(L - 1, 1), dtype=capi.POSE)
+        lists = np.zeros(cap, dtype=capi.POSE) if want_lists else None
+        counts = np.zeros(L, np.uint32)
+        self._check(self.lib.malio_scan_uncertainty(self._h, C.byref(a), capi.ptr(table), cap, capi.ptr(off), capi.ptr(tc),
+                                                    capi.ptr(lists), capi.ptr(counts)))
+        tc = tc[: L - 1]
+        rigid = None
+        if L > 1:
+            rigid = np.zeros(L - 1, dtype=capi.RIGID)
+            rigid["q"], rigid["t"] = tc["q"], tc["t"]
+        lu = None
+        if want_lists:
+            ends = np.cumsum(counts)
+            lu = [lists[e - c:e].copy() for c, e in zip(counts.astype(np.int64), ends.astype(np.int64))]
+        return dict(table=table[: off[L]].copy(), table_off=off, temporal_comp=tc, temporal_comp_rigid=rigid, lidar_unc=lu)
+
     # ---- after the update: publish_frame_world and the saved map (laserMapping.cpp:448-489)
     def publish_frame_world(self, s: capi.PassState | capi.State, dense: bool, slot_tag=None) -> np.ndarray:
         """The registered cloud of publish_frame_world (scan_pub_en) with the updated state: float32[n,4] {x, y, z, intensity}.
