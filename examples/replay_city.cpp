@@ -20,12 +20,14 @@
 //   g++ -O2 -std=c++14 -fopenmp -pthread -w -Ioracle/pcl_shim -I<reference>/MA_LIO/include/ikd-Tree -Iinclude \
 //       examples/replay_city.cpp -Lma-lio_b200/malio_b200 -lmalio_b200 -o oracle/_ref/replay_city
 //   ./replay_city ouster.bin avia.bin tele.bin      (no arguments: one synthetic scan per LiDAR)
+#include <chrono>
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <random>
+#include <thread>
 #include <vector>
 
 #include "ikd_Tree.cpp"        // the reference's tree, from where it lies (resolved through -I; nothing is copied)
@@ -246,8 +248,11 @@ int main(int argc, char** argv) {
   }
   uint32_t live = 0, slots = 0;
   CHECK(malio_map_info(g_h, &live, &slots));
-  std::printf("map: tree holds %d valid points, device %u live points in %u slots; %zu + %zu points added\n", ikdtree.validnum(), live, slots,
+  // validnum() answers -1 while the tree's background thread rebuilds the root: wait until it can count
+  int valid = ikdtree.validnum();
+  while (valid < 0) { std::this_thread::sleep_for(std::chrono::milliseconds(1)); valid = ikdtree.validnum(); }
+  std::printf("map: tree holds %d valid points, device %u live points in %u slots; %zu + %zu points added\n", valid, live, slots,
               PointToAdd.size(), PointNoNeedDownsample.size());
   malio_destroy(g_h);
-  return (int)live == ikdtree.validnum() ? 0 : 2;
+  return (int)live == valid ? 0 : 2;
 }

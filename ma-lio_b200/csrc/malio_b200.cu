@@ -396,9 +396,7 @@ knn_list_kernel(const float4* __restrict__ nodes, uint32_t n_nodes, const malio_
                 const uint32_t* __restrict__ perm, const float* __restrict__ queries, uint32_t N, PassConst pc,
                 float max_sqdist, const uint32_t* __restrict__ plist, const uint32_t* __restrict__ pcount,
                 uint32_t* __restrict__ nn_idx, float* __restrict__ nn_d2, uint8_t* __restrict__ sel,
-                uint32_t* __restrict__ count_out, const ScanCtl* __restrict__ ctl) {
-  if (ctl && !(ctl->active && ctl->redo)) return;
-  const PassConst& pcr = ctl ? ctl->pc : pc;
+                uint32_t* __restrict__ count_out) {
   const uint32_t count = *pcount;
   if (blockIdx.x == 0 && threadIdx.x == 0) { count_out[0] = count; count_out[2] = count_out[1]; }   // [1] = ring-2 counter
   const uint32_t lane = threadIdx.x & 31u;
@@ -408,7 +406,7 @@ knn_list_kernel(const float4* __restrict__ nodes, uint32_t n_nodes, const malio_
     const bool valid = (lane < lanes) && (base + lane < count);
     const uint32_t p = valid ? plist[base + lane] : 0u;
     float qx = 0.f, qy = 0.f, qz = 0.f;
-    if (valid) load_query<MODE>(pts, perm, queries, p, pcr, qx, qy, qz);
+    if (valid) load_query<MODE>(pts, perm, queries, p, pc, qx, qy, qz);
     uint32_t oi[MALIO_K];
     float od[MALIO_K];
     int found = 0;
@@ -698,128 +696,11 @@ __device__ __forceinline__ void ring2_query_warp(const float4* __restrict__ cell
   }
 }
 
-// Staged scan.  The candidates of one query are 9 (25) short contiguous runs of the cell-sorted point array.  Read
-// run by run with ordinary loads, every run costs a dependent memory round trip (profile: ~90 % of stall samples on the
-// first use of a loaded candidate).  Instead each thread fires cp.async (LDGSTS, 16 B) copies for ALL its candidates into
-// a private column of shared memory — they are in flight together, one round trip — and then scans them from shared
-// memory.  Column layout [slot][thread] keeps both the asynchronous writes and the LDS.128 reads conflict-free.
-constexpr int GK_THREADS = 64;
-constexpr int GK_CAP = 40;                 // staged candidates per thread and round (more: another round)
-constexpr int GK_ROWS1 = 9, GK_ROWS2 = 25;
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc));
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-
 // One query per thread (3x3x3 cells).  Queries whose 5th neighbour is not proven inside the block are retried on the
 // 5x5x5 block by the whole warp (ring2_query_warp) before the kernel ends; tie hazards and out-of-grid queries go to the
-// traversal list.  (RING = 1 is the only instantiation; the constants keep the block geometry in one place.)
-template <int MODE, int RING, bool CTL>
-__global__ void __launch_bounds__(GK_THREADS)
-knn_grid_kernel(const float4* __restrict__ cell_pts, const uint32_t* __restrict__ cell_start, GridConst G,
-                const malio_scan_pt* __restrict__ pts, const uint32_t* __restrict__ perm,
-                const float* __restrict__ queries, uint32_t N, PassConst pc, float max_sqdist,
-                float4* __restrict__ world, uint32_t* __restrict__ nn_idx, float* __restrict__ nn_d2,
-                uint8_t* __restrict__ sel, uint32_t* __restrict__ r2_count, uint32_t* __restrict__ fb_list,
-                uint32_t* __restrict__ fb_count, unsigned long long* __restrict__ cand_total, const ScanCtl* __restrict__ ctl) {
-  // device-side iterated update: this launch was enqueued before it was known whether the pass repeats the search
-  if (CTL && !(ctl->active && ctl->redo)) return;
-  const PassConst& pcr = CTL ? ctl->pc : pc;
-  constexpr int ROWS = RING == 1 ? GK_ROWS1 : GK_ROWS2;
-  uint32_t n_cand = 0;   // candidates this thread scanned (statistics for the roofline; only summed when asked for)
-  constexpr int HALF = RING == 1 ? 1 : 2;       // the block is (2*HALF+1)^3 cells
-  extern __shared__ float4 s_dyn[];
-  float4* s_cand = s_dyn;                                              // [GK_CAP][GK_THREADS]
-  uint2* s_rng = reinterpret_cast<uint2*>(s_dyn + GK_CAP * GK_THREADS);   // [ROWS][GK_THREADS]
-  // one query per thread (the grid covers N); warps stay whole because the 5x5x5 retry below is warp-cooperative
-  const uint32_t p = blockIdx.x * GK_THREADS + threadIdx.x;
-  bool want_r2 = false;
-  float qx = 0.f, qy = 0.f, qz = 0.f;
-  if (p < N) {
-    load_query<MODE>(pts, perm, queries, p, pcr, qx, qy, qz);
-    if (MODE == 0 && RING == 1) world[p] = make_float4(qx, qy, qz, 0.f);
-    const float ux = (qx - G.ox) * G.inv_h, uy = (qy - G.oy) * G.inv_h, uz = (qz - G.oz) * G.inv_h;
-    const float flx = floorf(ux), fly = floorf(uy), flz = floorf(uz);
-    // own cell in [-1, n] per axis: the 5x5x5 block then stays inside the GRID_PAD = 3 border of empty cells
-    const bool in_grid = flx >= -1.f && fly >= -1.f && flz >= -1.f && flx <= (float)G.nx && fly <= (float)G.ny && flz <= (float)G.nz;
-    bool settled = false, hazard = false;
-    Top6 t;
-    t.reset();
-    if (in_grid) {
-      const int cx = (int)flx, cy = (int)fly, cz = (int)flz;
-      const float fx = ux - flx, fy = uy - fly, fz = uz - flz;
-      const float fmin = fminf(fminf(fminf(fx, 1.f - fx), fminf(fy, 1.f - fy)), fminf(fz, 1.f - fz));
-      // the block's x-rows: (2*HALF+1)^2 runs of 2*HALF+1 consecutive cells
-#pragma unroll
-      for (int r = 0; r < ROWS; ++r) {
-        constexpr int W = 2 * HALF + 1;
-        const int dy = (r % W) - HALF, dz = (r / W) - HALF;
-        const uint32_t row = grid_cell_index(G, cx, cy + dy, cz + dz);
-        s_rng[r * GK_THREADS + threadIdx.x] = make_uint2(__ldg(cell_start + row - HALF), __ldg(cell_start + row + HALF + 1));
-      }
-      int r = 0;
-      uint2 cur = s_rng[threadIdx.x];
-      for (;;) {
-        // ---- stage up to GK_CAP candidates
-        int k = 0;
-        while (k < GK_CAP && r < ROWS) {
-          if (cur.x < cur.y) {
-            cp_async16(s_cand + k * GK_THREADS + threadIdx.x, cell_pts + cur.x);
-            ++cur.x; ++k;
-          } else {
-            ++r;   // past the last row the (clamped) re-read is never used: the loop ends on r == ROWS
-            cur = s_rng[min(r, ROWS - 1) * GK_THREADS + threadIdx.x];
-          }
-        }
-        cp_async_wait_all();
-        n_cand += (uint32_t)k;
-        // ---- scan them
-#pragma unroll 4
-        for (int i = 0; i < k; ++i) {
-          const float4 c = s_cand[i * GK_THREADS + threadIdx.x];
-          const float dist = (qx - c.x) * (qx - c.x) + (qy - c.y) * (qy - c.y) + (qz - c.z) * (qz - c.z);   // calc_dist
-          if (dist < t.d5) t.insert(dist, __float_as_uint(c.w));
-        }
-        if (r >= ROWS) break;
-      }
-      const float rg = ((float)HALF + fmin - GRID_MARGIN) * G.h;
-      hazard = t.tie_hazard();
-      settled = (t.d4 < rg * rg) & !hazard;
-    }
-    if (settled) {
-      nn_idx[p] = t.i0;                  nn_d2[p] = t.d0;
-      nn_idx[(size_t)N + p] = t.i1;      nn_d2[(size_t)N + p] = t.d1;
-      nn_idx[(size_t)2 * N + p] = t.i2;  nn_d2[(size_t)2 * N + p] = t.d2;
-      nn_idx[(size_t)3 * N + p] = t.i3;  nn_d2[(size_t)3 * N + p] = t.d3;
-      nn_idx[(size_t)4 * N + p] = t.i4;  nn_d2[(size_t)4 * N + p] = t.d4;
-      if (MODE == 0) sel[p] = (t.d4 > max_sqdist) ? 0 : 1;   // laserMapping.cpp:587 (five were found)
-    } else if (in_grid && !hazard) {
-      want_r2 = true;                    // 5th neighbour not proven inside the 3x3x3 block
-    } else {
-      fb_list[atomicAdd(fb_count, 1u)] = p;
-    }
-  }
-  // ---- 5x5x5 retry, one query at a time with the whole warp (rare: ~0.1 % of the queries on dense maps)
-  unsigned r2mask = __ballot_sync(0xffffffffu, want_r2);
-  if (r2mask && (threadIdx.x & 31u) == 0) atomicAdd(r2_count, (uint32_t)__popc(r2mask));   // statistics
-  while (r2mask) {
-    const int src = __ffs(r2mask) - 1;
-    r2mask &= r2mask - 1;
-    const float bx = __shfl_sync(0xffffffffu, qx, src), by = __shfl_sync(0xffffffffu, qy, src), bz = __shfl_sync(0xffffffffu, qz, src);
-    const uint32_t bp = __shfl_sync(0xffffffffu, p, src);
-    ring2_query_warp<MODE>(cell_pts, cell_start, G, bx, by, bz, bp, N, max_sqdist, nn_idx, nn_d2, sel, fb_list, fb_count);
-  }
-  if (cand_total) {
-    const uint32_t act = __activemask();
-    const uint32_t tot = __reduce_add_sync(act, n_cand);
-    if ((threadIdx.x & 31u) == (uint32_t)(__ffs(act) - 1)) atomicAdd(cand_total, (unsigned long long)tot);
-  }
-}
-
-// Direct-load variant of the 3x3x3 scan (no shared-memory staging): the nine cell ranges are fetched up front, the candidates are
-// read with independent 16-byte loads in batches of four straight into registers.  No dynamic shared memory, so occupancy is
-// bounded by registers only (many more warps per SM than the staged kernel's 10) and the latency of a batch is hidden by other
-// warps instead of by having all of a thread's candidates in flight at once.  Same arithmetic, same hand-over rules.
+// traversal list.  The nine cell ranges are fetched up front, the candidates are read with independent 16-byte loads in
+// batches of four straight into registers.  No dynamic shared memory, so occupancy is bounded by registers only and the
+// latency of a batch is hidden by other warps.
 #ifndef MALIO_GD_THREADS
 #define MALIO_GD_THREADS 128
 #endif
@@ -828,25 +709,24 @@ knn_grid_kernel(const float4* __restrict__ cell_pts, const uint32_t* __restrict_
 #endif
 constexpr int GD_THREADS = MALIO_GD_THREADS;
 constexpr int GD_BATCH = MALIO_GD_BATCH;     // independent candidate loads in flight per thread
-template <int MODE, bool CTL>
+template <int MODE>
 __global__ void __launch_bounds__(GD_THREADS)
 knn_direct_kernel(const float4* __restrict__ cell_pts, const uint32_t* __restrict__ cell_start, GridConst G,
                   const malio_scan_pt* __restrict__ pts, const uint32_t* __restrict__ perm,
                   const float* __restrict__ queries, uint32_t N, PassConst pc, float max_sqdist,
                   float4* __restrict__ world, uint32_t* __restrict__ nn_idx, float* __restrict__ nn_d2,
                   uint8_t* __restrict__ sel, uint32_t* __restrict__ r2_count, uint32_t* __restrict__ fb_list,
-                  uint32_t* __restrict__ fb_count, unsigned long long* __restrict__ cand_total, const ScanCtl* __restrict__ ctl) {
-  if (CTL && !(ctl->active && ctl->redo)) return;
-  const PassConst& pcr = CTL ? ctl->pc : pc;
-  uint32_t n_cand = 0;
+                  uint32_t* __restrict__ fb_count, unsigned long long* __restrict__ cand_total) {
+  uint32_t n_cand = 0;   // candidates this thread scanned (statistics for the roofline; only summed when asked for)
   const uint32_t p = blockIdx.x * GD_THREADS + threadIdx.x;
   bool want_r2 = false;
   float qx = 0.f, qy = 0.f, qz = 0.f;
   if (p < N) {
-    load_query<MODE>(pts, perm, queries, p, pcr, qx, qy, qz);
+    load_query<MODE>(pts, perm, queries, p, pc, qx, qy, qz);
     if (MODE == 0) world[p] = make_float4(qx, qy, qz, 0.f);
     const float ux = (qx - G.ox) * G.inv_h, uy = (qy - G.oy) * G.inv_h, uz = (qz - G.oz) * G.inv_h;
     const float flx = floorf(ux), fly = floorf(uy), flz = floorf(uz);
+    // own cell in [-1, n] per axis: the 5x5x5 block then stays inside the GRID_PAD = 3 border of empty cells
     const bool in_grid = flx >= -1.f && fly >= -1.f && flz >= -1.f && flx <= (float)G.nx && fly <= (float)G.ny && flz <= (float)G.nz;
     bool settled = false, hazard = false;
     Top6 t;
@@ -918,7 +798,7 @@ knn_direct_kernel(const float4* __restrict__ cell_pts, const uint32_t* __restric
 
 // Key scan: the 3x3x3 scan with ONE 32-bit key per kept candidate and G lanes per query (G = 2, 4; the template also covers 1, 8).
 //
-// (1) Keys.  The thread-per-query scans above spend most of their instructions on the sorted insertion of (distance, index)
+// (1) Keys.  The thread-per-query scan above spends most of its instructions on the sorted insertion of (distance, index)
 // pairs (5 compares + ~20 selects per candidate, executed by the whole warp whenever one lane inserts).  Here a candidate is
 // the key  (float bits of dist with the low 10 mantissa bits cleared) | row << 6 | offset-in-row : squared distances are
 // non-negative, so their bit patterns order like the numbers, the low bits make every key of a query unique, and the six
@@ -929,7 +809,7 @@ knn_direct_kernel(const float4* __restrict__ cell_pts, const uint32_t* __restric
 // (~0.06 % of the queries: 5th and 6th distance agree in 13 bits) the query is redone by the exact warp-cooperative 5x5x5
 // scan, as are the queries whose 5th neighbour is not proven inside the block; ties among the five go to the traversal list.
 // Rows longer than 64 candidates do not fit the 6-bit offset: such queries (maps far denser than the 2..9 points per cell
-// the index is tuned for) are handed to the list as well.  Results are identical to the scans above by construction.
+// the index is tuned for) are handed to the list as well.  Results are identical to the scan above by construction.
 //
 // (2) Groups.  A 100k-query search is 0.59 waves of a thread-per-query kernel: it lasts as long as ONE warp's dependent chain
 // however few queries a GPU holds.  With G lanes per query the chain is G times shorter and there are G times more warps;
@@ -951,16 +831,14 @@ struct Keys6 {
   }
   __device__ __forceinline__ void pop() { k0 = k1; k1 = k2; k2 = k3; k3 = k4; k4 = k5; k5 = 0xFFFFFFFFu; }
 };
-template <int MODE, bool CTL, int G, bool PRE>
+template <int MODE, int G, bool PRE>
 __global__ void __launch_bounds__(GD_THREADS)
 knn_keys_kernel(const float4* __restrict__ cell_pts, const uint32_t* __restrict__ cell_start, GridConst Gc,
                 const malio_scan_pt* __restrict__ pts, const uint32_t* __restrict__ perm,
                 const float* __restrict__ queries, uint32_t N, PassConst pc, float max_sqdist,
                 float4* __restrict__ world, uint32_t* __restrict__ nn_idx, float* __restrict__ nn_d2,
                 uint8_t* __restrict__ sel, uint32_t* __restrict__ r2_count, uint32_t* __restrict__ fb_list,
-                uint32_t* __restrict__ fb_count, unsigned long long* __restrict__ cand_total, const ScanCtl* __restrict__ ctl) {
-  if (CTL && !(ctl->active && ctl->redo)) return;
-  const PassConst& pcr = CTL ? ctl->pc : pc;
+                uint32_t* __restrict__ fb_count, unsigned long long* __restrict__ cand_total) {
   constexpr int QPB = GD_THREADS / G;          // queries per block
   constexpr int B = G == 1 ? 4 : 2;            // independent candidate loads in flight per lane
   __shared__ float4 s_q[QPB];                  // x, y, z, containment radius^2 (-1: outside the grid, -2: row too long for the key)
@@ -973,7 +851,7 @@ knn_keys_kernel(const float4* __restrict__ cell_pts, const uint32_t* __restrict_
 #pragma unroll
     for (int r = 0; r < 9; ++r) rng[r] = make_uint2(0u, 0u);
     if (p < N) {
-      load_query<MODE>(pts, perm, queries, p, pcr, q.x, q.y, q.z);
+      load_query<MODE>(pts, perm, queries, p, pc, q.x, q.y, q.z);
       if (MODE == 0) world[p] = make_float4(q.x, q.y, q.z, 0.f);
       const float ux = (q.x - Gc.ox) * Gc.inv_h, uy = (q.y - Gc.oy) * Gc.inv_h, uz = (q.z - Gc.oz) * Gc.inv_h;
       const float flx = floorf(ux), fly = floorf(uy), flz = floorf(uz);
@@ -1249,16 +1127,14 @@ knn_ring_kernel(const float4* __restrict__ cell_pts, const uint32_t* __restrict_
                 const malio_scan_pt* __restrict__ pts, const uint32_t* __restrict__ perm, const float* __restrict__ queries,
                 uint32_t N, PassConst pc, float max_sqdist, const uint32_t* __restrict__ plist, const uint32_t* __restrict__ pcount,
                 uint32_t* __restrict__ nn_idx, float* __restrict__ nn_d2, uint8_t* __restrict__ sel, uint32_t* __restrict__ count_out,
-                uint32_t* __restrict__ tie_count, const ScanCtl* __restrict__ ctl) {
-  if (ctl && !(ctl->active && ctl->redo)) return;
-  const PassConst& pcr = ctl ? ctl->pc : pc;
+                uint32_t* __restrict__ tie_count) {
   const uint32_t count = *pcount;
   if (blockIdx.x == 0 && threadIdx.x == 0) { count_out[0] = count; count_out[2] = count_out[1]; }
   const uint32_t warp = (blockIdx.x * KNN_THREADS + threadIdx.x) >> 5, nwarps = (gridDim.x * KNN_THREADS) >> 5;
   for (uint32_t k = warp; k < count; k += nwarps) {
     const uint32_t p = plist[k];
     float qx, qy, qz;
-    load_query<MODE>(pts, perm, queries, p, pcr, qx, qy, qz);
+    load_query<MODE>(pts, perm, queries, p, pc, qx, qy, qz);
     ring_search_warp<MODE>(cell_pts, cell_start, G, qx, qy, qz, p, N, max_sqdist, nn_idx, nn_d2, sel, tie_count);
   }
 }
@@ -1977,8 +1853,6 @@ struct PassArgs {
   double* block_red; double* d_res;
   double* h_res;           // mapped host memory: MALIO_RED_DOUBLES result | 4 min/max keys | flag
   uint32_t seq;
-  // device-side iterated update: non-null -> run / repeat-the-plane-fit / parity / sequence number come from the control block
-  const ScanCtl* ctl; unsigned long long* mmkey_base; uint32_t* cnt_base;
   unsigned long long* dbg; // optional [grid][8] %globaltimer stamps at the phase boundaries (MALIO_PASS_TRACE=1)
   unsigned long long* xwait;   // multi-GPU: [0] ns spent in the MIN exchange (push + wait for every peer), [1] same for the SUM exchange, [2] passes
 };
@@ -1995,8 +1869,8 @@ __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
   return v;
 }
 // all threads of all blocks call this; returns when `expected` arrivals have been counted
-// Gives up after ~2 s (a block of the grid that never became resident: only possible when the launch was not cooperative
-// and another kernel holds the SMs) and raises the fault word of the mapped result buffer, which measure() reports.
+// Gives up after ~2 s (a block of the grid that never became resident) and raises the fault word of the mapped result buffer,
+// which measure() reports.
 __device__ __forceinline__ void grid_barrier(uint32_t* counter, uint32_t target, uint32_t* fault) {
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -2029,28 +1903,9 @@ constexpr int PASS_MIN_BLOCKS = MALIO_PASS_MINB;    // co-resident blocks per SM
 constexpr int PASS_ROW_STRIDE = 15;        // doubles per staged row: a*J12 (12) | 1/rho^ | z | rho^   (odd: conflict-free)
 constexpr int PASS_FAST_SMEM_DOUBLES = PASS_FAST_TILES * RED_THREADS * PASS_ROW_STRIDE + RED_TASKS * RED_KS * 16;
 static_assert(PASS_FAST_SMEM_DOUBLES <= RED_SMEM_DOUBLES, "the fast path must fit the generic path's shared memory");
-template <bool FAST, bool CTL>
+template <bool FAST>
 __global__ void __launch_bounds__(RED_THREADS, FAST ? PASS_MIN_BLOCKS : 4)
-pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
-  if (CTL && !a_in.ctl->active) return;
-  // the per-pass quantities: launch arguments, or (device-side update) the control block the solve kernel maintains
-  struct Eff {
-    int do_tau, do_fit; unsigned long long *mmkey, *mmkey_next; uint32_t *cnt_cell, *cnt_next; uint32_t bar_base[3]; uint32_t seq;
-  } ef;
-  if (CTL) {
-    const int par = a_in.ctl->parity;
-    ef.do_tau = 0; ef.do_fit = a_in.ctl->redo;
-    ef.mmkey = a_in.mmkey_base + 4 * par; ef.mmkey_next = a_in.mmkey_base + 4 * (1 - par);
-    ef.cnt_cell = a_in.cnt_base + par; ef.cnt_next = a_in.cnt_base + (1 - par);
-    ef.bar_base[0] = a_in.ctl->bar_base[0]; ef.bar_base[1] = a_in.ctl->bar_base[1]; ef.bar_base[2] = a_in.ctl->bar_base[2];
-    ef.seq = a_in.ctl->seq;
-  } else {
-    ef.do_tau = a_in.do_tau; ef.do_fit = a_in.do_fit; ef.mmkey = a_in.mmkey; ef.mmkey_next = a_in.mmkey_next; ef.cnt_cell = a_in.cnt_cell;
-    ef.cnt_next = a_in.cnt_next; ef.bar_base[0] = a_in.bar_base[0]; ef.bar_base[1] = a_in.bar_base[1]; ef.bar_base[2] = a_in.bar_base[2];
-    ef.seq = a_in.seq;
-  }
-  const PassConst& pc = CTL ? a_in.ctl->pc : pc_in;   // CTL == false: the launch arguments themselves (constant bank)
-  const PassArgs& a = a_in;
+pass_kernel(PassArgs a, PassConst pc, ParamConst prm) {
   uint32_t t0, t1;
   block_tiles(a.n_tiles, t0, t1);
   extern __shared__ double smem[];
@@ -2073,8 +1928,8 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
         const uint32_t p = tile * RED_THREADS + threadIdx.x;
         if (tile < t1 && p < a.N) {
           const malio_scan_pt pt = a.pts[a.perm ? a.perm[p] : p];
-          if (ef.do_tau) tau_point(pt, pc, a.table, a.tau2, p);
-          if (ef.do_fit && a.sel[p]) fit_point(a.nodes, a.node_cov, a.N, prm, a.nn_idx, a.sel, a.plane, a.ucov, p);
+          if (a.do_tau) tau_point(pt, pc, a.table, a.tau2, p);
+          if (a.do_fit && a.sel[p]) fit_point(a.nodes, a.node_cov, a.N, prm, a.nn_idx, a.sel, a.plane, a.ucov, p);
           gate_point(pt, p, pc, a.plane, a.ucov, a.tau2, a.sel, a.world, a.pd2, a.tau, a.normal_y, a.rows12, a.lid8, mm,
                      smem + (size_t)(k * RED_THREADS + threadIdx.x) * PASS_ROW_STRIDE, &go[k]);
         }
@@ -2092,17 +1947,17 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
         const uint32_t p = tile * RED_THREADS + threadIdx.x;
         if (p < a.N) {
           const malio_scan_pt pt = a.pts[a.perm ? a.perm[p] : p];
-          if (ef.do_tau) tau_point(pt, pc, a.table, a.tau2, p);
-          if (ef.do_fit && a.sel[p]) fit_point(a.nodes, a.node_cov, a.N, prm, a.nn_idx, a.sel, a.plane, a.ucov, p);
+          if (a.do_tau) tau_point(pt, pc, a.table, a.tau2, p);
+          if (a.do_fit && a.sel[p]) fit_point(a.nodes, a.node_cov, a.N, prm, a.nn_idx, a.sel, a.plane, a.ucov, p);
           gate_point(pt, p, pc, a.plane, a.ucov, a.tau2, a.sel, a.world, a.pd2, a.tau, a.normal_y, a.rows12, a.lid8, mm);
         }
       }
     }
-    minmax_block_commit<RED_THREADS>(mm, ef.mmkey, ef.cnt_cell);
+    minmax_block_commit<RED_THREADS>(mm, a.mmkey, a.cnt_cell);
   }
   pass_stamp(a, 1);
   if (a.peer.world <= 1) {
-    grid_barrier(a.bar + 0, ef.bar_base[0] + gridDim.x, reinterpret_cast<uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 9));
+    grid_barrier(a.bar + 0, a.bar_base[0] + gridDim.x, reinterpret_cast<uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 9));
   } else {
     // barrier 1 fused with the cross-GPU MIN: every block arrives; warp 0 of block 0 waits for the local arrivals, pushes
     // this GPU's four keys into every peer's mailbox, waits for the peers' keys, writes the global minima into the local
@@ -2111,22 +1966,22 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
     if (threadIdx.x == 0) { __threadfence(); atomicAdd(a.bar + 0, 1u); }
     if (blockIdx.x == 0 && threadIdx.x < 32) {
       const int lane = threadIdx.x, me = a.peer.rank, W = a.peer.world;
-      if (lane == 0) while ((int32_t)(ld_acquire_u32(a.bar + 0) - (ef.bar_base[0] + gridDim.x)) < 0) { }
+      if (lane == 0) while ((int32_t)(ld_acquire_u32(a.bar + 0) - (a.bar_base[0] + gridDim.x)) < 0) { }
       __syncwarp();
       unsigned long long xw0 = 0;
       if (lane == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(xw0));
       unsigned long long k[4];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) k[c] = __ldcg(ef.mmkey + c);
+      for (int c = 0; c < 4; ++c) k[c] = __ldcg(a.mmkey + c);
       bool ok = true;
       if (lane < W && lane != me) {
-        unsigned char* dst = mail_min_slot(a.peer.mail[lane], ef.seq, me);
+        unsigned char* dst = mail_min_slot(a.peer.mail[lane], a.seq, me);
         volatile unsigned long long* dk = reinterpret_cast<volatile unsigned long long*>(dst);
 #pragma unroll
         for (int c = 0; c < 4; ++c) dk[c] = k[c];
-        st_release_sys_u32(reinterpret_cast<uint32_t*>(dst + 40), ef.seq);
-        const unsigned char* src = mail_min_slot(a.peer.mail[me], ef.seq, lane);
-        ok = wait_seq_sys(reinterpret_cast<const uint32_t*>(src + 40), ef.seq);
+        st_release_sys_u32(reinterpret_cast<uint32_t*>(dst + 40), a.seq);
+        const unsigned char* src = mail_min_slot(a.peer.mail[me], a.seq, lane);
+        ok = wait_seq_sys(reinterpret_cast<const uint32_t*>(src + 40), a.seq);
         const volatile unsigned long long* sk = reinterpret_cast<const volatile unsigned long long*>(src);
 #pragma unroll
         for (int c = 0; c < 4; ++c) k[c] = sk[c];
@@ -2146,27 +2001,27 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
         a.xwait[0] += xw1 - xw0;      // only this thread of this GPU ever writes these words
         a.xwait[2] += 1;
 #pragma unroll
-        for (int c = 0; c < 4; ++c) ef.mmkey[c] = k[c];
+        for (int c = 0; c < 4; ++c) a.mmkey[c] = k[c];
         if (!all_ok) *reinterpret_cast<volatile uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 9) = 1u;   // peer timeout
         __threadfence();
-        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(a.bar + 3), "r"(ef.seq) : "memory");
+        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(a.bar + 3), "r"(a.seq) : "memory");
       }
     }
-    if (threadIdx.x == 0) while (ld_acquire_u32(a.bar + 3) != ef.seq) { }
+    if (threadIdx.x == 0) while (ld_acquire_u32(a.bar + 3) != a.seq) { }
     __syncthreads();
   }
   pass_stamp(a, 2);
   if (blockIdx.x == 0 && threadIdx.x == 0) {   // arm the other parity's min/max cell for the next pass
-    ef.mmkey_next[0] = dkey(1000.0); ef.mmkey_next[1] = dkey(-0.0);
-    ef.mmkey_next[2] = dkey(9999.0); ef.mmkey_next[3] = dkey(-0.0);
-    *ef.cnt_next = 0;
+    a.mmkey_next[0] = dkey(1000.0); a.mmkey_next[1] = dkey(-0.0);
+    a.mmkey_next[2] = dkey(9999.0); a.mmkey_next[3] = dkey(-0.0);
+    *a.cnt_next = 0;
     a.gstats[2] = 0; a.gstats[4] = 0;
   }
   // ---- phase 2: weights + accumulation into this block's slot
   double* slot = a.block_red + (size_t)blockIdx.x * MALIO_RED_DOUBLES;
   if (FAST) {
     double* s_flush = smem + PASS_FAST_TILES * RED_THREADS * PASS_ROW_STRIDE;
-    const double umin = dkey_inv(ef.mmkey[0]), umax = -dkey_inv(ef.mmkey[1]), tmin = dkey_inv(ef.mmkey[2]), tmax = -dkey_inv(ef.mmkey[3]);
+    const double umin = dkey_inv(a.mmkey[0]), umax = -dkey_inv(a.mmkey[1]), tmin = dkey_inv(a.mmkey[2]), tmax = -dkey_inv(a.mmkey[3]);
     uint32_t mine = 0;
     // segment table of the block: seg[k][l] = [beg, end) inside tile k's list (every thread derives it from s_wc)
     uint32_t seg_beg[PASS_FAST_TILES][MALIO_MAX_LIDAR], seg_end[PASS_FAST_TILES][MALIO_MAX_LIDAR];
@@ -2263,10 +2118,10 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
     }
     if (threadIdx.x == 0) { slot[MALIO_RED_BLOCKS * 16] = (double)s_cnt; slot[MALIO_RED_BLOCKS * 16 + 1] = 0.0; }
   } else {
-    reduce_block(a.N, prm, pc.ext_en, a.sel, a.lid8, a.rows12, a.pd2, a.ucov, a.tau, ef.mmkey, t0, t1, slot);
+    reduce_block(a.N, prm, pc.ext_en, a.sel, a.lid8, a.rows12, a.pd2, a.ucov, a.tau, a.mmkey, t0, t1, slot);
   }
   pass_stamp(a, 3);
-  grid_barrier(a.bar + 1, ef.bar_base[1] + gridDim.x, reinterpret_cast<uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 9));
+  grid_barrier(a.bar + 1, a.bar_base[1] + gridDim.x, reinterpret_cast<uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 9));
   pass_stamp(a, 4);
   // ---- phase 3: fold the slots, one warp per entry, in fold_kernel's order
   const uint32_t lane = threadIdx.x & 31u, wpb = RED_THREADS / 32;
@@ -2286,7 +2141,7 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
       done = atomicAdd(a.bar + 2, folded) + folded;
     }
     done = __shfl_sync(0xffffffffu, done, 0);
-    if (done == ef.bar_base[2] + MALIO_RED_DOUBLES) {
+    if (done == a.bar_base[2] + MALIO_RED_DOUBLES) {
       // this warp folded the last entry: ship result + min/max keys to the mapped host buffer (posted PCIe writes, one
       // system-scope fence), then the sequence flag the host is spinning on
       __threadfence();
@@ -2303,7 +2158,7 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
 #pragma unroll
           for (uint32_t j = 0; j < (MALIO_RED_DOUBLES + 31) / 32; ++j) { const uint32_t e = lane + 32 * j; v[j] = e < MALIO_RED_DOUBLES ? __ldcg(a.d_res + e) : 0.0; }
           for (int r = 0; r < W; ++r) {
-            double* dst = reinterpret_cast<double*>(mail_sum_slot(a.peer.mail[r], ef.seq, me));
+            double* dst = reinterpret_cast<double*>(mail_sum_slot(a.peer.mail[r], a.seq, me));
 #pragma unroll
             for (uint32_t j = 0; j < (MALIO_RED_DOUBLES + 31) / 32; ++j) { const uint32_t e = lane + 32 * j; if (e < MALIO_RED_DOUBLES) dst[e] = v[j]; }
           }
@@ -2312,8 +2167,8 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
         __syncwarp();
         bool ok = true;
         if ((int)lane < W && (int)lane != me) {
-          st_release_sys_u32(reinterpret_cast<uint32_t*>(mail_sum_slot(a.peer.mail[lane], ef.seq, me) + MAIL_SUM_SEQ_OFF), ef.seq);
-          ok = wait_seq_sys(reinterpret_cast<const uint32_t*>(mail_sum_slot(a.peer.mail[me], ef.seq, (int)lane) + MAIL_SUM_SEQ_OFF), ef.seq);
+          st_release_sys_u32(reinterpret_cast<uint32_t*>(mail_sum_slot(a.peer.mail[lane], a.seq, me) + MAIL_SUM_SEQ_OFF), a.seq);
+          ok = wait_seq_sys(reinterpret_cast<const uint32_t*>(mail_sum_slot(a.peer.mail[me], a.seq, (int)lane) + MAIL_SUM_SEQ_OFF), a.seq);
         }
         if (!__all_sync(0xffffffffu, ok) && lane == 0) *reinterpret_cast<volatile uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 9) = 1u;
         if (lane == 0) {
@@ -2324,50 +2179,22 @@ pass_kernel(PassArgs a_in, PassConst pc_in, ParamConst prm) {
         __syncwarp();     // every lane's peer has published (acquire loads above); L2 is the coherence point for the peers' writes
         for (uint32_t e = lane; e < MALIO_RED_DOUBLES; e += 32) {
           double sum = 0.0;
-          for (int r = 0; r < W; ++r) sum += __ldcg(reinterpret_cast<const double*>(mail_sum_slot(a.peer.mail[me], ef.seq, r)) + e);
+          for (int r = 0; r < W; ++r) sum += __ldcg(reinterpret_cast<const double*>(mail_sum_slot(a.peer.mail[me], a.seq, r)) + e);
           a.d_res[e] = sum;
           a.h_res[e] = sum;
         }
       } else {
         for (uint32_t e = lane; e < MALIO_RED_DOUBLES; e += 32) a.h_res[e] = __ldcg(a.d_res + e);
       }
-      if (lane < 4) reinterpret_cast<unsigned long long*>(a.h_res + MALIO_RED_DOUBLES)[lane] = ef.mmkey[lane];
+      if (lane < 4) reinterpret_cast<unsigned long long*>(a.h_res + MALIO_RED_DOUBLES)[lane] = a.mmkey[lane];
       // k-NN list statistics of the last search as knn_list_kernel published them ([3] traversal list, [5] 5x5x5 retries)
       if (lane == 4) { uint32_t* hg = reinterpret_cast<uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 4); hg[3] = a.gstats[3]; hg[5] = a.gstats[5]; hg[6] = g_fault_word; hg[7] = a.gstats[7]; }
       __threadfence_system();
       __syncwarp();
-      if (lane == 0) *reinterpret_cast<volatile uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 8) = ef.seq;
+      if (lane == 0) *reinterpret_cast<volatile uint32_t*>(a.h_res + MALIO_RED_DOUBLES + 8) = a.seq;
     }
   }
   pass_stamp(a, 5);
-}
-
-// Pipelined host loop: this one-block kernel sits in the stream in front of a pass that was enqueued before the host knew its
-// state.  It waits for the host's ticket in mapped memory, then copies the published pass constants and flags into the
-// control block the following (predicated) kernels read.  Gives up after ~5 s and marks the pass inactive.
-__global__ void fetch_ctl_kernel(ScanCtl* __restrict__ ctl, const PubCtl* __restrict__ pub, uint32_t ticket) {
-  __shared__ int s_ok;
-  if (threadIdx.x == 0) {
-    unsigned long long t0 = 0;
-    int ok = 1;
-    for (uint32_t it = 0; ld_acquire_sys_u32(&pub->ticket) != ticket; ++it) {
-      if ((it & 0x3FFu) == 0x3FFu) {
-        unsigned long long t1;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-        if (t0 == 0) t0 = t1;
-        else if (t1 - t0 > 5000000000ull) { ok = 0; break; }
-      }
-    }
-    s_ok = ok;
-  }
-  __syncthreads();
-  const uint32_t* src = reinterpret_cast<const uint32_t*>(&pub->pc);
-  uint32_t* dst = reinterpret_cast<uint32_t*>(&ctl->pc);
-  if (s_ok) for (int k = threadIdx.x; k < (int)(sizeof(PassConst) / 4); k += blockDim.x) dst[k] = src[k];
-  if (threadIdx.x == 0) {
-    ctl->redo = s_ok ? pub->redo : 0; ctl->active = s_ok ? pub->active : 0; ctl->parity = pub->parity; ctl->seq = pub->seq;
-    ctl->bar_base[0] = pub->bar_base[0]; ctl->bar_base[1] = pub->bar_base[1]; ctl->bar_base[2] = pub->bar_base[2];
-  }
 }
 
 // second stage: one warp per entry of the reduced system folds the per-block slots in a fixed order
@@ -2580,10 +2407,7 @@ ParamConst make_param_const(const malio_params& p) {
 }
 
 // queries per warp for knn_kernel: halve the logical warp width while fewer than ~8 warps per SM would be resident
-// (MALIO_KNN_LANES overrides, for experiments)
 int pick_lanes(uint32_t n, int sm_count) {
-  static const int forced = [] { const char* e = getenv("MALIO_KNN_LANES"); return e ? atoi(e) : 0; }();
-  if (forced == 4 || forced == 8 || forced == 16 || forced == 32) return forced;
   const uint64_t target = (uint64_t)sm_count * 8;
   int lanes = 32;
   while (lanes > 4 && (n + lanes - 1) / lanes < target) lanes >>= 1;
@@ -2595,7 +2419,7 @@ uint32_t knn_blocks(uint32_t n, int lanes) {
 }
 
 // blocks in one wave of the fused pass's FAST variant: its co-resident blocks, capped at the slots for the per-block
-// systems (red_grid).  measure(), update_on_device() and the sort's LiDAR-major switch derive the launch from it.
+// systems (red_grid).  measure() and the sort's LiDAR-major switch derive the launch from it.
 static uint32_t fast_wave(const DeviceState* D) {
   return (D->pass_max_blocks > 0 && (uint32_t)D->pass_max_blocks < D->red_grid) ? (uint32_t)D->pass_max_blocks : D->red_grid;
 }
@@ -2679,10 +2503,8 @@ int grid_build(malio_handle* h, DeviceState* D, const GridConst& G) {
 }
 
 // lanes per query of the cell-list scan: small searches are latency-bound (one warp's chain), large ones issue-bound (the merge and
-// the replicated preamble are pure overhead there).  MALIO_KNN_GROUP=1|2|4 overrides (experiments).
+// the replicated preamble are pure overhead there).
 static int pick_group(uint32_t n, int sm_count) {
-  static const int forced = [] { const char* e = getenv("MALIO_KNN_GROUP"); return e ? atoi(e) : 0; }();
-  if (forced == 1 || forced == 2 || forced == 4) return forced;
   const uint64_t per_sm = (uint64_t)n / (uint64_t)(sm_count > 0 ? sm_count : 1);
   if (per_sm <= 256) return 4;        // <= ~34k queries on 132 SMs
   if (per_sm <= 1280) return 2;       // <= ~169k
@@ -2693,7 +2515,7 @@ static int pick_group(uint32_t n, int sm_count) {
 // traversal alone when the index is off
 template <int MODE>
 int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pts_in, const uint32_t* perm,
-            const PassConst& pc, float max_sqdist, const ScanCtl* ctl = nullptr) {
+            const PassConst& pc, float max_sqdist) {
   cudaStream_t st = D->stream;
   const bool smem_stack = D->depth + KNN_POP_WIDTH <= (uint32_t)KNN_SMEM_DEPTH;
   const malio_scan_pt* pts = MODE == 0 ? pts_in : nullptr;
@@ -2706,43 +2528,25 @@ int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pt
   };
   if (D->grid_on) {
     // d_gstats: [2] traversal-list length, [4] ring-2 list length (both zeroed by the previous pass / the re-arm)
-    constexpr size_t smem1 = (size_t)GK_CAP * GK_THREADS * sizeof(float4) + (size_t)GK_ROWS1 * GK_THREADS * sizeof(uint2);
-    const int grp = (D->knn_direct && D->knn_keys) ? pick_group(n, D->sm_count) : 1;
+    const int grp = pick_group(n, D->sm_count);
     if (grp > 1) {
 #define MALIO_LAUNCH_KEYS(GG, PP)                                                                                                \
   do {                                                                                                                         \
     const uint32_t qpb = GD_THREADS / GG;                                                                                      \
-    if (ctl)                                                                                                                   \
-      knn_keys_kernel<MODE, true, GG, PP><<<(n + qpb - 1) / qpb, GD_THREADS, 0, st>>>(                                         \
-          D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,      \
-          D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr, ctl);                               \
-    else                                                                                                                       \
-      knn_keys_kernel<MODE, false, GG, PP><<<(n + qpb - 1) / qpb, GD_THREADS, 0, st>>>(                                        \
-          D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,      \
-          D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr, ctl);                               \
+    knn_keys_kernel<MODE, GG, PP><<<(n + qpb - 1) / qpb, GD_THREADS, 0, st>>>(                                                 \
+        D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,        \
+        D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr);                                      \
   } while (0)
       // measured (ncu kernel time, C2 sub-sampled): 12.5k queries 31 -> 12 us with 4 lanes + row preload; 100k 29.5 -> 24 us with
       // 2 lanes; from ~200k queries on (C4, C5) the thread-per-query kernel is as fast or faster and stays
       if (grp == 2) MALIO_LAUNCH_KEYS(2, false);
       else MALIO_LAUNCH_KEYS(4, true);
 #undef MALIO_LAUNCH_KEYS
-    } else if (D->knn_direct) {
-      if (ctl)
-        knn_direct_kernel<MODE, true><<<(n + GD_THREADS - 1) / GD_THREADS, GD_THREADS, 0, st>>>(
-            D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,
-            D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr, ctl);
-      else
-        knn_direct_kernel<MODE, false><<<(n + GD_THREADS - 1) / GD_THREADS, GD_THREADS, 0, st>>>(
-            D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,
-            D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr, ctl);
-    } else if (ctl)
-      knn_grid_kernel<MODE, 1, true><<<(n + GK_THREADS - 1) / GK_THREADS, GK_THREADS, smem1, st>>>(
+    } else {
+      knn_direct_kernel<MODE><<<(n + GD_THREADS - 1) / GD_THREADS, GD_THREADS, 0, st>>>(
           D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,
-          D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr, ctl);
-    else
-      knn_grid_kernel<MODE, 1, false><<<(n + GK_THREADS - 1) / GK_THREADS, GK_THREADS, smem1, st>>>(
-          D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,
-          D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr, ctl);
+          D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr);
+    }
     // 8 queries per warp and iteration; at most one resident wave of 64-thread blocks
     uint32_t fb_blocks = (n + 15) / 16;
     const uint32_t wave = (uint32_t)D->sm_count * 2;   // the list is usually (near) empty: a small grid walks it by stride
@@ -2750,7 +2554,7 @@ int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pt
     if (D->tree_free) {   // device-resident map: no tree to walk, the open queries are settled on the cell list itself
       knn_ring_kernel<MODE><<<fb_blocks, KNN_THREADS, 0, st>>>(D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist,
                                                              D->d_fb_list, D->d_gstats + 2, D->d_nn_idx, D->d_nn_d2, sel, D->d_gstats + 3,
-                                                             D->d_gstats + 7, ctl);
+                                                             D->d_gstats + 7);
       D->ctr.kernel_launches += 2;
       CUDA_TRY(cudaGetLastError());
       return MALIO_OK;
@@ -2758,10 +2562,10 @@ int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pt
     if (int rc = need_boxes()) return rc;
     if (smem_stack)
       knn_list_kernel<MODE, true><<<fb_blocks, KNN_THREADS, 0, st>>>(D->d_nodes, D->n_nodes, pts, perm, qs, n, pc, max_sqdist,
-                                                                    D->d_fb_list, D->d_gstats + 2, D->d_nn_idx, D->d_nn_d2, sel, D->d_gstats + 3, ctl);
+                                                                    D->d_fb_list, D->d_gstats + 2, D->d_nn_idx, D->d_nn_d2, sel, D->d_gstats + 3);
     else
       knn_list_kernel<MODE, false><<<fb_blocks, KNN_THREADS, 0, st>>>(D->d_nodes, D->n_nodes, pts, perm, qs, n, pc, max_sqdist,
-                                                                     D->d_fb_list, D->d_gstats + 2, D->d_nn_idx, D->d_nn_d2, sel, D->d_gstats + 3, ctl);
+                                                                     D->d_fb_list, D->d_gstats + 2, D->d_nn_idx, D->d_nn_d2, sel, D->d_gstats + 3);
     D->ctr.kernel_launches += 2;
   } else {
     // device-resident map without a live point: n_nodes = 0, the traversal below answers with empty lists as for an empty snapshot
@@ -2831,43 +2635,21 @@ int create(malio_handle* h) {
   CUDA_TRY(cudaHostGetDevicePointer((void**)&D->h_res_dev, D->h_res, 0));
   CUDA_TRY(cudaMalloc((void**)&D->d_bar, 4 * sizeof(uint32_t)));
   CUDA_TRY(cudaMemset(D->d_bar, 0, 4 * sizeof(uint32_t)));
-  CUDA_TRY(cudaFuncSetAttribute(pass_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RED_SMEM_DOUBLES * (int)sizeof(double)));
-  CUDA_TRY(cudaFuncSetAttribute(pass_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RED_SMEM_DOUBLES * (int)sizeof(double)));
-  CUDA_TRY(cudaFuncSetAttribute(pass_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RED_SMEM_DOUBLES * (int)sizeof(double)));
-  CUDA_TRY(cudaFuncSetAttribute(pass_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RED_SMEM_DOUBLES * (int)sizeof(double)));
+  CUDA_TRY(cudaFuncSetAttribute(pass_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RED_SMEM_DOUBLES * (int)sizeof(double)));
+  CUDA_TRY(cudaFuncSetAttribute(pass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RED_SMEM_DOUBLES * (int)sizeof(double)));
   {
     int per_sm = 0, per_sm2 = 0;
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pass_kernel<true, true>, RED_THREADS, PASS_FAST_SMEM_DOUBLES * sizeof(double)));
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm2, pass_kernel<false, true>, RED_THREADS, RED_SMEM_DOUBLES * sizeof(double)));
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pass_kernel<true>, RED_THREADS, PASS_FAST_SMEM_DOUBLES * sizeof(double)));
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm2, pass_kernel<false>, RED_THREADS, RED_SMEM_DOUBLES * sizeof(double)));
     D->pass_max_blocks_generic = per_sm2 * D->sm_count;
     int coop = 0;
     CUDA_TRY(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, D->device));
     D->pass_max_blocks = per_sm * D->sm_count;
     D->fused = coop && per_sm > 0;
     if (const char* e = getenv("MALIO_FUSED_PASS")) D->fused = D->fused && atoi(e) != 0;
-    if (const char* e = getenv("MALIO_COOP_LAUNCH")) D->coop_launch = atoi(e) != 0;
-    D->tau_inline = getenv("MALIO_TAU_INLINE") != nullptr;
-    if (const char* e = getenv("MALIO_KNN_DIRECT")) D->knn_direct = atoi(e) != 0;
-    if (const char* e = getenv("MALIO_KNN_KEYS")) D->knn_keys = atoi(e) != 0;
     if (const char* e = getenv("MALIO_PASS_TRACE")) D->trace_passes = atoi(e);
     if (const char* e = getenv("MALIO_KNN_CELL")) { D->env_knn_cell = (float)atof(e); D->env_knn_cell_set = true; }
     D->host_prof = getenv("MALIO_HOST_PROF") != nullptr;
-  }
-  {   // iterated update on the device (malio_solve.cu)
-    CUDA_TRY(cudaMalloc((void**)&D->d_ctl, sizeof(ScanCtl)));
-    CUDA_TRY(cudaMemset(D->d_ctl, 0, sizeof(ScanCtl)));
-    CUDA_TRY(cudaHostAlloc((void**)&D->h_ctl, sizeof(ScanCtl), cudaHostAllocDefault));
-    CUDA_TRY(cudaHostAlloc((void**)&D->h_upd, UPD_DOUBLES * sizeof(double), cudaHostAllocMapped));
-    std::memset(D->h_upd, 0, UPD_DOUBLES * sizeof(double));
-    CUDA_TRY(cudaHostGetDevicePointer((void**)&D->h_upd_dev, D->h_upd, 0));
-    CUDA_TRY(cudaEventCreate(&D->ev_seq[0])); CUDA_TRY(cudaEventCreate(&D->ev_seq[1]));
-    for (int k = 0; k < 3; ++k) for (int j = 0; j < MALIO_MAX_PASSES; ++j) CUDA_TRY(cudaEventCreate(&D->ev_pass[k][j]));
-    CUDA_TRY(cudaHostAlloc((void**)&D->h_pub, sizeof(PubCtl), cudaHostAllocMapped));
-    std::memset(D->h_pub, 0, sizeof(PubCtl));
-    CUDA_TRY(cudaHostGetDevicePointer((void**)&D->h_pub_dev, D->h_pub, 0));
-    if (const char* e = getenv("MALIO_PIPELINE")) D->pipeline = atoi(e) != 0;
-    if (int rc = malio_solve::setup(h)) return rc;
-    if (const char* e = getenv("MALIO_DEVICE_SOLVE")) D->device_solve = atoi(e) != 0;
   }
   D->h_gstats = reinterpret_cast<uint32_t*>(D->h_res + MALIO_RED_DOUBLES + 4);
   std::memset(D->h_gstats, 0, 8 * sizeof(uint32_t));
@@ -2877,33 +2659,12 @@ int create(malio_handle* h) {
   return MALIO_OK;
 }
 
-// publish a decision for the pass that was enqueued ahead of its state
-static void publish_pass(DeviceState* D, const PassConst* pc, int redo, int active, int parity, uint32_t seq, const uint32_t bar_base[3]) {
-  PubCtl* pub = D->h_pub;
-  if (pc) std::memcpy(&pub->pc, pc, sizeof(PassConst));
-  pub->redo = redo; pub->active = active; pub->parity = parity; pub->seq = seq;
-  for (int k = 0; k < 3; ++k) pub->bar_base[k] = bar_base[k];
-  std::atomic_thread_fence(std::memory_order_release);
-  *reinterpret_cast<volatile uint32_t*>(&pub->ticket) = D->pre_ticket;
-}
-int cancel_prelaunch(malio_handle* h) {
-  DeviceState* D = (DeviceState*)h->dev;
-  if (!D || !D->pre_armed) return MALIO_OK;
-  publish_pass(D, nullptr, 0, 0, D->parity, D->seq, D->bar_base);
-  D->pre_armed = false;
-  return MALIO_OK;
-}
-
 void destroy(malio_handle* h) {
   DeviceState* D = (DeviceState*)h->dev;
   if (!D) return;
-  cancel_prelaunch(h);
   malio_pre::destroy(h);
   malio_map::destroy(h);
   if (D->d_ids) cudaFree(D->d_ids);
-  if (D->host_prof && D->solve_n)
-    fprintf(stderr, "[malio] device-side update: %.1f us per solve kernel (%llu timed), %.1f us per update (%llu timed)\n",
-            1e3 * D->solve_ms / D->solve_n, (unsigned long long)D->solve_n, 1e3 * D->upd_ms / (D->upd_n ? D->upd_n : 1), (unsigned long long)D->upd_n);
   if (D->host_prof && D->host_passes)
     fprintf(stderr, "[malio] passes %llu: host launch %.1f us/pass, host wait-for-device %.1f us/pass\n",
             (unsigned long long)D->host_passes, D->host_launch_us / D->host_passes, D->host_wait_us / D->host_passes);
@@ -2916,12 +2677,6 @@ void destroy(malio_handle* h) {
                   D->d_cell_start, D->d_cell_cnt, D->d_cell_of, D->d_ctot, D->d_cbase, D->d_cell_pts, D->d_fb_list, D->d_gstats, D->d_bar, D->d_cand};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (D->h_res) cudaFreeHost(D->h_res);
-  if (D->d_ctl) cudaFree(D->d_ctl);
-  if (D->h_ctl) cudaFreeHost(D->h_ctl);
-  if (D->h_upd) cudaFreeHost(D->h_upd);
-  if (D->h_pub) cudaFreeHost(D->h_pub);
-  for (auto& e : D->ev_seq) if (e) cudaEventDestroy(e);
-  for (auto& row : D->ev_pass) for (auto& e : row) if (e) cudaEventDestroy(e);
   for (auto& e : D->ev) if (e) cudaEventDestroy(e);
   if (D->stream2) { cudaStreamSynchronize(D->stream2); cudaStreamDestroy(D->stream2); }
   if (D->stream3) { cudaStreamSynchronize(D->stream3); cudaStreamDestroy(D->stream3); }
@@ -3242,12 +2997,7 @@ int measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* Ht
   // the per-pass kernels read the scan in position order: the sorted copy when the scan was sorted, else the upload itself
   const malio_scan_pt* pts_k = (h->cfg.sort_queries && N > 0) ? D->d_pts_sorted : D->d_pts;
   const uint32_t* perm_k = nullptr;
-  // pipelined host loop: the kernels of THIS pass were enqueued while the previous pass ran and are waiting (fetch_ctl_kernel)
-  // for the state decided since; nothing is launched for it here, the decision is published below
-  const bool consume_pre = D->pre_armed;
-  if (consume_pre) {
-    if (redo_knn) { knn_now = true; D->searched_once = true; }
-  } else if (N > 0) {
+  if (N > 0) {
     if (h->cfg.sort_queries) {
       if (!D->perm_valid) {
         if (int rc = sort_queries<0>(h, D, N, pc)) return rc;
@@ -3261,7 +3011,7 @@ int measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* Ht
     // a scan that is a search pass it runs on the second stream beside the k-NN kernels (which leave most of the SMs'
     // warp slots empty) instead of inside the pass kernel.
     bool tau_async = false;
-    if (!D->tau_valid && redo_knn && D->fused && !D->tau_inline) {
+    if (!D->tau_valid && redo_knn && D->fused) {
       CUDA_TRY(cudaEventRecord(D->ev_sorted, st_));
       CUDA_TRY(cudaStreamWaitEvent(D->stream2, D->ev_sorted, 0));
       tau_kernel<<<(N + PLANE_THREADS - 1) / PLANE_THREADS, PLANE_THREADS, 0, D->stream2>>>(pts_k, perm_k, N, pc, D->d_table, D->d_tau2);
@@ -3330,40 +3080,9 @@ int measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* Ht
     void* kargs[] = {&a, &pc_arg, &prm_arg};
     const bool fast = per_block <= (uint32_t)PASS_FAST_TILES;
     const size_t pass_smem = (fast ? PASS_FAST_SMEM_DOUBLES : RED_SMEM_DOUBLES) * sizeof(double);
-    auto launch_pass = [&]() -> int {
-      const void* kfn = a.ctl ? (fast ? (const void*)pass_kernel<true, true> : (const void*)pass_kernel<false, true>)
-                              : (fast ? (const void*)pass_kernel<true, false> : (const void*)pass_kernel<false, false>);
-      if (D->coop_launch) {
-        CUDA_TRY(cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(RED_THREADS), kargs, pass_smem, st_));
-      } else {
-        // plain launch (MALIO_COOP_LAUNCH=0): the grid never exceeds the co-resident capacity, so the in-kernel barriers are
-        // safe as long as no OTHER grid-synchronising kernel competes for the same GPU at the same time (one handle in flight)
-        CUDA_TRY(cudaLaunchKernel(kfn, dim3(grid), dim3(RED_THREADS), kargs, pass_smem, st_));
-      }
-      D->ctr.kernel_launches += 1;
-      return MALIO_OK;
-    };
-    if (consume_pre) {
-      // the pass is already in the stream: hand it its state (a.seq / a.bar_base / parity were advanced above exactly as for a
-      // direct launch)
-      publish_pass(D, &pc, redo_knn ? 1 : 0, 1, D->parity, a.seq, a.bar_base);
-      D->pre_armed = false;
-      D->ctr.kernel_launches += 2;   // the fetch kernel and the pass kernel ran; the k-NN pair was counted by run_knn at enqueue time
-    } else {
-      if (int rc = launch_pass()) return rc;
-    }
-    // enqueue the NEXT pass's kernels now, while this pass runs: they wait on the device for the decision the host takes after
-    // this pass's result (its own step), which hides the launch path of every pass but the first
-    if (h->want_prelaunch && D->pipeline && !D->timing && N > 0 && D->grid_on && a.dbg == nullptr) {
-      D->pre_ticket += 1;
-      fetch_ctl_kernel<<<1, 128, 0, st_>>>(D->d_ctl, D->h_pub_dev, D->pre_ticket);
-      if (int rc = run_knn<0>(h, D, N, pts_k, perm_k, pc, P.knn_max_sqdist, D->d_ctl)) return rc;
-      a.ctl = D->d_ctl; a.mmkey_base = D->d_mmkey; a.cnt_base = D->d_counters + 4;
-      if (int rc = launch_pass()) return rc;
-      a.ctl = nullptr;
-      D->ctr.kernel_launches -= 1;   // counted when (if) it is consumed
-      D->pre_armed = true;
-    }
+    CUDA_TRY(cudaLaunchCooperativeKernel(fast ? (const void*)pass_kernel<true> : (const void*)pass_kernel<false>, dim3(grid),
+                                         dim3(RED_THREADS), kargs, pass_smem, st_));
+    D->ctr.kernel_launches += 1;
     D->tau_valid = D->tau_valid || N > 0;
     if (D->timing) { CUDA_TRY(cudaEventRecord(D->ev[2], st_)); CUDA_TRY(cudaEventRecord(D->ev[3], st_)); CUDA_TRY(cudaEventRecord(D->ev[4], st_)); }
     D->last_parity = D->parity;
@@ -3521,166 +3240,6 @@ int measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* Ht
   }
   if (st) *st = S;
   return MALIO_OK;
-}
-
-// ---- the whole iterated update as ONE enqueued sequence (malio_solve.cu has the per-pass algebra).
-// Returns MALIO_OK with *handled = 1 when the update was done here; *handled = 0 asks the caller to run its own loop
-// (configuration not eligible, or the degenerate n > N_eff branch was hit — the per-scan state has been re-armed then).
-int update_on_device(malio_handle* h, malio_state* x, double* P, int max_iter, malio_update_report* rep, int* handled) {
-  DeviceState* D = (DeviceState*)h->dev;
-  *handled = 0;
-  if (!D->device_solve || !D->fused || (D->comm && !D->p2p) || max_iter + 1 > MALIO_MAX_PASSES || max_iter < 1) return MALIO_OK;
-  if (h->mapst) { if (int rc = malio_map::commit(h)) return rc; }
-  if (!D->map_ready || !D->scan_ready) { h->err = "update before upload_map/upload_scan"; return MALIO_ERR_STATE; }
-  if (!D->grid_on || D->N == 0) return MALIO_OK;   // index-off mode and empty scans keep the host loop
-  CUDA_TRY(cudaSetDevice(D->device));
-  const malio_params& Pm = h->cfg.params;
-  const int L = Pm.n_lidar, n = 17 + 6 * L, c = 6 * (L + 1);
-  const uint32_t N = D->N;
-  cudaStream_t st_ = D->stream;
-  // ---- inputs of the control block
-  ScanCtl* hc = D->h_ctl;
-  hc->L = L; hc->n = n; hc->c = c; hc->max_iter = max_iter; hc->ext_en = Pm.extrinsic_est_en; hc->pad0 = 0;
-  hc->loc_thresh_max = Pm.localize_thresh_max; hc->loc_thresh_min = Pm.localize_thresh_min;
-  hc->loc_cov_max = Pm.localize_cov_max; hc->loc_cov_min = Pm.localize_cov_min;
-  hc->x_prop = *x;
-  std::memcpy(hc->P_prop, P, sizeof(double) * n * n);
-  for (int l = 0; l < MALIO_MAX_LIDAR; ++l) hc->tcomp[l] = D->tcomp[l];
-  for (int l = 0; l <= MALIO_MAX_LIDAR; ++l) hc->table_off[l] = D->table_off[l];
-  hc->scan_id = ++D->scan_id;
-  CUDA_TRY(cudaMemcpyAsync(D->d_ctl, hc, offsetof(ScanCtl, x), cudaMemcpyHostToDevice, st_));
-  if (D->timing) CUDA_TRY(cudaEventRecord(D->ev_seq[0], st_));
-  const uint32_t seq0 = D->seq + 1;
-  if (int rc = malio_solve::launch_init(h, st_, D->d_ctl, seq0, D->parity, D->d_bar)) return rc;
-  D->ctr.kernel_launches += 1;
-  // ---- state-independent preparation with the initial state: internal order of the scan, point covariance traces
-  malio_pass_state ps0;
-  std::memcpy(ps0.rot, x->rot, sizeof(ps0.rot)); std::memcpy(ps0.pos, x->pos, sizeof(ps0.pos)); std::memcpy(ps0.ext, x->ext, sizeof(ps0.ext));
-  const PassConst pc0 = make_pass_const(h, D, &ps0);
-  const ParamConst prm = make_param_const(Pm);
-  D->last_pc = pc0;
-  const malio_scan_pt* pts_k = h->cfg.sort_queries ? D->d_pts_sorted : D->d_pts;
-  bool sorted_now = false;
-  if (h->cfg.sort_queries && !D->perm_valid) {
-    if (int rc = sort_queries<0>(h, D, N, pc0)) return rc;
-    D->perm_valid = true;
-    sorted_now = true;
-  }
-  bool tau_async = false;
-  if (!D->tau_valid) {
-    CUDA_TRY(cudaEventRecord(D->ev_sorted, st_));
-    CUDA_TRY(cudaStreamWaitEvent(D->stream2, D->ev_sorted, 0));
-    tau_kernel<<<(N + PLANE_THREADS - 1) / PLANE_THREADS, PLANE_THREADS, 0, D->stream2>>>(pts_k, nullptr, N, pc0, D->d_table, D->d_tau2);
-    CUDA_TRY(cudaEventRecord(D->ev_tau, D->stream2));
-    D->tau_valid = true;
-    D->ctr.kernel_launches += 1;
-    tau_async = true;
-  }
-  // ---- the passes: k-NN (runs only where the control block says the search is repeated), pass kernel, solve kernel
-  const uint32_t n_tiles = (N + RED_THREADS - 1) / RED_THREADS;
-  uint32_t wave = fast_wave(D);
-  uint32_t per_block = (n_tiles + wave - 1) / wave;
-  if (per_block > (uint32_t)PASS_FAST_TILES) {
-    wave = (uint32_t)D->pass_max_blocks_generic < D->red_grid ? (uint32_t)D->pass_max_blocks_generic : D->red_grid;
-    per_block = (n_tiles + wave - 1) / wave;
-  }
-  const uint32_t grid = (n_tiles + per_block - 1) / per_block;
-  const size_t pass_smem = (per_block <= (uint32_t)PASS_FAST_TILES ? PASS_FAST_SMEM_DOUBLES : RED_SMEM_DOUBLES) * sizeof(double);
-  PassArgs a{};
-  a.pts = pts_k; a.perm = nullptr; a.N = N; a.table = D->d_table; a.nodes = D->d_mpts; a.node_cov = D->d_cov;
-  a.nn_idx = D->d_nn_idx; a.sel = D->d_sel; a.world = D->d_world; a.plane = D->d_plane; a.ucov = D->d_ucov;
-  a.tau2 = D->d_tau2; a.pd2 = D->d_pd2; a.tau = D->d_tau; a.normal_y = D->d_normal_y; a.rows12 = D->d_rows12; a.lid8 = D->d_lid8;
-  a.gstats = D->d_gstats; a.bar = D->d_bar;
-  a.n_tiles = n_tiles; a.block_red = D->d_block_red; a.d_res = D->d_res; a.h_res = D->h_res_dev;
-  a.peer.rank = D->rank; a.peer.world = D->p2p ? D->world : 1;
-  for (int r = 0; r < MAIL_MAX_WORLD; ++r) a.peer.mail[r] = D->mail_peer[r];
-  a.ctl = D->d_ctl; a.mmkey_base = D->d_mmkey; a.cnt_base = D->d_counters + 4;
-  a.dbg = nullptr;
-  a.xwait = D->d_cand + 1;
-  *reinterpret_cast<volatile uint32_t*>(D->h_res + MALIO_RED_DOUBLES + 9) = 0u;
-  PassConst pc_arg = pc0;
-  ParamConst prm_arg = prm;
-  void* kargs[] = {&a, &pc_arg, &prm_arg};
-  const void* kfn = per_block <= (uint32_t)PASS_FAST_TILES ? (const void*)pass_kernel<true, true> : (const void*)pass_kernel<false, true>;
-  volatile uint32_t* flag = reinterpret_cast<volatile uint32_t*>(D->h_upd + UPD_DOUBLES - 1);
-  for (int k = 0; k <= max_iter; ++k) {
-    if (D->timing) CUDA_TRY(cudaEventRecord(D->ev_pass[0][k], st_));
-    if (int rc = run_knn<0>(h, D, N, pts_k, nullptr, pc0, Pm.knn_max_sqdist, D->d_ctl)) return rc;
-    if (D->timing) CUDA_TRY(cudaEventRecord(D->ev_pass[1][k], st_));
-    if (k == 0 && tau_async) CUDA_TRY(cudaStreamWaitEvent(st_, D->ev_tau, 0));
-    if (D->coop_launch) CUDA_TRY(cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(RED_THREADS), kargs, pass_smem, st_));
-    else CUDA_TRY(cudaLaunchKernel(kfn, dim3(grid), dim3(RED_THREADS), kargs, pass_smem, st_));
-    if (D->timing) CUDA_TRY(cudaEventRecord(D->ev_pass[2][k], st_));
-    if (int rc = malio_solve::launch_solve(h, st_, D->d_ctl, D->d_res, D->d_bar, D->h_upd_dev, reinterpret_cast<uint32_t*>(D->h_upd_dev + UPD_DOUBLES - 1))) return rc;
-    D->ctr.kernel_launches += 2;
-  }
-  if (D->timing) CUDA_TRY(cudaEventRecord(D->ev_seq[1], st_));
-  // ---- one wait for the whole update
-  const auto t_wait = std::chrono::steady_clock::now();
-  for (uint64_t spins = 1; *flag != hc->scan_id; ++spins) {
-    __builtin_ia32_pause();
-    if ((spins & 0x3FFF) == 0) {
-      const cudaError_t q = cudaStreamQuery(st_);
-      if (q == cudaErrorNotReady) {
-        if (std::chrono::duration<double>(std::chrono::steady_clock::now() - t_wait).count() > 30.0) { h->err = "device-side update: no result after 30 s"; return MALIO_ERR_CUDA; }
-        continue;
-      }
-      if (q != cudaSuccess) { h->err = std::string("device-side update: ") + cudaGetErrorString(q); return MALIO_ERR_CUDA; }
-      if (*flag != hc->scan_id) { h->err = "device-side update finished without publishing its result"; return MALIO_ERR_CUDA; }
-    }
-  }
-  std::atomic_thread_fence(std::memory_order_acquire);
-  CUDA_TRY(cudaStreamSynchronize(st_));   // the remaining (skipped) launches drain in a few microseconds; later calls may reuse buffers
-  if (const uint32_t fault = *reinterpret_cast<volatile uint32_t*>(D->h_res + MALIO_RED_DOUBLES + 9)) {
-    if (fault == 2u) { h->err = "pass_kernel: a grid barrier did not complete within 2 s (blocks not co-resident)"; return MALIO_ERR_CUDA; }
-    h->err = "pass_kernel: a peer GPU did not answer the in-kernel exchange within 2 s";
-    return MALIO_ERR_NCCL;
-  }
-  if (D->h_gstats[6] & FAULT_STACK_OVERFLOW) { h->err = "k-NN traversal stack overflow: the snapshot is deeper than the max_depth declared at upload"; return MALIO_ERR_TREE_TOO_DEEP; }
-  const double* up = D->h_upd;
-  const int32_t* r = reinterpret_cast<const int32_t*>(up + MALIO_MAX_DOF * MALIO_MAX_DOF + 64 + MALIO_MAX_DOF);
-  const int passes = r[0], searches = r[1], status = r[2], need_host = r[3];
-  D->seq = (uint32_t)r[6]; D->parity = r[7]; D->last_parity = 1 - r[7];
-  const uint32_t smask = (uint32_t)r[8];
-  D->bar_base[0] = D->bar_base[1] = D->bar_base[2] = 0;   // the solve kernel leaves the barrier counters at zero ...
-  CUDA_TRY(cudaMemsetAsync(D->d_bar, 0, 3 * sizeof(uint32_t), st_));   // ... except after the very last pass
-  D->pass_done = true; D->searched_once = true;
-  D->host_passes += passes;
-  if (D->grid_on) { D->ctr.knn_fallback_queries += (uint64_t)D->h_gstats[3] * searches; D->ctr.knn_ring2_queries += (uint64_t)D->h_gstats[5] * searches; }
-  float ms_total = 0.f;
-  if (D->timing) {
-    cudaEventElapsedTime(&ms_total, D->ev_seq[0], D->ev_seq[1]);
-    for (int k = 0; k < passes && k <= max_iter; ++k) {
-      float ms = 0.f;
-      if (smask & (1u << k)) { cudaEventElapsedTime(&ms, D->ev_pass[0][k], D->ev_pass[1][k]); D->ctr.knn_launches += 1; D->ctr.knn_queries += N; D->ctr.knn_ms += ms; D->ctr.pass_fit_launches += 1; }
-      cudaEventElapsedTime(&ms, D->ev_pass[1][k], D->ev_pass[2][k]);
-      D->ctr.pass_launches += 1; D->ctr.pass_points += N; D->ctr.pass_ms += ms;
-      cudaEventElapsedTime(&ms, D->ev_pass[2][k], k < max_iter ? D->ev_pass[0][k + 1] : D->ev_seq[1]);
-      D->solve_ms += ms; D->solve_n += 1;
-    }
-    D->upd_ms += ms_total; D->upd_n += 1;
-  }
-  D->ctr.d2h_bytes += UPD_DOUBLES * sizeof(double);
-  (void)sorted_now;
-  if (need_host) {   // degenerate branch: the dense rows are needed -> the caller's loop redoes this scan from its start
-    reset_scan_kernel<<<(D->capN + 255) / 256, 256, 0, st_>>>(D->capN, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st_));
-    D->pass_done = false; D->searched_once = false;   // sort order and point covariance traces stay valid
-    return MALIO_OK;
-  }
-  *handled = 1;
-  std::memcpy(P, up, sizeof(double) * n * n);
-  std::memcpy(x, up + MALIO_MAX_DOF * MALIO_MAX_DOF, sizeof(malio_state));
-  if (rep) {
-    malio_update_report rp{};
-    rp.passes = passes; rp.searches = searches; rp.converged_count = r[5]; rp.last_status = status == MALIO_ERR_NO_EFFECTIVE_POINTS ? status : MALIO_OK;
-    rp.n_eff_last = (uint32_t)r[4]; rp.ms_device_total = ms_total; rp.ms_host_solve = 0.f;
-    std::memcpy(rp.dx_last, up + MALIO_MAX_DOF * MALIO_MAX_DOF + 64, sizeof(double) * MALIO_MAX_DOF);
-    *rep = rp;
-  }
-  if (status == MALIO_ERR_INVALID_ARG) { h->err = "singular information matrix"; return MALIO_ERR_INVALID_ARG; }
-  return status == MALIO_ERR_NO_EFFECTIVE_POINTS ? MALIO_ERR_NO_EFFECTIVE_POINTS : MALIO_OK;
 }
 
 int download_rows(malio_handle* h, double* h_x, double* hvec, uint32_t cap, uint32_t* n_rows) {

@@ -33,8 +33,6 @@ constexpr int RED_TASKS = 9;              // upper-triangular 4x4 blocks of the 
 constexpr int RED_KS = 14;                // row-splits per task: 9 x 14 = 126 of the 128 threads work
 constexpr int RED_SMEM_DOUBLES = RED_THREADS * (RED_HS_STRIDE + RED_HX_STRIDE) + RED_TASKS * RED_KS * 16;   // staging + flush scratch
 constexpr int TABLE_DOUBLES = 52;         // malio_pose_entry
-constexpr int MALIO_MAX_PASSES = 12;      // max_iter + 1 passes the device-side update can enqueue
-constexpr int UPD_DOUBLES = MALIO_MAX_DOF * MALIO_MAX_DOF + 64 + MALIO_MAX_DOF + 8;   // result block of the device-side update (+ flag)
 
 struct PassConst {
   double rot[4], pos[3];
@@ -83,43 +81,6 @@ __device__ __forceinline__ void body_to_world(const PassConst& pc, int lid, floa
 struct ParamConst {
   float plane_th, knn_max_sqdist;
   double cov_threshold, point_cov_max, point_cov_min, plane_cov_max, plane_cov_min, range_min, range_max;
-};
-
-// Control block of one iterated update run entirely on the device (malio_solve.cu): the per-pass kernels are enqueued for all
-// max_iter + 1 passes up front and read from here whether they run, with which state, and whether the search is repeated; the
-// one-block solve kernel after every pass takes the IESKF step (esekfom.hpp:521-718) and rewrites it.
-struct ScanCtl {
-  // ---- written by the host before the sequence is enqueued
-  int32_t L, n, c, max_iter;
-  int32_t ext_en, pad0;
-  double loc_thresh_max, loc_thresh_min, loc_cov_max, loc_cov_min;   // localization weight (laserMapping.cpp:749-756)
-  malio_state x_prop;
-  double P_prop[MALIO_MAX_DOF * MALIO_MAX_DOF];
-  malio_rigid tcomp[MALIO_MAX_LIDAR];
-  uint32_t table_off[MALIO_MAX_LIDAR + 1];
-  uint32_t scan_id;                 // written to the host's done flag when the update has finished
-  // ---- evolving on the device
-  malio_state x;
-  PassConst pc;                     // pass constants of the NEXT pass
-  int32_t it, redo, active, t, parity, pad1;
-  uint32_t seq, pad2;               // sequence number of the next pass (peer mailboxes, host result flag)
-  uint32_t bar_base[4];             // values of the grid-barrier counters before the next pass (monotone counters)
-  double P_cur[MALIO_MAX_DOF * MALIO_MAX_DOF];   // P_ of the last valid pass (esekfom.hpp:530 + projections)
-  // ---- report
-  int32_t passes, searches, status, need_host;   // need_host: the degenerate n > N_eff branch was hit (host finishes the scan)
-  uint32_t n_eff_last, converged_count;
-  uint32_t searched_mask, pad3;     // bit k: pass k repeated the search
-  double dx_last[MALIO_MAX_DOF];
-  double P_out[MALIO_MAX_DOF * MALIO_MAX_DOF];
-};
-
-// What the HOST publishes for a pass whose kernels were enqueued before its state was known (pipelined host loop): lives in
-// mapped pinned memory; fetch_ctl_kernel waits for `ticket` and copies the rest into the device's ScanCtl.
-struct PubCtl {
-  PassConst pc;
-  int32_t redo, active, parity, pad;
-  uint32_t seq, bar_base[3];
-  uint32_t ticket, pad2[3];
 };
 
 struct GridConst {
@@ -198,23 +159,12 @@ struct DeviceState {
   uint32_t cap_cells = 0, cap_cell_pts = 0;
   float4* d_cell_pts = nullptr;
   uint32_t* d_fb_list = nullptr;          // positions the fast path could not settle (-> exact traversal)
-  unsigned long long* d_cand = nullptr;   // candidates scanned by knn_grid_kernel since create (summed only while timing is on)
+  unsigned long long* d_cand = nullptr;   // [0] candidates scanned by the cell-list scans since create (summed only while timing is on)
   uint32_t* d_gstats = nullptr;           // [0] occupied cells, [1] live points, [2] fb count, [3] fb count of the last search, [4] ring-2 queries
   uint32_t* h_gstats = nullptr;            // pinned mirror (8 words, carved out of h_res)
   // fused pass (single cooperative launch per measurement pass)
-  bool fused = true; int pass_max_blocks = 0, pass_max_blocks_generic = 0; bool coop_launch = true;
-  // iterated update on the device (malio_solve.cu)
-  bool device_solve = false; ScanCtl* d_ctl = nullptr; ScanCtl* h_ctl = nullptr;   // h_ctl: pinned staging of the inputs
-  double* h_upd = nullptr; double* h_upd_dev = nullptr;   // mapped: P_out | state | dx_last | report ints | done flag (last 8 bytes)
-  uint32_t scan_id = 0;
-  // pipelined host loop: the next pass's kernels are enqueued while the current pass runs and wait for the host's decision
-  // (opt-in, MALIO_PIPELINE=1: measured break-even, see DESIGN.md)
-  bool pipeline = false; bool pre_armed = false; uint32_t pre_ticket = 0; PubCtl* h_pub = nullptr; PubCtl* h_pub_dev = nullptr;
-  double solve_ms = 0, upd_ms = 0; uint64_t solve_n = 0, upd_n = 0;   // MALIO_HOST_PROF=1 prints them at destroy
-  cudaEvent_t ev_seq[2] = {nullptr, nullptr}; cudaEvent_t ev_pass[3][MALIO_MAX_PASSES] = {};
-  bool knn_direct = true;    // 3x3x3 scan with direct register loads (MALIO_KNN_DIRECT=0: the shared-memory-staged kernel)
-  bool knn_keys = true;      // ... with one 32-bit key per kept candidate and G lanes per query (MALIO_KNN_KEYS=0: knn_direct_kernel)
-  bool tau_inline = false; int trace_passes = 0; float env_knn_cell = -1.f; bool env_knn_cell_set = false; bool host_prof = false;   // environment switches, read once in create()
+  bool fused = true; int pass_max_blocks = 0, pass_max_blocks_generic = 0;
+  int trace_passes = 0; float env_knn_cell = -1.f; bool env_knn_cell_set = false; bool host_prof = false;   // environment switches, read once in create()
   uint32_t* d_bar = nullptr; uint32_t bar_base[3] = {0, 0, 0}; uint32_t seq = 0;
   double* h_res_dev = nullptr;     // device-side address of the mapped host result buffer
   unsigned long long* d_dbg = nullptr; int trace_left = 0;

@@ -289,18 +289,9 @@ int malio_knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* nn_idx, fl
 // ---------------------------------------------------------------- IESKF (esekfom.hpp:495-721)
 int malio_ieskf_update(malio_handle* h, malio_state* x, double* Pio, int max_iter, double R, malio_update_report* rep) {
   if (!h || !x || !Pio || max_iter < 0) return MALIO_ERR_INVALID_ARG;
-  {   // the whole update as one enqueued kernel sequence with the step taken on the device (malio_solve.cu), where eligible
-    int handled = 0;
-    const int rc = malio_dev::update_on_device(h, x, Pio, max_iter, rep, &handled);
-    if (handled || (rc != MALIO_OK && rc != MALIO_ERR_NO_EFFECTIVE_POINTS)) return rc;
-  }
   const StateLayout ly(h->cfg.params.n_lidar);
   const int n = ly.n, c = ly.c;
   malio_update_report rp{};
-  struct PrelaunchGuard {   // a pass enqueued ahead of its state must always be told whether to run
-    malio_handle* h;
-    ~PrelaunchGuard() { malio_dev::cancel_prelaunch(h); }
-  } prelaunch_guard{h};
   const malio_state x_prop = *x;
   Mat P_prop(n, n);
   std::memcpy(P_prop.a.data(), Pio, sizeof(double) * n * n);
@@ -319,9 +310,7 @@ int malio_ieskf_update(malio_handle* h, malio_state* x, double* Pio, int max_ite
     std::memcpy(ps.pos, x->pos, sizeof(ps.pos));
     std::memcpy(ps.ext, x->ext, sizeof(ps.ext));
     malio_pass_stats st{};
-    h->want_prelaunch = (it < max_iter - 1) ? 1 : 0;   // another pass may follow: its kernels are enqueued while this one runs
     const int rc = malio_dev::measure(h, &ps, redo ? 1 : 0, G.a.data(), g.data(), &st);   // h_dyn_share, :512
-    h->want_prelaunch = 0;
     rp.passes++;
     if (redo) rp.searches++;
     rp.ms_device_total += st.ms_total;
@@ -352,7 +341,6 @@ int malio_ieskf_update(malio_handle* h, malio_state* x, double* Pio, int max_ite
       right_block_T<2>(P, ly.grav, J2);
     }
     if (n > (int)st.n_eff) {   // degenerate branch :574-582 — needs the rows, scalar R
-      malio_dev::cancel_prelaunch(h);   // download_rows puts work on the stream: nothing may be waiting in front of it
       const int m = (int)st.n_eff;
       std::vector<double> rows((size_t)MALIO_MAX_DOF * c), hv(MALIO_MAX_DOF);
       uint32_t nr = 0;

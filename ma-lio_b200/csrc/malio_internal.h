@@ -25,7 +25,6 @@ struct malio_handle {
   void* dev = nullptr;   // DeviceState*, owned by the CUDA TU
   void* pre = nullptr;   // PreState*, owned by malio_preproc.cu (undistortion / voxel grid buffers)
   void* mapst = nullptr; // MapOpsState*, owned by malio_mapops.cu (device-resident map replay)
-  int want_prelaunch = 0; // set by malio_ieskf_update around malio_dev::measure: another pass may follow this one
 };
 
 // CUDA TU entry points used by the C-ABI wrappers
@@ -46,8 +45,6 @@ int knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, 
 int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world);
 int rearm_scan(malio_handle* h);
 int reserve_scan(malio_handle* h, uint32_t n);
-int cancel_prelaunch(malio_handle* h);   // a pass enqueued ahead of its state is told not to run (no-op when none is pending)
-int update_on_device(malio_handle* h, malio_state* x, double* P, int max_iter, malio_update_report* rep, int* handled);
 int grow_slots(malio_handle* h, uint32_t n, uint32_t keep);
 int index_from_slots(malio_handle* h, uint32_t n_slots, const float box[6]);
 int get_counters(malio_handle* h, malio_counters* out);
@@ -55,17 +52,6 @@ int set_timing(malio_handle* h, int enable);
 int comm_init(malio_handle* h, const uint8_t* id, int rank, int world);
 int get_unique_id(uint8_t* id);
 }  // namespace malio_dev
-
-// malio_solve.cu — the IESKF step on the device; ScanCtl is defined in malio_device.cuh (CUDA translation units only)
-#ifdef __CUDACC__
-namespace malio_devstate { struct ScanCtl; }
-namespace malio_solve {
-int setup(malio_handle* h);
-int launch_init(malio_handle* h, cudaStream_t st, malio_devstate::ScanCtl* d_ctl, uint32_t seq0, int parity, uint32_t* d_bar);
-int launch_solve(malio_handle* h, cudaStream_t st, malio_devstate::ScanCtl* d_ctl, const double* d_res, uint32_t* d_bar, double* h_out_dev,
-                 uint32_t* h_flag_dev);
-}  // namespace malio_solve
-#endif
 
 // malio_mapops.cu — the device-resident map (SURVEY.md §8f N1)
 namespace malio_map {

@@ -1,5 +1,5 @@
-// malio_manifold.h — the state manifold of the filter (MTK SO3 / S2 / vect operators, A_matrix) shared by the host IESKF
-// (malio_host.cpp) and the device-side IESKF step (malio_solve.cu).  One source for both: __host__ __device__ inline.
+// malio_manifold.h — the state manifold of the filter (MTK SO3 / S2 / vect operators, A_matrix) used by the host IESKF
+// (malio_host.cpp).
 //
 // Reference interface mirrored (paths relative to /root/reference/MA_LIO):
 //   state_ikfom manifold                        src/use-ikfom.hpp:14-27
@@ -13,32 +13,26 @@
 
 #include "malio_b200.h"
 
-#ifdef __CUDACC__
-#define MALIO_HD __host__ __device__
-#else
-#define MALIO_HD
-#endif
-
 namespace malio_manifold {
 
 // ---------------------------------------------------------------- rotations
 struct Quat { double w, x, y, z; };
-MALIO_HD inline Quat qload(const double* q) { return Quat{q[0], q[1], q[2], q[3]}; }
-MALIO_HD inline void qstore(const Quat& q, double* o) { o[0] = q.w; o[1] = q.x; o[2] = q.y; o[3] = q.z; }
-MALIO_HD inline Quat qconj(const Quat& q) { return Quat{q.w, -q.x, -q.y, -q.z}; }
-MALIO_HD inline Quat qmul(const Quat& a, const Quat& b) {
+inline Quat qload(const double* q) { return Quat{q[0], q[1], q[2], q[3]}; }
+inline void qstore(const Quat& q, double* o) { o[0] = q.w; o[1] = q.x; o[2] = q.y; o[3] = q.z; }
+inline Quat qconj(const Quat& q) { return Quat{q.w, -q.x, -q.y, -q.z}; }
+inline Quat qmul(const Quat& a, const Quat& b) {
   return Quat{a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
               a.w * b.y + a.y * b.w + a.z * b.x - a.x * b.z, a.w * b.z + a.z * b.w + a.x * b.y - a.y * b.x};
 }
 struct M3 { double m[3][3]; };
-MALIO_HD inline M3 hat3(const double v[3]) { return M3{{{0, -v[2], v[1]}, {v[2], 0, -v[0]}, {-v[1], v[0], 0}}}; }
-MALIO_HD inline M3 mul3(const M3& A, const M3& B) {
+inline M3 hat3(const double v[3]) { return M3{{{0, -v[2], v[1]}, {v[2], 0, -v[0]}, {-v[1], v[0], 0}}}; }
+inline M3 mul3(const M3& A, const M3& B) {
   M3 C{};
   for (int i = 0; i < 3; ++i)
     for (int j = 0; j < 3; ++j) C.m[i][j] = A.m[i][0] * B.m[0][j] + A.m[i][1] * B.m[1][j] + A.m[i][2] * B.m[2][j];
   return C;
 }
-MALIO_HD inline M3 rotmat(const Quat& q) {
+inline M3 rotmat(const Quat& q) {
   const double tx = 2 * q.x, ty = 2 * q.y, tz = 2 * q.z;
   const double twx = tx * q.w, twy = ty * q.w, twz = tz * q.w, txx = tx * q.x, txy = ty * q.x, txz = tz * q.x;
   const double tyy = ty * q.y, tyz = tz * q.y, tzz = tz * q.z;
@@ -49,7 +43,7 @@ constexpr double kTol = 1e-11;                    // MTK::tolerance<double>() (m
 constexpr double kGrav = 98090.0 / 10000.0;       // S2<double,98090,10000,1> (use-ikfom.hpp:8)
 
 // cos(sqrt(x2)), sinc(sqrt(x2))  (mtkmath.hpp:141-171)
-MALIO_HD inline void cos_sinc_sqrt(double x2, double& c, double& sc) {
+inline void cos_sinc_sqrt(double x2, double& c, double& sc) {
   const double b0 = std::numeric_limits<double>::epsilon();
   const double bn = std::sqrt(std::sqrt(b0));
   if (x2 >= bn) {
@@ -70,21 +64,21 @@ MALIO_HD inline void cos_sinc_sqrt(double x2, double& c, double& sc) {
   sc = si;
 }
 // quaternion of MTK::exp(vec, scale) (mtkmath.hpp:249-256)
-MALIO_HD inline Quat exp_quat(const double v[3], double scale) {
+inline Quat exp_quat(const double v[3], double scale) {
   double c, sc;
   cos_sinc_sqrt(scale * scale * (v[0] * v[0] + v[1] * v[1] + v[2] * v[2]), c, sc);
   const double m = sc * scale;
   return Quat{c, m * v[0], m * v[1], m * v[2]};
 }
 // SO3::log (SOn.hpp:341-345 -> mtkmath.hpp:268-289, scale 2, +-periodic)
-MALIO_HD inline void so3_log(const Quat& q, double out[3]) {
+inline void so3_log(const Quat& q, double out[3]) {
   double nv = std::sqrt(q.x * q.x + q.y * q.y + q.z * q.z);
   if (nv < kTol) nv = kTol;
   const double s = 2.0 / nv * std::atan(nv / q.w);
   out[0] = s * q.x; out[1] = s * q.y; out[2] = s * q.z;
 }
 // MTK::A_matrix (mtkmath.hpp:235-247)
-MALIO_HD inline M3 A_matrix(const double v[3]) {
+inline M3 A_matrix(const double v[3]) {
   const double sq = v[0] * v[0] + v[1] * v[1] + v[2] * v[2], nrm = std::sqrt(sq);
   M3 R{{{1, 0, 0}, {0, 1, 0}, {0, 0, 1}}};
   if (nrm < kTol) return R;
@@ -94,14 +88,14 @@ MALIO_HD inline M3 A_matrix(const double v[3]) {
     for (int j = 0; j < 3; ++j) R.m[i][j] += a * H.m[i][j] + b * HH.m[i][j];
   return R;
 }
-MALIO_HD inline M3 transpose3(const M3& A) {
+inline M3 transpose3(const M3& A) {
   M3 T{};
   for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) T.m[i][j] = A.m[j][i];
   return T;
 }
 
 // S2 chart with the x axis as pole (S2_typ == 1, S2.hpp:225-243): Bx is 3x2
-MALIO_HD inline void S2_Bx(const double v[3], double B[3][2]) {
+inline void S2_Bx(const double v[3], double B[3][2]) {
   const double L = kGrav;
   if (v[0] + L > kTol) {
     const double d = L + v[0];
@@ -115,7 +109,7 @@ MALIO_HD inline void S2_Bx(const double v[3], double B[3][2]) {
     B[2][0] = 1;
   }
 }
-MALIO_HD inline void S2_boxplus(double v[3], const double d[2]) {   // S2.hpp:136-142
+inline void S2_boxplus(double v[3], const double d[2]) {   // S2.hpp:136-142
   double B[3][2];
   S2_Bx(v, B);
   const double Bu[3] = {B[0][0] * d[0] + B[0][1] * d[1], B[1][0] * d[0] + B[1][1] * d[1], B[2][0] * d[0] + B[2][1] * d[1]};
@@ -124,7 +118,7 @@ MALIO_HD inline void S2_boxplus(double v[3], const double d[2]) {   // S2.hpp:13
                        R.m[2][0] * v[0] + R.m[2][1] * v[1] + R.m[2][2] * v[2]};
   v[0] = o[0]; v[1] = o[1]; v[2] = o[2];
 }
-MALIO_HD inline void S2_boxminus(const double v[3], const double o[3], double res[2]) {   // S2.hpp:144-168
+inline void S2_boxminus(const double v[3], const double o[3], double res[2]) {   // S2.hpp:144-168
   const double cr[3] = {v[1] * o[2] - v[2] * o[1], v[2] * o[0] - v[0] * o[2], v[0] * o[1] - v[1] * o[0]};
   const double v_sin = std::sqrt(cr[0] * cr[0] + cr[1] * cr[1] + cr[2] * cr[2]);
   const double v_cos = v[0] * o[0] + v[1] * o[1] + v[2] * o[2];
@@ -143,7 +137,7 @@ MALIO_HD inline void S2_boxminus(const double v[3], const double o[3], double re
 }
 // J = Nx(x) * Mx(x0, delta), the 2x2 projection of the S2 block (esekfom.hpp:560-564; S2.hpp:269-291).
 // Mx's exp_delta uses scalar(1/2) == 0 in the reference, i.e. the identity rotation.
-MALIO_HD inline void S2_projection(const double x[3], const double x0[3], const double delta[2], double J[2][2]) {
+inline void S2_projection(const double x[3], const double x0[3], const double delta[2], double J[2][2]) {
   double Bx[3][2], B0[3][2];
   S2_Bx(x, Bx);
   S2_Bx(x0, B0);
@@ -171,14 +165,14 @@ struct StateLayout {
   int L, n, c, rot, vel, bg, ba, grav;
   int offR[MALIO_MAX_LIDAR], offT[MALIO_MAX_LIDAR];
   int so3[1 + MALIO_MAX_LIDAR];
-  MALIO_HD explicit StateLayout(int L_) : L(L_) {
+  explicit StateLayout(int L_) : L(L_) {
     n = 17 + 6 * L; c = 6 * (L + 1); rot = 3;
     so3[0] = rot;
     for (int l = 0; l < L; ++l) { offR[l] = 6 + 3 * l; offT[l] = 6 + 3 * L + 3 * l; so3[1 + l] = offR[l]; }
     vel = 6 + 6 * L; bg = vel + 3; ba = bg + 3; grav = ba + 3;
   }
 };
-MALIO_HD inline void boxminus(const StateLayout& ly, const malio_state& x, const malio_state& x0, double* d) {
+inline void boxminus(const StateLayout& ly, const malio_state& x, const malio_state& x0, double* d) {
   for (int k = 0; k < 3; ++k) d[k] = x.pos[k] - x0.pos[k];
   so3_log(qmul(qconj(qload(x0.rot)), qload(x.rot)), d + ly.rot);
   for (int l = 0; l < ly.L; ++l) {
@@ -192,7 +186,7 @@ MALIO_HD inline void boxminus(const StateLayout& ly, const malio_state& x, const
   }
   S2_boxminus(x.grav, x0.grav, d + ly.grav);
 }
-MALIO_HD inline void boxplus(const StateLayout& ly, malio_state& x, const double* d) {
+inline void boxplus(const StateLayout& ly, malio_state& x, const double* d) {
   for (int k = 0; k < 3; ++k) x.pos[k] += d[k];
   qstore(qmul(qload(x.rot), exp_quat(d + ly.rot, 0.5)), x.rot);
   for (int l = 0; l < ly.L; ++l) {
@@ -208,7 +202,7 @@ MALIO_HD inline void boxplus(const StateLayout& ly, malio_state& x, const double
 }
 
 // singular values of the N x 3 matrix whose Gram matrix is S (descending) = sqrt(eig(S)): cyclic Jacobi on the 3x3
-MALIO_HD inline void sym3_singular_values(const double S[6], double sv[3]) {
+inline void sym3_singular_values(const double S[6], double sv[3]) {
   double A[3][3] = {{S[0], S[1], S[2]}, {S[1], S[3], S[4]}, {S[2], S[4], S[5]}};
   for (int sweep = 0; sweep < 50; ++sweep) {
     const double off = std::fabs(A[0][1]) + std::fabs(A[0][2]) + std::fabs(A[1][2]);

@@ -34,8 +34,6 @@ int knn(malio_handle*, const float*, uint32_t, uint32_t*, float*, float*) { retu
 int map_incremental(malio_handle*, const malio_pass_state*, double, int, uint8_t*, float*) { return MALIO_ERR_STATE; }
 int rearm_scan(malio_handle*) { return MALIO_OK; }
 int reserve_scan(malio_handle*, uint32_t) { return MALIO_OK; }
-int cancel_prelaunch(malio_handle*) { return MALIO_OK; }
-int update_on_device(malio_handle*, malio_state*, double*, int, malio_update_report*, int* handled) { *handled = 0; return MALIO_OK; }
 int get_counters(malio_handle*, malio_counters* out) { std::memset(out, 0, sizeof(*out)); return MALIO_OK; }
 int set_timing(malio_handle*, int) { return MALIO_OK; }
 int comm_init(malio_handle*, const uint8_t*, int, int) { return MALIO_ERR_NCCL; }

@@ -1,5 +1,5 @@
-"""GPU parity of the k-NN fast path (cell-list index over the snapshot, knn_grid_kernel) and its hand-over to the
-exact ikd-Tree-order traversal (knn_list_kernel).  Whatever the cell edge — automatic, tiny, huge, or the index
+"""GPU parity of the k-NN fast path (cell-list index over the snapshot, knn_direct_kernel / knn_keys_kernel) and its
+hand-over to the exact ikd-Tree-order traversal (knn_list_kernel).  Whatever the cell edge — automatic, tiny, huge, or the index
 switched off — the neighbour lists and float distances must be the reference's, index for index: compared with
 the restated Search (oracle) and, through the golden file, with the real ikd_Tree.cpp."""
 import os

@@ -118,24 +118,6 @@ def test_frozen_extrinsics_rows_of_the_degenerate_branch(L):
     model.close(); orc.close()
 
 
-def test_frozen_extrinsics_device_side_update(monkeypatch):
-    """malio_solve.cu carries its own copy of extrinsic_est_en."""
-    case = _frozen(synth.make_case("fds", 20000, 200000, 3, 3, varied_map_cov=True))
-    snap = plugin.build_static_snapshot(case.map_xyz, case.map_normal_y)
-    monkeypatch.setenv("MALIO_DEVICE_SOLVE", "1")
-    dev = H.make_model(case, snap)
-    monkeypatch.setenv("MALIO_DEVICE_SOLVE", "0")
-    host = H.make_model(case, snap)
-    monkeypatch.delenv("MALIO_DEVICE_SOLVE")
-    rep, xd, Pd = _compare_update(dev, H.make_oracle(case, snap), case)
-    assert rep.ms_host_solve == 0.0
-    xh, Ph = case.x_prop.copy(), case.P_prop.copy()
-    rh = host.update_iterated_dyn_share_modified(xh, Ph, case.max_iter)
-    assert rh.passes == rep.passes and np.abs(synth.state_to_vec(xd, 3) - synth.state_to_vec(xh, 3)).max() < 1e-9
-    assert H.rel_err(Pd, Ph) < 1e-8
-    dev.close(); host.close()
-
-
 # ------------------------------------------------------------------ pose tables: uneven lengths, indices beyond the end
 TABLES = (2, 7, 40)
 

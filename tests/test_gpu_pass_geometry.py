@@ -292,26 +292,22 @@ def test_boundaries_unfused(worlds, shape, monkeypatch, capfd):
 
 
 @pytest.mark.parametrize("shape", ["N=256W", "N=256W+1"])
-def test_device_solve_at_the_fast_generic_switch(worlds, shape, monkeypatch):
-    """update_on_device derives the launch on its own: the last FAST and the first generic launch give the host loop's
-    passes, searches and state."""
+def test_host_update_at_the_fast_generic_switch(worlds, shape):
+    """The whole iterated update at the last FAST and the first generic launch: the oracle's passes, searches, N_eff,
+    state and covariance."""
     base, pw, snap = worlds(3)
     N = boundary_n(shape)
     case = layout(base, pw, N, "interleaved", rr.launch_geometry(N, sm_count()))
-    monkeypatch.setenv("MALIO_DEVICE_SOLVE", "1")
-    dev = H.make_model(case, snap)
-    monkeypatch.setenv("MALIO_DEVICE_SOLVE", "0")
-    host = H.make_model(case, snap)
-    monkeypatch.delenv("MALIO_DEVICE_SOLVE")
+    model = H.make_model(case, snap)
+    orc = H.make_oracle(case, snap)
     try:
-        xd, Pd = case.x_prop.copy(), case.P_prop.copy()
         xh, Ph = case.x_prop.copy(), case.P_prop.copy()
-        rd = dev.update_iterated_dyn_share_modified(xd, Pd, case.max_iter)
-        rh = host.update_iterated_dyn_share_modified(xh, Ph, case.max_iter)
-        assert rd.last_status == 0 and rh.last_status == 0
-        assert rd.ms_host_solve == 0.0
-        assert rd.passes == rh.passes and rd.searches == rh.searches and rd.n_eff_last == rh.n_eff_last
-        assert np.abs(synth.state_to_vec(xd, 3) - synth.state_to_vec(xh, 3)).max() < 1e-9
-        assert H.rel_err(Pd, Ph) < 1e-8
+        xo, Po = case.x_prop.copy(), case.P_prop.copy()
+        rh = model.update_iterated_dyn_share_modified(xh, Ph, case.max_iter)
+        rc, _, _, ro = orc.update_iterated(xo, Po, case.max_iter, nthreads=8)
+        assert rc == 0 and rh.last_status == 0 and rh.ms_host_solve > 0.0
+        assert rh.passes == ro.passes and rh.searches == ro.searches and rh.n_eff_last == ro.n_eff_last
+        assert np.abs(synth.state_to_vec(xh, 3) - synth.state_to_vec(xo, 3)).max() < 1e-8
+        assert H.rel_err(Ph, Po) < 1e-6
     finally:
-        dev.close(); host.close()
+        model.close(); orc.close()

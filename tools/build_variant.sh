@@ -10,7 +10,7 @@ mkdir -p $out
 cd $root/ma-lio_b200/csrc
 NVCC=${NVCC:-nvcc}
 NV="$NVCC -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -fmad=false -Xcompiler -fPIC -ccbin /usr/bin/g++ -I../../include -I. $extra"
-for f in malio_b200 malio_preproc malio_mapops malio_solve; do
+for f in malio_b200 malio_preproc malio_mapops; do
   $NV -Xptxas -v -c $f.cu -o $out/$f.o 2> $out/ptxas_$f.log &
 done
 /usr/bin/g++ -O3 -std=c++17 -fPIC -fopenmp -Wall -I../../include -I. -c malio_host.cpp -o $out/malio_host.o

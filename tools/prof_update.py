@@ -1,4 +1,4 @@
-"""Workload for ncu / timing: C2, a few full iterated updates on a resident scan (device-side IESKF step)."""
+"""Workload for ncu / timing: C2, a few full iterated updates on a resident scan."""
 import sys, os, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "ma-lio_b200"))
