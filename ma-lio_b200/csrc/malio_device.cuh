@@ -1,6 +1,11 @@
-// malio_device.cuh — device-side state of one handle and the constants shared by the CUDA translation units of
-// libmalio_b200.so (malio_b200.cu: k-NN / pass kernels and the per-scan entry points; malio_preproc.cu: undistortion and
-// voxel grid; malio_mapops.cu: the device-resident map and its Add_Points / Delete_Point_Boxes replay).
+// malio_device.cuh — device-side state of one handle, the device math and constants shared by the CUDA translation units
+// of libmalio_b200.so, and the host functions they call in each other.  The units (no relocatable device code: each one
+// launches only its own kernels):
+//   malio_knn.cu      the k-NN search and the map it searches (snapshot upload, cell-list index, query sort)
+//   malio_pass.cu     the measurement pass (plane fit, gate, reduction, the fused pass_kernel and its multi-GPU exchange)
+//   malio_b200.cu     handle lifecycle and per-scan data movement (create / destroy, scan upload, downloads)
+//   malio_preproc.cu  undistortion, voxel grid, world registration
+//   malio_mapops.cu   the device-resident map and its Add_Points / Delete_Point_Boxes replay
 #ifndef MALIO_DEVICE_CUH_
 #define MALIO_DEVICE_CUH_
 
@@ -8,6 +13,7 @@
 #include <nccl.h>
 
 #include <cstdint>
+#include <cstring>
 #include <string>
 
 #include "malio_internal.h"
@@ -33,6 +39,9 @@ constexpr int RED_TASKS = 9;              // upper-triangular 4x4 blocks of the 
 constexpr int RED_KS = 14;                // row-splits per task: 9 x 14 = 126 of the 128 threads work
 constexpr int RED_SMEM_DOUBLES = RED_THREADS * (RED_HS_STRIDE + RED_HX_STRIDE) + RED_TASKS * RED_KS * 16;   // staging + flush scratch
 constexpr int TABLE_DOUBLES = 52;         // malio_pose_entry
+constexpr int SORT_BINS = 1 << 16;        // counting sort of the queries (malio_knn.cu): bins ...
+constexpr int SCAN_BLOCKS = 64;           // ... and blocks of its prefix scan
+constexpr uint32_t FAULT_STACK_OVERFLOW = 1u;   // d_gstats[6]: a traversal stack overflowed (snapshot deeper than declared)
 
 struct PassConst {
   double rot[4], pos[3];
@@ -48,15 +57,57 @@ struct PassConst {
   double RcT[MALIO_MAX_LIDAR][9];      // R(temporal_comp_l)^T  (entry 0 unused)
 };
 
-// Quaternion * vector as Eigen's _transformVector: v + w*uv + qv x uv, uv = 2 (qv x v); q = (w,x,y,z).  The same operations,
-// in the same order, as malio_b200.cu's q_rot.
-__device__ __forceinline__ void eigen_q_rot(const double q[4], const double v[3], double o[3]) {
-  const double uv0 = q[2] * v[2] - q[3] * v[1], uv1 = q[3] * v[0] - q[1] * v[2], uv2 = q[1] * v[1] - q[2] * v[0];
-  const double u[3] = {uv0 + uv0, uv1 + uv1, uv2 + uv2};
-  const double c0 = q[2] * u[2] - q[3] * u[1], c1 = q[3] * u[0] - q[1] * u[2], c2 = q[1] * u[1] - q[2] * u[0];
-  o[0] = v[0] + q[0] * u[0] + c0;
-  o[1] = v[1] + q[0] * u[1] + c1;
-  o[2] = v[2] + q[0] * u[2] + c2;
+// ------------------------------------------------------------------ small device algebra (mirrors Eigen's op order)
+__device__ __forceinline__ void cross3(const double a[3], const double b[3], double o[3]) {
+  o[0] = a[1] * b[2] - a[2] * b[1];
+  o[1] = a[2] * b[0] - a[0] * b[2];
+  o[2] = a[0] * b[1] - a[1] * b[0];
+}
+// Quaternion * vector as Eigen's _transformVector: v + w*uv + qv x uv, uv = 2 (qv x v); q = (w,x,y,z)
+__device__ __forceinline__ void q_rot(const double q[4], const double v[3], double o[3]) {
+  const double qv[3] = {q[1], q[2], q[3]};
+  double uv[3], c2[3];
+  cross3(qv, v, uv);
+  uv[0] += uv[0]; uv[1] += uv[1]; uv[2] += uv[2];
+  cross3(qv, uv, c2);
+  o[0] = v[0] + q[0] * uv[0] + c2[0];
+  o[1] = v[1] + q[0] * uv[1] + c2[1];
+  o[2] = v[2] + q[0] * uv[2] + c2[2];
+}
+__device__ __forceinline__ void q_rot_conj(const double q[4], const double v[3], double o[3]) {
+  const double qc[4] = {q[0], -q[1], -q[2], -q[3]};
+  q_rot(qc, v, o);
+}
+// laserMapping.cpp:569-579: point in its LiDAR frame -> LiDAR-0 body frame b, IMU frame m, world g
+__device__ __forceinline__ void transform_point(const PassConst& pc, float px, float py, float pz, int lid,
+                                                double b[3], double m[3], double g[3]) {
+  b[0] = px; b[1] = py; b[2] = pz;
+  if (lid != 0) {
+    double a[3], t[3], d[3];
+    q_rot(pc.eq[lid], b, a);
+    a[0] += pc.et[lid][0]; a[1] += pc.et[lid][1]; a[2] += pc.et[lid][2];
+    q_rot(pc.cq[lid], a, t);
+    d[0] = (t[0] + pc.ct[lid][0]) - pc.et[0][0];
+    d[1] = (t[1] + pc.ct[lid][1]) - pc.et[0][1];
+    d[2] = (t[2] + pc.ct[lid][2]) - pc.et[0][2];
+    q_rot_conj(pc.eq[0], d, b);
+  }
+  q_rot(pc.eq[0], b, m);
+  m[0] += pc.et[0][0]; m[1] += pc.et[0][1]; m[2] += pc.et[0][2];
+  q_rot(pc.rot, m, g);
+  g[0] += pc.pos[0]; g[1] += pc.pos[1]; g[2] += pc.pos[2];
+}
+// order-preserving map double <-> uint64 (so that min/max can use integer atomics: exact and order-independent)
+__host__ __device__ __forceinline__ unsigned long long dkey(double v) {
+  unsigned long long b;
+  memcpy(&b, &v, 8);
+  return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
+}
+__host__ __device__ __forceinline__ double dkey_inv(unsigned long long k) {
+  const unsigned long long b = (k & 0x8000000000000000ull) ? (k & 0x7FFFFFFFFFFFFFFFull) : ~k;
+  double v;
+  memcpy(&v, &b, 8);
+  return v;
 }
 
 // pointBodyToWorld / RGBpointBodyToWorld (laserMapping.cpp:134-163) in the reference's own operation order (no detour through
@@ -67,14 +118,14 @@ __device__ __forceinline__ void eigen_q_rot(const double q[4], const double v[3]
 __device__ __forceinline__ void body_to_world(const PassConst& pc, int lid, float x, float y, float z, float w[3]) {
   const double pb[3] = {(double)x, (double)y, (double)z};
   double a[3], g[3];
-  eigen_q_rot(pc.eq[lid], pb, a);
+  q_rot(pc.eq[lid], pb, a);
   a[0] += pc.et[lid][0]; a[1] += pc.et[lid][1]; a[2] += pc.et[lid][2];
   if (lid != 0) {                                                                               // :142, :157
     double b[3];
-    eigen_q_rot(pc.cq[lid], a, b);
+    q_rot(pc.cq[lid], a, b);
     a[0] = b[0] + pc.ct[lid][0]; a[1] = b[1] + pc.ct[lid][1]; a[2] = b[2] + pc.ct[lid][2];
   }
-  eigen_q_rot(pc.rot, a, g);
+  q_rot(pc.rot, a, g);
   w[0] = (float)(g[0] + pc.pos[0]); w[1] = (float)(g[1] + pc.pos[1]); w[2] = (float)(g[2] + pc.pos[2]);
 }
 
@@ -133,7 +184,7 @@ struct DeviceState {
   double* d_table = nullptr; uint32_t cap_table = 0;
   uint32_t table_off[MALIO_MAX_LIDAR + 1] = {0, 0, 0, 0};
   malio_rigid tcomp[MALIO_MAX_LIDAR];
-  bool scan_ready = false, map_ready = false, pass_done = false, searched_once = false;
+  bool scan_ready = false, map_ready = false, pass_done = false;
   // per point, position space
   uint32_t* d_nn_idx = nullptr; float* d_nn_d2 = nullptr; uint8_t* d_sel = nullptr;
   float4 *d_world = nullptr, *d_plane = nullptr; double *d_ucov = nullptr, *d_tau = nullptr; float* d_normal_y = nullptr;
@@ -142,9 +193,8 @@ struct DeviceState {
   // aux staging (caller order)
   float* d_o_ny = nullptr; uint32_t* d_o_idx = nullptr; float* d_o_d2 = nullptr; uint8_t* d_o_sel = nullptr; float* d_o_world = nullptr;
   // reductions
-  double* d_block_mm = nullptr; uint32_t* d_block_cnt = nullptr; uint32_t cap_blocks = 0;
-  uint32_t* d_counters = nullptr;   // [0] plane, [1] reduce, [2] n_eff local, [3] n_rows
-  unsigned long long* d_mmkey = nullptr;   // 2 parities x 4 keys (+ counts in d_counters[4+parity])
+  uint32_t* d_counters = nullptr;   // [3] rows rows_kernel found (download_rows); [0..2] unused
+  unsigned long long* d_mmkey = nullptr;   // 2 parities x 4 keys
   int parity = 0, last_parity = 0;
   double* d_block_red = nullptr; uint32_t red_grid = 0;
   double* d_res = nullptr;          // MALIO_RED_DOUBLES
@@ -160,7 +210,9 @@ struct DeviceState {
   float4* d_cell_pts = nullptr;
   uint32_t* d_fb_list = nullptr;          // positions the fast path could not settle (-> exact traversal)
   unsigned long long* d_cand = nullptr;   // [0] candidates scanned by the cell-list scans since create (summed only while timing is on)
-  uint32_t* d_gstats = nullptr;           // [0] occupied cells, [1] live points, [2] fb count, [3] fb count of the last search, [4] ring-2 queries
+  // [0] occupied cells, [1] live points, [2] fb count, [3] fb count of the last search, [4] ring-2 queries, [5] ring-2 queries
+  // of the last search, [6] traversal fault bits (FAULT_STACK_OVERFLOW; cleared only by a map upload), [7] tie queries
+  uint32_t* d_gstats = nullptr;
   uint32_t* h_gstats = nullptr;            // pinned mirror (8 words, carved out of h_res)
   // fused pass (single cooperative launch per measurement pass)
   bool fused = true; int pass_max_blocks = 0, pass_max_blocks_generic = 0;
@@ -173,12 +225,30 @@ struct DeviceState {
   bool p2p = false; unsigned char* d_mail = nullptr; unsigned char* mail_peer[MAIL_MAX_WORLD] = {nullptr};
 };
 
+// (re)allocate ptr for count elements; the old contents are not kept
 template <class T>
 int ensure(malio_handle* h, T*& ptr, size_t count) {
   if (ptr) { cudaFree(ptr); ptr = nullptr; }
   CUDA_TRY(cudaMalloc((void**)&ptr, count * sizeof(T)));
   return MALIO_OK;
 }
+
+// ---- host functions one unit calls in another
+// malio_knn.cu.  MODE 0: the scan's points through pc, MODE 1: the stand-alone queries in D->d_queries.
+// keys + counting sort of n queries into D->d_perm; lid_major: LiDAR id as the major key (large scans, see count_kernel)
+template <int MODE>
+int sort_queries(malio_handle* h, DeviceState* D, uint32_t n, const PassConst& pc, int lid_major);
+template <int MODE>
+int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pts_in, const uint32_t* perm,
+            const PassConst& pc, float max_sqdist);
+// d_gstats[2..7] of the last search -> h_gstats[2..7], enqueued on st
+int fetch_knn_stats(malio_handle* h, DeviceState* D, cudaStream_t st);
+// MALIO_ERR_TREE_TOO_DEEP if a traversal of this handle overflowed its stack since the last map upload (h_gstats[6])
+int knn_fault(malio_handle* h, const DeviceState* D);
+// malio_pass.cu
+PassConst make_pass_const(const malio_handle* h, const DeviceState* D, const malio_pass_state* s);
+int pass_init(malio_handle* h, DeviceState* D);   // part of create(): per-block result slots, pass_kernel launch limits
+void comm_destroy(DeviceState* D);
 
 }  // namespace malio_devstate
 

@@ -1,6 +1,6 @@
 // malio_host.cpp — host C++ side of libmalio_b200.so: the C-ABI wrappers, the iterated error-state Kalman
 // update on the state manifold, and the static snapshot builder.  No CUDA here; the device work is behind
-// malio_dev:: (malio_b200.cu).  There is NO CPU fallback for the measurement: without a usable GPU
+// malio_dev:: (malio_knn.cu, malio_pass.cu, malio_b200.cu).  There is NO CPU fallback for the measurement: without a usable GPU
 // malio_create fails with MALIO_ERR_CUDA.
 //
 // Reference interface mirrored (paths relative to /root/reference/MA_LIO):

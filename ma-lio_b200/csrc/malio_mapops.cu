@@ -10,7 +10,7 @@
 // Storage: slots in DeviceState::d_mpts (x, y, z, link word = MALIO_LINK_POINT_DELETED or 0), d_cov (normal_y), d_ids.
 // Deltas append slots and set deleted bits; nothing moves until a commit finds more than half of the slots dead, then a
 // stable compaction packs the live ones.  commit() = bounding box of the live points (one reduction, 24 B back to the host
-// for the grid geometry) + the same five-kernel cell-list build a snapshot upload runs (malio_b200.cu: grid_build).
+// for the grid geometry) + the same five-kernel cell-list build a snapshot upload runs (malio_knn.cu: grid_build).
 // Killing the content of a voxel box uses the CURRENT index (cells overlapping the box, exact half-open test per point),
 // so a sync after uncommitted appends commits first; boxes of one call are distinct voxels and cannot see each other's points.
 #include <cuda_runtime.h>
@@ -53,12 +53,6 @@ int state(malio_handle* h, MapOps*& M) {
   h->mapst = M;
   CUDA_TRY(cudaMalloc((void**)&M->d_small, 8 * sizeof(uint32_t)));
   CUDA_TRY(cudaHostAlloc((void**)&M->h_small, 8 * sizeof(uint32_t), cudaHostAllocDefault));
-  return MALIO_OK;
-}
-template <class T>
-int grow(malio_handle* h, T*& p, size_t count) {
-  if (p) { cudaFree(p); p = nullptr; }
-  CUDA_TRY(cudaMalloc((void**)&p, count * sizeof(T)));
   return MALIO_OK;
 }
 
@@ -256,7 +250,7 @@ __global__ void gather_live_kernel(const float4* __restrict__ mpts, const float*
 // host arrays -> staging buffer on the device: xyz | normal_y | ids
 int stage(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const float* ny, const int32_t* ids, uint32_t n, const float** d_xyz,
           const float** d_ny, const int32_t** d_ids, bool* synced_needed) {
-  if (n > M->cap_stage) { if (int rc = grow(h, M->d_stage, (size_t)(n + n / 4 + 1024) * 5)) return rc; M->cap_stage = n + n / 4 + 1024; }
+  if (n > M->cap_stage) { if (int rc = ensure(h, M->d_stage, (size_t)(n + n / 4 + 1024) * 5)) return rc; M->cap_stage = n + n / 4 + 1024; }
   float* base = M->d_stage;
   *d_xyz = base; *d_ny = base + 3 * (size_t)M->cap_stage;
   *d_ids = ids ? reinterpret_cast<const int32_t*>(base + 4 * (size_t)M->cap_stage) : nullptr;
@@ -355,15 +349,15 @@ int commit(malio_handle* h) {
   if (n > 65536 && M->n_live * 2 < n) {
     const uint32_t nblk = (n + CP_T - 1) / CP_T;
     if (nblk + 1 > M->cap_blk) {
-      if (int rc = grow(h, M->d_blk, nblk + 1024)) return rc;
-      if (int rc = grow(h, M->d_blkoff, nblk + 1025)) return rc;
+      if (int rc = ensure(h, M->d_blk, nblk + 1024)) return rc;
+      if (int rc = ensure(h, M->d_blkoff, nblk + 1025)) return rc;
       M->cap_blk = nblk + 1024;
     }
     const uint32_t cap2 = D->cap_slots;
     if (cap2 > M->cap2) {
-      if (int rc = grow(h, M->d_mpts2, cap2)) return rc;
-      if (int rc = grow(h, M->d_cov2, cap2)) return rc;
-      if (int rc = grow(h, M->d_ids2, cap2)) return rc;
+      if (int rc = ensure(h, M->d_mpts2, cap2)) return rc;
+      if (int rc = ensure(h, M->d_cov2, cap2)) return rc;
+      if (int rc = ensure(h, M->d_ids2, cap2)) return rc;
       M->cap2 = cap2;
     }
     cp_count_kernel<<<nblk, CP_T, 0, st>>>(D->d_mpts, n, M->d_blk);
@@ -444,7 +438,7 @@ int sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* x
   if (M->appended || !D->tree_free) { if (int rc = commit(h)) return rc; }   // the kill below reads the index: it must know every live slot
   uint32_t killed = 0;
   if (nb && D->grid_on) {
-    if (nb > M->cap_boxes) { if (int rc = grow(h, M->d_boxes, (size_t)(nb + nb / 4 + 1024) * 6)) return rc; M->cap_boxes = nb + nb / 4 + 1024; }
+    if (nb > M->cap_boxes) { if (int rc = ensure(h, M->d_boxes, (size_t)(nb + nb / 4 + 1024) * 6)) return rc; M->cap_boxes = nb + nb / 4 + 1024; }
     const bool via_bounce = !n_deleted && nb <= BOUNCE_BOXES;
     if (via_bounce) {
       if (!M->h_bounce_box) {
@@ -499,8 +493,8 @@ int download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_
   if (cap < live) { h->err = "malio_map_download: capacity below the number of live points"; return MALIO_ERR_CAPACITY; }
   const uint32_t nblk = (n + CP_T - 1) / CP_T;
   if (nblk + 1 > M->cap_blk) {
-    if (int rc = grow(h, M->d_blk, nblk + 1024)) return rc;
-    if (int rc = grow(h, M->d_blkoff, nblk + 1025)) return rc;
+    if (int rc = ensure(h, M->d_blk, nblk + 1024)) return rc;
+    if (int rc = ensure(h, M->d_blkoff, nblk + 1025)) return rc;
     M->cap_blk = nblk + 1024;
   }
   float* d_out = nullptr;

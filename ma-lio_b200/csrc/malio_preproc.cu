@@ -69,13 +69,6 @@ struct PreState {
   float4* h_bounce = nullptr;         // pinned, malio_pcd::CHUNK points: malio_world_save_pcd's D2H staging
 };
 
-template <class T>
-int grow(malio_handle* h, T*& p, size_t count) {
-  if (p) { cudaFree(p); p = nullptr; }
-  CUDA_TRY(cudaMalloc((void**)&p, count * sizeof(T)));
-  return MALIO_OK;
-}
-
 int get_state(malio_handle* h, PreState*& S) {
   S = (PreState*)h->pre;
   if (S) return MALIO_OK;
@@ -575,20 +568,6 @@ __global__ void world_kernel(const float* __restrict__ ud, int slot, float tag, 
 
 constexpr uint64_t WORLD_ACC_MIN = 1u << 16;   // first capacity of the accumulated cloud (points); it doubles from there
 
-// the constants body_to_world reads: the updated state and, for LiDARs 1.., the scan's temporal compensation
-PassConst world_const(const malio_pass_state* s, const DeviceState* D) {
-  PassConst pc{};
-  std::memcpy(pc.rot, s->rot, sizeof(pc.rot));
-  std::memcpy(pc.pos, s->pos, sizeof(pc.pos));
-  for (int l = 0; l < MALIO_MAX_LIDAR; ++l) {
-    std::memcpy(pc.eq[l], s->ext[l].q, sizeof(pc.eq[l]));
-    std::memcpy(pc.et[l], s->ext[l].t, sizeof(pc.et[l]));
-    std::memcpy(pc.cq[l], D->tcomp[l].q, sizeof(pc.cq[l]));
-    std::memcpy(pc.ct[l], D->tcomp[l].t, sizeof(pc.ct[l]));
-  }
-  return pc;
-}
-
 // size of the cloud `source` registers, or a state error when it is not on the device
 int world_count(malio_handle* h, PreState* S, DeviceState* D, int source, uint64_t& n) {
   n = 0;
@@ -607,7 +586,7 @@ int world_count(malio_handle* h, PreState* S, DeviceState* D, int source, uint64
 // enqueue the registration of `source` into dst[0 .. n) on the handle's stream
 int world_launch(malio_handle* h, PreState* S, DeviceState* D, const malio_pass_state* s, int source, const float* slot_tag,
                  float4* dst) {
-  const PassConst pc = world_const(s, D);
+  const PassConst pc = make_pass_const(h, D, s);   // body_to_world reads the state and the temporal compensation
   if (source == MALIO_WORLD_DENSE) {
     uint64_t at = 0;
     for (int l = 0; l < h->cfg.params.n_lidar; ++l) {
@@ -714,15 +693,15 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   L.ud_valid = false;
   if (n > L.cap) {
     const uint32_t cap = n + n / 8 + 1024;
-    if (int rc = grow(h, L.d_raw, cap)) return rc;
-    if (int rc = grow(h, L.d_ud, (size_t)cap * 5)) return rc;
-    if (int rc = grow(h, L.d_need, cap)) return rc;
-    if (int rc = grow(h, L.d_idx, cap)) return rc;
-    if (int rc = grow(h, L.d_ok, cap)) return rc;
-    if (int rc = grow(h, L.d_pose, (size_t)cap * 7)) return rc;
+    if (int rc = ensure(h, L.d_raw, cap)) return rc;
+    if (int rc = ensure(h, L.d_ud, (size_t)cap * 5)) return rc;
+    if (int rc = ensure(h, L.d_need, cap)) return rc;
+    if (int rc = ensure(h, L.d_idx, cap)) return rc;
+    if (int rc = ensure(h, L.d_ok, cap)) return rc;
+    if (int rc = ensure(h, L.d_pose, (size_t)cap * 7)) return rc;
     L.cap = cap;
   }
-  if (!L.d_pop) { if (int rc = grow(h, L.d_pop, MALIO_MAX_COV + 1)) return rc; }
+  if (!L.d_pop) { if (int rc = ensure(h, L.d_pop, MALIO_MAX_COV + 1)) return rc; }
   L.n = n;
   L.ds_valid = false;
   L.n_cov = a->n_cov;
@@ -775,7 +754,7 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
   cudaStream_t st = S->stream;
   const float* d_in;
   if (in) {
-    if (n > S->cap_vin) { if (int rc = grow(h, S->d_vin, (size_t)(n + 1024) * 5)) return rc; S->cap_vin = n + 1024; }
+    if (n > S->cap_vin) { if (int rc = ensure(h, S->d_vin, (size_t)(n + 1024) * 5)) return rc; S->cap_vin = n + 1024; }
     if (n) CUDA_TRY(cudaMemcpyAsync(S->d_vin, in, (size_t)n * 5 * sizeof(float), cudaMemcpyHostToDevice, st));
     D->ctr.h2d_bytes += (uint64_t)n * 20;
     d_in = S->d_vin;
@@ -789,9 +768,9 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
   if (n == 0) { L.ds_valid = true; return MALIO_OK; }
   if (n > S->cap_vpts) {
     const uint32_t cap = n + n / 8 + 1024;
-    if (int rc = grow(h, S->d_vidx, cap)) return rc;
-    if (int rc = grow(h, S->d_vtmp, cap)) return rc;
-    if (int rc = grow(h, S->d_vorder, cap)) return rc;
+    if (int rc = ensure(h, S->d_vidx, cap)) return rc;
+    if (int rc = ensure(h, S->d_vtmp, cap)) return rc;
+    if (int rc = ensure(h, S->d_vorder, cap)) return rc;
     S->cap_vpts = cap;
   }
   // ---- bounds (getMinMax3D), then the grid geometry on the host exactly as PCL derives it
@@ -829,10 +808,10 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
   c.dx = dx; c.dxy = dx * dy;
   if ((uint64_t)cells > S->cap_cells) {
     const uint64_t cap = (uint64_t)cells + (uint64_t)cells / 4 + 4096;
-    if (int rc = grow(h, S->d_vcnt, cap)) return rc;
-    if (int rc = grow(h, S->d_voff, cap)) return rc;
-    if (int rc = grow(h, S->d_vocc, cap)) return rc;
-    if (int rc = grow(h, S->d_vcur, cap)) return rc;
+    if (int rc = ensure(h, S->d_vcnt, cap)) return rc;
+    if (int rc = ensure(h, S->d_voff, cap)) return rc;
+    if (int rc = ensure(h, S->d_vocc, cap)) return rc;
+    if (int rc = ensure(h, S->d_vcur, cap)) return rc;
     S->cap_cells = cap;
   }
   const uint32_t nchunk = (uint32_t)((cells + VS_CHUNK - 1) / VS_CHUNK);   // <= 65536
@@ -847,7 +826,7 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
   CUDA_TRY(cudaMemcpyAsync(S->h_small, S->d_bounds + 6, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   const uint32_t m = S->h_small[1];
-  if (m > L.cap_ds) { if (int rc = grow(h, L.d_ds, (size_t)(m + m / 8 + 1024) * 5)) return rc; L.cap_ds = m + m / 8 + 1024; }
+  if (m > L.cap_ds) { if (int rc = ensure(h, L.d_ds, (size_t)(m + m / 8 + 1024) * 5)) return rc; L.cap_ds = m + m / 8 + 1024; }
   vg_centroid_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_in, S->d_vidx, n, S->d_voff, S->d_vcnt, S->d_vocc, S->d_vorder, L.d_ds, m);
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 7;
@@ -906,7 +885,7 @@ int world_register(malio_handle* h, const malio_pass_state* s, int source, const
   if (!out || k == 0) return MALIO_OK;
   if (n > S->cap_wstage) {
     const uint64_t c = n + n / 8 + 1024;
-    if (int rc = grow(h, S->d_wstage, c)) { S->cap_wstage = 0; return rc; }
+    if (int rc = ensure(h, S->d_wstage, c)) { S->cap_wstage = 0; return rc; }
     S->cap_wstage = c;
   }
   if (int rc = world_launch(h, S, D, s, source, slot_tag, S->d_wstage)) return rc;
@@ -1015,8 +994,8 @@ int scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_e
   const size_t tab_bytes = (size_t)n_tab * sizeof(malio_pose_entry);
   const size_t out_bytes = tab_bytes + (size_t)(Ln - 1 + (lidar_unc ? n_unc : 0)) * sizeof(malio_pose);
   if (!S->d_ucov) {   // sized for the largest lists: L x MALIO_MAX_COV pops, L - 1 compensations
-    if (int rc = grow(h, S->d_ucov, (size_t)MALIO_MAX_COV * 36)) return rc;
-    if (int rc = grow(h, S->d_uout, (size_t)MALIO_MAX_LIDAR * MALIO_MAX_COV * (sizeof(malio_pose_entry) + sizeof(malio_pose)) +
+    if (int rc = ensure(h, S->d_ucov, (size_t)MALIO_MAX_COV * 36)) return rc;
+    if (int rc = ensure(h, S->d_uout, (size_t)MALIO_MAX_LIDAR * MALIO_MAX_COV * (sizeof(malio_pose_entry) + sizeof(malio_pose)) +
                                         MALIO_MAX_LIDAR * sizeof(malio_pose)))
       return rc;
   }

@@ -1,4 +1,4 @@
-// TEST INFRASTRUCTURE ONLY — a stand-in for the CUDA translation unit (ma-lio_b200/csrc/malio_b200.cu) so that the
+// TEST INFRASTRUCTURE ONLY — a stand-in for the CUDA translation units (ma-lio_b200/csrc/malio_*.cu) so that the
 // product's HOST code (malio_host.cpp: malio_ieskf_update, the degenerate branch, manifold operators, C-ABI argument
 // checks) can be driven on a machine without a GPU: malio_dev::measure / download_rows call back into the test, which
 // supplies the reduced system (from the oracle).  Linked only into tests/hoststub/libmalio_hoststub.so, never shipped.

@@ -81,7 +81,7 @@ def reduce_ref(h_x, h, R, method: str | None = None):
 
 
 def launch_geometry(n_points: int, sm_count: int, fused: bool = True, blocks_per_sm: int = 4):
-    """The pass launch the host picks (malio_b200.cu measure()): n_tiles tiles of 128
+    """The pass launch the host picks (malio_pass.cu pass_geometry()): n_tiles tiles of 128
     points, one co-resident wave of W = blocks_per_sm * SMs blocks (also the slot count red_grid), per_block tiles per
     block, grid blocks; FAST (rows kept in shared memory) while per_block <= 2.  The unfused kernels always use the
     generic reduction over a wave of red_grid blocks."""

@@ -1,5 +1,5 @@
 """CPU property test of the geometric guarantee the k-NN fast path rests on (DESIGN.md (c), knn_direct_kernel /
-knn_keys_kernel / ring2_query_warp in ma-lio_b200/csrc/malio_b200.cu).
+knn_keys_kernel / ring2_query_warp in ma-lio_b200/csrc/malio_knn.cu).
 
 The device accepts the result of a (2H+1)^3 cell-block scan iff the 5th squared distance (float32, calc_dist's
 expression) is below ((H + fmin - 0.005) * h)^2, claiming that every map point OUTSIDE the block is farther than that.

@@ -104,6 +104,50 @@ def test_deep_snapshot_uses_local_stack_variant():
     m.close()
 
 
+def test_traversal_fault_stays_with_its_handle():
+    """A snapshot deeper than its declared max_depth trips the in-kernel stack guard of the handle that searches it, and
+    only that handle: another handle on the same GPU keeps searching and updating, and a valid re-upload clears it."""
+    # chain snapshot whose every left leaf is closer to the query than the spine points seen so far: the traversal
+    # descends the spine and pushes every leaf, so its stack grows with the real depth (~m), not the declared one
+    m_ = 60
+    pts = []
+    for k in range(m_):
+        pts.append((2.0 * k, 0.0, 0.0))          # leaf k: distance 2m - 2k from the query, decreasing with depth
+        pts.append((2.0 * k + 1, 1000.0, 0.0))   # spine point k: ~1000 away
+    deep = _chain_snapshot(np.array(pts, np.float32))
+    assert deep.max_depth > 40
+    understated = plugin.MapSnapshot(deep.nodes, deep.node_cov, deep.node_ids, 8)   # -> 32-entry shared-memory stack
+    q = np.array([[2.0 * m_, 0.0, 0.0], [2.0 * m_ + 0.5, 0.25, 0.0]], np.float32)
+
+    case = synth.case_C1()
+    snap_b = plugin.build_static_snapshot(case.map_xyz, case.map_normal_y)
+    a = plugin.MeasurementModel(1, knn_cell_size=-1.0)
+    b = plugin.MeasurementModel(case.n_lidar, params=case.params, knn_cell_size=-1.0)
+    b.upload_map(snap_b)
+    b.upload_scan(case.pts, case.table, case.table_off, case.temporal_comp)
+    a.upload_map(understated)
+    with pytest.raises(capi.MalioError) as e:
+        a.Nearest_Search(q)
+    assert e.value.status == capi.ERR_TREE_TOO_DEEP
+
+    x, P = case.x_prop.copy(), case.P_prop.copy()
+    rep = b.update_iterated_dyn_share_modified(x, P, case.max_iter)   # raises on any status but "no effective points"
+    assert rep.passes >= 1 and rep.n_eff_last > 0
+    qb = case.map_xyz[::97] + np.float32(0.05)   # after the update: stand-alone queries take over the scan's buffers
+    idx, d2, _ = b.Nearest_Search(qb)
+    o_idx, o_d2, _, _ = po.knn_snapshot(snap_b.nodes, snap_b.node_cov, qb)
+    assert np.array_equal(idx.astype(np.int64), o_idx.astype(np.int64))
+    assert np.array_equal(d2, o_d2)
+
+    a.upload_map(deep)   # the same tree with its true depth: the fault is gone and the lists are the reference's
+    idx, d2, _ = a.Nearest_Search(q)
+    o_idx, o_d2, _, _ = po.knn_snapshot(deep.nodes, deep.node_cov, q)
+    assert np.array_equal(idx.astype(np.int64), o_idx.astype(np.int64))
+    assert np.array_equal(d2, o_d2)
+    a.close()
+    b.close()
+
+
 def test_degenerate_branches_match_oracle():
     base = synth.make_case("b", 3000, 40000, 3, 3, varied_map_cov=True)
     snap = plugin.build_static_snapshot(base.map_xyz, base.map_normal_y)
