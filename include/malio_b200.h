@@ -483,6 +483,44 @@ int malio_set_timing(malio_handle* h, int enable);
 int malio_knn(malio_handle* h, const float* queries_xyz, uint32_t n_queries,
               uint32_t* nn_idx, float* nn_sqdist, float* ms_device);
 
+/* ---- device-memory entry points: inputs and outputs stay in device memory, the work is ordered on the caller's stream ----------
+ * queries / nn_idx / nn_sqdist / xyz / normal_y / ids are device memory of the handle's device (cudaMalloc, cudaMallocAsync or a
+ * memory pool, e.g. torch's CUDA tensors).  stream is a cudaStream_t of that device (NULL = the legacy default stream).
+ * Results are bit-identical to the host-pointer call on the same inputs: malio_knn_device gives malio_knn's lists (caller order,
+ * ascending by (distance, x), 0xFFFFFFFF / +inf where fewer than 5 were found; slot indices in device-resident map mode), with
+ * and without sort_queries; malio_map_build_device / _add_points_device give malio_map_build / _add_points' slots, ids (ids ==
+ * NULL numbers them as there), commit and compaction.
+ * Stream order, no host wait for the call's own work:
+ *   - on entry the handle's stream waits on an event recorded on `stream`: everything enqueued there before the call is seen;
+ *   - on exit `stream` waits on an event recorded after the last access to the caller's buffers: work enqueued on `stream` after
+ *     the call sees the results, and the caller's input buffers may be reused (or freed) once `stream` has passed the call;
+ *   - malio_knn_device returns after enqueueing (no cudaStreamSynchronize).  malio_map_build_device still waits, as
+ *     malio_map_build does, for the bounding box its commit reads back; malio_map_add_points_device returns after enqueueing.
+ *   - a call that must grow the handle's buffers first waits for the handle's earlier work (not for `stream`'s).
+ * Arguments checked on the host before anything is enqueued: a NULL, misaligned (not 4-byte), host (pageable or pinned),
+ * managed or other-device pointer returns MALIO_ERR_INVALID_ARG.  Managed memory is refused: these calls exist for data already
+ * resident in HBM, and a page migration in the middle of a search would make its cost depend on where the pages happen to be;
+ * prefetch into plain device memory, or use the host-pointer calls.  n == 0: no pointer is read and nothing is enqueued on
+ * `stream` (malio_map_build_device with n == 0 builds an empty map exactly as malio_map_build does).  malio_knn_device before a
+ * map exists returns MALIO_ERR_STATE, malio_map_add_points_device before malio_map_build* too.
+ * Deferred device-side results — the one behaviour that differs from malio_knn: the traversal fault bit (the stack guard of the
+ * exact ikd-Tree-order search, see MALIO_ERR_TREE_TOO_DEEP) and the fallback / ring-2 / tie counters of a malio_knn_device call
+ * are only known once the device has run it.  They are copied behind the search and folded in by the NEXT call on the handle,
+ * whatever its entry point (malio_get_counters included), which first waits for that copy.  A fault is returned by that next
+ * call as MALIO_ERR_TREE_TOO_DEEP instead of running it; the fault stays with its handle as for malio_knn (later searches on the
+ * same map report it again, the next malio_upload_map* clears it) and other handles are not affected.  A CUDA error of the
+ * enqueued work surfaces the same way, as MALIO_ERR_CUDA of the next call.
+ * Shared buffers: like malio_knn, malio_knn_device uses the per-point buffers of the scan path: a malio_measure after it needs a
+ * new malio_upload_scan* (MALIO_ERR_STATE otherwise).
+ * Counters: knn_launches, knn_queries and kernel_launches grow as for malio_knn; knn_ms is not (reading it would need a host
+ * wait) and h2d_bytes / d2h_bytes do not grow. */
+int malio_knn_device(malio_handle* h, const float* d_queries, uint32_t n_queries, uint32_t* d_nn_idx, float* d_nn_sqdist,
+                     void* stream);
+int malio_map_build_device(malio_handle* h, const float* d_xyz, const float* d_normal_y, const int32_t* d_ids, uint32_t n,
+                           void* stream);
+int malio_map_add_points_device(malio_handle* h, const float* d_xyz, const float* d_normal_y, const int32_t* d_ids, uint32_t n,
+                                void* stream);
+
 /* ---- host IESKF -----------------------------------------------------------------------------
  * state_ikfom for L LiDARs (use-ikfom.hpp:14-27): DOF n = 17+6L laid out as
  *   pos 0-2 | rot 3-5 | offset_R_l 6+3l | offset_T_l 6+3L+3l | vel | bg | ba | grav (S2, 2 DOF). */

@@ -1,6 +1,6 @@
 // malio_b200.cu — handle lifecycle and per-scan data movement of libmalio_b200.so, sm_90a: create / destroy, the scan
-// upload and its per-scan reset, the downloads in caller order, stand-alone k-NN queries (the search itself is in
-// malio_knn.cu) and map_incremental's per-point decision.  The measurement pass is in malio_pass.cu.
+// upload and its per-scan reset, the downloads in caller order, stand-alone k-NN queries from host or device memory (the
+// search itself is in malio_knn.cu) and map_incremental's per-point decision.  The measurement pass is in malio_pass.cu.
 // Compiled with -fmad=false like the rest of the library (bit parity with the reference's non-FMA x86-64 build).
 #include <cuda_runtime.h>
 
@@ -99,6 +99,47 @@ __global__ void scatter_aux_kernel(const uint32_t* __restrict__ perm, uint32_t N
 
 }  // namespace
 
+// ------------------------------------------------------------------ device-memory entry points
+namespace malio_devstate {
+int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const char* what) {
+  if (!p) { h->err = std::string(what) + ": NULL"; return MALIO_ERR_INVALID_ARG; }
+  if (reinterpret_cast<uintptr_t>(p) & 3u) { h->err = std::string(what) + ": not 4-byte aligned"; return MALIO_ERR_INVALID_ARG; }
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();   // not sticky: clear it so that it does not surface in a later call
+    h->err = std::string(what) + ": not a CUDA pointer";
+    return MALIO_ERR_INVALID_ARG;
+  }
+  if (a.type == cudaMemoryTypeManaged) { h->err = std::string(what) + ": managed memory is not accepted (use cudaMalloc'ed memory)"; return MALIO_ERR_INVALID_ARG; }
+  if (a.type != cudaMemoryTypeDevice) { h->err = std::string(what) + ": host memory (the *_device calls take device memory)"; return MALIO_ERR_INVALID_ARG; }
+  if (a.device != D->device) { h->err = std::string(what) + ": memory of another device than the handle's"; return MALIO_ERR_INVALID_ARG; }
+  return MALIO_OK;
+}
+
+int caller_enter(malio_handle* h, DeviceState* D, cudaStream_t caller) {
+  CUDA_TRY(cudaEventRecord(D->ev_caller_in, caller));
+  CUDA_TRY(cudaStreamWaitEvent(D->stream, D->ev_caller_in, 0));
+  return MALIO_OK;
+}
+int caller_leave(malio_handle* h, DeviceState* D, cudaStream_t caller) {
+  CUDA_TRY(cudaEventRecord(D->ev_caller_out, D->stream));
+  CUDA_TRY(cudaStreamWaitEvent(caller, D->ev_caller_out, 0));
+  return MALIO_OK;
+}
+}  // namespace malio_devstate
+
+namespace {
+// h->deferred of malio_knn_device: wait for its statistics, fold the fast-path counters in, report a traversal fault
+int settle_knn_device(malio_handle* h) {
+  DeviceState* D = (DeviceState*)h->dev;
+  h->deferred = nullptr;
+  CUDA_TRY(cudaSetDevice(D->device));
+  CUDA_TRY(cudaEventSynchronize(D->ev_deferred));
+  if (D->deferred_grid) { D->ctr.knn_fallback_queries += D->h_gstats[3]; D->ctr.knn_ring2_queries += D->h_gstats[5]; }
+  return knn_fault(h, D);
+}
+}  // namespace
+
 namespace malio_dev {
 
 int create(malio_handle* h) {
@@ -120,6 +161,9 @@ int create(malio_handle* h) {
   CUDA_TRY(cudaEventCreateWithFlags(&D->ev_cov, cudaEventDisableTiming));
   CUDA_TRY(cudaEventCreateWithFlags(&D->ev_sorted, cudaEventDisableTiming));
   CUDA_TRY(cudaEventCreateWithFlags(&D->ev_tau, cudaEventDisableTiming));
+  CUDA_TRY(cudaEventCreateWithFlags(&D->ev_caller_in, cudaEventDisableTiming));
+  CUDA_TRY(cudaEventCreateWithFlags(&D->ev_caller_out, cudaEventDisableTiming));
+  CUDA_TRY(cudaEventCreateWithFlags(&D->ev_deferred, cudaEventDisableTiming));
   for (auto& e : D->ev) CUDA_TRY(cudaEventCreate(&e));
   CUDA_TRY(cudaMalloc((void**)&D->d_counters, 4 * sizeof(uint32_t)));
   CUDA_TRY(cudaMemset(D->d_counters, 0, 4 * sizeof(uint32_t)));
@@ -155,6 +199,9 @@ int create(malio_handle* h) {
 void destroy(malio_handle* h) {
   DeviceState* D = (DeviceState*)h->dev;
   if (!D) return;
+  cudaSetDevice(D->device);
+  if (D->stream) cudaStreamSynchronize(D->stream);   // an enqueued call (malio_knn_device) may still use the buffers below
+  h->deferred = nullptr;
   malio_pre::destroy(h);
   malio_map::destroy(h);
   if (D->d_ids) cudaFree(D->d_ids);
@@ -178,6 +225,7 @@ void destroy(malio_handle* h) {
   if (D->ev_cov) cudaEventDestroy(D->ev_cov);
   if (D->ev_sorted) cudaEventDestroy(D->ev_sorted);
   if (D->ev_tau) cudaEventDestroy(D->ev_tau);
+  for (cudaEvent_t e : {D->ev_caller_in, D->ev_caller_out, D->ev_deferred}) if (e) cudaEventDestroy(e);
   if (D->stream) cudaStreamDestroy(D->stream);
   delete D;
   h->dev = nullptr;
@@ -355,6 +403,51 @@ int knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, 
   return MALIO_OK;
 }
 
+// malio_knn on device memory, ordered on the caller's stream: the same sort, search and caller-order scatter, with the queries
+// read where the caller keeps them and the lists written straight into the caller's arrays.  Returns after enqueueing; the
+// statistics malio_knn waits for are copied behind the search and folded in by the next call on the handle (settle_knn_device).
+int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, cudaStream_t caller) {
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (nq) {
+    if (int rc = check_device_ptr(h, D, q, "malio_knn_device queries")) return rc;
+    if (int rc = check_device_ptr(h, D, idx, "malio_knn_device nn_idx")) return rc;
+    if (int rc = check_device_ptr(h, D, d2, "malio_knn_device nn_sqdist")) return rc;
+  }
+  if (!D->map_ready) { h->err = "knn before upload_map"; return MALIO_ERR_STATE; }
+  if (nq == 0) return MALIO_OK;
+  if (h->mapst) { if (int rc = malio_map::commit(h)) return rc; }
+  if (int rc = knn_fault(h, D)) return rc;   // this map already overflowed a traversal stack: no search on it is trusted
+  if (nq > D->capN) {
+    // ensure() frees the old buffers: an earlier enqueued search of this handle must be done with them first (cudaFree would
+    // wait for the whole device as well; this does not rely on it).  Nothing of this call is enqueued yet.
+    CUDA_TRY(cudaStreamSynchronize(D->stream));
+    if (int rc = ensure_point_buffers(h, D, nq)) return rc;
+  }
+  D->scan_ready = false;   // point buffers are shared with the scan path
+  D->pass_done = false;
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  PassConst pc{};
+  const uint32_t* perm = nullptr;
+  if (h->cfg.sort_queries) {
+    if (int rc = sort_queries<1>(h, D, nq, pc, 0, q)) return rc;
+    perm = D->d_perm;
+  }
+  CUDA_TRY(cudaMemsetAsync(D->d_gstats + 2, 0, 4 * sizeof(uint32_t), D->stream));
+  if (int rc = run_knn<1>(h, D, nq, nullptr, perm, pc, 0.f, q)) return rc;
+  scatter_aux_kernel<<<(nq + 255) / 256, 256, 0, D->stream>>>(perm, nq, nullptr, D->d_nn_idx, D->d_nn_d2, nullptr,
+                                                               nullptr, nullptr, idx, d2, nullptr, nullptr);
+  CUDA_TRY(cudaGetLastError());
+  if (int rc = caller_leave(h, D, caller)) return rc;
+  if (int rc = fetch_knn_stats(h, D, D->stream)) return rc;   // behind the caller's event: the caller does not wait for it
+  CUDA_TRY(cudaEventRecord(D->ev_deferred, D->stream));
+  D->deferred_grid = D->grid_on;
+  h->deferred = settle_knn_device;
+  D->ctr.kernel_launches += 1;   // scatter (the sort and the k-NN count their own)
+  D->ctr.knn_launches += 1; D->ctr.knn_queries += nq;
+  return MALIO_OK;
+}
+
 int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world) {
   DeviceState* D = (DeviceState*)h->dev;
   if (!D->pass_done) { h->err = "map_incremental before measure"; return MALIO_ERR_STATE; }
@@ -377,3 +470,10 @@ int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int e
 }
 
 }  // namespace malio_dev
+
+extern "C" int malio_knn_device(malio_handle* h, const float* d_queries, uint32_t n_queries, uint32_t* d_nn_idx,
+                                float* d_nn_sqdist, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_dev::knn_device(h, d_queries, n_queries, d_nn_idx, d_nn_sqdist, (cudaStream_t)stream);
+}

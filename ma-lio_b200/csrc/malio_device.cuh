@@ -165,6 +165,10 @@ struct DeviceState {
   cudaEvent_t ev_cov = nullptr;
   cudaEvent_t ev_sorted = nullptr, ev_tau = nullptr;   // point-covariance traces run beside the first search of a scan
   cudaEvent_t ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // [5] after sort, [6] after knn kernel
+  // calls on device memory ordered on the caller's stream (malio_knn_device, malio_map_*_device): ev_caller_in is recorded on
+  // the caller's stream and waited for by this handle's, ev_caller_out the other way round; ev_deferred follows the copy of the
+  // search statistics the next entry point folds in (settle_deferred), deferred_grid whether that search ran on the cell list
+  cudaEvent_t ev_caller_in = nullptr, ev_caller_out = nullptr, ev_deferred = nullptr; bool deferred_grid = false;
   malio_counters ctr{};
   bool timing = true;   // per-pass CUDA-event timing (malio_set_timing)
   double host_launch_us = 0, host_wait_us = 0; uint64_t host_passes = 0;   // MALIO_HOST_PROF=1 prints them at destroy
@@ -234,17 +238,25 @@ int ensure(malio_handle* h, T*& ptr, size_t count) {
 }
 
 // ---- host functions one unit calls in another
-// malio_knn.cu.  MODE 0: the scan's points through pc, MODE 1: the stand-alone queries in D->d_queries.
+// malio_knn.cu.  MODE 0: the scan's points through pc, MODE 1: stand-alone world-frame queries, n x 3 floats in `queries`
+// (device memory; NULL = D->d_queries).
 // keys + counting sort of n queries into D->d_perm; lid_major: LiDAR id as the major key (large scans, see count_kernel)
 template <int MODE>
-int sort_queries(malio_handle* h, DeviceState* D, uint32_t n, const PassConst& pc, int lid_major);
+int sort_queries(malio_handle* h, DeviceState* D, uint32_t n, const PassConst& pc, int lid_major, const float* queries = nullptr);
 template <int MODE>
 int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pts_in, const uint32_t* perm,
-            const PassConst& pc, float max_sqdist);
+            const PassConst& pc, float max_sqdist, const float* queries = nullptr);
 // d_gstats[2..7] of the last search -> h_gstats[2..7], enqueued on st
 int fetch_knn_stats(malio_handle* h, DeviceState* D, cudaStream_t st);
 // MALIO_ERR_TREE_TOO_DEEP if a traversal of this handle overflowed its stack since the last map upload (h_gstats[6])
 int knn_fault(malio_handle* h, const DeviceState* D);
+// malio_b200.cu: the device-memory entry points.
+// MALIO_OK when p is 4-byte aligned device memory of D's device (cudaMalloc / a memory pool: what torch allocates); NULL, host,
+// pinned, managed or another device's memory -> MALIO_ERR_INVALID_ARG with h->err naming `what`
+int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const char* what);
+// D->stream waits for everything enqueued on the caller's stream so far / the caller's stream waits for D->stream
+int caller_enter(malio_handle* h, DeviceState* D, cudaStream_t caller);
+int caller_leave(malio_handle* h, DeviceState* D, cudaStream_t caller);
 // malio_pass.cu
 PassConst make_pass_const(const malio_handle* h, const DeviceState* D, const malio_pass_state* s);
 int pass_init(malio_handle* h, DeviceState* D);   // part of create(): per-block result slots, pass_kernel launch limits

@@ -165,68 +165,103 @@ void malio_destroy(malio_handle* h) {
 int malio_get_nccl_unique_id(uint8_t id[MALIO_NCCL_UNIQUE_ID_BYTES]) { return id ? malio_dev::get_unique_id(id) : MALIO_ERR_INVALID_ARG; }
 int malio_comm_init(malio_handle* h, const uint8_t id[MALIO_NCCL_UNIQUE_ID_BYTES], int rank, int world) {
   if (!h || !id || world < 1 || rank < 0 || rank >= world) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::comm_init(h, id, rank, world);
 }
 int malio_upload_map(malio_handle* h, const malio_map_node* nodes, const float* node_cov, uint32_t n_nodes, uint32_t max_depth) {
   if (!h || (n_nodes && (!nodes || !node_cov))) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::upload_map(h, nodes, node_cov, n_nodes, max_depth);
 }
 int malio_upload_map_compact(malio_handle* h, const malio_map_point* pts, const float* node_cov, uint32_t n_nodes, uint32_t max_depth,
                              const float* root_box) {
   if (!h || (n_nodes && (!pts || !node_cov))) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::upload_map_compact(h, pts, node_cov, n_nodes, max_depth, root_box);
 }
 int malio_download_map_nodes(malio_handle* h, malio_map_node* out, uint32_t capacity) {
   if (!h || !out) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::download_map_nodes(h, out, capacity);
 }
 int malio_upload_scan(malio_handle* h, const malio_scan_pt* pts, uint32_t n_pts, const malio_pose_entry* table,
                       const uint32_t* table_off, const malio_rigid* temporal_comp) {
   if (!h || (n_pts && !pts) || !table || !table_off) return MALIO_ERR_INVALID_ARG;
   if (h->cfg.params.n_lidar > 1 && !temporal_comp) { h->err = "temporal_comp required for L > 1"; return MALIO_ERR_INVALID_ARG; }
+  MALIO_SETTLE(h);
   return malio_dev::upload_scan(h, pts, n_pts, table, table_off, temporal_comp);
 }
-int malio_rearm_scan(malio_handle* h) { return h ? malio_dev::rearm_scan(h) : MALIO_ERR_INVALID_ARG; }
-int malio_set_timing(malio_handle* h, int enable) { return h ? malio_dev::set_timing(h, enable) : MALIO_ERR_INVALID_ARG; }
-int malio_get_counters(malio_handle* h, malio_counters* out) { return (h && out) ? malio_dev::get_counters(h, out) : MALIO_ERR_INVALID_ARG; }
+int malio_rearm_scan(malio_handle* h) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_dev::rearm_scan(h);
+}
+int malio_set_timing(malio_handle* h, int enable) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_dev::set_timing(h, enable);
+}
+int malio_get_counters(malio_handle* h, malio_counters* out) {
+  if (!h || !out) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_dev::get_counters(h, out);
+}
 int malio_measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* HtRinvH, double* HtRinvh, malio_pass_stats* stats) {
   if (!h || !s || !HtRinvH || !HtRinvh) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::measure(h, s, redo_knn, HtRinvH, HtRinvh, stats);
 }
 int malio_download_rows(malio_handle* h, double* h_x, double* hvec, uint32_t cap, uint32_t* n_rows) {
   if (!h || !h_x || !hvec || !n_rows) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::download_rows(h, h_x, hvec, cap, n_rows);
 }
 int malio_download_aux(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_sqdist, uint8_t* selected, float* world) {
   if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::download_aux(h, normal_y, nn_idx, nn_sqdist, selected, world);
 }
 int malio_map_incremental(malio_handle* h, const malio_pass_state* s, double filter_size_map, int ekf_inited, uint8_t* cls, float* world) {
   if (!h || !s || !cls || !(filter_size_map > 0.0)) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::map_incremental(h, s, filter_size_map, ekf_inited, cls, world);
 }
 // ---------------------------------------------------------------- N1 wrappers (malio_mapops.cu)
 int malio_map_build(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n) {
   if (!h || (n && (!xyz || !normal_y))) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_map::build(h, xyz, normal_y, ids, n);
 }
 int malio_map_add_points(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n) {
   if (!h || (n && (!xyz || !normal_y))) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_map::add_points(h, xyz, normal_y, ids, n);
 }
 int malio_map_delete_boxes(malio_handle* h, const float* boxes, uint32_t nb, uint32_t* n_deleted) {
   if (!h || (nb && !boxes)) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_map::delete_boxes(h, boxes, nb, n_deleted);
 }
 int malio_map_sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* xyz, const float* normal_y, const int32_t* ids,
                           uint32_t n_points, uint32_t* n_deleted) {
   if (!h || (nb && !boxes) || (n_points && (!xyz || !normal_y))) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_map::sync_voxels(h, boxes, nb, xyz, normal_y, ids, n_points, n_deleted);
 }
-int malio_map_commit(malio_handle* h) { return h ? malio_map::commit(h) : MALIO_ERR_INVALID_ARG; }
-int malio_map_info(malio_handle* h, uint32_t* n_live, uint32_t* n_slots) { return h ? malio_map::info(h, n_live, n_slots) : MALIO_ERR_INVALID_ARG; }
+int malio_map_commit(malio_handle* h) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_map::commit(h);
+}
+int malio_map_info(malio_handle* h, uint32_t* n_live, uint32_t* n_slots) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_map::info(h, n_live, n_slots);
+}
 int malio_map_download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_t* slots, uint32_t cap, uint32_t* n) {
-  return h ? malio_map::download(h, xyz, normal_y, ids, slots, cap, n) : MALIO_ERR_INVALID_ARG;
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_map::download(h, xyz, normal_y, ids, slots, cap, n);
 }
 
 // ---------------------------------------------------------------- N2 / N3 wrappers (malio_preproc.cu)
@@ -236,16 +271,19 @@ int malio_undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_
   // the walk of IMU_Processing.hpp:476-486 assumes the cloud sorted by time (sort at :232): checked, not assumed
   for (uint32_t i = 1; i < n; ++i)
     if (pts[i].curvature < pts[i - 1].curvature) { h->err = "malio_undistort: points must be sorted by curvature (IMU_Processing.hpp:232)"; return MALIO_ERR_INVALID_ARG; }
+  MALIO_SETTLE(h);
   return malio_pre::undistort(h, lidar, pts, n, a, xyz, idx, ok, pop_point, n_pops, pose);
 }
 int malio_voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap, uint32_t* n_out) {
   if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_pre::voxel_grid(h, lidar, in, n, leaf, out, out_cap, n_out);
 }
 int malio_upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uint32_t* table_off, const malio_rigid* temporal_comp,
                              uint32_t* n_total) {
   if (!h || !table || !table_off) return MALIO_ERR_INVALID_ARG;
   if (h->cfg.params.n_lidar > 1 && !temporal_comp) { h->err = "temporal_comp required for L > 1"; return MALIO_ERR_INVALID_ARG; }
+  MALIO_SETTLE(h);
   return malio_pre::upload_scan_device(h, table, table_off, temporal_comp, n_total);
 }
 
@@ -283,12 +321,14 @@ int malio_build_pose_unc(int n_lidar, const malio_pose* extrinsic, const malio_p
 
 int malio_knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* nn_idx, float* nn_sqdist, float* ms_device) {
   if (!h || (nq && !q)) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_dev::knn(h, q, nq, nn_idx, nn_sqdist, ms_device);
 }
 
 // ---------------------------------------------------------------- IESKF (esekfom.hpp:495-721)
 int malio_ieskf_update(malio_handle* h, malio_state* x, double* Pio, int max_iter, double R, malio_update_report* rep) {
   if (!h || !x || !Pio || max_iter < 0) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   const StateLayout ly(h->cfg.params.n_lidar);
   const int n = ly.n, c = ly.c;
   malio_update_report rp{};

@@ -25,7 +25,19 @@ struct malio_handle {
   void* dev = nullptr;   // DeviceState*, owned by the CUDA TU
   void* pre = nullptr;   // PreState*, owned by malio_preproc.cu (undistortion / voxel grid buffers)
   void* mapst = nullptr; // MapOpsState*, owned by malio_mapops.cu (device-resident map replay)
+  // set while a call that returned after enqueueing (malio_knn_device) still has device-side results to hand over: its
+  // traversal fault bit and search statistics.  The next entry point on the handle runs it first (MALIO_SETTLE).
+  int (*deferred)(malio_handle* h) = nullptr;
 };
+
+// first thing every C-ABI entry point that takes a handle does: wait for and fold in what an earlier enqueued call left on
+// the device; a fault found there is that call's status, returned instead of running this one
+#define MALIO_SETTLE(h)                                              \
+  do {                                                               \
+    if ((h)->deferred) {                                             \
+      if (int settle_rc_ = (h)->deferred(h)) return settle_rc_;      \
+    }                                                                \
+  } while (0)
 
 // CUDA TU entry points used by the C-ABI wrappers
 namespace malio_dev {
@@ -42,6 +54,8 @@ int measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* Ht
 int download_rows(malio_handle* h, double* h_x, double* hvec, uint32_t cap, uint32_t* n_rows);
 int download_aux(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world);
 int knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, float* ms);
+// device-memory queries and lists, ordered on the caller's stream (a cudaStream_t); malio_b200.cu
+int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, struct CUstream_st* caller);
 int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world);
 int rearm_scan(malio_handle* h);
 int reserve_scan(malio_handle* h, uint32_t n);
@@ -60,6 +74,9 @@ int commit(malio_handle* h);   // pending deltas -> compaction (when worth it) +
 void leave(malio_handle* h);   // a snapshot upload took the handle: back to snapshot mode, the map_* calls refuse until the next build
 int build(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n);
 int add_points(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n);
+// the same with device arrays read in place, ordered on the caller's stream; pointers checked first (MALIO_ERR_INVALID_ARG)
+int build_device(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, struct CUstream_st* caller);
+int add_points_device(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, struct CUstream_st* caller);
 int delete_boxes(malio_handle* h, const float* boxes, uint32_t nb, uint32_t* n_deleted);
 int sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t m,
                 uint32_t* n_deleted);

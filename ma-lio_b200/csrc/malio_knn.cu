@@ -1263,10 +1263,10 @@ static int pick_group(uint32_t n, int sm_count) {
 namespace malio_devstate {
 
 template <int MODE>
-int sort_queries(malio_handle* h, DeviceState* D, uint32_t n, const PassConst& pc, int lid_major) {
+int sort_queries(malio_handle* h, DeviceState* D, uint32_t n, const PassConst& pc, int lid_major, const float* queries) {
   cudaStream_t st = D->stream;
   CUDA_TRY(cudaMemsetAsync(D->d_hist, 0, SORT_BINS * sizeof(uint32_t), st));
-  count_kernel<MODE><<<(n + 255) / 256, 256, 0, st>>>(D->d_pts, D->d_queries, n, pc, lid_major, D->d_keys16, D->d_hist);
+  count_kernel<MODE><<<(n + 255) / 256, 256, 0, st>>>(D->d_pts, queries ? queries : D->d_queries, n, pc, lid_major, D->d_keys16, D->d_hist);
   scan_kernel<<<SCAN_BLOCKS, SCAN_THREADS, 0, st>>>(D->d_hist, D->d_offs, D->d_cursor, D->d_btot);
   // d_fb_list (the k-NN hand-over list, filled only later in the pass) doubles as the arrival-slot array of the sort
   scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(D->d_keys16, n, D->d_offs, D->d_btot, D->d_cursor, D->d_tmp_ids, D->d_fb_list);
@@ -1281,11 +1281,11 @@ int sort_queries(malio_handle* h, DeviceState* D, uint32_t n, const PassConst& p
 // traversal alone when the index is off
 template <int MODE>
 int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pts_in, const uint32_t* perm,
-            const PassConst& pc, float max_sqdist) {
+            const PassConst& pc, float max_sqdist, const float* queries) {
   cudaStream_t st = D->stream;
   const bool smem_stack = D->depth + KNN_POP_WIDTH <= (uint32_t)KNN_SMEM_DEPTH;
   const malio_scan_pt* pts = MODE == 0 ? pts_in : nullptr;
-  const float* qs = MODE == 0 ? nullptr : D->d_queries;
+  const float* qs = MODE == 0 ? nullptr : (queries ? queries : D->d_queries);
   float4* world = MODE == 0 ? D->d_world : nullptr;
   uint8_t* sel = MODE == 0 ? D->d_sel : nullptr;
   auto need_boxes = [&]() -> int {   // the exact traversal reads the 64-byte records: wait for a rebuild still in flight
@@ -1351,10 +1351,10 @@ int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pt
   CUDA_TRY(cudaGetLastError());
   return MALIO_OK;
 }
-template int sort_queries<0>(malio_handle*, DeviceState*, uint32_t, const PassConst&, int);
-template int sort_queries<1>(malio_handle*, DeviceState*, uint32_t, const PassConst&, int);
-template int run_knn<0>(malio_handle*, DeviceState*, uint32_t, const malio_scan_pt*, const uint32_t*, const PassConst&, float);
-template int run_knn<1>(malio_handle*, DeviceState*, uint32_t, const malio_scan_pt*, const uint32_t*, const PassConst&, float);
+template int sort_queries<0>(malio_handle*, DeviceState*, uint32_t, const PassConst&, int, const float*);
+template int sort_queries<1>(malio_handle*, DeviceState*, uint32_t, const PassConst&, int, const float*);
+template int run_knn<0>(malio_handle*, DeviceState*, uint32_t, const malio_scan_pt*, const uint32_t*, const PassConst&, float, const float*);
+template int run_knn<1>(malio_handle*, DeviceState*, uint32_t, const malio_scan_pt*, const uint32_t*, const PassConst&, float, const float*);
 
 int fetch_knn_stats(malio_handle* h, DeviceState* D, cudaStream_t st) {
   CUDA_TRY(cudaMemcpyAsync(D->h_gstats + 2, D->d_gstats + 2, 6 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));

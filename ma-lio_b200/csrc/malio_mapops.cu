@@ -283,17 +283,25 @@ int stage(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const fl
   if (ids) CUDA_TRY(cudaMemcpyAsync(base + 4 * (size_t)M->cap_stage, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, D->stream));
   return MALIO_OK;
 }
-int append(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const float* ny, const int32_t* ids, uint32_t n) {
+// on_device: xyz / ny / ids are device memory the append kernel reads in place, ordered on the caller's stream `caller`
+// (no staging, no host wait); otherwise host arrays, staged as above
+int append(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const float* ny, const int32_t* ids, uint32_t n,
+           bool on_device = false, cudaStream_t caller = nullptr) {
   if (n == 0) return MALIO_OK;
   if ((uint64_t)M->n_slots + n > MALIO_LINK_INDEX_MASK) { h->err = "device-resident map: too many slots"; return MALIO_ERR_CAPACITY; }
-  if (int rc = malio_dev::grow_slots(h, M->n_slots + n, M->n_slots)) return rc;
+  if (int rc = malio_dev::grow_slots(h, M->n_slots + n, M->n_slots)) return rc;   // (drains D->stream before it frees anything)
   if (M->n_slots + n > D->cap_slots) { h->err = "device-resident map: slot storage smaller than its recorded use"; return MALIO_ERR_CAPACITY; }
-  const float *d_xyz, *d_ny;
-  const int32_t* d_ids;
-  bool need_sync = true;
-  if (int rc = stage(h, D, M, xyz, ny, ids, n, &d_xyz, &d_ny, &d_ids, &need_sync)) return rc;
+  const float *d_xyz = xyz, *d_ny = ny;
+  const int32_t* d_ids = ids;
+  bool need_sync = false;
+  if (on_device) {
+    if (int rc = caller_enter(h, D, caller)) return rc;
+  } else {
+    if (int rc = stage(h, D, M, xyz, ny, ids, n, &d_xyz, &d_ny, &d_ids, &need_sync)) return rc;
+  }
   append_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(d_xyz, d_ny, d_ids, n, M->n_slots, (int32_t)M->n_slots, D->d_mpts, D->d_cov, D->d_ids);
   CUDA_TRY(cudaGetLastError());
+  if (on_device) { if (int rc = caller_leave(h, D, caller)) return rc; }   // the kernel is the last reader of the caller's arrays
   // large batches are copied straight from the caller's arrays: wait until they are consumed.  (The device staging buffer itself is
   // reused in stream order.)
   if (need_sync) CUDA_TRY(cudaStreamSynchronize(D->stream));
@@ -384,7 +392,9 @@ int commit(malio_handle* h) {
   return MALIO_OK;
 }
 
-int build(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n) {
+// build / add_points from host arrays (on_device false) or from device arrays ordered on `caller`
+static int build_from(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, bool on_device,
+                      cudaStream_t caller) {
   MapOps* M;
   if (int rc = state(h, M)) return rc;
   DeviceState* D = (DeviceState*)h->dev;
@@ -395,16 +405,42 @@ int build(malio_handle* h, const float* xyz, const float* normal_y, const int32_
   D->tree_free = true;      // grow_slots copies existing slots only in this mode; none are kept here
   if (int rc = malio_dev::grow_slots(h, n > 0 ? n : 1, 0)) return rc;
   M->dirty = true;
-  if (int rc = append(h, D, M, xyz, normal_y, ids, n)) return rc;
+  if (int rc = append(h, D, M, xyz, normal_y, ids, n, on_device, caller)) return rc;
   return commit(h);
 }
 
-int add_points(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n) {
+static int add_points_from(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, bool on_device,
+                           cudaStream_t caller) {
   MapOps* M = (MapOps*)h->mapst;
   if (!M || !M->active) { h->err = "malio_map_add_points before malio_map_build"; return MALIO_ERR_STATE; }
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
-  return append(h, D, M, xyz, normal_y, ids, n);
+  return append(h, D, M, xyz, normal_y, ids, n, on_device, caller);
+}
+int build(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n) {
+  return build_from(h, xyz, normal_y, ids, n, false, nullptr);
+}
+int add_points(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n) {
+  return add_points_from(h, xyz, normal_y, ids, n, false, nullptr);
+}
+
+// the device-memory variants: every argument the host can check is checked before anything is launched
+static int check_device_points(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n) {
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (n == 0) return MALIO_OK;
+  if (int rc = check_device_ptr(h, D, xyz, "xyz")) return rc;
+  if (int rc = check_device_ptr(h, D, normal_y, "normal_y")) return rc;
+  if (ids) { if (int rc = check_device_ptr(h, D, ids, "ids")) return rc; }
+  return MALIO_OK;
+}
+int build_device(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, cudaStream_t caller) {
+  if (int rc = check_device_points(h, xyz, normal_y, ids, n)) return rc;
+  return build_from(h, xyz, normal_y, ids, n, true, caller);
+}
+int add_points_device(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, cudaStream_t caller) {
+  if (int rc = check_device_points(h, xyz, normal_y, ids, n)) return rc;
+  return add_points_from(h, xyz, normal_y, ids, n, true, caller);
 }
 
 int delete_boxes(malio_handle* h, const float* boxes, uint32_t nb, uint32_t* n_deleted) {
@@ -516,3 +552,16 @@ int download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_
 }
 
 }  // namespace malio_map
+
+extern "C" int malio_map_build_device(malio_handle* h, const float* d_xyz, const float* d_normal_y, const int32_t* d_ids, uint32_t n,
+                                      void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_map::build_device(h, d_xyz, d_normal_y, d_ids, n, (cudaStream_t)stream);
+}
+extern "C" int malio_map_add_points_device(malio_handle* h, const float* d_xyz, const float* d_normal_y, const int32_t* d_ids,
+                                           uint32_t n, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_map::add_points_device(h, d_xyz, d_normal_y, d_ids, n, (cudaStream_t)stream);
+}

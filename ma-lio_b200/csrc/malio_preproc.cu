@@ -1040,6 +1040,7 @@ extern "C" int malio_scan_uncertainty(malio_handle* h, const malio_scan_unc_args
                                       uint32_t* table_off, malio_pose* temporal_comp, malio_pose* lidar_unc, uint32_t* lidar_unc_counts) {
   if (!h || !a || !table || !table_off || !a->extrinsic || !a->uncertainty || (a->n_cov && !a->imu_cov)) return MALIO_ERR_INVALID_ARG;
   if (h->cfg.params.n_lidar > 1 && !temporal_comp) { h->err = "scan_uncertainty: temporal_comp required for L > 1"; return MALIO_ERR_INVALID_ARG; }
+  MALIO_SETTLE(h);
   return malio_pre::scan_uncertainty(h, a, table, table_cap, table_off, temporal_comp, lidar_unc, lidar_unc_counts);
 }
 
@@ -1049,14 +1050,17 @@ extern "C" int malio_world_register(malio_handle* h, const malio_pass_state* s, 
   if (!h || !s || !n_out || (cap && !out)) return MALIO_ERR_INVALID_ARG;
   if (source != MALIO_WORLD_DOWNSAMPLED && source != MALIO_WORLD_DENSE) { h->err = "world register: unknown source"; return MALIO_ERR_INVALID_ARG; }
   if (source == MALIO_WORLD_DENSE && !slot_tag) { h->err = "world register: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
+  MALIO_SETTLE(h);
   return malio_pre::world_register(h, s, source, slot_tag, out, cap, n_out);
 }
 extern "C" int malio_world_accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, uint64_t* n_total) {
   if (!h || !s) return MALIO_ERR_INVALID_ARG;
   if (!slot_tag) { h->err = "world accumulate: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
+  MALIO_SETTLE(h);
   return malio_pre::world_accumulate(h, s, slot_tag, n_total);
 }
 extern "C" int malio_world_save_pcd(malio_handle* h, const char* path, int clear) {
   if (!h || !path) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
   return malio_pre::world_save_pcd(h, path, clear);
 }

@@ -127,6 +127,7 @@ EXPORTS = [
     "malio_undistort", "malio_bspline_get_pose", "malio_voxel_grid", "malio_upload_scan_device", "malio_scan_uncertainty",
     "malio_pose_initial", "malio_compound_pose_with_cov", "malio_compound_inv_pose_with_cov", "malio_build_pose_unc",
     "malio_world_register", "malio_world_accumulate", "malio_world_save_pcd", "malio_write_pcd_binary",
+    "malio_knn_device", "malio_map_build_device", "malio_map_add_points_device",
 ]
 
 
@@ -192,6 +193,10 @@ def load() -> C.CDLL:
     lib.malio_download_rows.argtypes = [vp, vp, vp, u32, C.POINTER(u32)]
     lib.malio_download_aux.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.malio_knn.argtypes = [vp, vp, u32, vp, vp, C.POINTER(C.c_float)]
+    # device pointers and a cudaStream_t (torch: tensor.data_ptr(), torch.cuda.Stream.cuda_stream)
+    lib.malio_knn_device.argtypes = [vp, vp, u32, vp, vp, vp]
+    lib.malio_map_build_device.argtypes = [vp, vp, vp, vp, u32, vp]
+    lib.malio_map_add_points_device.argtypes = [vp, vp, vp, vp, u32, vp]
     lib.malio_ieskf_update.argtypes = [vp, C.POINTER(State), vp, i32, C.c_double, C.POINTER(UpdateReport)]
     lib.malio_build_static_snapshot.argtypes = [vp, u32, vp, vp, C.POINTER(u32)]
     lib.malio_rearm_scan.argtypes = [vp]

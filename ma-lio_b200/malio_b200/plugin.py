@@ -138,6 +138,7 @@ class MeasurementModel:
         cfg.params = params if params is not None else capi.default_params(n_lidar)
         cfg.params.n_lidar = n_lidar
         cfg.device = device
+        self.device = device
         cfg.sort_queries = 1 if sort_queries else 0
         cfg.knn_cell_size = float(knn_cell_size)
         self.n_lidar = n_lidar
@@ -449,3 +450,59 @@ class MeasurementModel:
         ms = C.c_float(0)
         self._check(self.lib.malio_knn(self._h, capi.ptr(q), n, capi.ptr(idx), capi.ptr(d2), C.byref(ms)))
         return idx, d2, float(ms.value)
+
+    # ---- the same on torch CUDA tensors: no host copy, ordered on torch.cuda.current_stream() (malio_knn_device & co.)
+    def knn_tensor(self, q):
+        """Nearest_Search on a contiguous float32 CUDA tensor (n, 3) on the handle's device.  Returns (idx int32 (n, 5), sqdist
+        float32 (n, 5)), allocated on and ordered with the current stream; idx holds the bits of the uint32 indices, so a missing
+        neighbour reads -1.  Returns once the search is enqueued; a traversal fault is reported by the next call on the model."""
+        import torch
+        _check_tensor(q, "q", torch.float32, 3, self.device)
+        n = q.shape[0]
+        idx = torch.empty((n, capi.K), dtype=torch.int32, device=q.device)
+        d2 = torch.empty((n, capi.K), dtype=torch.float32, device=q.device)
+        st = torch.cuda.current_stream(q.device)
+        self._check(self.lib.malio_knn_device(self._h, _dptr(q), n, _dptr(idx), _dptr(d2), st.cuda_stream))
+        return idx, d2
+
+    def map_build_tensor(self, xyz, normal_y, ids=None):
+        """map_build from CUDA tensors: xyz float32 (n, 3), normal_y float32 (n,), ids int32 (n,) or None, contiguous, on the
+        handle's device; read in place, ordered on torch.cuda.current_stream()."""
+        self._map_tensor("malio_map_build_device", xyz, normal_y, ids)
+
+    def map_add_points_tensor(self, xyz, normal_y, ids=None):
+        """map_add_points from CUDA tensors (as map_build_tensor); returns once the append is enqueued."""
+        self._map_tensor("malio_map_add_points_device", xyz, normal_y, ids)
+
+    def _map_tensor(self, name, xyz, normal_y, ids):
+        import torch
+        _check_tensor(xyz, "xyz", torch.float32, 3, self.device)
+        n = xyz.shape[0]
+        _check_tensor(normal_y, "normal_y", torch.float32, None, self.device, n)
+        if ids is not None:
+            _check_tensor(ids, "ids", torch.int32, None, self.device, n)
+        st = torch.cuda.current_stream(xyz.device)
+        self._check(getattr(self.lib, name)(self._h, _dptr(xyz), _dptr(normal_y), _dptr(ids), n, st.cuda_stream))
+
+
+def _dptr(t):
+    """Device address of a tensor for the C-ABI (None for None or an empty tensor: the calls take NULL with n == 0)."""
+    return None if t is None or t.numel() == 0 else t.data_ptr()
+
+
+def _check_tensor(t, name, dtype, cols, device, rows=None):
+    """Raise ValueError unless t is a contiguous CUDA tensor of dtype on cuda:device with shape (rows, cols) — (rows,) when cols
+    is None; rows None = any."""
+    import torch
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{name}: expected a torch.Tensor, got {type(t).__name__}")
+    if t.dtype != dtype:
+        raise ValueError(f"{name}: dtype {t.dtype}, expected {dtype}")
+    shape_ok = (t.dim() == 1) if cols is None else (t.dim() == 2 and t.shape[1] == cols)
+    if not shape_ok or (rows is not None and t.shape[0] != rows):
+        want = f"({rows if rows is not None else 'n'},)" if cols is None else f"({rows if rows is not None else 'n'}, {cols})"
+        raise ValueError(f"{name}: shape {tuple(t.shape)}, expected {want}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name}: not contiguous")
+    if t.device.type != "cuda" or t.device.index != device:
+        raise ValueError(f"{name}: on {t.device}, expected cuda:{device} (the handle's device)")
