@@ -521,6 +521,48 @@ int malio_map_build_device(malio_handle* h, const float* d_xyz, const float* d_n
 int malio_map_add_points_device(malio_handle* h, const float* d_xyz, const float* d_normal_y, const int32_t* d_ids, uint32_t n,
                                 void* stream);
 
+/* ---- the measurement path on device memory: the scan in, the per-point outputs out, ordered on the caller's stream ----------
+ * The same contract as the block above, for malio_upload_scan, malio_download_aux, malio_map_incremental and
+ * malio_world_register.  d_* pointers are device memory of the handle's device; table, table_off, temporal_comp, s, slot_tag and
+ * n_out stay host memory exactly as in the host calls (the tables are small and built on the host, table_off is read there).
+ * Results are bit-identical to the host call on the same inputs (the same kernels write the caller's arrays instead of the
+ * library's staging buffers), with and without sort_queries, in snapshot and in device-resident map mode.
+ * Stream order as above: the handle's stream waits on an event recorded on `stream` on entry, and `stream` waits on an event
+ * recorded after the last access to the caller's buffers on exit.  A call that must grow the handle's buffers first waits for
+ * the handle's earlier work (not for `stream`'s); so does a later host call that grows them (malio_upload_scan, malio_undistort,
+ * malio_world_register, malio_upload_map*).
+ * Checks, in this order: the wrapper's argument checks of the host call (NULL s / n_out / table / table_off, temporal_comp for
+ * L > 1, filter_size_map <= 0, source, slot_tag) -> MALIO_ERR_INVALID_ARG; the host call's state errors (MALIO_ERR_STATE before a
+ * malio_measure on the current scan, before malio_undistort of every slot for MALIO_WORLD_DENSE); then, when there is a point
+ * to read or write, every d_* pointer given: NULL (where the host call needs it), not 4-byte aligned (d_out: not 16-byte
+ * aligned, world_kernel stores float4), host (pageable or pinned), managed or other-device memory -> MALIO_ERR_INVALID_ARG.
+ * Nothing is enqueued on any error.  n == 0 (no scan point, an empty cloud, cap == 0): no d_* pointer is read and nothing is
+ * enqueued on `stream`.
+ *
+ * malio_upload_scan_from_device: n_pts malio_scan_pt records (16 B: x, y, z, lidar | table_idx << 16) in device memory, 4-byte
+ * aligned.  They are copied device-to-device into the handle (about 1 us per 100k points), since the passes of several
+ * malio_measure calls read them and the caller may reuse its buffer as soon as `stream` has passed the call.  Like
+ * malio_upload_scan it rejects a record with lidar >= n_lidar before it changes anything: a small kernel checks the records
+ * where they are and the call WAITS for its verdict, so it returns only after `stream` has reached it (as
+ * malio_map_build_device waits for its bounding box).  On such a record it returns MALIO_ERR_INVALID_ARG and the previous scan
+ * is still resident and measurable.  Counters: kernel_launches + 1 (the check), h2d_bytes + the table only.
+ * malio_download_aux_device: malio_download_aux's outputs in caller order: d_normal_y N floats, d_nn_idx / d_nn_sqdist N x 5,
+ * d_selected N bytes, d_world N x 3 floats; any of them may be NULL (skipped).  Returns after enqueueing.
+ * malio_map_incremental_device: d_cls N bytes (required), d_world N x 3 floats (may be NULL).  Returns after enqueueing.
+ * malio_world_register_device: malio_world_register's protocol: d_out == NULL with cap == 0 asks for the size, *n_out = the
+ * full count, at most cap points {x, y, z, intensity} are written to d_out.  With cap >= the count the points are registered
+ * straight into d_out, otherwise into the handle's staging buffer followed by a device-to-device copy of the first cap points.
+ * Returns after enqueueing.
+ * The three output calls add their kernel launches to kernel_launches; d2h_bytes does not grow. */
+int malio_upload_scan_from_device(malio_handle* h, const malio_scan_pt* d_pts, uint32_t n_pts, const malio_pose_entry* table,
+                                  const uint32_t* table_off, const malio_rigid* temporal_comp, void* stream);
+int malio_download_aux_device(malio_handle* h, float* d_normal_y, uint32_t* d_nn_idx, float* d_nn_sqdist, uint8_t* d_selected,
+                              float* d_world, void* stream);
+int malio_map_incremental_device(malio_handle* h, const malio_pass_state* s, double filter_size_map, int ekf_inited,
+                                 uint8_t* d_cls, float* d_world, void* stream);
+int malio_world_register_device(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* d_out,
+                                uint32_t cap, uint32_t* n_out, void* stream);
+
 /* ---- host IESKF -----------------------------------------------------------------------------
  * state_ikfom for L LiDARs (use-ikfom.hpp:14-27): DOF n = 17+6L laid out as
  *   pos 0-2 | rot 3-5 | offset_R_l 6+3l | offset_T_l 6+3L+3l | vel | bg | ba | grav (S2, 2 DOF). */

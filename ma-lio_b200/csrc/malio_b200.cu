@@ -1,6 +1,7 @@
 // malio_b200.cu — handle lifecycle and per-scan data movement of libmalio_b200.so, sm_90a: create / destroy, the scan
-// upload and its per-scan reset, the downloads in caller order, stand-alone k-NN queries from host or device memory (the
-// search itself is in malio_knn.cu) and map_incremental's per-point decision.  The measurement pass is in malio_pass.cu.
+// upload (from host or device memory) and its per-scan reset, the downloads in caller order (to host or device memory),
+// stand-alone k-NN queries from host or device memory (the search itself is in malio_knn.cu) and map_incremental's per-point
+// decision.  The measurement pass is in malio_pass.cu.
 // Compiled with -fmad=false like the rest of the library (bit parity with the reference's non-FMA x86-64 build).
 #include <cuda_runtime.h>
 
@@ -95,6 +96,15 @@ __global__ void scatter_aux_kernel(const uint32_t* __restrict__ perm, uint32_t N
 #pragma unroll
     for (int j = 0; j < MALIO_K; ++j) o_d2[(size_t)i * MALIO_K + j] = nn_d2[(size_t)j * N + p];
   }
+}
+
+// malio_upload_scan_from_device's record check, upload_scan's host sweep on device memory: word 3 of a malio_scan_pt is
+// lidar | table_idx << 16, and lidar must be < L.  A warp with a bad record ORs 1 into *bad.  The records are read as words:
+// the caller's buffer need only be 4-byte aligned.
+__global__ void scan_lidar_check_kernel(const uint32_t* __restrict__ words, uint32_t n, uint32_t L, uint32_t* __restrict__ bad) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool b = i < n && (words[4 * (size_t)i + 3] & 0xFFFFu) >= L;
+  if (__any_sync(0xFFFFFFFFu, b) && (threadIdx.x & 31u) == 0) atomicOr(bad, 1u);
 }
 
 }  // namespace
@@ -214,9 +224,11 @@ void destroy(malio_handle* h) {
                   D->d_table, D->d_nn_idx, D->d_nn_d2, D->d_sel, D->d_world, D->d_plane, D->d_ucov, D->d_tau, D->d_tau2, D->d_pd2, D->d_rows12, D->d_lid8,
                   D->d_normal_y, D->d_o_ny, D->d_o_idx, D->d_o_d2, D->d_o_sel, D->d_o_world,
                   D->d_counters, D->d_mmkey, D->d_block_red, D->d_res, D->d_rows, D->d_queries,
-                  D->d_cell_start, D->d_cell_cnt, D->d_cell_of, D->d_ctot, D->d_cbase, D->d_cell_pts, D->d_fb_list, D->d_gstats, D->d_bar, D->d_cand};
+                  D->d_cell_start, D->d_cell_cnt, D->d_cell_of, D->d_ctot, D->d_cbase, D->d_cell_pts, D->d_fb_list, D->d_gstats, D->d_bar, D->d_cand,
+                  D->d_scan_check};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (D->h_res) cudaFreeHost(D->h_res);
+  if (D->h_scan_check) cudaFreeHost(D->h_scan_check);
   for (auto& e : D->ev) if (e) cudaEventDestroy(e);
   if (D->stream2) { cudaStreamSynchronize(D->stream2); cudaStreamDestroy(D->stream2); }
   if (D->stream3) { cudaStreamSynchronize(D->stream3); cudaStreamDestroy(D->stream3); }
@@ -233,6 +245,9 @@ void destroy(malio_handle* h) {
 
 static int ensure_point_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
   if (n <= D->capN) return MALIO_OK;
+  // ensure() frees the old buffers: a call that returned after enqueueing (the *_device outputs, malio_knn_device) may still
+  // read or write them.  Drain this handle's stream first rather than rely on cudaFree waiting for the device.
+  CUDA_TRY(cudaStreamSynchronize(D->stream));
   uint32_t cap = n + n / 8 + 1024;
   if (cap < h->cfg.max_points) cap = h->cfg.max_points;
   int rc = 0;
@@ -290,6 +305,51 @@ int upload_scan(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const mal
   for (int l = 1; l < L; ++l) D->tcomp[l] = tcomp[l - 1];
   D->N = n; D->scan_ready = true; D->perm_valid = false; D->tau_valid = false; D->pass_done = false;
   D->ctr.h2d_bytes += (uint64_t)n * sizeof(malio_scan_pt) + (uint64_t)n_tab * sizeof(malio_pose_entry);
+  return MALIO_OK;
+}
+
+// malio_upload_scan with the records in device memory, ordered on the caller's stream.  The records are checked where they are
+// and the host waits for the verdict, so that a bad scan changes nothing (as upload_scan's host sweep); then they are copied
+// D2D into d_pts, because the passes keep reading d_pts over several malio_measure calls while the caller may reuse its buffer.
+int upload_scan_from_device(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
+                            const uint32_t* table_off, const malio_rigid* tcomp, cudaStream_t caller) {
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  const int L = h->cfg.params.n_lidar;
+  for (int l = 0; l < L; ++l)
+    if (table_off[l + 1] < table_off[l] + 2) { h->err = "pose table of each LiDAR needs >= 2 entries"; return MALIO_ERR_INVALID_ARG; }
+  if (n) { if (int rc = check_device_ptr(h, D, pts, "malio_upload_scan_from_device pts")) return rc; }
+  if (n == 0) return upload_scan(h, nullptr, 0, table, table_off, tcomp);   // no record to read: nothing on `caller`
+  if (!D->d_scan_check) {
+    CUDA_TRY(cudaMalloc((void**)&D->d_scan_check, sizeof(uint32_t)));
+    CUDA_TRY(cudaHostAlloc((void**)&D->h_scan_check, sizeof(uint32_t), cudaHostAllocDefault));
+  }
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  CUDA_TRY(cudaMemsetAsync(D->d_scan_check, 0, sizeof(uint32_t), D->stream));
+  scan_lidar_check_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(reinterpret_cast<const uint32_t*>(pts), n, (uint32_t)L,
+                                                                  D->d_scan_check);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(D->h_scan_check, D->d_scan_check, sizeof(uint32_t), cudaMemcpyDeviceToHost, D->stream));
+  // also drains every earlier enqueued call of this handle, so the buffers below may grow
+  CUDA_TRY(cudaStreamSynchronize(D->stream));
+  D->ctr.kernel_launches += 1;
+  if (*D->h_scan_check) { h->err = "scan point with lidar id >= n_lidar"; return MALIO_ERR_INVALID_ARG; }
+  if (int rc = ensure_point_buffers(h, D, n)) return rc;
+  const uint32_t n_tab = table_off[L];
+  if (n_tab > D->cap_table) {
+    if (int rc = ensure(h, D->d_table, (size_t)(n_tab + 64) * TABLE_DOUBLES)) return rc;
+    D->cap_table = n_tab + 64;
+  }
+  CUDA_TRY(cudaMemcpyAsync(D->d_pts, pts, (size_t)n * sizeof(malio_scan_pt), cudaMemcpyDeviceToDevice, D->stream));
+  if (int rc = caller_leave(h, D, caller)) return rc;   // the copy is the last read of the caller's records
+  CUDA_TRY(cudaMemcpyAsync(D->d_table, table, (size_t)n_tab * sizeof(malio_pose_entry), cudaMemcpyHostToDevice, D->stream));
+  reset_scan_kernel<<<(D->capN + 255) / 256, 256, 0, D->stream>>>(D->capN, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaStreamSynchronize(D->stream));
+  for (int l = 0; l <= MALIO_MAX_LIDAR; ++l) D->table_off[l] = (l <= L) ? table_off[l] : table_off[L];
+  for (int l = 1; l < L; ++l) D->tcomp[l] = tcomp[l - 1];
+  D->N = n; D->scan_ready = true; D->perm_valid = false; D->tau_valid = false; D->pass_done = false;
+  D->ctr.h2d_bytes += (uint64_t)n_tab * sizeof(malio_pose_entry);
   return MALIO_OK;
 }
 
@@ -356,6 +416,31 @@ int download_aux(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d
   D->ctr.d2h_bytes += (uint64_t)N * ((normal_y ? 4 : 0) + (nn_idx ? 20 : 0) + (nn_d2 ? 20 : 0) + (sel ? 1 : 0) + (world ? 12 : 0));
   CUDA_TRY(cudaStreamSynchronize(D->stream));
   CUDA_TRY(cudaGetLastError());
+  return MALIO_OK;
+}
+
+// download_aux into the caller's device arrays: the same scatter, writing them instead of the d_o_* staging buffers, ordered
+// on the caller's stream; returns after enqueueing
+int download_aux_device(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world,
+                        cudaStream_t caller) {
+  DeviceState* D = (DeviceState*)h->dev;
+  if (!D->pass_done) { h->err = "download_aux before measure"; return MALIO_ERR_STATE; }
+  CUDA_TRY(cudaSetDevice(D->device));
+  const uint32_t N = D->N;
+  if (N == 0) return MALIO_OK;
+  const void* out[5] = {normal_y, nn_idx, nn_d2, sel, world};
+  const char* what[5] = {"malio_download_aux_device normal_y", "malio_download_aux_device nn_idx",
+                         "malio_download_aux_device nn_sqdist", "malio_download_aux_device selected",
+                         "malio_download_aux_device world"};
+  for (int k = 0; k < 5; ++k)
+    if (out[k]) { if (int rc = check_device_ptr(h, D, out[k], what[k])) return rc; }
+  const uint32_t* perm = (h->cfg.sort_queries && D->perm_valid) ? D->d_perm : nullptr;
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  scatter_aux_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(perm, N, D->d_normal_y, D->d_nn_idx, D->d_nn_d2, D->d_sel, D->d_world,
+                                                             normal_y, nn_idx, nn_d2, sel, world);
+  CUDA_TRY(cudaGetLastError());
+  if (int rc = caller_leave(h, D, caller)) return rc;
+  D->ctr.kernel_launches += 1;
   return MALIO_OK;
 }
 
@@ -469,6 +554,28 @@ int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int e
   return MALIO_OK;
 }
 
+// map_incremental into the caller's device arrays (world may be NULL), ordered on the caller's stream; returns after enqueueing
+int map_incremental_device(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world,
+                           cudaStream_t caller) {
+  DeviceState* D = (DeviceState*)h->dev;
+  if (!D->pass_done) { h->err = "map_incremental before measure"; return MALIO_ERR_STATE; }
+  CUDA_TRY(cudaSetDevice(D->device));
+  const uint32_t N = D->N;
+  if (N == 0) return MALIO_OK;
+  if (int rc = check_device_ptr(h, D, cls, "malio_map_incremental_device cls")) return rc;
+  if (world) { if (int rc = check_device_ptr(h, D, world, "malio_map_incremental_device world")) return rc; }
+  const bool sorted = h->cfg.sort_queries && D->perm_valid;
+  const PassConst pc = make_pass_const(h, D, s);
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  map_incr_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(sorted ? D->d_pts_sorted : D->d_pts, sorted ? D->d_perm : nullptr, N, pc,
+                                                           D->d_mpts, D->d_nn_idx, D->d_normal_y, h->cfg.params.cov_threshold, fs,
+                                                           ekf_inited, cls, world);
+  CUDA_TRY(cudaGetLastError());
+  if (int rc = caller_leave(h, D, caller)) return rc;
+  D->ctr.kernel_launches += 1;
+  return MALIO_OK;
+}
+
 }  // namespace malio_dev
 
 extern "C" int malio_knn_device(malio_handle* h, const float* d_queries, uint32_t n_queries, uint32_t* d_nn_idx,
@@ -476,4 +583,28 @@ extern "C" int malio_knn_device(malio_handle* h, const float* d_queries, uint32_
   if (!h) return MALIO_ERR_INVALID_ARG;
   MALIO_SETTLE(h);
   return malio_dev::knn_device(h, d_queries, n_queries, d_nn_idx, d_nn_sqdist, (cudaStream_t)stream);
+}
+
+// the wrappers check what malio_upload_scan / _download_aux / _map_incremental check on the host; the device pointers are
+// checked inside, once the point count is known
+extern "C" int malio_upload_scan_from_device(malio_handle* h, const malio_scan_pt* d_pts, uint32_t n_pts, const malio_pose_entry* table,
+                                             const uint32_t* table_off, const malio_rigid* temporal_comp, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  if (!table || !table_off) return MALIO_ERR_INVALID_ARG;
+  if (h->cfg.params.n_lidar > 1 && !temporal_comp) { h->err = "temporal_comp required for L > 1"; return MALIO_ERR_INVALID_ARG; }
+  return malio_dev::upload_scan_from_device(h, d_pts, n_pts, table, table_off, temporal_comp, (cudaStream_t)stream);
+}
+extern "C" int malio_download_aux_device(malio_handle* h, float* d_normal_y, uint32_t* d_nn_idx, float* d_nn_sqdist,
+                                         uint8_t* d_selected, float* d_world, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_dev::download_aux_device(h, d_normal_y, d_nn_idx, d_nn_sqdist, d_selected, d_world, (cudaStream_t)stream);
+}
+extern "C" int malio_map_incremental_device(malio_handle* h, const malio_pass_state* s, double filter_size_map, int ekf_inited,
+                                            uint8_t* d_cls, float* d_world, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  if (!s || !(filter_size_map > 0.0)) return MALIO_ERR_INVALID_ARG;
+  return malio_dev::map_incremental_device(h, s, filter_size_map, ekf_inited, d_cls, d_world, (cudaStream_t)stream);
 }

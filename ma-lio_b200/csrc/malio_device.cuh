@@ -169,6 +169,8 @@ struct DeviceState {
   // the caller's stream and waited for by this handle's, ev_caller_out the other way round; ev_deferred follows the copy of the
   // search statistics the next entry point folds in (settle_deferred), deferred_grid whether that search ran on the cell list
   cudaEvent_t ev_caller_in = nullptr, ev_caller_out = nullptr, ev_deferred = nullptr; bool deferred_grid = false;
+  // malio_upload_scan_from_device: the record check's flag word and its pinned host copy (allocated on first use)
+  uint32_t *d_scan_check = nullptr, *h_scan_check = nullptr;
   malio_counters ctr{};
   bool timing = true;   // per-pass CUDA-event timing (malio_set_timing)
   double host_launch_us = 0, host_wait_us = 0; uint64_t host_passes = 0;   // MALIO_HOST_PROF=1 prints them at destroy

@@ -568,6 +568,17 @@ __global__ void world_kernel(const float* __restrict__ ud, int slot, float tag, 
 
 constexpr uint64_t WORLD_ACC_MIN = 1u << 16;   // first capacity of the accumulated cloud (points); it doubles from there
 
+// d_wstage large enough for n points.  ensure() frees the old buffer, which a malio_world_register_device that returned after
+// enqueueing may still use: the stream is drained first rather than relying on cudaFree waiting for the device.
+int grow_wstage(malio_handle* h, PreState* S, uint64_t n) {
+  if (n <= S->cap_wstage) return MALIO_OK;
+  CUDA_TRY(cudaStreamSynchronize(S->stream));
+  const uint64_t c = n + n / 8 + 1024;
+  if (int rc = ensure(h, S->d_wstage, c)) { S->cap_wstage = 0; return rc; }
+  S->cap_wstage = c;
+  return MALIO_OK;
+}
+
 // size of the cloud `source` registers, or a state error when it is not on the device
 int world_count(malio_handle* h, PreState* S, DeviceState* D, int source, uint64_t& n) {
   n = 0;
@@ -692,6 +703,9 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   cudaStream_t st = S->stream;
   L.ud_valid = false;
   if (n > L.cap) {
+    // ensure() frees the slot's buffers: a malio_world_register_device that returned after enqueueing may still read d_ud.
+    // Drain the stream first rather than rely on cudaFree waiting for the device.
+    CUDA_TRY(cudaStreamSynchronize(st));
     const uint32_t cap = n + n / 8 + 1024;
     if (int rc = ensure(h, L.d_raw, cap)) return rc;
     if (int rc = ensure(h, L.d_ud, (size_t)cap * 5)) return rc;
@@ -883,15 +897,42 @@ int world_register(malio_handle* h, const malio_pass_state* s, int source, const
   *n_out = (uint32_t)n;
   const uint64_t k = n < cap ? n : cap;
   if (!out || k == 0) return MALIO_OK;
-  if (n > S->cap_wstage) {
-    const uint64_t c = n + n / 8 + 1024;
-    if (int rc = ensure(h, S->d_wstage, c)) { S->cap_wstage = 0; return rc; }
-    S->cap_wstage = c;
-  }
+  if (int rc = grow_wstage(h, S, n)) return rc;
   if (int rc = world_launch(h, S, D, s, source, slot_tag, S->d_wstage)) return rc;
   CUDA_TRY(cudaMemcpyAsync(out, S->d_wstage, (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, S->stream));
   CUDA_TRY(cudaStreamSynchronize(S->stream));
   D->ctr.d2h_bytes += k * sizeof(float4);
+  return MALIO_OK;
+}
+
+// world_register into the caller's device array (16-byte aligned: world_kernel stores float4), ordered on the caller's stream;
+// returns after enqueueing.  world_kernel writes the caller's array directly when all n points fit, and d_wstage otherwise,
+// followed by a D2D copy of the first cap points.
+int world_register_device(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out, uint32_t cap,
+                          uint32_t* n_out, cudaStream_t caller) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  uint64_t n = 0;
+  if (int rc = world_count(h, S, D, source, n)) return rc;
+  if (n > 0xFFFFFFFFull) { h->err = "world registration: more than 2^32-1 points"; return MALIO_ERR_CAPACITY; }
+  const uint64_t k = n < cap ? n : cap;
+  if (out && k) {
+    if (int rc = check_device_ptr(h, D, out, "malio_world_register_device out")) return rc;
+    if (reinterpret_cast<uintptr_t>(out) & 15u) {
+      h->err = "malio_world_register_device out: not 16-byte aligned (the points are stored as float4)";
+      return MALIO_ERR_INVALID_ARG;
+    }
+  }
+  *n_out = (uint32_t)n;
+  if (!out || k == 0) return MALIO_OK;
+  const bool whole = k == n;
+  if (!whole) { if (int rc = grow_wstage(h, S, n)) return rc; }
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  if (int rc = world_launch(h, S, D, s, source, slot_tag, whole ? reinterpret_cast<float4*>(out) : S->d_wstage)) return rc;
+  if (!whole) CUDA_TRY(cudaMemcpyAsync(out, S->d_wstage, (size_t)k * sizeof(float4), cudaMemcpyDeviceToDevice, S->stream));
+  if (int rc = caller_leave(h, D, caller)) return rc;   // (S->stream is D->stream)
   return MALIO_OK;
 }
 
@@ -1052,6 +1093,15 @@ extern "C" int malio_world_register(malio_handle* h, const malio_pass_state* s, 
   if (source == MALIO_WORLD_DENSE && !slot_tag) { h->err = "world register: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
   MALIO_SETTLE(h);
   return malio_pre::world_register(h, s, source, slot_tag, out, cap, n_out);
+}
+extern "C" int malio_world_register_device(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* d_out,
+                                           uint32_t cap, uint32_t* n_out, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  if (!s || !n_out || (cap && !d_out)) return MALIO_ERR_INVALID_ARG;
+  if (source != MALIO_WORLD_DOWNSAMPLED && source != MALIO_WORLD_DENSE) { h->err = "world register: unknown source"; return MALIO_ERR_INVALID_ARG; }
+  if (source == MALIO_WORLD_DENSE && !slot_tag) { h->err = "world register: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
+  return malio_pre::world_register_device(h, s, source, slot_tag, d_out, cap, n_out, (cudaStream_t)stream);
 }
 extern "C" int malio_world_accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, uint64_t* n_total) {
   if (!h || !s) return MALIO_ERR_INVALID_ARG;

@@ -128,6 +128,7 @@ EXPORTS = [
     "malio_pose_initial", "malio_compound_pose_with_cov", "malio_compound_inv_pose_with_cov", "malio_build_pose_unc",
     "malio_world_register", "malio_world_accumulate", "malio_world_save_pcd", "malio_write_pcd_binary",
     "malio_knn_device", "malio_map_build_device", "malio_map_add_points_device",
+    "malio_upload_scan_from_device", "malio_download_aux_device", "malio_map_incremental_device", "malio_world_register_device",
 ]
 
 
@@ -197,6 +198,10 @@ def load() -> C.CDLL:
     lib.malio_knn_device.argtypes = [vp, vp, u32, vp, vp, vp]
     lib.malio_map_build_device.argtypes = [vp, vp, vp, vp, u32, vp]
     lib.malio_map_add_points_device.argtypes = [vp, vp, vp, vp, u32, vp]
+    lib.malio_upload_scan_from_device.argtypes = [vp, vp, u32, vp, vp, vp, vp]
+    lib.malio_download_aux_device.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.malio_map_incremental_device.argtypes = [vp, vp, C.c_double, i32, vp, vp, vp]
+    lib.malio_world_register_device.argtypes = [vp, vp, i32, vp, vp, u32, vp, vp]
     lib.malio_ieskf_update.argtypes = [vp, C.POINTER(State), vp, i32, C.c_double, C.POINTER(UpdateReport)]
     lib.malio_build_static_snapshot.argtypes = [vp, u32, vp, vp, C.POINTER(u32)]
     lib.malio_rearm_scan.argtypes = [vp]

@@ -484,6 +484,102 @@ class MeasurementModel:
         st = torch.cuda.current_stream(xyz.device)
         self._check(getattr(self.lib, name)(self._h, _dptr(xyz), _dptr(normal_y), _dptr(ids), n, st.cuda_stream))
 
+    # ---- the measurement path on torch CUDA tensors: the scan in, the per-point outputs out, ordered on
+    # torch.cuda.current_stream() (malio_upload_scan_from_device & co.)
+    def upload_scan_tensor(self, pts, table: np.ndarray, table_off: np.ndarray, temporal_comp: np.ndarray | None):
+        """upload_scan from a contiguous int32 CUDA tensor (n, 4) of malio_scan_pt records (pack_scan_tensor builds them) on the
+        handle's device; table / table_off / temporal_comp are host arrays as for upload_scan.  The records are copied into the
+        handle, so pts may be reused afterwards.  Waits until the current stream has reached the call (a record with
+        lidar >= n_lidar is rejected before the resident scan changes)."""
+        import torch
+        _check_tensor(pts, "pts", torch.int32, 4, self.device)
+        table = np.ascontiguousarray(table)
+        assert table.dtype == capi.POSE_ENTRY
+        table_off = np.ascontiguousarray(table_off, dtype=np.uint32)
+        tc = None if temporal_comp is None else np.ascontiguousarray(temporal_comp)
+        n = pts.shape[0]
+        st = torch.cuda.current_stream(pts.device)
+        self._check(self.lib.malio_upload_scan_from_device(self._h, _dptr(pts), n, capi.ptr(table), capi.ptr(table_off),
+                                                           capi.ptr(tc), st.cuda_stream))
+        self.n_points = int(n)
+
+    def _empty(self, shape, dtype, want=True):
+        import torch
+        return torch.empty(shape, dtype=dtype, device=torch.device("cuda", self.device)) if want else None
+
+    def aux_tensor(self, normal_y=True, nn_idx=True, nn_sqdist=True, selected=True, world=True):
+        """aux() into CUDA tensors allocated on the current stream: normal_y float32 (n,), nn_idx int32 (n, 5) (the bits of the
+        uint32 indices: a missing neighbour reads -1), nn_sqdist float32 (n, 5), selected uint8 (n,), world float32 (n, 3); the
+        ones not asked for are None.  Returns once the scatter is enqueued."""
+        import torch
+        n = self.n_points
+        o = dict(normal_y=self._empty((n,), torch.float32, normal_y), nn_idx=self._empty((n, capi.K), torch.int32, nn_idx),
+                 nn_sqdist=self._empty((n, capi.K), torch.float32, nn_sqdist), selected=self._empty((n,), torch.uint8, selected),
+                 world=self._empty((n, 3), torch.float32, world))
+        st = torch.cuda.current_stream(self.device)
+        self._check(self.lib.malio_download_aux_device(self._h, _dptr(o["normal_y"]), _dptr(o["nn_idx"]), _dptr(o["nn_sqdist"]),
+                                                       _dptr(o["selected"]), _dptr(o["world"]), st.cuda_stream))
+        return o
+
+    def map_incremental_tensor(self, s: capi.PassState | capi.State, filter_size_map: float = 0.5, ekf_inited: bool = True,
+                               world: bool = True):
+        """map_incremental() into CUDA tensors: (cls uint8 (n,) with capi.MAP_* codes, feats_down_world float32 (n, 3) or None).
+        Returns once the kernel is enqueued on the current stream."""
+        import torch
+        ps = s.pass_state() if isinstance(s, capi.State) else s
+        cls = self._empty((self.n_points,), torch.uint8)
+        w = self._empty((self.n_points, 3), torch.float32, world)
+        st = torch.cuda.current_stream(self.device)
+        self._check(self.lib.malio_map_incremental_device(self._h, C.byref(ps), C.c_double(filter_size_map), 1 if ekf_inited else 0,
+                                                          _dptr(cls), _dptr(w), st.cuda_stream))
+        return cls, w
+
+    def publish_frame_world_tensor(self, s: capi.PassState | capi.State, dense: bool, slot_tag=None):
+        """publish_frame_world() into a CUDA tensor float32 (n, 4) {x, y, z, intensity}, allocated on the current stream.  Returns
+        once the registration is enqueued."""
+        import torch
+        ps = s.pass_state() if isinstance(s, capi.State) else s
+        src = capi.WORLD_DENSE if dense else capi.WORLD_DOWNSAMPLED
+        tag = None if slot_tag is None else np.ascontiguousarray(slot_tag, np.float32)
+        n = C.c_uint32(0)
+        st = torch.cuda.current_stream(self.device)
+        self._check(self.lib.malio_world_register_device(self._h, C.byref(ps), src, capi.ptr(tag), None, 0, C.byref(n), st.cuda_stream))
+        out = self._empty((n.value, 4), torch.float32)
+        if n.value:
+            self._check(self.lib.malio_world_register_device(self._h, C.byref(ps), src, capi.ptr(tag), _dptr(out), n.value, C.byref(n),
+                                                             st.cuda_stream))
+        return out
+
+
+def pack_scan_tensor(xyz, lidar, table_idx):
+    """malio_scan_pt records built with torch ops, on the inputs' device: int32 (n, 4), words 0..2 the bits of xyz (float32
+    (n, 3)), word 3 = lidar | table_idx << 16 (integer tensors (n,)).  Raises ValueError for an id outside [0, 65535]; that
+    check reads the ids' range back to the host (one synchronisation)."""
+    import torch
+    if not isinstance(xyz, torch.Tensor) or xyz.dtype != torch.float32 or xyz.dim() != 2 or xyz.shape[1] != 3:
+        raise ValueError(f"xyz: expected a float32 tensor (n, 3), got {getattr(xyz, 'dtype', type(xyz).__name__)} "
+                         f"{tuple(getattr(xyz, 'shape', ()))}")
+    n = xyz.shape[0]
+    ids = []
+    for name, t in (("lidar", lidar), ("table_idx", table_idx)):
+        if not isinstance(t, torch.Tensor) or t.dim() != 1 or t.shape[0] != n:
+            raise ValueError(f"{name}: expected a tensor ({n},)")
+        if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+            raise ValueError(f"{name}: dtype {t.dtype}, expected an integer dtype")
+        if t.device != xyz.device:
+            raise ValueError(f"{name}: on {t.device}, xyz on {xyz.device}")
+        ids.append(t.to(torch.int64))
+    if n:
+        lo_l, hi_l, lo_t, hi_t = torch.stack([ids[0].min(), ids[0].max(), ids[1].min(), ids[1].max()]).tolist()
+        for name, lo, hi in (("lidar", lo_l, hi_l), ("table_idx", lo_t, hi_t)):
+            if lo < 0 or hi > 0xFFFF:
+                raise ValueError(f"{name}: values in [{lo}, {hi}], outside [0, 65535]")
+    out = torch.empty((n, 4), dtype=torch.int32, device=xyz.device)
+    out[:, :3] = xyz.contiguous().view(torch.int32)
+    w = ids[0] | (ids[1] << 16)
+    out[:, 3] = torch.where(w >= 1 << 31, w - (1 << 32), w).to(torch.int32)   # the uint32 word's bits
+    return out
+
 
 def _dptr(t):
     """Device address of a tensor for the C-ABI (None for None or an empty tensor: the calls take NULL with n == 0)."""
