@@ -300,8 +300,9 @@ int malio_bspline_get_pose(const double* ctrl_t, const double* ctrl_T, uint32_t 
  * floor(x / leaf) relative to the cloud's minimum, one output point per occupied voxel in ascending voxel index, every
  * field the centroid of the voxel's points (float sums taken in ascending input index).  What the hot path reads of the
  * result is x, y, z and the averaged `intensity` (the table index, moved to normal_x at :975).
- * in == NULL: take the device-resident output of the last malio_undistort(h, lidar, ...) (x, y, z, intensity = idx,
- * curvature; points the undistortion left untouched keep intensity 0).  in != NULL: n x 5 floats
+ * in == NULL: take the device-resident output of the last malio_undistort*(h, lidar, ...) (x, y, z, intensity = idx,
+ * curvature; points the undistortion left untouched keep intensity 0); MALIO_ERR_STATE when that call did not complete (an
+ * unordered cloud given to malio_undistort_device).  in != NULL: n x 5 floats
  * {x, y, z, intensity, curvature} from the host.  Outputs (may be NULL): out n_out x 5 floats, same layout, at most out_cap
  * of them; *n_out = the full count.  Non-finite points are skipped; a cloud without a finite point gives n_out = 0.
  * MALIO_ERR_CAPACITY (nothing computed) when the grid has more than 2^28 voxels, more than 2^24 voxels along one axis, or
@@ -562,6 +563,55 @@ int malio_map_incremental_device(malio_handle* h, const malio_pass_state* s, dou
                                  uint8_t* d_cls, float* d_world, void* stream);
 int malio_world_register_device(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* d_out,
                                 uint32_t cap, uint32_t* n_out, void* stream);
+
+/* ---- the front half of a scan on device memory: raw clouds in, the pose table kept on the device ------------------------------
+ * The same contract as the two blocks above, for malio_undistort, malio_voxel_grid, malio_scan_uncertainty and
+ * malio_upload_scan_device: with these a scan goes from raw clouds in device memory to the updated state and every per-point
+ * output without a point or a table entry crossing the bus.  d_* pointers are plain device memory of the handle's device
+ * (a NULL where one is required, a misaligned (not 4-byte), host (pageable or pinned), managed or other-device pointer ->
+ * MALIO_ERR_INVALID_ARG before anything is enqueued or the slot is touched); `stream` is the caller's cudaStream_t; the handle's
+ * stream waits on an event recorded on `stream` on entry, `stream` waits on an event recorded after the last access to the
+ * caller's buffers; with no point to read (n == 0, an empty slot) no d_* pointer is read and nothing is enqueued on `stream`;
+ * growing the handle's buffers first waits for the handle's earlier work.  The small host-side inputs (malio_undistort_args with
+ * its control points and IMU times, malio_scan_unc_args, leaf) and the scalar outputs (n_pops, n_out, table_off, temporal_comp,
+ * n_total) are host memory as in the host calls.  Every kernel is the host call's: results are bit-identical to the host calls
+ * on the same inputs.
+ *
+ * malio_undistort_device: malio_undistort of n raw points (16 B: x, y, z, curvature) read where they are; they are not copied
+ * and nothing reads them once `stream` has passed the call.  Outputs (any may be NULL) are device-to-device copies of what the
+ * slot holds: d_cloud n x 5 floats {x, y, z, intensity (= idx as float, 0 where untouched), curvature}, the rows
+ * malio_voxel_grid* takes as input (there is no separate xyz output); d_idx n; d_ok n bytes; d_pop_point n_cov entries (the first
+ * *n_pops are pop points, the rest -1); d_pose n x 7 doubles.  The argument errors are malio_undistort's, in its order, before
+ * anything is enqueued.  The time-order check runs on the device (a point whose time is below its predecessor's; a NaN time is
+ * accepted exactly where malio_undistort accepts it) and its verdict comes back with the pop count in the call's ONE host wait, at
+ * its end, behind the undistortion itself.  So, unlike malio_undistort, which refuses an unordered cloud before it touches the
+ * slot, malio_undistort_device returns MALIO_ERR_INVALID_ARG (malio_undistort's message) with the slot left WITHOUT a valid
+ * result: malio_voxel_grid*(.., NULL input), malio_scan_uncertainty*, the dense world registration and malio_upload_scan_resident
+ * return MALIO_ERR_STATE until the slot is undistorted again, and the outputs given hold unspecified values.  Counters:
+ * kernel_launches + malio_undistort's + 1 (the check), h2d_bytes + the control points and IMU times only, d2h_bytes unchanged.
+ *
+ * malio_voxel_grid_device: malio_voxel_grid with d_in (n x 5 floats; NULL = the slot's undistorted cloud) read where it is and
+ * min(*n_out, out_cap) rows copied device-to-device to d_out (may be NULL).  *n_out is the full count.  The call waits, as
+ * malio_voxel_grid does, for the grid geometry and for the output count (they size allocations) and returns with the last kernel
+ * and the copy enqueued.  The result also stays in the slot for malio_upload_scan_device / _resident.  MALIO_ERR_CAPACITY cases,
+ * non-finite points, a cloud without a finite point, n == 0: as malio_voxel_grid, nothing written.
+ *
+ * malio_scan_uncertainty_resident: malio_scan_uncertainty without the table transfer: the same checks, error codes and kernel,
+ * but only the L - 1 temporal compensations come back (table_off L + 1 and temporal_comp L - 1 may be NULL); the table stays on
+ * the device and the handle remembers its offsets and the compensations.  malio_scan_uncertainty leaves its table resident too.
+ * Counters: h2d_bytes + imu_cov, d2h_bytes + (L - 1) * sizeof(malio_pose).
+ * malio_upload_scan_resident: malio_upload_scan_device with the table (copied device-to-device into the scan's own buffer, so
+ * the next scan's malio_scan_uncertainty* may run while this scan is measured), offsets and compensations of the last
+ * malio_scan_uncertainty*.  MALIO_ERR_STATE when there is none, when a slot was undistorted again since it was built, or when a
+ * slot has no down-sampled cloud; MALIO_ERR_INVALID_ARG when a LiDAR's table has fewer than two entries.  h2d_bytes does not
+ * grow. */
+int malio_undistort_device(malio_handle* h, int lidar, const malio_raw_pt* d_pts, uint32_t n, const malio_undistort_args* a,
+                           float* d_cloud, int32_t* d_idx, uint8_t* d_ok, int32_t* d_pop_point, double* d_pose, uint32_t* n_pops,
+                           void* stream);
+int malio_voxel_grid_device(malio_handle* h, int lidar, const float* d_in, uint32_t n, float leaf, float* d_out, uint32_t out_cap,
+                            uint32_t* n_out, void* stream);
+int malio_scan_uncertainty_resident(malio_handle* h, const malio_scan_unc_args* a, uint32_t* table_off, malio_pose* temporal_comp);
+int malio_upload_scan_resident(malio_handle* h, uint32_t* n_total);
 
 /* ---- host IESKF -----------------------------------------------------------------------------
  * state_ikfom for L LiDARs (use-ikfom.hpp:14-27): DOF n = 17+6L laid out as

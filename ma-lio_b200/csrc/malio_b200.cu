@@ -278,8 +278,9 @@ static int ensure_point_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
   return MALIO_OK;
 }
 
-int upload_scan(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
-                const uint32_t* table_off, const malio_rigid* tcomp) {
+// table_kind: where `table` lives: host memory (malio_upload_scan*) or this device's (upload_scan_table_on_device)
+static int upload_scan_from(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
+                            cudaMemcpyKind table_kind, const uint32_t* table_off, const malio_rigid* tcomp) {
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
   const int L = h->cfg.params.n_lidar;
@@ -297,15 +298,27 @@ int upload_scan(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const mal
     D->cap_table = n_tab + 64;
   }
   if (n) CUDA_TRY(cudaMemcpyAsync(D->d_pts, pts, (size_t)n * sizeof(malio_scan_pt), cudaMemcpyHostToDevice, D->stream));
-  CUDA_TRY(cudaMemcpyAsync(D->d_table, table, (size_t)n_tab * sizeof(malio_pose_entry), cudaMemcpyHostToDevice, D->stream));
+  CUDA_TRY(cudaMemcpyAsync(D->d_table, table, (size_t)n_tab * sizeof(malio_pose_entry), table_kind, D->stream));
   reset_scan_kernel<<<(D->capN + 255) / 256, 256, 0, D->stream>>>(D->capN, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaStreamSynchronize(D->stream));
   for (int l = 0; l <= MALIO_MAX_LIDAR; ++l) D->table_off[l] = (l <= L) ? table_off[l] : table_off[L];
   for (int l = 1; l < L; ++l) D->tcomp[l] = tcomp[l - 1];
   D->N = n; D->scan_ready = true; D->perm_valid = false; D->tau_valid = false; D->pass_done = false;
-  D->ctr.h2d_bytes += (uint64_t)n * sizeof(malio_scan_pt) + (uint64_t)n_tab * sizeof(malio_pose_entry);
+  D->ctr.h2d_bytes += (uint64_t)n * sizeof(malio_scan_pt);
+  if (table_kind == cudaMemcpyHostToDevice) D->ctr.h2d_bytes += (uint64_t)n_tab * sizeof(malio_pose_entry);
   return MALIO_OK;
+}
+
+int upload_scan(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
+                const uint32_t* table_off, const malio_rigid* tcomp) {
+  return upload_scan_from(h, pts, n, table, cudaMemcpyHostToDevice, table_off, tcomp);
+}
+
+// an empty scan whose table is already in this device's memory (malio_upload_scan_resident: the table malio_scan_uncertainty*
+// built), copied device-to-device; the caller fills the points in afterwards as malio_upload_scan_device does
+int upload_scan_table_on_device(malio_handle* h, const malio_pose_entry* d_table, const uint32_t* table_off, const malio_rigid* tcomp) {
+  return upload_scan_from(h, nullptr, 0, d_table, cudaMemcpyDeviceToDevice, table_off, tcomp);
 }
 
 // malio_upload_scan with the records in device memory, ordered on the caller's stream.  The records are checked where they are

@@ -266,4 +266,9 @@ void comm_destroy(DeviceState* D);
 
 }  // namespace malio_devstate
 
+// malio_b200.cu, for malio_preproc.cu: malio_dev::upload_scan of an empty scan with the pose table taken from device memory
+namespace malio_dev {
+int upload_scan_table_on_device(malio_handle* h, const malio_pose_entry* d_table, const uint32_t* table_off, const malio_rigid* tcomp);
+}
+
 #endif  // MALIO_DEVICE_CUH_

@@ -62,7 +62,14 @@ struct PreState {
   uint32_t *d_vcnt = nullptr, *d_voff = nullptr, *d_vocc = nullptr, *d_vcur = nullptr; uint64_t cap_cells = 0;
   uint32_t *d_ctot = nullptr, *d_cbase = nullptr;     // chunk totals / bases of the two cell scans (2 x 65536)
   uint32_t* d_bounds = nullptr;       // 6 order-preserving keys + out count
-  uint32_t* h_small = nullptr;        // pinned: 8 words
+  uint32_t* d_order_bad = nullptr;    // malio_undistort_device: raw_order_check_kernel's flag word
+  // pinned, 8 words: the voxel grid's bounds and counts in [0..5]; malio_undistort_device's order flag and pop count in [6..7]
+  uint32_t* h_small = nullptr;
+  // the table malio_scan_uncertainty* left at the head of d_uout, for malio_upload_scan_resident: its offsets, the rigid part
+  // of the temporal compensations, and whether it still describes the slots (any malio_undistort* since then clears it)
+  bool table_resident = false;
+  uint32_t res_table_off[MALIO_MAX_LIDAR + 1] = {0, 0, 0, 0};
+  malio_rigid res_tcomp[MALIO_MAX_LIDAR] = {};
   // publish_frame_world / pcd_save (world registration): {x, y, z, intensity} per point
   float4* d_wstage = nullptr; uint64_t cap_wstage = 0;   // malio_world_register's result before its one D2H copy
   float4* d_acc = nullptr; uint64_t n_acc = 0, cap_acc = 0;   // pcl_wait_save (laserMapping.cpp:475), device-resident
@@ -82,6 +89,7 @@ int get_state(malio_handle* h, PreState*& S) {
   CUDA_TRY(cudaMalloc((void**)&S->d_seglog, (size_t)MALIO_MAX_CTRL * 6 * sizeof(double)));
   CUDA_TRY(cudaMalloc((void**)&S->d_covt, MALIO_MAX_COV * sizeof(double)));
   CUDA_TRY(cudaMalloc((void**)&S->d_bounds, 8 * sizeof(uint32_t)));
+  CUDA_TRY(cudaMalloc((void**)&S->d_order_bad, sizeof(uint32_t)));
   CUDA_TRY(cudaMalloc((void**)&S->d_ctot, 2 * 65536 * sizeof(uint32_t)));
   CUDA_TRY(cudaMalloc((void**)&S->d_cbase, 2 * 65536 * sizeof(uint32_t)));
   CUDA_TRY(cudaHostAlloc((void**)&S->h_small, 8 * sizeof(uint32_t), cudaHostAllocDefault));
@@ -367,6 +375,15 @@ idx_scan_kernel(const int32_t* __restrict__ need, const uint8_t* __restrict__ ok
     const int32_t total = steps ? (int32_t)(steps - 1) + s_carry : 0;
     pop_point[n_cov] = total < 0 ? 0 : total;
   }
+}
+
+// malio_undistort_device's time-order check, malio_undistort's host loop on device memory: point i >= 1 is out of order when
+// its time is below its predecessor's (the same comparison, so a NaN time passes exactly where the host loop lets it pass).
+// A warp with such a point ORs 1 into *bad.  Only the time word of each 16-byte record is read.
+__global__ void __launch_bounds__(256) raw_order_check_kernel(const malio_raw_pt* __restrict__ raw, uint32_t n, uint32_t* __restrict__ bad) {
+  const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+  const bool b = i >= 1 && i < n && raw[i].curvature < raw[i - 1].curvature;
+  if (__any_sync(0xFFFFFFFFu, b) && (threadIdx.x & 31u) == 0) atomicOr(bad, 1u);
 }
 
 // ------------------------------------------------------------------ N3: voxel grid
@@ -668,44 +685,24 @@ scan_unc_kernel(const UncConst c, const double* __restrict__ imu_cov, malio_pose
   if (k < c.n_pops[num] - 1) pose_unc_entry(num, c.ext, &tcomp, &pc, &tab[c.tab_off[num] + k]);
 }
 
-}  // namespace
-
-namespace malio_pre {
-
-void destroy(malio_handle* h) {
-  PreState* S = (PreState*)h->pre;
-  if (!S) return;
-  for (auto& L : S->lid) {
-    void* p[] = {L.d_raw, L.d_ud, L.d_need, L.d_idx, L.d_ok, L.d_pose, L.d_pop, L.d_ds};
-    for (void* q : p) if (q) cudaFree(q);
-  }
-  void* p[] = {S->d_ct, S->d_cT, S->d_seglog, S->d_covt, S->d_ucov, S->d_uout, S->d_vin, S->d_vidx, S->d_vtmp, S->d_vorder, S->d_vcnt, S->d_voff,
-               S->d_vocc, S->d_vcur, S->d_ctot, S->d_cbase, S->d_bounds, S->d_wstage, S->d_acc};
-  for (void* q : p) if (q) cudaFree(q);
-  if (S->h_small) cudaFreeHost(S->h_small);
-  if (S->h_bounce) cudaFreeHost(S->h_bounce);
-  delete S;
-  h->pre = nullptr;
-}
-
-int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, const malio_undistort_args* a, float* xyz,
-              int32_t* idx, uint8_t* ok, int32_t* pop_point, uint32_t* n_pops, double* pose) {
-  PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+// ---- malio_undistort and malio_undistort_device share three steps: the argument checks, the slot's preparation, the launches
+int undistort_check_args(malio_handle* h, int lidar, const malio_undistort_args* a) {
   if (lidar < 0 || lidar >= MALIO_MAX_LIDAR) { h->err = "lidar slot out of range"; return MALIO_ERR_INVALID_ARG; }
   if (a->n_ctrl > MALIO_MAX_CTRL || a->n_cov > MALIO_MAX_COV) { h->err = "too many control points / covariance entries"; return MALIO_ERR_CAPACITY; }
   for (uint32_t k = 1; k < a->n_ctrl; ++k) if (!(a->ctrl_t[k] > a->ctrl_t[k - 1])) { h->err = "control-point times must ascend"; return MALIO_ERR_INVALID_ARG; }
   for (uint32_t k = 1; k < a->n_cov; ++k) if (!(a->imu_cov_t[k] >= a->imu_cov_t[k - 1])) { h->err = "imu_cov times must ascend"; return MALIO_ERR_INVALID_ARG; }
   if (a->cov_pointer < -1 || a->cov_pointer >= (int32_t)a->n_cov) { h->err = "cov_pointer outside the list"; return MALIO_ERR_INVALID_ARG; }
-  PreLidar& L = S->lid[lidar];
-  cudaStream_t st = S->stream;
+  return MALIO_OK;
+}
+
+// the slot takes the call's sizes and arguments and holds no valid result until the caller sets ud_valid; buffers grown for n
+int undistort_prepare_slot(malio_handle* h, PreState* S, PreLidar& L, uint32_t n, const malio_undistort_args* a) {
   L.ud_valid = false;
+  S->table_resident = false;   // the table in d_uout was built from this slot's previous undistortion
   if (n > L.cap) {
-    // ensure() frees the slot's buffers: a malio_world_register_device that returned after enqueueing may still read d_ud.
-    // Drain the stream first rather than rely on cudaFree waiting for the device.
-    CUDA_TRY(cudaStreamSynchronize(st));
+    // ensure() frees the slot's buffers: a call that returned after enqueueing (malio_world_register_device,
+    // malio_voxel_grid_device) may still read d_ud.  Drain the stream first rather than rely on cudaFree waiting for the device.
+    CUDA_TRY(cudaStreamSynchronize(S->stream));
     const uint32_t cap = n + n / 8 + 1024;
     if (int rc = ensure(h, L.d_raw, cap)) return rc;
     if (int rc = ensure(h, L.d_ud, (size_t)cap * 5)) return rc;
@@ -722,8 +719,14 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   L.cov_pointer = a->cov_pointer;
   L.lt_imu_frame = a->lt_imu_frame;
   L.n_pops = 0;
-  if (n == 0) { if (n_pops) *n_pops = 0; L.ud_valid = true; return MALIO_OK; }
-  CUDA_TRY(cudaMemcpyAsync(L.d_raw, pts, (size_t)n * sizeof(malio_raw_pt), cudaMemcpyHostToDevice, st));
+  return MALIO_OK;
+}
+
+// control points and IMU times to the device, then the three kernels over d_raw[0 .. n), n > 0 (the slot's d_raw, or the
+// caller's device array read in place); results in the slot's buffers
+int undistort_launch(malio_handle* h, PreState* S, DeviceState* D, PreLidar& L, const malio_raw_pt* d_raw, uint32_t n,
+                     const malio_undistort_args* a) {
+  cudaStream_t st = S->stream;
   CUDA_TRY(cudaMemcpyAsync(S->d_ct, a->ctrl_t, a->n_ctrl * sizeof(double), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(S->d_cT, a->ctrl_T, (size_t)a->n_ctrl * 16 * sizeof(double), cudaMemcpyHostToDevice, st));
   if (a->n_cov) CUDA_TRY(cudaMemcpyAsync(S->d_covt, a->imu_cov_t, a->n_cov * sizeof(double), cudaMemcpyHostToDevice, st));
@@ -734,12 +737,49 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   c.n_ctrl = (int)a->n_ctrl; c.n_cov = (int)a->n_cov; c.cov_pointer = a->cov_pointer;
   if (a->n_ctrl > 1) seglog_kernel<<<(a->n_ctrl + 63) / 64, 64, 0, st>>>(S->d_cT, (int)a->n_ctrl, S->d_seglog);
   const size_t smem = (size_t)(a->n_ctrl + a->n_cov) * sizeof(double);
-  undistort_kernel<<<(n + UD_THREADS - 1) / UD_THREADS, UD_THREADS, smem, st>>>(L.d_raw, n, c, S->d_ct, S->d_cT, S->d_seglog, S->d_covt,
+  undistort_kernel<<<(n + UD_THREADS - 1) / UD_THREADS, UD_THREADS, smem, st>>>(d_raw, n, c, S->d_ct, S->d_cT, S->d_seglog, S->d_covt,
                                                                                   L.d_ud, L.d_need, L.d_ok, L.d_pose);
   idx_scan_kernel<<<1, SCAN_T, 0, st>>>(L.d_need, L.d_ok, n, L.d_ud, L.d_idx, L.d_pop, (int)a->n_cov);
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 3;
-  D->ctr.h2d_bytes += (uint64_t)n * sizeof(malio_raw_pt) + (uint64_t)a->n_ctrl * 17 * 8 + (uint64_t)a->n_cov * 8;
+  D->ctr.h2d_bytes += (uint64_t)a->n_ctrl * 17 * 8 + (uint64_t)a->n_cov * 8;
+  return MALIO_OK;
+}
+
+}  // namespace
+
+namespace malio_pre {
+
+void destroy(malio_handle* h) {
+  PreState* S = (PreState*)h->pre;
+  if (!S) return;
+  for (auto& L : S->lid) {
+    void* p[] = {L.d_raw, L.d_ud, L.d_need, L.d_idx, L.d_ok, L.d_pose, L.d_pop, L.d_ds};
+    for (void* q : p) if (q) cudaFree(q);
+  }
+  void* p[] = {S->d_ct, S->d_cT, S->d_seglog, S->d_covt, S->d_ucov, S->d_uout, S->d_vin, S->d_vidx, S->d_vtmp, S->d_vorder, S->d_vcnt, S->d_voff,
+               S->d_vocc, S->d_vcur, S->d_ctot, S->d_cbase, S->d_bounds, S->d_order_bad, S->d_wstage, S->d_acc};
+  for (void* q : p) if (q) cudaFree(q);
+  if (S->h_small) cudaFreeHost(S->h_small);
+  if (S->h_bounce) cudaFreeHost(S->h_bounce);
+  delete S;
+  h->pre = nullptr;
+}
+
+int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, const malio_undistort_args* a, float* xyz,
+              int32_t* idx, uint8_t* ok, int32_t* pop_point, uint32_t* n_pops, double* pose) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (int rc = undistort_check_args(h, lidar, a)) return rc;
+  PreLidar& L = S->lid[lidar];
+  cudaStream_t st = S->stream;
+  if (int rc = undistort_prepare_slot(h, S, L, n, a)) return rc;
+  if (n == 0) { if (n_pops) *n_pops = 0; L.ud_valid = true; return MALIO_OK; }
+  CUDA_TRY(cudaMemcpyAsync(L.d_raw, pts, (size_t)n * sizeof(malio_raw_pt), cudaMemcpyHostToDevice, st));
+  D->ctr.h2d_bytes += (uint64_t)n * sizeof(malio_raw_pt);
+  if (int rc = undistort_launch(h, S, D, L, L.d_raw, n, a)) return rc;
   std::vector<float> ud_host;
   if (xyz) ud_host.resize((size_t)n * 5);
   std::vector<int32_t> pops(a->n_cov + 1);
@@ -758,29 +798,65 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
   return MALIO_OK;
 }
 
-int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap, uint32_t* n_out) {
+// malio_undistort on a raw cloud in device memory, ordered on the caller's stream.  The cloud is read where it is by the order
+// check and by undistort_kernel; the slot's d_raw is not used.  The check's verdict and the pop count are fetched together
+// behind the kernels, so the host waits once.  That is safe on a cloud that turns out to be unordered: undistort_kernel treats
+// every point on its own (need = entries of the list above the point's time, in [0, n_cov] whatever the order), and in
+// idx_scan_kernel pops_s = s + min(1, min_{j<=s}(need_j - j)) lies in [0, need_s], so pop_point is written at pops - 1 < n_cov
+// only and everything else at a point's own index.  Such a cloud leaves the slot without a valid result.
+int undistort_device(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, const malio_undistort_args* a, float* cloud,
+                     int32_t* idx, uint8_t* ok, int32_t* pop_point, double* pose, uint32_t* n_pops, cudaStream_t caller) {
   PreState* S;
   if (int rc = get_state(h, S)) return rc;
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
-  if (lidar < 0 || lidar >= MALIO_MAX_LIDAR || !(leaf > 0.f)) { h->err = "voxel_grid: bad lidar slot or leaf size"; return MALIO_ERR_INVALID_ARG; }
+  if (int rc = undistort_check_args(h, lidar, a)) return rc;
+  if (n) {
+    if (int rc = check_device_ptr(h, D, pts, "malio_undistort_device pts")) return rc;
+    if (cloud) { if (int rc = check_device_ptr(h, D, cloud, "malio_undistort_device cloud")) return rc; }
+    if (idx) { if (int rc = check_device_ptr(h, D, idx, "malio_undistort_device idx")) return rc; }
+    if (ok) { if (int rc = check_device_ptr(h, D, ok, "malio_undistort_device ok")) return rc; }
+    if (pop_point && a->n_cov) { if (int rc = check_device_ptr(h, D, pop_point, "malio_undistort_device pop_point")) return rc; }
+    if (pose) { if (int rc = check_device_ptr(h, D, pose, "malio_undistort_device pose")) return rc; }
+  }
   PreLidar& L = S->lid[lidar];
   cudaStream_t st = S->stream;
-  const float* d_in;
-  if (in) {
-    if (n > S->cap_vin) { if (int rc = ensure(h, S->d_vin, (size_t)(n + 1024) * 5)) return rc; S->cap_vin = n + 1024; }
-    if (n) CUDA_TRY(cudaMemcpyAsync(S->d_vin, in, (size_t)n * 5 * sizeof(float), cudaMemcpyHostToDevice, st));
-    D->ctr.h2d_bytes += (uint64_t)n * 20;
-    d_in = S->d_vin;
-  } else {
-    n = L.n;
-    d_in = L.d_ud;
-  }
+  if (int rc = undistort_prepare_slot(h, S, L, n, a)) return rc;
+  if (n == 0) { if (n_pops) *n_pops = 0; L.ud_valid = true; return MALIO_OK; }
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  CUDA_TRY(cudaMemsetAsync(S->d_order_bad, 0, sizeof(uint32_t), st));
+  raw_order_check_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, S->d_order_bad);
+  D->ctr.kernel_launches += 1;
+  if (int rc = undistort_launch(h, S, D, L, pts, n, a)) return rc;
+  if (cloud) CUDA_TRY(cudaMemcpyAsync(cloud, L.d_ud, (size_t)n * 5 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (idx) CUDA_TRY(cudaMemcpyAsync(idx, L.d_idx, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  if (ok) CUDA_TRY(cudaMemcpyAsync(ok, L.d_ok, (size_t)n, cudaMemcpyDeviceToDevice, st));
+  if (pop_point && a->n_cov) CUDA_TRY(cudaMemcpyAsync(pop_point, L.d_pop, a->n_cov * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  if (pose) CUDA_TRY(cudaMemcpyAsync(pose, L.d_pose, (size_t)n * 7 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  if (int rc = caller_leave(h, D, caller)) return rc;   // the copies are the last access to the caller's arrays
+  CUDA_TRY(cudaMemcpyAsync(S->h_small + 6, S->d_order_bad, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(S->h_small + 7, L.d_pop + a->n_cov, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (S->h_small[6]) { h->err = "malio_undistort: points must be sorted by curvature (IMU_Processing.hpp:232)"; return MALIO_ERR_INVALID_ARG; }
+  L.n_pops = S->h_small[7];
+  if (n_pops) *n_pops = L.n_pops;
+  L.ud_valid = true;
+  return MALIO_OK;
+}
+
+// the filter over d_in[0 .. n) (device memory: the slot's undistorted cloud, the staged host input or the caller's device
+// array), shared by malio_voxel_grid and malio_voxel_grid_device.  Waits twice, for the grid geometry and for the output count
+// (they size allocations), and returns with vg_centroid_kernel enqueued: the result is the slot's d_ds, n_ds rows.
+static int voxel_grid_run(malio_handle* h, PreState* S, DeviceState* D, PreLidar& L, const float* d_in, uint32_t n, float leaf,
+                          uint32_t* n_out) {
+  cudaStream_t st = S->stream;
   L.ds_valid = false;
   L.n_ds = 0;
   if (n_out) *n_out = 0;
   if (n == 0) { L.ds_valid = true; return MALIO_OK; }
   if (n > S->cap_vpts) {
+    // ensure() frees the scratch a malio_voxel_grid_device that returned after enqueueing may still use: drain the stream first
+    CUDA_TRY(cudaStreamSynchronize(st));
     const uint32_t cap = n + n / 8 + 1024;
     if (int rc = ensure(h, S->d_vidx, cap)) return rc;
     if (int rc = ensure(h, S->d_vtmp, cap)) return rc;
@@ -847,8 +923,38 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
   L.n_ds = m;
   L.ds_valid = true;
   if (n_out) *n_out = m;
-  if (out) {
-    const uint32_t k = m < out_cap ? m : out_cap;
+  return MALIO_OK;
+}
+
+// the slot's own cloud as the filter's input.  A slot whose last undistortion did not complete (an unordered cloud given to
+// malio_undistort_device, a failed allocation) holds no cloud to filter; a slot never undistorted is an empty cloud.
+static int voxel_slot_input(malio_handle* h, const PreLidar& L, const float*& d_in, uint32_t& n) {
+  if (!L.ud_valid && L.n) { h->err = "voxel_grid: the slot's last undistortion did not complete (undistort it again)"; return MALIO_ERR_STATE; }
+  n = L.n;
+  d_in = L.d_ud;
+  return MALIO_OK;
+}
+
+int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap, uint32_t* n_out) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (lidar < 0 || lidar >= MALIO_MAX_LIDAR || !(leaf > 0.f)) { h->err = "voxel_grid: bad lidar slot or leaf size"; return MALIO_ERR_INVALID_ARG; }
+  PreLidar& L = S->lid[lidar];
+  cudaStream_t st = S->stream;
+  const float* d_in;
+  if (in) {
+    if (n > S->cap_vin) { if (int rc = ensure(h, S->d_vin, (size_t)(n + 1024) * 5)) return rc; S->cap_vin = n + 1024; }
+    if (n) CUDA_TRY(cudaMemcpyAsync(S->d_vin, in, (size_t)n * 5 * sizeof(float), cudaMemcpyHostToDevice, st));
+    D->ctr.h2d_bytes += (uint64_t)n * 20;
+    d_in = S->d_vin;
+  } else if (int rc = voxel_slot_input(h, L, d_in, n)) {
+    return rc;
+  }
+  if (int rc = voxel_grid_run(h, S, D, L, d_in, n, leaf, n_out)) return rc;
+  if (out && L.n_ds) {
+    const uint32_t k = L.n_ds < out_cap ? L.n_ds : out_cap;
     CUDA_TRY(cudaMemcpyAsync(out, L.d_ds, (size_t)k * 5 * sizeof(float), cudaMemcpyDeviceToHost, st));
     D->ctr.d2h_bytes += (uint64_t)k * 20;
   }
@@ -856,12 +962,35 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
   return MALIO_OK;
 }
 
-int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uint32_t* table_off, const malio_rigid* tcomp,
-                       uint32_t* n_total) {
+// malio_voxel_grid with the explicit input and the output in device memory, ordered on the caller's stream.  The input is read
+// where it is (nothing reads it after vg_centroid_kernel); the call returns with that kernel and the copy of the output enqueued.
+int voxel_grid_device(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap, uint32_t* n_out,
+                      cudaStream_t caller) {
   PreState* S;
   if (int rc = get_state(h, S)) return rc;
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
+  if (lidar < 0 || lidar >= MALIO_MAX_LIDAR || !(leaf > 0.f)) { h->err = "voxel_grid: bad lidar slot or leaf size"; return MALIO_ERR_INVALID_ARG; }
+  PreLidar& L = S->lid[lidar];
+  const float* d_in = in;
+  if (!in) { if (int rc = voxel_slot_input(h, L, d_in, n)) return rc; }
+  if (n) {
+    if (in) { if (int rc = check_device_ptr(h, D, in, "malio_voxel_grid_device in")) return rc; }
+    if (out && out_cap) { if (int rc = check_device_ptr(h, D, out, "malio_voxel_grid_device out")) return rc; }
+    if (int rc = caller_enter(h, D, caller)) return rc;
+  }
+  // an early return below (no finite point, MALIO_ERR_CAPACITY) comes after a wait for the last kernel that read `in`
+  if (int rc = voxel_grid_run(h, S, D, L, d_in, n, leaf, n_out)) return rc;
+  if (L.n_ds == 0) return MALIO_OK;
+  const uint32_t k = L.n_ds < out_cap ? L.n_ds : out_cap;
+  if (out && k) CUDA_TRY(cudaMemcpyAsync(out, L.d_ds, (size_t)k * 5 * sizeof(float), cudaMemcpyDeviceToDevice, S->stream));
+  return caller_leave(h, D, caller);
+}
+
+// the slots' down-sampled clouds merged into the handle's scan.  table: host memory, or (table_on_device) the table
+// malio_scan_uncertainty* left in d_uout, copied device-to-device
+static int merge_scan(malio_handle* h, PreState* S, DeviceState* D, const malio_pose_entry* table, bool table_on_device,
+                      const uint32_t* table_off, const malio_rigid* tcomp, uint32_t* n_total) {
   const int Ln = h->cfg.params.n_lidar;
   uint32_t total = 0;
   for (int l = 0; l < Ln; ++l) {
@@ -869,7 +998,9 @@ int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uin
     total += S->lid[l].n_ds;
   }
   // size the scan buffers and tables through the regular entry point (no points copied), then fill d_pts on the device
-  if (int rc = malio_dev::upload_scan(h, nullptr, 0, table, table_off, tcomp)) return rc;
+  if (int rc = table_on_device ? malio_dev::upload_scan_table_on_device(h, table, table_off, tcomp)
+                               : malio_dev::upload_scan(h, nullptr, 0, table, table_off, tcomp))
+    return rc;
   if (int rc = malio_dev::reserve_scan(h, total)) return rc;
   uint32_t at = 0;
   for (int l = 0; l < Ln; ++l) {
@@ -883,6 +1014,28 @@ int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uin
   D->ctr.kernel_launches += Ln;
   if (n_total) *n_total = total;
   return MALIO_OK;
+}
+
+int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uint32_t* table_off, const malio_rigid* tcomp,
+                       uint32_t* n_total) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  return merge_scan(h, S, D, table, false, table_off, tcomp, n_total);
+}
+
+// malio_upload_scan_device with the table, its offsets and the temporal compensations of the last malio_scan_uncertainty*
+int upload_scan_resident(malio_handle* h, uint32_t* n_total) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (!S->table_resident) {
+    h->err = "upload_scan_resident: no pose table on the device (run malio_scan_uncertainty* after the last malio_undistort* of the scan)";
+    return MALIO_ERR_STATE;
+  }
+  return merge_scan(h, S, D, (const malio_pose_entry*)S->d_uout, true, S->res_table_off, S->res_tcomp, n_total);
 }
 
 int world_register(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out, uint32_t cap,
@@ -994,9 +1147,15 @@ int world_save_pcd(malio_handle* h, const char* path, int clear) {
   return rc;
 }
 
+// malio_scan_uncertainty, and with table == NULL malio_scan_uncertainty_resident: the table is built in d_uout either way and
+// stays there for malio_upload_scan_resident; the resident call fetches the L - 1 temporal compensations only (the passes take
+// them as kernel constants, and the host's sin / cos differ from the device's in the last place, so they are not recomputed),
+// and table_off, temporal_comp may be NULL
 int scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_entry* table, uint32_t table_cap, uint32_t* table_off,
                      malio_pose* temporal_comp, malio_pose* lidar_unc, uint32_t* lidar_unc_counts) {
   PreState* S = (PreState*)h->pre;
+  uint32_t off_local[MALIO_MAX_LIDAR + 1];
+  if (!table_off) table_off = off_local;
   const int Ln = h->cfg.params.n_lidar;
   UncConst c{};
   c.L = Ln;
@@ -1019,7 +1178,7 @@ int scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_e
   }
   c.first[Ln] = n_thr;
   table_off[Ln] = n_tab;
-  if (n_tab > table_cap) {
+  if (table && n_tab > table_cap) {
     h->err = "scan_uncertainty: the table needs " + std::to_string(n_tab) + " entries (table_off[L]), table_cap is " + std::to_string(table_cap);
     return MALIO_ERR_CAPACITY;
   }
@@ -1040,22 +1199,32 @@ int scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_e
                                         MALIO_MAX_LIDAR * sizeof(malio_pose)))
       return rc;
   }
+  S->table_resident = false;
   if (a->n_cov) CUDA_TRY(cudaMemcpyAsync(S->d_ucov, a->imu_cov, (size_t)a->n_cov * 36 * sizeof(double), cudaMemcpyHostToDevice, st));
   malio_pose_entry* d_tab = (malio_pose_entry*)S->d_uout;
   malio_pose* d_tc = (malio_pose*)(S->d_uout + tab_bytes);
   malio_pose* d_unc = d_tc + (Ln - 1);
   scan_unc_kernel<<<(n_thr + UNC_THREADS - 1) / UNC_THREADS, UNC_THREADS, 0, st>>>(c, S->d_ucov, d_tab, d_tc, d_unc);
   CUDA_TRY(cudaGetLastError());
-  std::vector<char> out(out_bytes);
-  CUDA_TRY(cudaMemcpyAsync(out.data(), S->d_uout, out_bytes, cudaMemcpyDeviceToHost, st));
+  const size_t tc_bytes = (size_t)(Ln - 1) * sizeof(malio_pose);
+  const size_t skip = table ? 0 : tab_bytes, fetch = table ? out_bytes : tc_bytes;
+  std::vector<char> out(fetch);
+  if (fetch) CUDA_TRY(cudaMemcpyAsync(out.data(), S->d_uout + skip, fetch, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   D->ctr.kernel_launches += 1;
   D->ctr.h2d_bytes += (uint64_t)a->n_cov * 36 * 8;
-  D->ctr.d2h_bytes += out_bytes;
-  std::memcpy(table, out.data(), tab_bytes);
-  if (Ln > 1) std::memcpy(temporal_comp, out.data() + tab_bytes, (size_t)(Ln - 1) * sizeof(malio_pose));
-  if (lidar_unc) std::memcpy(lidar_unc, out.data() + tab_bytes + (size_t)(Ln - 1) * sizeof(malio_pose), (size_t)n_unc * sizeof(malio_pose));
+  D->ctr.d2h_bytes += fetch;
+  const malio_pose* tc = (const malio_pose*)(out.data() + tab_bytes - skip);
+  if (table) std::memcpy(table, out.data(), tab_bytes);
+  if (Ln > 1 && temporal_comp) std::memcpy(temporal_comp, tc, tc_bytes);
+  if (lidar_unc) std::memcpy(lidar_unc, out.data() + tab_bytes + tc_bytes, (size_t)n_unc * sizeof(malio_pose));
   if (lidar_unc_counts) for (int l = 0; l < Ln; ++l) lidar_unc_counts[l] = (uint32_t)c.n_pops[l];
+  for (int l = 0; l <= Ln; ++l) S->res_table_off[l] = table_off[l];
+  for (int l = 0; l + 1 < Ln; ++l) {
+    std::memcpy(S->res_tcomp[l].q, tc[l].q, sizeof(tc[l].q));
+    std::memcpy(S->res_tcomp[l].t, tc[l].t, sizeof(tc[l].t));
+  }
+  S->table_resident = true;
   return MALIO_OK;
 }
 
@@ -1083,6 +1252,34 @@ extern "C" int malio_scan_uncertainty(malio_handle* h, const malio_scan_unc_args
   if (h->cfg.params.n_lidar > 1 && !temporal_comp) { h->err = "scan_uncertainty: temporal_comp required for L > 1"; return MALIO_ERR_INVALID_ARG; }
   MALIO_SETTLE(h);
   return malio_pre::scan_uncertainty(h, a, table, table_cap, table_off, temporal_comp, lidar_unc, lidar_unc_counts);
+}
+
+extern "C" int malio_scan_uncertainty_resident(malio_handle* h, const malio_scan_unc_args* a, uint32_t* table_off, malio_pose* temporal_comp) {
+  if (!h || !a || !a->extrinsic || !a->uncertainty || (a->n_cov && !a->imu_cov)) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_pre::scan_uncertainty(h, a, nullptr, 0, table_off, temporal_comp, nullptr, nullptr);
+}
+
+// the front half of a scan on device memory (malio_b200.h): the wrappers check what malio_undistort / malio_voxel_grid /
+// malio_upload_scan_device check on the host; the device pointers are checked inside, once the point count is known
+extern "C" int malio_undistort_device(malio_handle* h, int lidar, const malio_raw_pt* d_pts, uint32_t n, const malio_undistort_args* a,
+                                      float* d_cloud, int32_t* d_idx, uint8_t* d_ok, int32_t* d_pop_point, double* d_pose, uint32_t* n_pops,
+                                      void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  if (!a || !a->ctrl_t || !a->ctrl_T || (a->n_cov && !a->imu_cov_t)) return MALIO_ERR_INVALID_ARG;
+  return malio_pre::undistort_device(h, lidar, d_pts, n, a, d_cloud, d_idx, d_ok, d_pop_point, d_pose, n_pops, (cudaStream_t)stream);
+}
+extern "C" int malio_voxel_grid_device(malio_handle* h, int lidar, const float* d_in, uint32_t n, float leaf, float* d_out, uint32_t out_cap,
+                                       uint32_t* n_out, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_pre::voxel_grid_device(h, lidar, d_in, n, leaf, d_out, out_cap, n_out, (cudaStream_t)stream);
+}
+extern "C" int malio_upload_scan_resident(malio_handle* h, uint32_t* n_total) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_pre::upload_scan_resident(h, n_total);
 }
 
 // publish_frame_world / pcd_save (laserMapping.cpp:448-489)

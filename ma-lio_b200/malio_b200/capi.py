@@ -129,6 +129,7 @@ EXPORTS = [
     "malio_world_register", "malio_world_accumulate", "malio_world_save_pcd", "malio_write_pcd_binary",
     "malio_knn_device", "malio_map_build_device", "malio_map_add_points_device",
     "malio_upload_scan_from_device", "malio_download_aux_device", "malio_map_incremental_device", "malio_world_register_device",
+    "malio_undistort_device", "malio_voxel_grid_device", "malio_scan_uncertainty_resident", "malio_upload_scan_resident",
 ]
 
 
@@ -202,6 +203,10 @@ def load() -> C.CDLL:
     lib.malio_download_aux_device.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.malio_map_incremental_device.argtypes = [vp, vp, C.c_double, i32, vp, vp, vp]
     lib.malio_world_register_device.argtypes = [vp, vp, i32, vp, vp, u32, vp, vp]
+    lib.malio_undistort_device.argtypes = [vp, i32, vp, u32, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.malio_voxel_grid_device.argtypes = [vp, i32, vp, u32, C.c_float, vp, u32, vp, vp]
+    lib.malio_scan_uncertainty_resident.argtypes = [vp, vp, vp, vp]
+    lib.malio_upload_scan_resident.argtypes = [vp, vp]
     lib.malio_ieskf_update.argtypes = [vp, C.POINTER(State), vp, i32, C.c_double, C.POINTER(UpdateReport)]
     lib.malio_build_static_snapshot.argtypes = [vp, u32, vp, vp, C.POINTER(u32)]
     lib.malio_rearm_scan.argtypes = [vp]

@@ -149,6 +149,7 @@ class MeasurementModel:
         if rc != capi.OK:
             raise capi.MalioError(rc, self.lib.malio_last_error(None).decode())
         self.n_points = 0
+        self._slot_rows = {}   # rows of the last undistort*() per LiDAR slot (voxel_grid_tensor sizes its output by them)
         self._keep = []   # host buffers must outlive the (synchronous) calls only; kept for clarity
 
     def close(self):
@@ -274,20 +275,13 @@ class MeasurementModel:
         pts = np.ascontiguousarray(pts)
         assert pts.dtype == capi.RAW_PT
         n = pts.shape[0]
-        ct = np.ascontiguousarray(ctrl_t, np.float64)
-        cT = np.ascontiguousarray(ctrl_T, np.float64).reshape(-1, 16)
-        cv = np.ascontiguousarray(imu_cov_t, np.float64)
-        a = capi.UndistortArgs()
-        a.beg_time = float(beg_time)
-        a.extrinsic.q[:] = list(map(float, extrinsic[0])); a.extrinsic.t[:] = list(map(float, extrinsic[1]))
-        a.lt_imu_frame.q[:] = list(map(float, lt_imu_frame[0])); a.lt_imu_frame.t[:] = list(map(float, lt_imu_frame[1]))
-        a.ctrl_t = ct.ctypes.data; a.ctrl_T = cT.ctypes.data; a.n_ctrl = ct.shape[0]
-        a.imu_cov_t = cv.ctypes.data if cv.shape[0] else None; a.n_cov = cv.shape[0]; a.cov_pointer = int(cov_pointer)
+        a, cv, _keep = _undistort_args(beg_time, extrinsic, lt_imu_frame, ctrl_t, ctrl_T, imu_cov_t, cov_pointer)
         xyz = np.zeros((n, 3), np.float32); idx = np.zeros(n, np.int32); ok = np.zeros(n, np.uint8)
         pop = np.full(max(cv.shape[0], 1), -1, np.int32); npop = C.c_uint32(0)
         pose = np.zeros((n, 7)) if want_pose else None
         self._check(self.lib.malio_undistort(self._h, lidar, capi.ptr(pts), n, C.byref(a), capi.ptr(xyz), capi.ptr(idx), capi.ptr(ok),
                                              capi.ptr(pop), C.byref(npop), capi.ptr(pose)))
+        self._slot_rows[lidar] = n
         return dict(xyz=xyz, idx=idx, ok=ok, pop_point=pop[: npop.value], pose=pose)
 
     def voxel_grid(self, lidar: int, pts5: np.ndarray | None, leaf: float):
@@ -318,14 +312,7 @@ class MeasurementModel:
         uncertainty; uncertainty: float64[6,6] (kf.getUncertainty()).  Returns dict(table, table_off, temporal_comp capi.POSE[L-1],
         temporal_comp_rigid capi.RIGID[L-1] or None (what upload_scan* take), lidar_unc: list of capi.POSE arrays or None)."""
         L = self.n_lidar
-        cov = np.ascontiguousarray(imu_cov, np.float64).reshape(-1, 36)
-        ext = np.ascontiguousarray(extrinsic, dtype=capi.POSE)
-        unc0 = np.ascontiguousarray(uncertainty, np.float64).reshape(36)
-        a = capi.ScanUncArgs()
-        a.imu_cov = cov.ctypes.data if cov.shape[0] else None
-        a.n_cov = cov.shape[0]
-        a.extrinsic = ext.ctypes.data
-        a.uncertainty = unc0.ctypes.data
+        a, _keep = _scan_unc_args(imu_cov, extrinsic, uncertainty)
         cap = L * capi.MAX_COV
         table = np.zeros(cap, dtype=capi.POSE_ENTRY)
         off = np.zeros(L + 1, np.uint32)
@@ -335,10 +322,7 @@ class MeasurementModel:
         self._check(self.lib.malio_scan_uncertainty(self._h, C.byref(a), capi.ptr(table), cap, capi.ptr(off), capi.ptr(tc),
                                                     capi.ptr(lists), capi.ptr(counts)))
         tc = tc[: L - 1]
-        rigid = None
-        if L > 1:
-            rigid = np.zeros(L - 1, dtype=capi.RIGID)
-            rigid["q"], rigid["t"] = tc["q"], tc["t"]
+        rigid = _rigid_of(tc)
         lu = None
         if want_lists:
             ends = np.cumsum(counts)
@@ -549,6 +533,115 @@ class MeasurementModel:
             self._check(self.lib.malio_world_register_device(self._h, C.byref(ps), src, capi.ptr(tag), _dptr(out), n.value, C.byref(n),
                                                              st.cuda_stream))
         return out
+
+    # ---- the front half of a scan on torch CUDA tensors: raw clouds in, the pose table kept on the device, ordered on
+    # torch.cuda.current_stream() (malio_undistort_device & co.)
+    UNDISTORT_OUTPUTS = ("cloud", "idx", "ok", "pop_point", "pose")
+
+    def undistort_tensor(self, lidar: int, pts, beg_time: float, extrinsic, lt_imu_frame, ctrl_t, ctrl_T, imu_cov_t, cov_pointer: int,
+                         want=UNDISTORT_OUTPUTS):
+        """undistort() of a contiguous float32 CUDA tensor (n, 4) {x, y, z, curvature} on the handle's device, sorted by
+        curvature and read in place; the other arguments are host values as for undistort().  Returns a dict with n_pops and the
+        tensors named in `want`: cloud float32 (n, 5) {x, y, z, idx as float (0 where untouched), curvature} — the rows
+        voxel_grid_tensor takes —, idx int32 (n,), ok uint8 (n,), pop_point int32 (n_pops,), pose float64 (n, 7).  Waits once, at
+        its end, for the pop count and the time-order check; an unordered cloud raises MalioError (ERR_INVALID_ARG) and leaves
+        the slot without a result until it is undistorted again."""
+        import torch
+        _check_tensor(pts, "pts", torch.float32, 4, self.device)
+        unknown = set(want) - set(self.UNDISTORT_OUTPUTS)
+        if unknown:
+            raise ValueError(f"want: unknown outputs {sorted(unknown)}")
+        n = pts.shape[0]
+        a, cv, _keep = _undistort_args(beg_time, extrinsic, lt_imu_frame, ctrl_t, ctrl_T, imu_cov_t, cov_pointer)
+        o = dict(cloud=self._empty((n, 5), torch.float32, "cloud" in want), idx=self._empty((n,), torch.int32, "idx" in want),
+                 ok=self._empty((n,), torch.uint8, "ok" in want), pop_point=self._empty((cv.shape[0],), torch.int32, "pop_point" in want),
+                 pose=self._empty((n, 7), torch.float64, "pose" in want))
+        npop = C.c_uint32(0)
+        st = torch.cuda.current_stream(pts.device)
+        self._check(self.lib.malio_undistort_device(self._h, lidar, _dptr(pts), n, C.addressof(a), _dptr(o["cloud"]), _dptr(o["idx"]),
+                                                    _dptr(o["ok"]), _dptr(o["pop_point"]), _dptr(o["pose"]), C.addressof(npop),
+                                                    st.cuda_stream))
+        self._slot_rows[lidar] = n
+        out = {k: v for k, v in o.items() if k in want}
+        if "pop_point" in want:
+            out["pop_point"] = o["pop_point"][: npop.value]   # (an empty cloud writes nothing: no pop, an empty slice)
+        out["n_pops"] = int(npop.value)
+        return out
+
+    def voxel_grid_tensor(self, lidar: int, pts5, leaf: float):
+        """voxel_grid() of a contiguous float32 CUDA tensor (n, 5) {x, y, z, intensity, curvature}, read in place, or with None of
+        the slot's undistorted cloud.  Returns float32 (n_out, 5), a view of a buffer allocated on the current stream; the result
+        is enqueued, not waited for.  The filter returns at most one row per input row, so the buffer is allocated with the input's
+        rows and sliced: the filter runs once, where the size-query protocol of voxel_grid() runs it twice.  For the slot's cloud
+        the rows are those of this model's last undistort*() on the slot; if the slot holds more (it was filled through the
+        C-ABI directly), a second call with the full size fetches the rest."""
+        import torch
+        if pts5 is not None:
+            _check_tensor(pts5, "pts5", torch.float32, 5, self.device)
+        rows = self._slot_rows.get(lidar, 0) if pts5 is None else pts5.shape[0]
+        st = torch.cuda.current_stream(self.device)
+        m = C.c_uint32(0)
+        call = lambda out, cap: self._check(self.lib.malio_voxel_grid_device(
+            self._h, lidar, _dptr(pts5), 0 if pts5 is None else pts5.shape[0], C.c_float(leaf), _dptr(out), cap, C.addressof(m), st.cuda_stream))
+        out = self._empty((rows, 5), torch.float32)
+        call(out, rows)
+        if m.value > rows:
+            out = self._empty((m.value, 5), torch.float32)
+            call(out, m.value)
+        return out[: m.value]
+
+    def scan_uncertainty_resident(self, imu_cov: np.ndarray, extrinsic: np.ndarray, uncertainty: np.ndarray):
+        """scan_uncertainty() with the table left on the device for upload_scan_resident().  Returns (table_off uint32[L+1],
+        temporal_comp capi.POSE[L-1])."""
+        L = self.n_lidar
+        a, _keep = _scan_unc_args(imu_cov, extrinsic, uncertainty)
+        off = np.zeros(L + 1, np.uint32)
+        tc = np.zeros(max(L - 1, 1), dtype=capi.POSE)
+        self._check(self.lib.malio_scan_uncertainty_resident(self._h, C.addressof(a), capi.ptr(off), capi.ptr(tc)))
+        return off, tc[: L - 1]
+
+    def upload_scan_resident(self) -> int:
+        """upload_scan_device() with the table, offsets and temporal compensations of the last scan_uncertainty*()."""
+        n = C.c_uint32(0)
+        self._check(self.lib.malio_upload_scan_resident(self._h, C.addressof(n)))
+        self.n_points = int(n.value)
+        return self.n_points
+
+
+def _undistort_args(beg_time, extrinsic, lt_imu_frame, ctrl_t, ctrl_T, imu_cov_t, cov_pointer):
+    """capi.UndistortArgs over host arrays: (args, the imu_cov times, the arrays the struct points into: keep them alive)."""
+    ct = np.ascontiguousarray(ctrl_t, np.float64)
+    cT = np.ascontiguousarray(ctrl_T, np.float64).reshape(-1, 16)
+    cv = np.ascontiguousarray(imu_cov_t, np.float64)
+    a = capi.UndistortArgs()
+    a.beg_time = float(beg_time)
+    a.extrinsic.q[:] = list(map(float, extrinsic[0])); a.extrinsic.t[:] = list(map(float, extrinsic[1]))
+    a.lt_imu_frame.q[:] = list(map(float, lt_imu_frame[0])); a.lt_imu_frame.t[:] = list(map(float, lt_imu_frame[1]))
+    a.ctrl_t = ct.ctypes.data; a.ctrl_T = cT.ctypes.data; a.n_ctrl = ct.shape[0]
+    a.imu_cov_t = cv.ctypes.data if cv.shape[0] else None; a.n_cov = cv.shape[0]; a.cov_pointer = int(cov_pointer)
+    return a, cv, (ct, cT)
+
+
+def _scan_unc_args(imu_cov, extrinsic, uncertainty):
+    """capi.ScanUncArgs over host arrays: (args, the arrays the struct points into: keep them alive)."""
+    cov = np.ascontiguousarray(imu_cov, np.float64).reshape(-1, 36)
+    ext = np.ascontiguousarray(extrinsic, dtype=capi.POSE)
+    unc0 = np.ascontiguousarray(uncertainty, np.float64).reshape(36)
+    a = capi.ScanUncArgs()
+    a.imu_cov = cov.ctypes.data if cov.shape[0] else None
+    a.n_cov = cov.shape[0]
+    a.extrinsic = ext.ctypes.data
+    a.uncertainty = unc0.ctypes.data
+    return a, (cov, ext, unc0)
+
+
+def _rigid_of(tc):
+    """capi.POSE[k] -> capi.RIGID[k] (what upload_scan* take as temporal_comp); None for k == 0."""
+    if tc.shape[0] == 0:
+        return None
+    rigid = np.zeros(tc.shape[0], dtype=capi.RIGID)
+    rigid["q"], rigid["t"] = tc["q"], tc["t"]
+    return rigid
 
 
 def pack_scan_tensor(xyz, lidar, table_idx):
