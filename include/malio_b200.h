@@ -385,6 +385,35 @@ int malio_world_accumulate(malio_handle* h, const malio_pass_state* s, const flo
  * empty cloud, MALIO_ERR_INVALID_ARG when the file cannot be opened or written; no file is left behind on any error.  The
  * scan_wait_num / pcd_save_interval bookkeeping and the file names (scans_<k>.pcd, result.pcd) stay with the caller. */
 int malio_world_save_pcd(malio_handle* h, const char* path, int clear);
+/* The saved map as a voxel map (opt-in, beside the dense cloud above; a deliberate extension beyond the reference's dense file):
+ * memory grows with the occupied voxels, work per call with the scan.  The map holds exactly the points malio_world_accumulate
+ * would append, in its order (slots 0..L-1, point order, scan after scan; the xyz are world_kernel's bits), folded per voxel
+ * into a centroid {x, y, z, intensity} with intensity = slot_tag averaged like every other field.  It is defined as
+ * malio_voxel_grid (pcl::VoxelGrid) applied to the concatenation of those dense clouds, with absolute voxel indices:
+ *   voxel of a point   (int)floorf(x * il) per axis, il = 1.0f / leaf in float (PCL's relative index gives the same voxel
+ *                      wherever |floorf(x * il)| < 2^24); points with a non-finite coordinate are skipped
+ *   centroid           float sums from 0.f continued point by point in that order across all scans, a u32 count, sum / count
+ *   order              ascending voxel index (k, j, i) as signed ints: z, then y, then x
+ * malio_world_voxel_accumulate folds the current dense cloud in: the preconditions and errors of malio_world_accumulate
+ * (MALIO_ERR_STATE until malio_undistort* has run on every slot 0..L-1, slot_tag required), and MALIO_ERR_INVALID_ARG for a leaf
+ * that is not finite and > 0 or that differs from the map's (fixed by the first call after creation or a clearing save).  A
+ * point whose voxel index falls outside int returns MALIO_ERR_CAPACITY with the map unchanged.  The call waits once, at its
+ * end, for the voxel count and that verdict; growing the table first drains the handle's stream.  n_voxels may be NULL.
+ * malio_world_voxel_download_device: the centroids in order as n x 4 floats into device memory, with the size protocol of
+ * malio_world_register_device (d_out == NULL and cap == 0 asks the size, *n_out = the full count, at most cap written) and its
+ * device-memory contract (pointer checks before anything is enqueued, 16-byte alignment, ordered on `stream`, returns after
+ * enqueueing).
+ * malio_world_voxel_save_pcd: the centroids in order through malio_world_save_pcd's writer; MALIO_ERR_STATE on an empty map;
+ * clear != 0 then empties the map and releases its leaf.
+ * Device memory: 32 B per entry (key, sums, count; the entries at least double when they grow) and a hash of 4 B per slot at
+ * most half full, plus scratch for the scan (48 B per point).  The sort by key of a download or a save needs 32 B per voxel more;
+ * a download keeps that area until the next save, a save releases it (and writes through it, with no further copy).
+ * malio_world_voxel_info: voxels in use, entry capacity, and the device bytes the voxel map holds now, scratch included (any may
+ * be NULL). */
+int malio_world_voxel_accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, float leaf, uint64_t* n_voxels);
+int malio_world_voxel_download_device(malio_handle* h, float* d_out, uint64_t cap, uint64_t* n_out, void* stream);
+int malio_world_voxel_save_pcd(malio_handle* h, const char* path, int clear);
+int malio_world_voxel_info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* device_bytes);
 /* Host: the same PCD file from n > 0 host points (n x 4 floats {x, y, z, intensity}): the header of PCDWriter::writeBinary for
  * PointXYZINormal (FIELDS x y z intensity normal_x normal_y normal_z curvature, WIDTH = POINTS = n, HEIGHT 1, DATA binary) and
  * n packed 32-byte records with normal_x/y/z = curvature = 0.  MALIO_ERR_INVALID_ARG for n == 0, a NULL argument or a file

@@ -213,6 +213,7 @@ void destroy(malio_handle* h) {
   if (D->stream) cudaStreamSynchronize(D->stream);   // an enqueued call (malio_knn_device) may still use the buffers below
   h->deferred = nullptr;
   malio_pre::destroy(h);
+  malio_vox::destroy(h);
   malio_map::destroy(h);
   if (D->d_ids) cudaFree(D->d_ids);
   if (D->host_prof && D->host_passes)

@@ -6,6 +6,7 @@
 //   malio_b200.cu     handle lifecycle and per-scan data movement (create / destroy, scan upload, downloads)
 //   malio_preproc.cu  undistortion, voxel grid, world registration
 //   malio_mapops.cu   the device-resident map and its Add_Points / Delete_Point_Boxes replay
+//   malio_voxmap.cu   the saved map as a voxel map
 #ifndef MALIO_DEVICE_CUH_
 #define MALIO_DEVICE_CUH_
 

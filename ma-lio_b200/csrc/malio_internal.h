@@ -25,6 +25,7 @@ struct malio_handle {
   void* dev = nullptr;   // DeviceState*, owned by the CUDA TU
   void* pre = nullptr;   // PreState*, owned by malio_preproc.cu (undistortion / voxel grid buffers)
   void* mapst = nullptr; // MapOpsState*, owned by malio_mapops.cu (device-resident map replay)
+  void* voxmap = nullptr; // VoxState*, owned by malio_voxmap.cu (the saved map as a voxel map)
   // set while a call that returned after enqueueing (malio_knn_device) still has device-side results to hand over: its
   // traversal fault bit and search statistics.  The next entry point on the handle runs it first (MALIO_SETTLE).
   int (*deferred)(malio_handle* h) = nullptr;
@@ -99,7 +100,15 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
 int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap, uint32_t* n_out);
 int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uint32_t* table_off, const malio_rigid* tcomp,
                        uint32_t* n_total);
+// the device-resident undistorted clouds of slots 0..L-1 (n x 5 floats each) for malio_voxmap.cu; MALIO_ERR_STATE until every
+// slot has been undistorted, as for the dense world registration
+int world_dense_source(malio_handle* h, const float* ud[MALIO_MAX_LIDAR], uint32_t n[MALIO_MAX_LIDAR]);
 }  // namespace malio_pre
+
+// malio_voxmap.cu — the saved map as a voxel map
+namespace malio_vox {
+void destroy(malio_handle* h);
+}  // namespace malio_vox
 
 // malio_pcd.cpp — pcl::PCDWriter::writeBinary for PointXYZINormal (host)
 namespace malio_pcd {

@@ -1128,6 +1128,18 @@ int world_accumulate(malio_handle* h, const malio_pass_state* s, const float* sl
   return MALIO_OK;
 }
 
+// the dense cloud for the voxel map (malio_voxmap.cu): the undistorted clouds of slots 0..L-1 (n x 5 rows on the device) and
+// their sizes, with world_count's state error
+int world_dense_source(malio_handle* h, const float* ud[MALIO_MAX_LIDAR], uint32_t n[MALIO_MAX_LIDAR]) {
+  PreState* S;
+  if (int rc = get_state(h, S)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  uint64_t total = 0;
+  if (int rc = world_count(h, S, D, MALIO_WORLD_DENSE, total)) return rc;
+  for (int l = 0; l < h->cfg.params.n_lidar; ++l) { ud[l] = S->lid[l].d_ud; n[l] = S->lid[l].n; }
+  return MALIO_OK;
+}
+
 int world_save_pcd(malio_handle* h, const char* path, int clear) {
   PreState* S;
   if (int rc = get_state(h, S)) return rc;

@@ -130,6 +130,7 @@ EXPORTS = [
     "malio_knn_device", "malio_map_build_device", "malio_map_add_points_device",
     "malio_upload_scan_from_device", "malio_download_aux_device", "malio_map_incremental_device", "malio_world_register_device",
     "malio_undistort_device", "malio_voxel_grid_device", "malio_scan_uncertainty_resident", "malio_upload_scan_resident",
+    "malio_world_voxel_accumulate", "malio_world_voxel_download_device", "malio_world_voxel_save_pcd", "malio_world_voxel_info",
 ]
 
 
@@ -190,6 +191,10 @@ def load() -> C.CDLL:
     lib.malio_world_register.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, u32, C.POINTER(u32)]
     lib.malio_world_accumulate.argtypes = [vp, C.POINTER(PassState), vp, C.POINTER(C.c_uint64)]
     lib.malio_world_save_pcd.argtypes = [vp, C.c_char_p, i32]
+    lib.malio_world_voxel_accumulate.argtypes = [vp, vp, vp, C.c_float, vp]
+    lib.malio_world_voxel_download_device.argtypes = [vp, vp, C.c_uint64, vp, vp]
+    lib.malio_world_voxel_save_pcd.argtypes = [vp, C.c_char_p, i32]
+    lib.malio_world_voxel_info.argtypes = [vp, vp, vp, vp]
     lib.malio_write_pcd_binary.argtypes = [C.c_char_p, vp, C.c_uint64]
     lib.malio_measure.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, C.POINTER(PassStats)]
     lib.malio_download_rows.argtypes = [vp, vp, vp, u32, C.POINTER(u32)]

@@ -97,22 +97,36 @@ def write_pcd_binary(path: str, xyzi: np.ndarray):
 
 class PcdSaver:
     """The pcd_save_en branch of publish_frame_world (laserMapping.cpp:466-488) and the map save at shutdown (:1083-1091) over
-    a MeasurementModel: the library keeps pcl_wait_save on the device; the scan counter and the file names live here."""
+    a MeasurementModel: the library keeps pcl_wait_save on the device; the scan counter and the file names live here.
+    leaf (m, optional): keep the saved map as a voxel map of that leaf instead of the dense cloud (MeasurementModel.voxel_map_*):
+    the files hold one centroid per voxel; the names and the interval logic are the same."""
 
-    def __init__(self, model: "MeasurementModel", directory: str, pcd_save_interval: int):
+    def __init__(self, model: "MeasurementModel", directory: str, pcd_save_interval: int, leaf: float | None = None):
         self.model, self.directory, self.interval = model, directory, int(pcd_save_interval)
+        self.leaf = None if leaf is None else _check_leaf(leaf)
         self.scan_wait_num = 0
         self.pcd_index = 0
         self.n_wait_save = 0
 
+    def _accumulate(self, s, slot_tag) -> int:
+        if self.leaf is None:
+            return self.model.pcd_accumulate(s, slot_tag)
+        return self.model.voxel_map_accumulate(s, slot_tag, self.leaf)
+
+    def _save(self, path, clear):
+        if self.leaf is None:
+            self.model.pcd_save(path, clear=clear)
+        else:
+            self.model.voxel_map_save(path, clear=clear)
+
     def after_update(self, s, slot_tag) -> str | None:
         """Once per scan after the update.  Returns the path written, if any."""
-        self.n_wait_save = self.model.pcd_accumulate(s, slot_tag)                          # :475
+        self.n_wait_save = self._accumulate(s, slot_tag)                                   # :475
         self.scan_wait_num += 1
         if self.n_wait_save > 0 and self.interval > 0 and self.scan_wait_num > self.interval:   # :478
             self.pcd_index += 1
             path = os.path.join(self.directory, f"scans_{self.pcd_index}.pcd")
-            self.model.pcd_save(path, clear=True)                                          # :484-485
+            self._save(path, clear=True)                                                   # :484-485
             self.n_wait_save = 0
             self.scan_wait_num = 0
             return path
@@ -123,7 +137,7 @@ class PcdSaver:
         if self.n_wait_save == 0:
             return None
         path = os.path.join(self.directory, "result.pcd")
-        self.model.pcd_save(path, clear=False)
+        self._save(path, clear=False)
         return path
 
 
@@ -355,6 +369,41 @@ class MeasurementModel:
     def pcd_save(self, path: str, clear: bool):
         """pcd_writer.writeBinary(path, *pcl_wait_save) (:484, :1090); clear=True also empties the cloud (:485)."""
         self._check(self.lib.malio_world_save_pcd(self._h, os.fsencode(path), 1 if clear else 0))
+
+    # ---- the saved map as a voxel map (malio_world_voxel_*): pcl::VoxelGrid of the accumulated dense cloud, kept per voxel
+    def voxel_map_accumulate(self, s: capi.PassState | capi.State, slot_tag, leaf: float) -> int:
+        """Fold the registered dense cloud into the device's voxel map (leaf in m, fixed by the first call after creation or a
+        clearing save).  Returns the number of voxels."""
+        leaf = _check_leaf(leaf)
+        tag = np.ascontiguousarray(slot_tag, np.float32).reshape(-1)
+        if tag.shape[0] != self.n_lidar:
+            raise ValueError(f"slot_tag: {tag.shape[0]} values, expected one per LiDAR slot ({self.n_lidar})")
+        ps = s.pass_state() if isinstance(s, capi.State) else s
+        n = C.c_uint64(0)
+        self._check(self.lib.malio_world_voxel_accumulate(self._h, C.byref(ps), capi.ptr(tag), C.c_float(leaf), C.byref(n)))
+        return int(n.value)
+
+    def voxel_map_tensor(self):
+        """The voxel map's centroids as a CUDA tensor float32 (n, 4) {x, y, z, intensity} in ascending (z, y, x) voxel order,
+        allocated on the current stream.  Returns once the sort and the copy are enqueued."""
+        import torch
+        n = C.c_uint64(0)
+        st = torch.cuda.current_stream(self.device)
+        self._check(self.lib.malio_world_voxel_download_device(self._h, None, 0, C.byref(n), st.cuda_stream))
+        out = self._empty((n.value, 4), torch.float32)
+        if n.value:
+            self._check(self.lib.malio_world_voxel_download_device(self._h, _dptr(out), n.value, C.byref(n), st.cuda_stream))
+        return out
+
+    def voxel_map_save(self, path: str, clear: bool):
+        """The voxel map as a binary PCD file (the writer of pcd_save); clear=True also empties it and releases its leaf."""
+        self._check(self.lib.malio_world_voxel_save_pcd(self._h, os.fsencode(path), 1 if clear else 0))
+
+    def voxel_map_info(self) -> dict:
+        """Voxels in use, entry capacity and the device bytes the voxel map holds."""
+        v, c, b = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.malio_world_voxel_info(self._h, C.byref(v), C.byref(c), C.byref(b)))
+        return dict(n_voxels=int(v.value), capacity=int(c.value), device_bytes=int(b.value))
 
     def rearm_scan(self):
         """Reset the per-scan state of the scan already resident on the device (no host copy)."""
@@ -672,6 +721,18 @@ def pack_scan_tensor(xyz, lidar, table_idx):
     w = ids[0] | (ids[1] << 16)
     out[:, 3] = torch.where(w >= 1 << 31, w - (1 << 32), w).to(torch.int32)   # the uint32 word's bits
     return out
+
+
+def _check_leaf(leaf) -> float:
+    """A voxel leaf size in m: a finite number > 0 (ValueError otherwise), as a float32 value."""
+    try:
+        with np.errstate(over="ignore"):
+            v = float(np.float32(leaf))
+    except (TypeError, ValueError):
+        raise ValueError(f"leaf: expected a number, got {type(leaf).__name__}") from None
+    if not (np.isfinite(v) and v > 0.0):
+        raise ValueError(f"leaf: {leaf!r}, expected a finite size > 0")
+    return v
 
 
 def _dptr(t):
