@@ -125,6 +125,11 @@ int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const
   if (a.device != D->device) { h->err = std::string(what) + ": memory of another device than the handle's"; return MALIO_ERR_INVALID_ARG; }
   return MALIO_OK;
 }
+int check_device_ptrs(malio_handle* h, const DeviceState* D, std::initializer_list<DevicePtrArg> args) {
+  for (const DevicePtrArg& a : args)
+    if (a.p) { if (int rc = check_device_ptr(h, D, a.p, a.what)) return rc; }
+  return MALIO_OK;
+}
 
 int caller_enter(malio_handle* h, DeviceState* D, cudaStream_t caller) {
   CUDA_TRY(cudaEventRecord(D->ev_caller_in, caller));
@@ -246,9 +251,6 @@ void destroy(malio_handle* h) {
 
 static int ensure_point_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
   if (n <= D->capN) return MALIO_OK;
-  // ensure() frees the old buffers: a call that returned after enqueueing (the *_device outputs, malio_knn_device) may still
-  // read or write them.  Drain this handle's stream first rather than rely on cudaFree waiting for the device.
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
   uint32_t cap = n + n / 8 + 1024;
   if (cap < h->cfg.max_points) cap = h->cfg.max_points;
   int rc = 0;
@@ -279,18 +281,34 @@ static int ensure_point_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
   return MALIO_OK;
 }
 
-// table_kind: where `table` lives: host memory (malio_upload_scan*) or this device's (upload_scan_table_on_device)
-static int upload_scan_from(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
-                            cudaMemcpyKind table_kind, const uint32_t* table_off, const malio_rigid* tcomp) {
+int upload_scan_from(malio_handle* h, ScanSource from, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
+                     cudaMemcpyKind table_kind, const uint32_t* table_off, const malio_rigid* tcomp, cudaStream_t caller) {
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
   const int L = h->cfg.params.n_lidar;
   for (int l = 0; l < L; ++l)
     if (table_off[l + 1] < table_off[l] + 2) { h->err = "pose table of each LiDAR needs >= 2 entries"; return MALIO_ERR_INVALID_ARG; }
-  {   // pt.lidar indexes per-LiDAR tables on the device: reject ids outside [0, L) here (one vectorisable sweep)
+  const bool on_device = from == SCAN_DEVICE && n > 0;   // no record to read: nothing on `caller`
+  // pt.lidar indexes per-LiDAR tables on the device: reject ids outside [0, L) before anything changes
+  if (from == SCAN_HOST) {   // one vectorisable sweep
     uint32_t bad = 0;
     for (uint32_t i = 0; i < n; ++i) bad |= (uint32_t)(pts[i].lidar >= (uint16_t)L);
     if (bad) { h->err = "scan point with lidar id >= n_lidar"; return MALIO_ERR_INVALID_ARG; }
+  } else if (on_device) {
+    if (int rc = check_device_ptr(h, D, pts, "malio_upload_scan_from_device pts")) return rc;
+    if (!D->d_scan_check) {
+      CUDA_TRY(cudaMalloc((void**)&D->d_scan_check, sizeof(uint32_t)));
+      CUDA_TRY(cudaHostAlloc((void**)&D->h_scan_check, sizeof(uint32_t), cudaHostAllocDefault));
+    }
+    if (int rc = caller_enter(h, D, caller)) return rc;
+    CUDA_TRY(cudaMemsetAsync(D->d_scan_check, 0, sizeof(uint32_t), D->stream));
+    scan_lidar_check_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(reinterpret_cast<const uint32_t*>(pts), n, (uint32_t)L,
+                                                                    D->d_scan_check);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(D->h_scan_check, D->d_scan_check, sizeof(uint32_t), cudaMemcpyDeviceToHost, D->stream));
+    CUDA_TRY(cudaStreamSynchronize(D->stream));
+    D->ctr.kernel_launches += 1;
+    if (*D->h_scan_check) { h->err = "scan point with lidar id >= n_lidar"; return MALIO_ERR_INVALID_ARG; }
   }
   if (int rc = ensure_point_buffers(h, D, n > 0 ? n : 1)) return rc;
   const uint32_t n_tab = table_off[L];
@@ -298,7 +316,10 @@ static int upload_scan_from(malio_handle* h, const malio_scan_pt* pts, uint32_t 
     if (int rc = ensure(h, D->d_table, (size_t)(n_tab + 64) * TABLE_DOUBLES)) return rc;
     D->cap_table = n_tab + 64;
   }
-  if (n) CUDA_TRY(cudaMemcpyAsync(D->d_pts, pts, (size_t)n * sizeof(malio_scan_pt), cudaMemcpyHostToDevice, D->stream));
+  if (n && from != SCAN_ROOM)
+    CUDA_TRY(cudaMemcpyAsync(D->d_pts, pts, (size_t)n * sizeof(malio_scan_pt), on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                             D->stream));
+  if (on_device) { if (int rc = caller_leave(h, D, caller)) return rc; }   // the copy is the last read of the caller's records
   CUDA_TRY(cudaMemcpyAsync(D->d_table, table, (size_t)n_tab * sizeof(malio_pose_entry), table_kind, D->stream));
   reset_scan_kernel<<<(D->capN + 255) / 256, 256, 0, D->stream>>>(D->capN, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
   CUDA_TRY(cudaGetLastError());
@@ -306,79 +327,14 @@ static int upload_scan_from(malio_handle* h, const malio_scan_pt* pts, uint32_t 
   for (int l = 0; l <= MALIO_MAX_LIDAR; ++l) D->table_off[l] = (l <= L) ? table_off[l] : table_off[L];
   for (int l = 1; l < L; ++l) D->tcomp[l] = tcomp[l - 1];
   D->N = n; D->scan_ready = true; D->perm_valid = false; D->tau_valid = false; D->pass_done = false;
-  D->ctr.h2d_bytes += (uint64_t)n * sizeof(malio_scan_pt);
+  if (from == SCAN_HOST) D->ctr.h2d_bytes += (uint64_t)n * sizeof(malio_scan_pt);
   if (table_kind == cudaMemcpyHostToDevice) D->ctr.h2d_bytes += (uint64_t)n_tab * sizeof(malio_pose_entry);
   return MALIO_OK;
 }
 
 int upload_scan(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
                 const uint32_t* table_off, const malio_rigid* tcomp) {
-  return upload_scan_from(h, pts, n, table, cudaMemcpyHostToDevice, table_off, tcomp);
-}
-
-// an empty scan whose table is already in this device's memory (malio_upload_scan_resident: the table malio_scan_uncertainty*
-// built), copied device-to-device; the caller fills the points in afterwards as malio_upload_scan_device does
-int upload_scan_table_on_device(malio_handle* h, const malio_pose_entry* d_table, const uint32_t* table_off, const malio_rigid* tcomp) {
-  return upload_scan_from(h, nullptr, 0, d_table, cudaMemcpyDeviceToDevice, table_off, tcomp);
-}
-
-// malio_upload_scan with the records in device memory, ordered on the caller's stream.  The records are checked where they are
-// and the host waits for the verdict, so that a bad scan changes nothing (as upload_scan's host sweep); then they are copied
-// D2D into d_pts, because the passes keep reading d_pts over several malio_measure calls while the caller may reuse its buffer.
-int upload_scan_from_device(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
-                            const uint32_t* table_off, const malio_rigid* tcomp, cudaStream_t caller) {
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
-  const int L = h->cfg.params.n_lidar;
-  for (int l = 0; l < L; ++l)
-    if (table_off[l + 1] < table_off[l] + 2) { h->err = "pose table of each LiDAR needs >= 2 entries"; return MALIO_ERR_INVALID_ARG; }
-  if (n) { if (int rc = check_device_ptr(h, D, pts, "malio_upload_scan_from_device pts")) return rc; }
-  if (n == 0) return upload_scan(h, nullptr, 0, table, table_off, tcomp);   // no record to read: nothing on `caller`
-  if (!D->d_scan_check) {
-    CUDA_TRY(cudaMalloc((void**)&D->d_scan_check, sizeof(uint32_t)));
-    CUDA_TRY(cudaHostAlloc((void**)&D->h_scan_check, sizeof(uint32_t), cudaHostAllocDefault));
-  }
-  if (int rc = caller_enter(h, D, caller)) return rc;
-  CUDA_TRY(cudaMemsetAsync(D->d_scan_check, 0, sizeof(uint32_t), D->stream));
-  scan_lidar_check_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(reinterpret_cast<const uint32_t*>(pts), n, (uint32_t)L,
-                                                                  D->d_scan_check);
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(D->h_scan_check, D->d_scan_check, sizeof(uint32_t), cudaMemcpyDeviceToHost, D->stream));
-  // also drains every earlier enqueued call of this handle, so the buffers below may grow
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
-  D->ctr.kernel_launches += 1;
-  if (*D->h_scan_check) { h->err = "scan point with lidar id >= n_lidar"; return MALIO_ERR_INVALID_ARG; }
-  if (int rc = ensure_point_buffers(h, D, n)) return rc;
-  const uint32_t n_tab = table_off[L];
-  if (n_tab > D->cap_table) {
-    if (int rc = ensure(h, D->d_table, (size_t)(n_tab + 64) * TABLE_DOUBLES)) return rc;
-    D->cap_table = n_tab + 64;
-  }
-  CUDA_TRY(cudaMemcpyAsync(D->d_pts, pts, (size_t)n * sizeof(malio_scan_pt), cudaMemcpyDeviceToDevice, D->stream));
-  if (int rc = caller_leave(h, D, caller)) return rc;   // the copy is the last read of the caller's records
-  CUDA_TRY(cudaMemcpyAsync(D->d_table, table, (size_t)n_tab * sizeof(malio_pose_entry), cudaMemcpyHostToDevice, D->stream));
-  reset_scan_kernel<<<(D->capN + 255) / 256, 256, 0, D->stream>>>(D->capN, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
-  for (int l = 0; l <= MALIO_MAX_LIDAR; ++l) D->table_off[l] = (l <= L) ? table_off[l] : table_off[L];
-  for (int l = 1; l < L; ++l) D->tcomp[l] = tcomp[l - 1];
-  D->N = n; D->scan_ready = true; D->perm_valid = false; D->tau_valid = false; D->pass_done = false;
-  D->ctr.h2d_bytes += (uint64_t)n_tab * sizeof(malio_pose_entry);
-  return MALIO_OK;
-}
-
-// grow the per-point buffers to hold n points of a scan that is assembled on the device (malio_upload_scan_device);
-// called right after upload_scan(.., 0 points, tables): the per-scan state is already reset, a re-allocation resets it again
-int reserve_scan(malio_handle* h, uint32_t n) {
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
-  if (n > D->capN) {
-    if (int rc = ensure_point_buffers(h, D, n)) return rc;
-    reset_scan_kernel<<<(D->capN + 255) / 256, 256, 0, D->stream>>>(D->capN, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(D->stream));
-  }
-  return MALIO_OK;
+  return upload_scan_from(h, SCAN_HOST, pts, n, table, cudaMemcpyHostToDevice, table_off, tcomp, nullptr);
 }
 
 int rearm_scan(malio_handle* h) {
@@ -410,51 +366,86 @@ int get_counters(malio_handle* h, malio_counters* out) {
   return MALIO_OK;
 }
 
-int download_aux(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world) {
+// download_aux's scatter from position space into caller order, into those of the five outputs that are not NULL: host arrays
+// (on_device false) through the d_o_* staging buffers, which download_aux copies out when D->N > 0, or the caller's device
+// arrays, ordered on `caller`
+static int scatter_aux_to(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world, bool on_device,
+                          cudaStream_t caller) {
   DeviceState* D = (DeviceState*)h->dev;
   if (!D->pass_done) { h->err = "download_aux before measure"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
   const uint32_t N = D->N;
   if (N == 0) return MALIO_OK;
+  if (on_device) {
+    if (int rc = check_device_ptrs(h, D, {{normal_y, "malio_download_aux_device normal_y"}, {nn_idx, "malio_download_aux_device nn_idx"},
+                                          {nn_d2, "malio_download_aux_device nn_sqdist"}, {sel, "malio_download_aux_device selected"},
+                                          {world, "malio_download_aux_device world"}}))
+      return rc;
+    if (int rc = caller_enter(h, D, caller)) return rc;
+  } else {
+    normal_y = normal_y ? D->d_o_ny : nullptr; nn_idx = nn_idx ? D->d_o_idx : nullptr; nn_d2 = nn_d2 ? D->d_o_d2 : nullptr;
+    sel = sel ? D->d_o_sel : nullptr; world = world ? D->d_o_world : nullptr;
+  }
   const uint32_t* perm = (h->cfg.sort_queries && D->perm_valid) ? D->d_perm : nullptr;
-  scatter_aux_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(
-      perm, N, D->d_normal_y, D->d_nn_idx, D->d_nn_d2, D->d_sel, D->d_world, normal_y ? D->d_o_ny : nullptr,
-      nn_idx ? D->d_o_idx : nullptr, nn_d2 ? D->d_o_d2 : nullptr, sel ? D->d_o_sel : nullptr,
-      world ? D->d_o_world : nullptr);
+  scatter_aux_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(perm, N, D->d_normal_y, D->d_nn_idx, D->d_nn_d2, D->d_sel, D->d_world,
+                                                             normal_y, nn_idx, nn_d2, sel, world);
+  CUDA_TRY(cudaGetLastError());
+  if (on_device) { if (int rc = caller_leave(h, D, caller)) return rc; }
+  D->ctr.kernel_launches += 1;
+  return MALIO_OK;
+}
+
+int download_aux(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world) {
+  if (int rc = scatter_aux_to(h, normal_y, nn_idx, nn_d2, sel, world, false, nullptr)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  const uint32_t N = D->N;
+  if (N == 0) return MALIO_OK;
   if (normal_y) CUDA_TRY(cudaMemcpyAsync(normal_y, D->d_o_ny, (size_t)N * sizeof(float), cudaMemcpyDeviceToHost, D->stream));
   if (nn_idx) CUDA_TRY(cudaMemcpyAsync(nn_idx, D->d_o_idx, (size_t)N * MALIO_K * sizeof(uint32_t), cudaMemcpyDeviceToHost, D->stream));
   if (nn_d2) CUDA_TRY(cudaMemcpyAsync(nn_d2, D->d_o_d2, (size_t)N * MALIO_K * sizeof(float), cudaMemcpyDeviceToHost, D->stream));
   if (sel) CUDA_TRY(cudaMemcpyAsync(sel, D->d_o_sel, (size_t)N, cudaMemcpyDeviceToHost, D->stream));
   if (world) CUDA_TRY(cudaMemcpyAsync(world, D->d_o_world, (size_t)N * 3 * sizeof(float), cudaMemcpyDeviceToHost, D->stream));
-  D->ctr.kernel_launches += 1;
   D->ctr.d2h_bytes += (uint64_t)N * ((normal_y ? 4 : 0) + (nn_idx ? 20 : 0) + (nn_d2 ? 20 : 0) + (sel ? 1 : 0) + (world ? 12 : 0));
   CUDA_TRY(cudaStreamSynchronize(D->stream));
   CUDA_TRY(cudaGetLastError());
   return MALIO_OK;
 }
 
-// download_aux into the caller's device arrays: the same scatter, writing them instead of the d_o_* staging buffers, ordered
-// on the caller's stream; returns after enqueueing
-int download_aux_device(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world,
-                        cudaStream_t caller) {
-  DeviceState* D = (DeviceState*)h->dev;
-  if (!D->pass_done) { h->err = "download_aux before measure"; return MALIO_ERR_STATE; }
-  CUDA_TRY(cudaSetDevice(D->device));
-  const uint32_t N = D->N;
-  if (N == 0) return MALIO_OK;
-  const void* out[5] = {normal_y, nn_idx, nn_d2, sel, world};
-  const char* what[5] = {"malio_download_aux_device normal_y", "malio_download_aux_device nn_idx",
-                         "malio_download_aux_device nn_sqdist", "malio_download_aux_device selected",
-                         "malio_download_aux_device world"};
-  for (int k = 0; k < 5; ++k)
-    if (out[k]) { if (int rc = check_device_ptr(h, D, out[k], what[k])) return rc; }
-  const uint32_t* perm = (h->cfg.sort_queries && D->perm_valid) ? D->d_perm : nullptr;
-  if (int rc = caller_enter(h, D, caller)) return rc;
-  scatter_aux_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(perm, N, D->d_normal_y, D->d_nn_idx, D->d_nn_d2, D->d_sel, D->d_world,
-                                                             normal_y, nn_idx, nn_d2, sel, world);
+// the stand-alone search of nq > 0 queries on the committed map: the point buffers grown, the sort, the search and the
+// caller-order scatter of the lists.  Host call (on_device false): the queries go through d_queries, the lists into the d_o_*
+// staging buffers, and ev[0] / ev[1] bracket the search kernels (knn_ms, ms_device).  Device call: the queries are read and the
+// lists written where the caller keeps them, ordered on `caller`.  The scatter is counted by the callers.
+static int knn_search(malio_handle* h, DeviceState* D, const float* q, uint32_t nq, uint32_t* idx, float* d2, bool on_device,
+                      cudaStream_t caller) {
+  if (int rc = ensure_point_buffers(h, D, nq)) return rc;
+  if (!on_device && nq > D->capQ) {
+    if (int rc = ensure(h, D->d_queries, (size_t)(nq + 1024) * 3)) return rc;
+    D->capQ = nq + 1024;
+  }
+  D->scan_ready = false;   // point buffers are shared with the scan path
+  D->pass_done = false;
+  if (on_device) {
+    if (int rc = caller_enter(h, D, caller)) return rc;
+  } else {
+    CUDA_TRY(cudaMemcpyAsync(D->d_queries, q, (size_t)nq * 3 * sizeof(float), cudaMemcpyHostToDevice, D->stream));
+    q = nullptr;   // sort_queries / run_knn: D->d_queries
+    idx = idx ? D->d_o_idx : nullptr;
+    d2 = d2 ? D->d_o_d2 : nullptr;
+  }
+  PassConst pc{};
+  const uint32_t* perm = nullptr;
+  if (h->cfg.sort_queries) {
+    if (int rc = sort_queries<1>(h, D, nq, pc, 0, q)) return rc;
+    perm = D->d_perm;
+  }
+  CUDA_TRY(cudaMemsetAsync(D->d_gstats + 2, 0, 4 * sizeof(uint32_t), D->stream));
+  if (!on_device) CUDA_TRY(cudaEventRecord(D->ev[0], D->stream));
+  if (int rc = run_knn<1>(h, D, nq, nullptr, perm, pc, 0.f, q)) return rc;
+  if (!on_device) CUDA_TRY(cudaEventRecord(D->ev[1], D->stream));
+  scatter_aux_kernel<<<(nq + 255) / 256, 256, 0, D->stream>>>(perm, nq, nullptr, D->d_nn_idx, D->d_nn_d2, nullptr,
+                                                               nullptr, nullptr, idx, d2, nullptr, nullptr);
   CUDA_TRY(cudaGetLastError());
-  if (int rc = caller_leave(h, D, caller)) return rc;
-  D->ctr.kernel_launches += 1;
+  if (on_device) { if (int rc = caller_leave(h, D, caller)) return rc; }
   return MALIO_OK;
 }
 
@@ -464,27 +455,7 @@ int knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, 
   if (!D->map_ready) { h->err = "knn before upload_map"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
   if (nq == 0) return MALIO_OK;
-  if (int rc = ensure_point_buffers(h, D, nq)) return rc;
-  if (nq > D->capQ) {
-    if (int rc = ensure(h, D->d_queries, (size_t)(nq + 1024) * 3)) return rc;
-    D->capQ = nq + 1024;
-  }
-  D->scan_ready = false;   // point buffers are shared with the scan path
-  D->pass_done = false;
-  CUDA_TRY(cudaMemcpyAsync(D->d_queries, q, (size_t)nq * 3 * sizeof(float), cudaMemcpyHostToDevice, D->stream));
-  PassConst pc{};
-  const uint32_t* perm = nullptr;
-  if (h->cfg.sort_queries) {
-    if (int rc = sort_queries<1>(h, D, nq, pc, 0)) return rc;
-    perm = D->d_perm;
-  }
-  CUDA_TRY(cudaMemsetAsync(D->d_gstats + 2, 0, 4 * sizeof(uint32_t), D->stream));
-  CUDA_TRY(cudaEventRecord(D->ev[0], D->stream));
-  if (int rc = run_knn<1>(h, D, nq, nullptr, perm, pc, 0.f)) return rc;
-  CUDA_TRY(cudaEventRecord(D->ev[1], D->stream));
-  scatter_aux_kernel<<<(nq + 255) / 256, 256, 0, D->stream>>>(perm, nq, nullptr, D->d_nn_idx, D->d_nn_d2, nullptr,
-                                                               nullptr, nullptr, idx ? D->d_o_idx : nullptr,
-                                                               d2 ? D->d_o_d2 : nullptr, nullptr, nullptr);
+  if (int rc = knn_search(h, D, q, nq, idx, d2, false, nullptr)) return rc;
   if (idx) CUDA_TRY(cudaMemcpyAsync(idx, D->d_o_idx, (size_t)nq * MALIO_K * sizeof(uint32_t), cudaMemcpyDeviceToHost, D->stream));
   if (d2) CUDA_TRY(cudaMemcpyAsync(d2, D->d_o_d2, (size_t)nq * MALIO_K * sizeof(float), cudaMemcpyDeviceToHost, D->stream));
   if (int rc = fetch_knn_stats(h, D, D->stream)) return rc;
@@ -502,9 +473,8 @@ int knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, 
   return MALIO_OK;
 }
 
-// malio_knn on device memory, ordered on the caller's stream: the same sort, search and caller-order scatter, with the queries
-// read where the caller keeps them and the lists written straight into the caller's arrays.  Returns after enqueueing; the
-// statistics malio_knn waits for are copied behind the search and folded in by the next call on the handle (settle_knn_device).
+// malio_knn on device memory, ordered on the caller's stream.  Returns after enqueueing; the statistics malio_knn waits for are
+// copied behind the search and folded in by the next call on the handle (settle_knn_device).
 int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, cudaStream_t caller) {
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
@@ -517,27 +487,7 @@ int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, floa
   if (nq == 0) return MALIO_OK;
   if (h->mapst) { if (int rc = malio_map::commit(h)) return rc; }
   if (int rc = knn_fault(h, D)) return rc;   // this map already overflowed a traversal stack: no search on it is trusted
-  if (nq > D->capN) {
-    // ensure() frees the old buffers: an earlier enqueued search of this handle must be done with them first (cudaFree would
-    // wait for the whole device as well; this does not rely on it).  Nothing of this call is enqueued yet.
-    CUDA_TRY(cudaStreamSynchronize(D->stream));
-    if (int rc = ensure_point_buffers(h, D, nq)) return rc;
-  }
-  D->scan_ready = false;   // point buffers are shared with the scan path
-  D->pass_done = false;
-  if (int rc = caller_enter(h, D, caller)) return rc;
-  PassConst pc{};
-  const uint32_t* perm = nullptr;
-  if (h->cfg.sort_queries) {
-    if (int rc = sort_queries<1>(h, D, nq, pc, 0, q)) return rc;
-    perm = D->d_perm;
-  }
-  CUDA_TRY(cudaMemsetAsync(D->d_gstats + 2, 0, 4 * sizeof(uint32_t), D->stream));
-  if (int rc = run_knn<1>(h, D, nq, nullptr, perm, pc, 0.f, q)) return rc;
-  scatter_aux_kernel<<<(nq + 255) / 256, 256, 0, D->stream>>>(perm, nq, nullptr, D->d_nn_idx, D->d_nn_d2, nullptr,
-                                                               nullptr, nullptr, idx, d2, nullptr, nullptr);
-  CUDA_TRY(cudaGetLastError());
-  if (int rc = caller_leave(h, D, caller)) return rc;
+  if (int rc = knn_search(h, D, q, nq, idx, d2, true, caller)) return rc;
   if (int rc = fetch_knn_stats(h, D, D->stream)) return rc;   // behind the caller's event: the caller does not wait for it
   CUDA_TRY(cudaEventRecord(D->ev_deferred, D->stream));
   D->deferred_grid = D->grid_on;
@@ -547,7 +497,11 @@ int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, floa
   return MALIO_OK;
 }
 
-int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world) {
+// map_incremental's decision per point of the last pass, in caller order, into cls (N bytes) and world (N x 3 floats, may be
+// NULL): host arrays (on_device false) through the d_o_sel / d_o_world staging buffers of download_aux, which map_incremental
+// copies out when D->N > 0, or the caller's device arrays, ordered on `caller`
+static int map_incr_to(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world, bool on_device,
+                       cudaStream_t caller) {
   DeviceState* D = (DeviceState*)h->dev;
   if (!D->pass_done) { h->err = "map_incremental before measure"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
@@ -555,38 +509,32 @@ int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int e
   if (N == 0) return MALIO_OK;
   const bool sorted = h->cfg.sort_queries && D->perm_valid;
   const PassConst pc = make_pass_const(h, D, s);
-  // d_o_sel / d_o_world: the caller-order staging buffers of download_aux
-  map_incr_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(sorted ? D->d_pts_sorted : D->d_pts, sorted ? D->d_perm : nullptr, N, pc,
-                                                           D->d_mpts, D->d_nn_idx, D->d_normal_y, h->cfg.params.cov_threshold, fs,
-                                                           ekf_inited, D->d_o_sel, world ? D->d_o_world : nullptr);
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(cls, D->d_o_sel, (size_t)N, cudaMemcpyDeviceToHost, D->stream));
-  if (world) CUDA_TRY(cudaMemcpyAsync(world, D->d_o_world, (size_t)N * 3 * sizeof(float), cudaMemcpyDeviceToHost, D->stream));
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
-  D->ctr.kernel_launches += 1;
-  D->ctr.d2h_bytes += (uint64_t)N * (1 + (world ? 12 : 0));
-  return MALIO_OK;
-}
-
-// map_incremental into the caller's device arrays (world may be NULL), ordered on the caller's stream; returns after enqueueing
-int map_incremental_device(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world,
-                           cudaStream_t caller) {
-  DeviceState* D = (DeviceState*)h->dev;
-  if (!D->pass_done) { h->err = "map_incremental before measure"; return MALIO_ERR_STATE; }
-  CUDA_TRY(cudaSetDevice(D->device));
-  const uint32_t N = D->N;
-  if (N == 0) return MALIO_OK;
-  if (int rc = check_device_ptr(h, D, cls, "malio_map_incremental_device cls")) return rc;
-  if (world) { if (int rc = check_device_ptr(h, D, world, "malio_map_incremental_device world")) return rc; }
-  const bool sorted = h->cfg.sort_queries && D->perm_valid;
-  const PassConst pc = make_pass_const(h, D, s);
-  if (int rc = caller_enter(h, D, caller)) return rc;
+  if (on_device) {
+    if (int rc = check_device_ptr(h, D, cls, "malio_map_incremental_device cls")) return rc;
+    if (int rc = check_device_ptrs(h, D, {{world, "malio_map_incremental_device world"}})) return rc;
+    if (int rc = caller_enter(h, D, caller)) return rc;
+  } else {
+    cls = D->d_o_sel;
+    world = world ? D->d_o_world : nullptr;
+  }
   map_incr_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(sorted ? D->d_pts_sorted : D->d_pts, sorted ? D->d_perm : nullptr, N, pc,
                                                            D->d_mpts, D->d_nn_idx, D->d_normal_y, h->cfg.params.cov_threshold, fs,
                                                            ekf_inited, cls, world);
   CUDA_TRY(cudaGetLastError());
-  if (int rc = caller_leave(h, D, caller)) return rc;
+  if (on_device) { if (int rc = caller_leave(h, D, caller)) return rc; }
   D->ctr.kernel_launches += 1;
+  return MALIO_OK;
+}
+
+int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world) {
+  if (int rc = map_incr_to(h, s, fs, ekf_inited, cls, world, false, nullptr)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  const uint32_t N = D->N;
+  if (N == 0) return MALIO_OK;
+  CUDA_TRY(cudaMemcpyAsync(cls, D->d_o_sel, (size_t)N, cudaMemcpyDeviceToHost, D->stream));
+  if (world) CUDA_TRY(cudaMemcpyAsync(world, D->d_o_world, (size_t)N * 3 * sizeof(float), cudaMemcpyDeviceToHost, D->stream));
+  CUDA_TRY(cudaStreamSynchronize(D->stream));
+  D->ctr.d2h_bytes += (uint64_t)N * (1 + (world ? 12 : 0));
   return MALIO_OK;
 }
 
@@ -607,18 +555,19 @@ extern "C" int malio_upload_scan_from_device(malio_handle* h, const malio_scan_p
   MALIO_SETTLE(h);
   if (!table || !table_off) return MALIO_ERR_INVALID_ARG;
   if (h->cfg.params.n_lidar > 1 && !temporal_comp) { h->err = "temporal_comp required for L > 1"; return MALIO_ERR_INVALID_ARG; }
-  return malio_dev::upload_scan_from_device(h, d_pts, n_pts, table, table_off, temporal_comp, (cudaStream_t)stream);
+  return malio_dev::upload_scan_from(h, malio_dev::SCAN_DEVICE, d_pts, n_pts, table, cudaMemcpyHostToDevice, table_off, temporal_comp,
+                                     (cudaStream_t)stream);
 }
 extern "C" int malio_download_aux_device(malio_handle* h, float* d_normal_y, uint32_t* d_nn_idx, float* d_nn_sqdist,
                                          uint8_t* d_selected, float* d_world, void* stream) {
   if (!h) return MALIO_ERR_INVALID_ARG;
   MALIO_SETTLE(h);
-  return malio_dev::download_aux_device(h, d_normal_y, d_nn_idx, d_nn_sqdist, d_selected, d_world, (cudaStream_t)stream);
+  return malio_dev::scatter_aux_to(h, d_normal_y, d_nn_idx, d_nn_sqdist, d_selected, d_world, true, (cudaStream_t)stream);
 }
 extern "C" int malio_map_incremental_device(malio_handle* h, const malio_pass_state* s, double filter_size_map, int ekf_inited,
                                             uint8_t* d_cls, float* d_world, void* stream) {
   if (!h) return MALIO_ERR_INVALID_ARG;
   MALIO_SETTLE(h);
   if (!s || !(filter_size_map > 0.0)) return MALIO_ERR_INVALID_ARG;
-  return malio_dev::map_incremental_device(h, s, filter_size_map, ekf_inited, d_cls, d_world, (cudaStream_t)stream);
+  return malio_dev::map_incr_to(h, s, filter_size_map, ekf_inited, d_cls, d_world, true, (cudaStream_t)stream);
 }

@@ -15,6 +15,7 @@
 
 #include <cstdint>
 #include <cstring>
+#include <initializer_list>
 #include <string>
 
 #include "malio_internal.h"
@@ -232,10 +233,19 @@ struct DeviceState {
   bool p2p = false; unsigned char* d_mail = nullptr; unsigned char* mail_peer[MAIL_MAX_WORLD] = {nullptr};
 };
 
-// (re)allocate ptr for count elements; the old contents are not kept
+// (re)allocate ptr for count elements; the old contents are not kept.  Every buffer of a handle that grows by replacement grows
+// here, because a call that returned after enqueueing (the *_device calls) may still read or write the old buffer on the
+// handle's stream: that stream is drained before a live buffer is freed, rather than relying on cudaFree waiting for the
+// device.  Growth that copies the old contents over (grow_slots, world_accumulate, the voxel map's grow_table) drains the
+// stream itself before the copy.
 template <class T>
 int ensure(malio_handle* h, T*& ptr, size_t count) {
-  if (ptr) { cudaFree(ptr); ptr = nullptr; }
+  if (ptr) {
+    const DeviceState* D = static_cast<const DeviceState*>(h->dev);
+    CUDA_TRY(cudaStreamSynchronize(D->stream));
+    cudaFree(ptr);
+    ptr = nullptr;
+  }
   CUDA_TRY(cudaMalloc((void**)&ptr, count * sizeof(T)));
   return MALIO_OK;
 }
@@ -257,6 +267,9 @@ int knn_fault(malio_handle* h, const DeviceState* D);
 // MALIO_OK when p is 4-byte aligned device memory of D's device (cudaMalloc / a memory pool: what torch allocates); NULL, host,
 // pinned, managed or another device's memory -> MALIO_ERR_INVALID_ARG with h->err naming `what`
 int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const char* what);
+// check_device_ptr on each pointer of the list that is not NULL (NULL: that output is not asked for), in list order
+struct DevicePtrArg { const void* p; const char* what; };
+int check_device_ptrs(malio_handle* h, const DeviceState* D, std::initializer_list<DevicePtrArg> args);
 // D->stream waits for everything enqueued on the caller's stream so far / the caller's stream waits for D->stream
 int caller_enter(malio_handle* h, DeviceState* D, cudaStream_t caller);
 int caller_leave(malio_handle* h, DeviceState* D, cudaStream_t caller);
@@ -267,9 +280,18 @@ void comm_destroy(DeviceState* D);
 
 }  // namespace malio_devstate
 
-// malio_b200.cu, for malio_preproc.cu: malio_dev::upload_scan of an empty scan with the pose table taken from device memory
+// malio_b200.cu: the scan upload of every entry point that sets the scan.  The n records come from
+//   SCAN_HOST    host memory (malio_upload_scan*): checked by a host sweep, copied H2D
+//   SCAN_DEVICE  the caller's device memory (malio_upload_scan_from_device), ordered on `caller`: checked where they are, the
+//                host waiting for the verdict so that a bad scan changes nothing, then copied D2D into d_pts, because the
+//                passes keep reading d_pts over several malio_measure calls while the caller may reuse its buffer
+//   SCAN_ROOM    nowhere: d_pts gets room for n records, which the caller fills on the handle's stream (malio_preproc.cu's
+//                merged scan)
+// table_kind: where `table` lives, host memory or this device's (malio_upload_scan_resident)
 namespace malio_dev {
-int upload_scan_table_on_device(malio_handle* h, const malio_pose_entry* d_table, const uint32_t* table_off, const malio_rigid* tcomp);
+enum ScanSource { SCAN_HOST, SCAN_DEVICE, SCAN_ROOM };
+int upload_scan_from(malio_handle* h, ScanSource from, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
+                     cudaMemcpyKind table_kind, const uint32_t* table_off, const malio_rigid* tcomp, cudaStream_t caller);
 }
 
 #endif  // MALIO_DEVICE_CUH_

@@ -58,15 +58,7 @@ int knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, 
 // device-memory queries and lists, ordered on the caller's stream (a cudaStream_t); malio_b200.cu
 int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, struct CUstream_st* caller);
 int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world);
-// the scan upload and the per-point outputs on device memory, ordered on the caller's stream; malio_b200.cu
-int upload_scan_from_device(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
-                            const uint32_t* table_off, const malio_rigid* tcomp, struct CUstream_st* caller);
-int download_aux_device(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world,
-                        struct CUstream_st* caller);
-int map_incremental_device(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world,
-                           struct CUstream_st* caller);
 int rearm_scan(malio_handle* h);
-int reserve_scan(malio_handle* h, uint32_t n);
 int grow_slots(malio_handle* h, uint32_t n, uint32_t keep);
 int index_from_slots(malio_handle* h, uint32_t n_slots, const float box[6]);
 int get_counters(malio_handle* h, malio_counters* out);

@@ -1375,9 +1375,6 @@ namespace malio_dev {
 
 static int ensure_map_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
   if (n <= D->cap_nodes && D->d_nodes) return MALIO_OK;   // (slot mode grows d_mpts / d_cov only: no tree records there)
-  // ensure() frees the old map: a call that returned after enqueueing (malio_knn_device, malio_map_incremental_device) may
-  // still read it.  Drain this handle's stream first rather than rely on cudaFree waiting for the device.
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
   uint32_t cap = n + n / 8 + 1024;
   if (cap < h->cfg.max_map_nodes) cap = h->cfg.max_map_nodes;
   if (int rc = ensure(h, D->d_nodes, (size_t)cap * 4)) return rc;

@@ -431,8 +431,7 @@ static int check_device_points(malio_handle* h, const float* xyz, const float* n
   if (n == 0) return MALIO_OK;
   if (int rc = check_device_ptr(h, D, xyz, "xyz")) return rc;
   if (int rc = check_device_ptr(h, D, normal_y, "normal_y")) return rc;
-  if (ids) { if (int rc = check_device_ptr(h, D, ids, "ids")) return rc; }
-  return MALIO_OK;
+  return check_device_ptrs(h, D, {{ids, "ids"}});
 }
 int build_device(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, cudaStream_t caller) {
   if (int rc = check_device_points(h, xyz, normal_y, ids, n)) return rc;

@@ -585,11 +585,9 @@ __global__ void world_kernel(const float* __restrict__ ud, int slot, float tag, 
 
 constexpr uint64_t WORLD_ACC_MIN = 1u << 16;   // first capacity of the accumulated cloud (points); it doubles from there
 
-// d_wstage large enough for n points.  ensure() frees the old buffer, which a malio_world_register_device that returned after
-// enqueueing may still use: the stream is drained first rather than relying on cudaFree waiting for the device.
+// d_wstage large enough for n points
 int grow_wstage(malio_handle* h, PreState* S, uint64_t n) {
   if (n <= S->cap_wstage) return MALIO_OK;
-  CUDA_TRY(cudaStreamSynchronize(S->stream));
   const uint64_t c = n + n / 8 + 1024;
   if (int rc = ensure(h, S->d_wstage, c)) { S->cap_wstage = 0; return rc; }
   S->cap_wstage = c;
@@ -700,9 +698,6 @@ int undistort_prepare_slot(malio_handle* h, PreState* S, PreLidar& L, uint32_t n
   L.ud_valid = false;
   S->table_resident = false;   // the table in d_uout was built from this slot's previous undistortion
   if (n > L.cap) {
-    // ensure() frees the slot's buffers: a call that returned after enqueueing (malio_world_register_device,
-    // malio_voxel_grid_device) may still read d_ud.  Drain the stream first rather than rely on cudaFree waiting for the device.
-    CUDA_TRY(cudaStreamSynchronize(S->stream));
     const uint32_t cap = n + n / 8 + 1024;
     if (int rc = ensure(h, L.d_raw, cap)) return rc;
     if (int rc = ensure(h, L.d_ud, (size_t)cap * 5)) return rc;
@@ -813,11 +808,10 @@ int undistort_device(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32
   if (int rc = undistort_check_args(h, lidar, a)) return rc;
   if (n) {
     if (int rc = check_device_ptr(h, D, pts, "malio_undistort_device pts")) return rc;
-    if (cloud) { if (int rc = check_device_ptr(h, D, cloud, "malio_undistort_device cloud")) return rc; }
-    if (idx) { if (int rc = check_device_ptr(h, D, idx, "malio_undistort_device idx")) return rc; }
-    if (ok) { if (int rc = check_device_ptr(h, D, ok, "malio_undistort_device ok")) return rc; }
-    if (pop_point && a->n_cov) { if (int rc = check_device_ptr(h, D, pop_point, "malio_undistort_device pop_point")) return rc; }
-    if (pose) { if (int rc = check_device_ptr(h, D, pose, "malio_undistort_device pose")) return rc; }
+    if (int rc = check_device_ptrs(h, D, {{cloud, "malio_undistort_device cloud"}, {idx, "malio_undistort_device idx"},
+                                          {ok, "malio_undistort_device ok"}, {a->n_cov ? pop_point : nullptr, "malio_undistort_device pop_point"},
+                                          {pose, "malio_undistort_device pose"}}))
+      return rc;
   }
   PreLidar& L = S->lid[lidar];
   cudaStream_t st = S->stream;
@@ -855,8 +849,6 @@ static int voxel_grid_run(malio_handle* h, PreState* S, DeviceState* D, PreLidar
   if (n_out) *n_out = 0;
   if (n == 0) { L.ds_valid = true; return MALIO_OK; }
   if (n > S->cap_vpts) {
-    // ensure() frees the scratch a malio_voxel_grid_device that returned after enqueueing may still use: drain the stream first
-    CUDA_TRY(cudaStreamSynchronize(st));
     const uint32_t cap = n + n / 8 + 1024;
     if (int rc = ensure(h, S->d_vidx, cap)) return rc;
     if (int rc = ensure(h, S->d_vtmp, cap)) return rc;
@@ -975,8 +967,8 @@ int voxel_grid_device(malio_handle* h, int lidar, const float* in, uint32_t n, f
   const float* d_in = in;
   if (!in) { if (int rc = voxel_slot_input(h, L, d_in, n)) return rc; }
   if (n) {
-    if (in) { if (int rc = check_device_ptr(h, D, in, "malio_voxel_grid_device in")) return rc; }
-    if (out && out_cap) { if (int rc = check_device_ptr(h, D, out, "malio_voxel_grid_device out")) return rc; }
+    if (int rc = check_device_ptrs(h, D, {{in, "malio_voxel_grid_device in"}, {out_cap ? out : nullptr, "malio_voxel_grid_device out"}}))
+      return rc;
     if (int rc = caller_enter(h, D, caller)) return rc;
   }
   // an early return below (no finite point, MALIO_ERR_CAPACITY) comes after a wait for the last kernel that read `in`
@@ -997,11 +989,9 @@ static int merge_scan(malio_handle* h, PreState* S, DeviceState* D, const malio_
     if (!S->lid[l].ds_valid) { h->err = "upload_scan_device: no down-sampled cloud for a LiDAR (call malio_voxel_grid first)"; return MALIO_ERR_STATE; }
     total += S->lid[l].n_ds;
   }
-  // size the scan buffers and tables through the regular entry point (no points copied), then fill d_pts on the device
-  if (int rc = table_on_device ? malio_dev::upload_scan_table_on_device(h, table, table_off, tcomp)
-                               : malio_dev::upload_scan(h, nullptr, 0, table, table_off, tcomp))
+  if (int rc = malio_dev::upload_scan_from(h, malio_dev::SCAN_ROOM, nullptr, total, table,
+                                           table_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, table_off, tcomp, nullptr))
     return rc;
-  if (int rc = malio_dev::reserve_scan(h, total)) return rc;
   uint32_t at = 0;
   for (int l = 0; l < Ln; ++l) {
     const uint32_t m = S->lid[l].n_ds;
@@ -1010,7 +1000,6 @@ static int merge_scan(malio_handle* h, PreState* S, DeviceState* D, const malio_
   }
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaStreamSynchronize(S->stream));
-  D->N = total;
   D->ctr.kernel_launches += Ln;
   if (n_total) *n_total = total;
   return MALIO_OK;
@@ -1038,31 +1027,13 @@ int upload_scan_resident(malio_handle* h, uint32_t* n_total) {
   return merge_scan(h, S, D, (const malio_pose_entry*)S->d_uout, true, S->res_table_off, S->res_tcomp, n_total);
 }
 
-int world_register(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out, uint32_t cap,
-                   uint32_t* n_out) {
-  PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
-  uint64_t n = 0;
-  if (int rc = world_count(h, S, D, source, n)) return rc;
-  if (n > 0xFFFFFFFFull) { h->err = "world registration: more than 2^32-1 points"; return MALIO_ERR_CAPACITY; }
-  *n_out = (uint32_t)n;
-  const uint64_t k = n < cap ? n : cap;
-  if (!out || k == 0) return MALIO_OK;
-  if (int rc = grow_wstage(h, S, n)) return rc;
-  if (int rc = world_launch(h, S, D, s, source, slot_tag, S->d_wstage)) return rc;
-  CUDA_TRY(cudaMemcpyAsync(out, S->d_wstage, (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, S->stream));
-  CUDA_TRY(cudaStreamSynchronize(S->stream));
-  D->ctr.d2h_bytes += k * sizeof(float4);
-  return MALIO_OK;
-}
-
-// world_register into the caller's device array (16-byte aligned: world_kernel stores float4), ordered on the caller's stream;
-// returns after enqueueing.  world_kernel writes the caller's array directly when all n points fit, and d_wstage otherwise,
-// followed by a D2D copy of the first cap points.
-int world_register_device(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out, uint32_t cap,
-                          uint32_t* n_out, cudaStream_t caller) {
+// the registration of `source` for world_register: *n_out = its point count n, and the first k = min(n, cap) points go to
+// `out`.  Host array (on_device false): world_kernel writes d_wstage, which world_register copies out when *k > 0.  Device
+// array (16-byte aligned: world_kernel stores float4), ordered on `caller`: world_kernel writes it directly when all n points
+// fit, and d_wstage otherwise, followed by a D2D copy of the first k points.
+static int world_register_to(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out, uint32_t cap,
+                             uint32_t* n_out, bool on_device, cudaStream_t caller, uint64_t* k_out) {
+  *k_out = 0;
   PreState* S;
   if (int rc = get_state(h, S)) return rc;
   DeviceState* D = (DeviceState*)h->dev;
@@ -1071,7 +1042,7 @@ int world_register_device(malio_handle* h, const malio_pass_state* s, int source
   if (int rc = world_count(h, S, D, source, n)) return rc;
   if (n > 0xFFFFFFFFull) { h->err = "world registration: more than 2^32-1 points"; return MALIO_ERR_CAPACITY; }
   const uint64_t k = n < cap ? n : cap;
-  if (out && k) {
+  if (on_device && out && k) {
     if (int rc = check_device_ptr(h, D, out, "malio_world_register_device out")) return rc;
     if (reinterpret_cast<uintptr_t>(out) & 15u) {
       h->err = "malio_world_register_device out: not 16-byte aligned (the points are stored as float4)";
@@ -1080,12 +1051,28 @@ int world_register_device(malio_handle* h, const malio_pass_state* s, int source
   }
   *n_out = (uint32_t)n;
   if (!out || k == 0) return MALIO_OK;
-  const bool whole = k == n;
+  const bool whole = on_device && k == n;
   if (!whole) { if (int rc = grow_wstage(h, S, n)) return rc; }
-  if (int rc = caller_enter(h, D, caller)) return rc;
+  if (on_device) { if (int rc = caller_enter(h, D, caller)) return rc; }
   if (int rc = world_launch(h, S, D, s, source, slot_tag, whole ? reinterpret_cast<float4*>(out) : S->d_wstage)) return rc;
-  if (!whole) CUDA_TRY(cudaMemcpyAsync(out, S->d_wstage, (size_t)k * sizeof(float4), cudaMemcpyDeviceToDevice, S->stream));
-  if (int rc = caller_leave(h, D, caller)) return rc;   // (S->stream is D->stream)
+  if (on_device) {
+    if (!whole) CUDA_TRY(cudaMemcpyAsync(out, S->d_wstage, (size_t)k * sizeof(float4), cudaMemcpyDeviceToDevice, S->stream));
+    if (int rc = caller_leave(h, D, caller)) return rc;   // (S->stream is D->stream)
+  }
+  *k_out = k;
+  return MALIO_OK;
+}
+
+int world_register(malio_handle* h, const malio_pass_state* s, int source, const float* slot_tag, float* out, uint32_t cap,
+                   uint32_t* n_out) {
+  uint64_t k = 0;
+  if (int rc = world_register_to(h, s, source, slot_tag, out, cap, n_out, false, nullptr, &k)) return rc;
+  if (k == 0) return MALIO_OK;
+  PreState* S = (PreState*)h->pre;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaMemcpyAsync(out, S->d_wstage, (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, S->stream));
+  CUDA_TRY(cudaStreamSynchronize(S->stream));
+  D->ctr.d2h_bytes += k * sizeof(float4);
   return MALIO_OK;
 }
 
@@ -1310,7 +1297,8 @@ extern "C" int malio_world_register_device(malio_handle* h, const malio_pass_sta
   if (!s || !n_out || (cap && !d_out)) return MALIO_ERR_INVALID_ARG;
   if (source != MALIO_WORLD_DOWNSAMPLED && source != MALIO_WORLD_DENSE) { h->err = "world register: unknown source"; return MALIO_ERR_INVALID_ARG; }
   if (source == MALIO_WORLD_DENSE && !slot_tag) { h->err = "world register: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
-  return malio_pre::world_register_device(h, s, source, slot_tag, d_out, cap, n_out, (cudaStream_t)stream);
+  uint64_t k = 0;
+  return malio_pre::world_register_to(h, s, source, slot_tag, d_out, cap, n_out, true, (cudaStream_t)stream, &k);
 }
 extern "C" int malio_world_accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, uint64_t* n_total) {
   if (!h || !s) return MALIO_ERR_INVALID_ARG;

@@ -231,11 +231,9 @@ int get_state(malio_handle* h, VoxState*& V) {
   return MALIO_OK;
 }
 
-// CUB's temporary storage for at least t bytes, and the sort area for n rows.  ensure() frees the old buffers, which a
-// download that returned after enqueueing may still use: the stream is drained first.
+// CUB's temporary storage for at least t bytes, and the sort area for n rows
 int grow_temp(malio_handle* h, VoxState* V, DeviceState* D, size_t t) {
   if (t <= V->cap_temp) return MALIO_OK;
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
   t += t / 8 + 4096;
   V->cap_temp = 0;
   if (int rc = ensure(h, V->d_temp, t)) return rc;
@@ -244,7 +242,6 @@ int grow_temp(malio_handle* h, VoxState* V, DeviceState* D, size_t t) {
 }
 int grow_sort(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
   if (n > V->cap_s) {
-    CUDA_TRY(cudaStreamSynchronize(D->stream));
     const uint64_t c = n + n / 8 + 1024;
     V->cap_s = 0;
     if (int rc = ensure(h, V->d_sort, c * SORT_ROW)) return rc;
@@ -258,7 +255,6 @@ int grow_sort(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
 // the run scratch for the n points of a scan
 int grow_runs(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
   if (n > V->cap_p) {
-    CUDA_TRY(cudaStreamSynchronize(D->stream));
     const uint64_t c = n + n / 8 + 1024;
     V->cap_p = 0;
     uint32_t** u[] = {&V->d_head, &V->d_run, &V->d_rent, &V->d_new};

@@ -33,7 +33,6 @@ int download_aux(malio_handle*, float*, uint32_t*, float*, uint8_t*, float*) { r
 int knn(malio_handle*, const float*, uint32_t, uint32_t*, float*, float*) { return MALIO_ERR_STATE; }
 int map_incremental(malio_handle*, const malio_pass_state*, double, int, uint8_t*, float*) { return MALIO_ERR_STATE; }
 int rearm_scan(malio_handle*) { return MALIO_OK; }
-int reserve_scan(malio_handle*, uint32_t) { return MALIO_OK; }
 int get_counters(malio_handle*, malio_counters* out) { std::memset(out, 0, sizeof(*out)); return MALIO_OK; }
 int set_timing(malio_handle*, int) { return MALIO_OK; }
 int comm_init(malio_handle*, const uint8_t*, int, int) { return MALIO_ERR_NCCL; }
