@@ -180,28 +180,29 @@ int create(malio_handle* h) {
   CUDA_TRY(cudaEventCreateWithFlags(&D->ev_caller_out, cudaEventDisableTiming));
   CUDA_TRY(cudaEventCreateWithFlags(&D->ev_deferred, cudaEventDisableTiming));
   for (auto& e : D->ev) CUDA_TRY(cudaEventCreate(&e));
-  CUDA_TRY(cudaMalloc((void**)&D->d_counters, 4 * sizeof(uint32_t)));
+  const cudaStream_t st = D->stream;
+  if (int rc = D->d_counters.allocate(h, st, 4)) return rc;
   CUDA_TRY(cudaMemset(D->d_counters, 0, 4 * sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_mmkey, 8 * sizeof(unsigned long long)));
+  if (int rc = D->d_mmkey.allocate(h, st, 8)) return rc;
   {
     const unsigned long long init[8] = {dkey(1000.0), dkey(-0.0), dkey(9999.0), dkey(-0.0), dkey(1000.0), dkey(-0.0), dkey(9999.0), dkey(-0.0)};
     CUDA_TRY(cudaMemcpy(D->d_mmkey, init, sizeof(init), cudaMemcpyHostToDevice));
   }
-  CUDA_TRY(cudaMalloc((void**)&D->d_res, MALIO_RED_DOUBLES * sizeof(double)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_cand, 4 * sizeof(unsigned long long)));   // [0] candidates, [1..3] multi-GPU exchange waits (ns, ns, passes)
+  if (int rc = D->d_res.allocate(h, st, MALIO_RED_DOUBLES)) return rc;
+  if (int rc = D->d_cand.allocate(h, st, 4)) return rc;   // [0] candidates, [1..3] multi-GPU exchange waits (ns, ns, passes)
   CUDA_TRY(cudaMemset(D->d_cand, 0, 4 * sizeof(unsigned long long)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_gstats, 8 * sizeof(uint32_t)));
+  if (int rc = D->d_gstats.allocate(h, st, 8)) return rc;
   CUDA_TRY(cudaMemset(D->d_gstats, 0, 8 * sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_hist, SORT_BINS * sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_offs, SORT_BINS * sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_cursor, SORT_BINS * sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_btot, SCAN_BLOCKS * sizeof(uint32_t)));
+  if (int rc = D->d_hist.allocate(h, st, SORT_BINS)) return rc;
+  if (int rc = D->d_offs.allocate(h, st, SORT_BINS)) return rc;
+  if (int rc = D->d_cursor.allocate(h, st, SORT_BINS)) return rc;
+  if (int rc = D->d_btot.allocate(h, st, SCAN_BLOCKS)) return rc;
   CUDA_TRY(cudaMemset(D->d_hist, 0, SORT_BINS * sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_rows, (size_t)ROWS_DOUBLES * (1 + MAIL_MAX_WORLD) * sizeof(double)));   // own rows | gathered rows of all ranks
+  if (int rc = D->d_rows.allocate(h, st, (size_t)ROWS_DOUBLES * (1 + MAIL_MAX_WORLD))) return rc;   // own rows | gathered rows of all ranks
   // pinned + mapped: [0, RED) result | +0..3 min/max keys | +4..7 k-NN list statistics | +8 pass sequence flag | +16.. rows
-  CUDA_TRY(cudaHostAlloc((void**)&D->h_res, (MALIO_RED_DOUBLES + 16 + MALIO_MAX_DOF * 25) * sizeof(double), cudaHostAllocMapped));
+  if (int rc = D->h_res.allocate(h, MALIO_RED_DOUBLES + 16 + MALIO_MAX_DOF * 25, cudaHostAllocMapped)) return rc;
   std::memset(D->h_res, 0, (MALIO_RED_DOUBLES + 16) * sizeof(double));
-  CUDA_TRY(cudaHostGetDevicePointer((void**)&D->h_res_dev, D->h_res, 0));
+  CUDA_TRY(cudaHostGetDevicePointer((void**)&D->h_res_dev, D->h_res.data(), 0));
   D->h_gstats = reinterpret_cast<uint32_t*>(D->h_res + MALIO_RED_DOUBLES + 4);
   std::memset(D->h_gstats, 0, 8 * sizeof(uint32_t));
   if (int rc = pass_init(h, D)) return rc;
@@ -220,21 +221,11 @@ void destroy(malio_handle* h) {
   malio_pre::destroy(h);
   malio_vox::destroy(h);
   malio_map::destroy(h);
-  if (D->d_ids) cudaFree(D->d_ids);
   if (D->host_prof && D->host_passes)
     fprintf(stderr, "[malio] passes %llu: host launch %.1f us/pass, host wait-for-device %.1f us/pass\n",
             (unsigned long long)D->host_passes, D->host_launch_us / D->host_passes, D->host_wait_us / D->host_passes);
   cudaSetDevice(D->device);
   comm_destroy(D);
-  void* ptrs[] = {D->d_nodes, D->d_cov, D->d_mpts, D->d_parent, D->d_arrived, D->d_pts, D->d_pts_sorted, D->d_perm, D->d_keys16, D->d_hist, D->d_offs, D->d_cursor, D->d_btot, D->d_tmp_ids,
-                  D->d_table, D->d_nn_idx, D->d_nn_d2, D->d_sel, D->d_world, D->d_plane, D->d_ucov, D->d_tau, D->d_tau2, D->d_pd2, D->d_rows12, D->d_lid8,
-                  D->d_normal_y, D->d_o_ny, D->d_o_idx, D->d_o_d2, D->d_o_sel, D->d_o_world,
-                  D->d_counters, D->d_mmkey, D->d_block_red, D->d_res, D->d_rows, D->d_queries,
-                  D->d_cell_start, D->d_cell_cnt, D->d_cell_of, D->d_ctot, D->d_cbase, D->d_cell_pts, D->d_fb_list, D->d_gstats, D->d_bar, D->d_cand,
-                  D->d_scan_check};
-  for (void* p : ptrs) if (p) cudaFree(p);
-  if (D->h_res) cudaFreeHost(D->h_res);
-  if (D->h_scan_check) cudaFreeHost(D->h_scan_check);
   for (auto& e : D->ev) if (e) cudaEventDestroy(e);
   if (D->stream2) { cudaStreamSynchronize(D->stream2); cudaStreamDestroy(D->stream2); }
   if (D->stream3) { cudaStreamSynchronize(D->stream3); cudaStreamDestroy(D->stream3); }
@@ -245,40 +236,21 @@ void destroy(malio_handle* h) {
   if (D->ev_tau) cudaEventDestroy(D->ev_tau);
   for (cudaEvent_t e : {D->ev_caller_in, D->ev_caller_out, D->ev_deferred}) if (e) cudaEventDestroy(e);
   if (D->stream) cudaStreamDestroy(D->stream);
-  delete D;
+  delete D;   // the buffers go back with it
   h->dev = nullptr;
 }
 
 static int ensure_point_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
-  if (n <= D->capN) return MALIO_OK;
+  if (n <= D->d_pts.size()) return MALIO_OK;
   uint32_t cap = n + n / 8 + 1024;
   if (cap < h->cfg.max_points) cap = h->cfg.max_points;
-  int rc = 0;
-  if ((rc = ensure(h, D->d_pts, cap))) return rc;
-  if ((rc = ensure(h, D->d_pts_sorted, cap))) return rc;
-  if ((rc = ensure(h, D->d_perm, cap))) return rc;
-  if ((rc = ensure(h, D->d_keys16, cap))) return rc;
-  if ((rc = ensure(h, D->d_tmp_ids, cap))) return rc;
-  if ((rc = ensure(h, D->d_nn_idx, (size_t)cap * MALIO_K))) return rc;
-  if ((rc = ensure(h, D->d_nn_d2, (size_t)cap * MALIO_K))) return rc;
-  if ((rc = ensure(h, D->d_sel, cap))) return rc;
-  if ((rc = ensure(h, D->d_world, cap))) return rc;
-  if ((rc = ensure(h, D->d_plane, cap))) return rc;
-  if ((rc = ensure(h, D->d_ucov, cap))) return rc;
-  if ((rc = ensure(h, D->d_tau, cap))) return rc;
-  if ((rc = ensure(h, D->d_tau2, cap))) return rc;
-  if ((rc = ensure(h, D->d_pd2, cap))) return rc;
-  if ((rc = ensure(h, D->d_rows12, (size_t)cap * 12))) return rc;
-  if ((rc = ensure(h, D->d_lid8, cap))) return rc;
-  if ((rc = ensure(h, D->d_normal_y, cap))) return rc;
-  if ((rc = ensure(h, D->d_o_ny, cap))) return rc;
-  if ((rc = ensure(h, D->d_o_idx, (size_t)cap * MALIO_K))) return rc;
-  if ((rc = ensure(h, D->d_o_d2, (size_t)cap * MALIO_K))) return rc;
-  if ((rc = ensure(h, D->d_o_sel, cap))) return rc;
-  if ((rc = ensure(h, D->d_o_world, (size_t)cap * 3))) return rc;
-  if ((rc = ensure(h, D->d_fb_list, cap))) return rc;
-  D->capN = cap;
-  return MALIO_OK;
+  const size_t capK = (size_t)cap * MALIO_K;
+  return malio_buf::allocate_group(h, D->stream, {{D->d_pts, cap}, {D->d_pts_sorted, cap}, {D->d_perm, cap}, {D->d_keys16, cap},
+                                                  {D->d_tmp_ids, cap}, {D->d_nn_idx, capK}, {D->d_nn_d2, capK}, {D->d_sel, cap},
+                                                  {D->d_world, cap}, {D->d_plane, cap}, {D->d_ucov, cap}, {D->d_tau, cap},
+                                                  {D->d_tau2, cap}, {D->d_pd2, cap}, {D->d_rows12, (size_t)cap * 12}, {D->d_lid8, cap},
+                                                  {D->d_normal_y, cap}, {D->d_o_ny, cap}, {D->d_o_idx, capK}, {D->d_o_d2, capK},
+                                                  {D->d_o_sel, cap}, {D->d_o_world, (size_t)cap * 3}, {D->d_fb_list, cap}});
 }
 
 int upload_scan_from(malio_handle* h, ScanSource from, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
@@ -296,10 +268,8 @@ int upload_scan_from(malio_handle* h, ScanSource from, const malio_scan_pt* pts,
     if (bad) { h->err = "scan point with lidar id >= n_lidar"; return MALIO_ERR_INVALID_ARG; }
   } else if (on_device) {
     if (int rc = check_device_ptr(h, D, pts, "malio_upload_scan_from_device pts")) return rc;
-    if (!D->d_scan_check) {
-      CUDA_TRY(cudaMalloc((void**)&D->d_scan_check, sizeof(uint32_t)));
-      CUDA_TRY(cudaHostAlloc((void**)&D->h_scan_check, sizeof(uint32_t), cudaHostAllocDefault));
-    }
+    if (!D->d_scan_check) { if (int rc = D->d_scan_check.allocate(h, D->stream, 1)) return rc; }
+    if (!D->h_scan_check) { if (int rc = D->h_scan_check.allocate(h, 1)) return rc; }
     if (int rc = caller_enter(h, D, caller)) return rc;
     CUDA_TRY(cudaMemsetAsync(D->d_scan_check, 0, sizeof(uint32_t), D->stream));
     scan_lidar_check_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(reinterpret_cast<const uint32_t*>(pts), n, (uint32_t)L,
@@ -312,16 +282,16 @@ int upload_scan_from(malio_handle* h, ScanSource from, const malio_scan_pt* pts,
   }
   if (int rc = ensure_point_buffers(h, D, n > 0 ? n : 1)) return rc;
   const uint32_t n_tab = table_off[L];
-  if (n_tab > D->cap_table) {
-    if (int rc = ensure(h, D->d_table, (size_t)(n_tab + 64) * TABLE_DOUBLES)) return rc;
-    D->cap_table = n_tab + 64;
+  if (n_tab > D->d_table.size() / TABLE_DOUBLES) {
+    if (int rc = D->d_table.allocate(h, D->stream, (size_t)(n_tab + 64) * TABLE_DOUBLES)) return rc;
   }
   if (n && from != SCAN_ROOM)
     CUDA_TRY(cudaMemcpyAsync(D->d_pts, pts, (size_t)n * sizeof(malio_scan_pt), on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
                              D->stream));
   if (on_device) { if (int rc = caller_leave(h, D, caller)) return rc; }   // the copy is the last read of the caller's records
   CUDA_TRY(cudaMemcpyAsync(D->d_table, table, (size_t)n_tab * sizeof(malio_pose_entry), table_kind, D->stream));
-  reset_scan_kernel<<<(D->capN + 255) / 256, 256, 0, D->stream>>>(D->capN, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
+  const uint32_t cap = (uint32_t)D->d_pts.size();
+  reset_scan_kernel<<<(cap + 255) / 256, 256, 0, D->stream>>>(cap, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaStreamSynchronize(D->stream));
   for (int l = 0; l <= MALIO_MAX_LIDAR; ++l) D->table_off[l] = (l <= L) ? table_off[l] : table_off[L];
@@ -341,7 +311,8 @@ int rearm_scan(malio_handle* h) {
   DeviceState* D = (DeviceState*)h->dev;
   if (!D->scan_ready) { h->err = "rearm_scan before upload_scan"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
-  reset_scan_kernel<<<(D->capN + 255) / 256, 256, 0, D->stream>>>(D->capN, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
+  const uint32_t cap = (uint32_t)D->d_pts.size();
+  reset_scan_kernel<<<(cap + 255) / 256, 256, 0, D->stream>>>(cap, D->d_sel, D->d_normal_y, D->d_nn_idx, D->d_gstats);
   CUDA_TRY(cudaGetLastError());
   D->perm_valid = false; D->tau_valid = false; D->pass_done = false;
   return MALIO_OK;
@@ -383,10 +354,10 @@ static int scatter_aux_to(malio_handle* h, float* normal_y, uint32_t* nn_idx, fl
       return rc;
     if (int rc = caller_enter(h, D, caller)) return rc;
   } else {
-    normal_y = normal_y ? D->d_o_ny : nullptr; nn_idx = nn_idx ? D->d_o_idx : nullptr; nn_d2 = nn_d2 ? D->d_o_d2 : nullptr;
-    sel = sel ? D->d_o_sel : nullptr; world = world ? D->d_o_world : nullptr;
+    normal_y = normal_y ? D->d_o_ny.data() : nullptr; nn_idx = nn_idx ? D->d_o_idx.data() : nullptr; nn_d2 = nn_d2 ? D->d_o_d2.data() : nullptr;
+    sel = sel ? D->d_o_sel.data() : nullptr; world = world ? D->d_o_world.data() : nullptr;
   }
-  const uint32_t* perm = (h->cfg.sort_queries && D->perm_valid) ? D->d_perm : nullptr;
+  const uint32_t* perm = (h->cfg.sort_queries && D->perm_valid) ? D->d_perm.data() : nullptr;
   scatter_aux_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(perm, N, D->d_normal_y, D->d_nn_idx, D->d_nn_d2, D->d_sel, D->d_world,
                                                              normal_y, nn_idx, nn_d2, sel, world);
   CUDA_TRY(cudaGetLastError());
@@ -418,9 +389,8 @@ int download_aux(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d
 static int knn_search(malio_handle* h, DeviceState* D, const float* q, uint32_t nq, uint32_t* idx, float* d2, bool on_device,
                       cudaStream_t caller) {
   if (int rc = ensure_point_buffers(h, D, nq)) return rc;
-  if (!on_device && nq > D->capQ) {
-    if (int rc = ensure(h, D->d_queries, (size_t)(nq + 1024) * 3)) return rc;
-    D->capQ = nq + 1024;
+  if (!on_device && nq > D->d_queries.size() / 3) {
+    if (int rc = D->d_queries.allocate(h, D->stream, (size_t)(nq + 1024) * 3)) return rc;
   }
   D->scan_ready = false;   // point buffers are shared with the scan path
   D->pass_done = false;
@@ -429,8 +399,8 @@ static int knn_search(malio_handle* h, DeviceState* D, const float* q, uint32_t 
   } else {
     CUDA_TRY(cudaMemcpyAsync(D->d_queries, q, (size_t)nq * 3 * sizeof(float), cudaMemcpyHostToDevice, D->stream));
     q = nullptr;   // sort_queries / run_knn: D->d_queries
-    idx = idx ? D->d_o_idx : nullptr;
-    d2 = d2 ? D->d_o_d2 : nullptr;
+    idx = idx ? D->d_o_idx.data() : nullptr;
+    d2 = d2 ? D->d_o_d2.data() : nullptr;
   }
   PassConst pc{};
   const uint32_t* perm = nullptr;
@@ -515,9 +485,9 @@ static int map_incr_to(malio_handle* h, const malio_pass_state* s, double fs, in
     if (int rc = caller_enter(h, D, caller)) return rc;
   } else {
     cls = D->d_o_sel;
-    world = world ? D->d_o_world : nullptr;
+    world = world ? D->d_o_world.data() : nullptr;
   }
-  map_incr_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(sorted ? D->d_pts_sorted : D->d_pts, sorted ? D->d_perm : nullptr, N, pc,
+  map_incr_kernel<<<(N + 255) / 256, 256, 0, D->stream>>>(sorted ? D->d_pts_sorted.data() : D->d_pts.data(), sorted ? D->d_perm.data() : nullptr, N, pc,
                                                            D->d_mpts, D->d_nn_idx, D->d_normal_y, h->cfg.params.cov_threshold, fs,
                                                            ekf_inited, cls, world);
   CUDA_TRY(cudaGetLastError());

@@ -18,9 +18,13 @@
 #include <initializer_list>
 #include <string>
 
+#include "malio_buffer.h"
 #include "malio_internal.h"
 
 namespace malio_devstate {
+
+using malio_buf::DeviceBuffer;
+using malio_buf::PinnedBuffer;
 
 #define CUDA_TRY(expr)                                                                     \
   do {                                                                                     \
@@ -172,83 +176,67 @@ struct DeviceState {
   // search statistics the next entry point folds in (settle_deferred), deferred_grid whether that search ran on the cell list
   cudaEvent_t ev_caller_in = nullptr, ev_caller_out = nullptr, ev_deferred = nullptr; bool deferred_grid = false;
   // malio_upload_scan_from_device: the record check's flag word and its pinned host copy (allocated on first use)
-  uint32_t *d_scan_check = nullptr, *h_scan_check = nullptr;
+  DeviceBuffer<uint32_t> d_scan_check; PinnedBuffer<uint32_t> h_scan_check;
   malio_counters ctr{};
   bool timing = true;   // per-pass CUDA-event timing (malio_set_timing)
   double host_launch_us = 0, host_wait_us = 0; uint64_t host_passes = 0;   // MALIO_HOST_PROF=1 prints them at destroy
   // map
-  float4* d_nodes = nullptr; float* d_cov = nullptr;
-  float4* d_mpts = nullptr;            // compact mirror: point + link of every node, 16 B stride
-  uint32_t *d_parent = nullptr, *d_arrived = nullptr;   // box rebuild of the compact upload
-  uint32_t n_nodes = 0, cap_nodes = 0, depth = 0;
+  DeviceBuffer<float4> d_nodes; DeviceBuffer<float> d_cov;   // 64-byte tree records (4 float4 each); map-side weights
+  DeviceBuffer<float4> d_mpts;         // compact mirror: point + link of every node, 16 B stride; its size sizes the cell lists
+  DeviceBuffer<uint32_t> d_parent, d_arrived;   // box rebuild of the compact upload
+  uint32_t n_nodes = 0, depth = 0;
   // device-resident map mode (malio_mapops.cu): d_mpts / d_cov / d_ids are slots of a point set (link word = deleted bit only),
-  // there are no 64-byte tree records and the search never walks a tree
-  bool tree_free = false; int32_t* d_ids = nullptr; uint32_t cap_slots = 0;
-  // scan (caller order) + internal order
-  malio_scan_pt* d_pts = nullptr; uint32_t N = 0, capN = 0;
-  malio_scan_pt* d_pts_sorted = nullptr;   // the scan in internal (position) order
-  uint32_t* d_perm = nullptr; bool perm_valid = false;
-  uint16_t* d_keys16 = nullptr; uint32_t *d_hist = nullptr, *d_offs = nullptr, *d_cursor = nullptr, *d_btot = nullptr, *d_tmp_ids = nullptr;   // counting sort
-  double* d_table = nullptr; uint32_t cap_table = 0;
+  // there are no 64-byte tree records and the search never walks a tree.  slot_store is a mode, not a size: false once a
+  // snapshot upload has taken d_mpts / d_cov, so that the next grow_slots re-creates the slot store
+  bool tree_free = false; DeviceBuffer<int32_t> d_ids; bool slot_store = false;
+  // scan (caller order) + internal order; the point buffers share one capacity, d_pts' size
+  DeviceBuffer<malio_scan_pt> d_pts; uint32_t N = 0;
+  DeviceBuffer<malio_scan_pt> d_pts_sorted;   // the scan in internal (position) order
+  DeviceBuffer<uint32_t> d_perm; bool perm_valid = false;
+  DeviceBuffer<uint16_t> d_keys16; DeviceBuffer<uint32_t> d_hist, d_offs, d_cursor, d_btot, d_tmp_ids;   // counting sort
+  DeviceBuffer<double> d_table;
   uint32_t table_off[MALIO_MAX_LIDAR + 1] = {0, 0, 0, 0};
   malio_rigid tcomp[MALIO_MAX_LIDAR];
   bool scan_ready = false, map_ready = false, pass_done = false;
   // per point, position space
-  uint32_t* d_nn_idx = nullptr; float* d_nn_d2 = nullptr; uint8_t* d_sel = nullptr;
-  float4 *d_world = nullptr, *d_plane = nullptr; double *d_ucov = nullptr, *d_tau = nullptr; float* d_normal_y = nullptr;
-  double2* d_tau2 = nullptr; float* d_pd2 = nullptr; bool tau_valid = false;
-  double* d_rows12 = nullptr; uint8_t* d_lid8 = nullptr;
+  DeviceBuffer<uint32_t> d_nn_idx; DeviceBuffer<float> d_nn_d2; DeviceBuffer<uint8_t> d_sel;
+  DeviceBuffer<float4> d_world, d_plane; DeviceBuffer<double> d_ucov, d_tau; DeviceBuffer<float> d_normal_y;
+  DeviceBuffer<double2> d_tau2; DeviceBuffer<float> d_pd2; bool tau_valid = false;
+  DeviceBuffer<double> d_rows12; DeviceBuffer<uint8_t> d_lid8;
   // aux staging (caller order)
-  float* d_o_ny = nullptr; uint32_t* d_o_idx = nullptr; float* d_o_d2 = nullptr; uint8_t* d_o_sel = nullptr; float* d_o_world = nullptr;
+  DeviceBuffer<float> d_o_ny; DeviceBuffer<uint32_t> d_o_idx; DeviceBuffer<float> d_o_d2; DeviceBuffer<uint8_t> d_o_sel; DeviceBuffer<float> d_o_world;
   // reductions
-  uint32_t* d_counters = nullptr;   // [3] rows rows_kernel found (download_rows); [0..2] unused
-  unsigned long long* d_mmkey = nullptr;   // 2 parities x 4 keys
+  DeviceBuffer<uint32_t> d_counters;   // [3] rows rows_kernel found (download_rows); [0..2] unused
+  DeviceBuffer<unsigned long long> d_mmkey;   // 2 parities x 4 keys
   int parity = 0, last_parity = 0;
-  double* d_block_red = nullptr; uint32_t red_grid = 0;
-  double* d_res = nullptr;          // MALIO_RED_DOUBLES
-  double* d_rows = nullptr;         // MALIO_MAX_DOF x 25
-  double* h_res = nullptr;          // pinned: res | mm(4) | cnt
+  DeviceBuffer<double> d_block_red; uint32_t red_grid = 0;
+  DeviceBuffer<double> d_res;          // MALIO_RED_DOUBLES
+  DeviceBuffer<double> d_rows;         // MALIO_MAX_DOF x 25
+  PinnedBuffer<double> h_res;          // pinned, mapped: res | mm(4) | cnt
   PassConst last_pc{};
   // stand-alone queries
-  float* d_queries = nullptr; uint32_t capQ = 0;
+  DeviceBuffer<float> d_queries;
   // cell-list index over the live snapshot points (k-NN fast path)
   bool grid_on = false; GridConst grid{}; float grid_h = 0.f;
-  uint32_t *d_cell_start = nullptr, *d_cell_cnt = nullptr, *d_cell_of = nullptr, *d_ctot = nullptr, *d_cbase = nullptr;
-  uint32_t cap_cells = 0, cap_cell_pts = 0;
-  float4* d_cell_pts = nullptr;
-  uint32_t* d_fb_list = nullptr;          // positions the fast path could not settle (-> exact traversal)
-  unsigned long long* d_cand = nullptr;   // [0] candidates scanned by the cell-list scans since create (summed only while timing is on)
+  DeviceBuffer<uint32_t> d_cell_start, d_cell_cnt, d_cell_of, d_ctot, d_cbase;
+  DeviceBuffer<float4> d_cell_pts;
+  DeviceBuffer<uint32_t> d_fb_list;          // positions the fast path could not settle (-> exact traversal)
+  DeviceBuffer<unsigned long long> d_cand;   // [0] candidates scanned by the cell-list scans since create (summed only while timing is on)
   // [0] occupied cells, [1] live points, [2] fb count, [3] fb count of the last search, [4] ring-2 queries, [5] ring-2 queries
   // of the last search, [6] traversal fault bits (FAULT_STACK_OVERFLOW; cleared only by a map upload), [7] tie queries
-  uint32_t* d_gstats = nullptr;
+  DeviceBuffer<uint32_t> d_gstats;
   uint32_t* h_gstats = nullptr;            // pinned mirror (8 words, carved out of h_res)
   // fused pass (single cooperative launch per measurement pass)
   bool fused = true; int pass_max_blocks = 0, pass_max_blocks_generic = 0;
   int trace_passes = 0; float env_knn_cell = -1.f; bool env_knn_cell_set = false; bool host_prof = false;   // environment switches, read once in create()
-  uint32_t* d_bar = nullptr; uint32_t bar_base[3] = {0, 0, 0}; uint32_t seq = 0;
+  DeviceBuffer<uint32_t> d_bar; uint32_t bar_base[3] = {0, 0, 0}; uint32_t seq = 0;
   double* h_res_dev = nullptr;     // device-side address of the mapped host result buffer
-  unsigned long long* d_dbg = nullptr; int trace_left = 0;
+  DeviceBuffer<unsigned long long> d_dbg; int trace_left = 0;
   // multi-GPU
   ncclComm_t comm = nullptr; int rank = 0, world = 1;
-  bool p2p = false; unsigned char* d_mail = nullptr; unsigned char* mail_peer[MAIL_MAX_WORLD] = {nullptr};
+  // d_mail: this rank's mailbox; mail_peer: every rank's, the peers' opened with cudaIpcOpenMemHandle (closed by comm_destroy)
+  bool p2p = false; DeviceBuffer<unsigned char> d_mail; unsigned char* mail_peer[MAIL_MAX_WORLD] = {nullptr};
 };
-
-// (re)allocate ptr for count elements; the old contents are not kept.  Every buffer of a handle that grows by replacement grows
-// here, because a call that returned after enqueueing (the *_device calls) may still read or write the old buffer on the
-// handle's stream: that stream is drained before a live buffer is freed, rather than relying on cudaFree waiting for the
-// device.  Growth that copies the old contents over (grow_slots, world_accumulate, the voxel map's grow_table) drains the
-// stream itself before the copy.
-template <class T>
-int ensure(malio_handle* h, T*& ptr, size_t count) {
-  if (ptr) {
-    const DeviceState* D = static_cast<const DeviceState*>(h->dev);
-    CUDA_TRY(cudaStreamSynchronize(D->stream));
-    cudaFree(ptr);
-    ptr = nullptr;
-  }
-  CUDA_TRY(cudaMalloc((void**)&ptr, count * sizeof(T)));
-  return MALIO_OK;
-}
 
 // ---- host functions one unit calls in another
 // malio_knn.cu.  MODE 0: the scan's points through pc, MODE 1: stand-alone world-frame queries, n x 3 floats in `queries`

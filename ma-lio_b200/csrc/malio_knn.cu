@@ -1224,16 +1224,12 @@ int grid_build(malio_handle* h, DeviceState* D, const GridConst& G) {
   cudaStream_t st = D->stream;
   const uint32_t n = D->n_nodes;
   const uint32_t ncell_pad = ((G.ncell + 1 + GRID_CHUNK - 1) / GRID_CHUNK) * GRID_CHUNK, nchunk = ncell_pad / GRID_CHUNK;
-  if (ncell_pad > D->cap_cells) {
-    if (int rc = ensure(h, D->d_cell_start, (size_t)ncell_pad)) return rc;
-    if (int rc = ensure(h, D->d_cell_cnt, (size_t)ncell_pad)) return rc;
-    if (!D->d_ctot) { if (int rc = ensure(h, D->d_ctot, 8192)) return rc; if (int rc = ensure(h, D->d_cbase, 8192)) return rc; }
-    D->cap_cells = ncell_pad;
+  if (ncell_pad > D->d_cell_start.size()) {
+    if (int rc = malio_buf::allocate_group(h, st, {{D->d_cell_start, ncell_pad}, {D->d_cell_cnt, ncell_pad}})) return rc;
+    if (!D->d_ctot) { if (int rc = malio_buf::allocate_group(h, st, {{D->d_ctot, 8192}, {D->d_cbase, 8192}})) return rc; }
   }
-  if (D->cap_nodes > D->cap_cell_pts) {
-    if (int rc = ensure(h, D->d_cell_of, (size_t)D->cap_nodes)) return rc;
-    if (int rc = ensure(h, D->d_cell_pts, (size_t)D->cap_nodes)) return rc;
-    D->cap_cell_pts = D->cap_nodes;
+  if (D->d_mpts.size() > D->d_cell_of.size()) {
+    if (int rc = malio_buf::allocate_group(h, st, {{D->d_cell_of, D->d_mpts.size()}, {D->d_cell_pts, D->d_mpts.size()}})) return rc;
   }
   CUDA_TRY(cudaMemsetAsync(D->d_cell_cnt, 0, (size_t)ncell_pad * sizeof(uint32_t), st));
   CUDA_TRY(cudaMemsetAsync(D->d_gstats, 0, 2 * sizeof(uint32_t), st));
@@ -1271,7 +1267,7 @@ int sort_queries(malio_handle* h, DeviceState* D, uint32_t n, const PassConst& p
   // d_fb_list (the k-NN hand-over list, filled only later in the pass) doubles as the arrival-slot array of the sort
   scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(D->d_keys16, n, D->d_offs, D->d_btot, D->d_cursor, D->d_tmp_ids, D->d_fb_list);
   rank_kernel<<<(n + 255) / 256, 256, 0, st>>>(D->d_keys16, n, D->d_offs, D->d_btot, D->d_hist, D->d_tmp_ids, D->d_fb_list, D->d_perm,
-                                               MODE == 0 ? D->d_pts : nullptr, MODE == 0 ? D->d_pts_sorted : nullptr);
+                                               MODE == 0 ? D->d_pts.data() : nullptr, MODE == 0 ? D->d_pts_sorted.data() : nullptr);
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 4;
   return MALIO_OK;
@@ -1286,8 +1282,8 @@ int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pt
   const bool smem_stack = D->depth + KNN_POP_WIDTH <= (uint32_t)KNN_SMEM_DEPTH;
   const malio_scan_pt* pts = MODE == 0 ? pts_in : nullptr;
   const float* qs = MODE == 0 ? nullptr : (queries ? queries : D->d_queries);
-  float4* world = MODE == 0 ? D->d_world : nullptr;
-  uint8_t* sel = MODE == 0 ? D->d_sel : nullptr;
+  float4* world = MODE == 0 ? D->d_world.data() : nullptr;
+  uint8_t* sel = MODE == 0 ? D->d_sel.data() : nullptr;
   auto need_boxes = [&]() -> int {   // the exact traversal reads the 64-byte records: wait for a rebuild still in flight
     if (D->refit_pending) { CUDA_TRY(cudaStreamWaitEvent(st, D->ev_refit, 0)); D->refit_pending = false; }
     return MALIO_OK;
@@ -1301,7 +1297,7 @@ int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pt
     const uint32_t qpb = GD_THREADS / GG;                                                                                      \
     knn_keys_kernel<MODE, GG, PP><<<(n + qpb - 1) / qpb, GD_THREADS, 0, st>>>(                                                 \
         D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,        \
-        D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr);                                      \
+        D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand.data() : nullptr);                                      \
   } while (0)
       // measured (ncu kernel time, C2 sub-sampled): 12.5k queries 31 -> 12 us with 4 lanes + row preload; 100k 29.5 -> 24 us with
       // 2 lanes; from ~200k queries on (C4, C5) the thread-per-query kernel is as fast or faster and stays
@@ -1311,7 +1307,7 @@ int run_knn(malio_handle* h, DeviceState* D, uint32_t n, const malio_scan_pt* pt
     } else {
       knn_direct_kernel<MODE><<<(n + GD_THREADS - 1) / GD_THREADS, GD_THREADS, 0, st>>>(
           D->d_cell_pts, D->d_cell_start, D->grid, pts, perm, qs, n, pc, max_sqdist, world, D->d_nn_idx, D->d_nn_d2, sel,
-          D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand : nullptr);
+          D->d_gstats + 4, D->d_fb_list, D->d_gstats + 2, D->timing ? D->d_cand.data() : nullptr);
     }
     // 8 queries per warp and iteration; at most one resident wave of 64-thread blocks
     uint32_t fb_blocks = (n + 15) / 16;
@@ -1374,16 +1370,13 @@ int knn_fault(malio_handle* h, const DeviceState* D) {
 namespace malio_dev {
 
 static int ensure_map_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
-  if (n <= D->cap_nodes && D->d_nodes) return MALIO_OK;   // (slot mode grows d_mpts / d_cov only: no tree records there)
+  if (n <= D->d_nodes.size() / 4 && D->d_nodes) return MALIO_OK;   // (slot mode grows d_mpts / d_cov only: no tree records there)
   uint32_t cap = n + n / 8 + 1024;
   if (cap < h->cfg.max_map_nodes) cap = h->cfg.max_map_nodes;
-  if (int rc = ensure(h, D->d_nodes, (size_t)cap * 4)) return rc;
-  if (int rc = ensure(h, D->d_mpts, (size_t)cap)) return rc;
-  if (int rc = ensure(h, D->d_cov, (size_t)cap)) return rc;
-  if (int rc = ensure(h, D->d_parent, (size_t)cap)) return rc;
-  if (int rc = ensure(h, D->d_arrived, (size_t)cap)) return rc;
-  D->cap_nodes = cap;
-  D->cap_slots = 0;        // d_mpts / d_cov now hold the snapshot: the next malio_map_build re-creates the slot storage (grow_slots)
+  if (int rc = malio_buf::allocate_group(h, D->stream, {{D->d_nodes, (size_t)cap * 4}, {D->d_mpts, cap}, {D->d_cov, cap}, {D->d_parent, cap},
+                                                        {D->d_arrived, cap}}))
+    return rc;
+  D->slot_store = false;   // d_mpts / d_cov now hold the snapshot: the next malio_map_build re-creates the slot storage (grow_slots)
   return MALIO_OK;
 }
 
@@ -1498,29 +1491,14 @@ int upload_map_compact(malio_handle* h, const malio_map_point* pts, const float*
 int grow_slots(malio_handle* h, uint32_t n, uint32_t keep) {
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
-  if (n <= D->cap_slots && D->d_ids) return MALIO_OK;
+  if (D->slot_store && n <= D->d_ids.size()) return MALIO_OK;
   uint32_t cap = n + n / 2 + 4096;
   if (cap < h->cfg.max_map_nodes) cap = h->cfg.max_map_nodes;
-  float4* nm = nullptr; float* nc = nullptr; int32_t* ni = nullptr;
-  CUDA_TRY(cudaMalloc((void**)&nm, (size_t)cap * sizeof(float4)));
-  CUDA_TRY(cudaMalloc((void**)&nc, (size_t)cap * sizeof(float)));
-  CUDA_TRY(cudaMalloc((void**)&ni, (size_t)cap * sizeof(int32_t)));
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
-  if (keep && D->tree_free) {
-    CUDA_TRY(cudaMemcpy(nm, D->d_mpts, (size_t)keep * sizeof(float4), cudaMemcpyDeviceToDevice));
-    CUDA_TRY(cudaMemcpy(nc, D->d_cov, (size_t)keep * sizeof(float), cudaMemcpyDeviceToDevice));
-    if (D->d_ids) CUDA_TRY(cudaMemcpy(ni, D->d_ids, (size_t)keep * sizeof(int32_t), cudaMemcpyDeviceToDevice));
-  }
-  if (D->d_mpts) cudaFree(D->d_mpts);
-  if (D->d_cov) cudaFree(D->d_cov);
-  if (D->d_ids) cudaFree(D->d_ids);
+  if (!D->tree_free) keep = 0;   // d_mpts / d_cov hold a snapshot, not slots
+  CUDA_TRY(malio_buf::grow_keep(D->stream, {{D->d_mpts, cap, keep}, {D->d_cov, cap, keep}, {D->d_ids, cap, keep}}));
   // the tree records belong to the snapshot mode; they are re-created by the next malio_upload_map* call
-  if (D->d_nodes) { cudaFree(D->d_nodes); D->d_nodes = nullptr; }
-  if (D->d_parent) { cudaFree(D->d_parent); D->d_parent = nullptr; }
-  if (D->d_arrived) { cudaFree(D->d_arrived); D->d_arrived = nullptr; }
-  D->d_mpts = nm; D->d_cov = nc; D->d_ids = ni;
-  D->cap_slots = cap;
-  D->cap_nodes = cap;      // sizes the cell-list arrays (grid_build)
+  D->d_nodes.release(); D->d_parent.release(); D->d_arrived.release();
+  D->slot_store = true;
   return MALIO_OK;
 }
 // (re)build the cell-list index over the n_slots slots; box = {x_min,x_max,y_min,y_max,z_min,z_max} of the live points

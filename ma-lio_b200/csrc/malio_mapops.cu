@@ -30,16 +30,16 @@ struct MapOps {
   bool dirty = false;            // slots changed since the index was built
   bool appended = false;         // ... by appends (those are invisible to the index until the next commit)
   bool active = false;           // a build() happened: the handle is in device-resident map mode
-  float* d_stage = nullptr; uint32_t cap_stage = 0;     // staged host input: xyz (3n) | normal_y (n) | ids (n)
-  float* d_boxes = nullptr; uint32_t cap_boxes = 0;
-  uint32_t* d_small = nullptr;   // [0..5] bbox keys, [6] kill counter, [7] live counter
-  uint32_t* h_small = nullptr;   // pinned mirror
-  uint32_t *d_blk = nullptr, *d_blkoff = nullptr; uint32_t cap_blk = 0;   // compaction: live count / offset per 1024-slot block
-  float4* d_mpts2 = nullptr; float* d_cov2 = nullptr; int32_t* d_ids2 = nullptr; uint32_t cap2 = 0;   // compaction targets
+  DeviceBuffer<float> d_stage;     // staged host input, 5 rows of size() / 5: xyz (3 rows) | normal_y | ids
+  DeviceBuffer<float> d_boxes;
+  DeviceBuffer<uint32_t> d_small;   // [0..5] bbox keys, [6] kill counter, [7] live counter
+  PinnedBuffer<uint32_t> h_small;   // pinned mirror
+  DeviceBuffer<uint32_t> d_blk, d_blkoff;   // compaction: live count / offset per 1024-slot block
+  DeviceBuffer<float4> d_mpts2; DeviceBuffer<float> d_cov2; DeviceBuffer<int32_t> d_ids2;   // compaction targets
   // small batches (the per-scan deltas) go through a pinned bounce buffer: one host memcpy, one H2D, and the call returns
   // without waiting for the device — the caller's arrays are consumed, the bounce buffer is protected by ev_bounce
-  float* h_bounce[2] = {nullptr, nullptr}; cudaEvent_t ev_bounce[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false}; int bounce_next = 0;
-  float* h_bounce_box = nullptr; cudaEvent_t ev_bounce_box = nullptr; bool bounce_box_busy = false;   // same for the voxel boxes
+  PinnedBuffer<float> h_bounce[2]; cudaEvent_t ev_bounce[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false}; int bounce_next = 0;
+  PinnedBuffer<float> h_bounce_box; cudaEvent_t ev_bounce_box = nullptr; bool bounce_box_busy = false;   // same for the voxel boxes
 };
 constexpr uint32_t BOUNCE_POINTS = 65536;      // 5 floats per point: 1.3 MB of pinned memory
 constexpr uint32_t BOUNCE_BOXES = 16384;       // 6 floats per box
@@ -51,9 +51,8 @@ int state(malio_handle* h, MapOps*& M) {
   CUDA_TRY(cudaSetDevice(D->device));
   M = new MapOps;
   h->mapst = M;
-  CUDA_TRY(cudaMalloc((void**)&M->d_small, 8 * sizeof(uint32_t)));
-  CUDA_TRY(cudaHostAlloc((void**)&M->h_small, 8 * sizeof(uint32_t), cudaHostAllocDefault));
-  return MALIO_OK;
+  if (int rc = M->d_small.allocate(h, D->stream, 8)) return rc;
+  return M->h_small.allocate(h, 8);
 }
 
 __device__ __forceinline__ uint32_t fkey(float f) {
@@ -250,10 +249,11 @@ __global__ void gather_live_kernel(const float4* __restrict__ mpts, const float*
 // host arrays -> staging buffer on the device: xyz | normal_y | ids
 int stage(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const float* ny, const int32_t* ids, uint32_t n, const float** d_xyz,
           const float** d_ny, const int32_t** d_ids, bool* synced_needed) {
-  if (n > M->cap_stage) { if (int rc = ensure(h, M->d_stage, (size_t)(n + n / 4 + 1024) * 5)) return rc; M->cap_stage = n + n / 4 + 1024; }
+  if (n > M->d_stage.size() / 5) { if (int rc = M->d_stage.allocate(h, D->stream, (size_t)(n + n / 4 + 1024) * 5)) return rc; }
   float* base = M->d_stage;
-  *d_xyz = base; *d_ny = base + 3 * (size_t)M->cap_stage;
-  *d_ids = ids ? reinterpret_cast<const int32_t*>(base + 4 * (size_t)M->cap_stage) : nullptr;
+  const size_t stride = M->d_stage.size() / 5;
+  *d_xyz = base; *d_ny = base + 3 * stride;
+  *d_ids = ids ? reinterpret_cast<const int32_t*>(base + 4 * stride) : nullptr;
   D->ctr.h2d_bytes += (uint64_t)n * (16 + (ids ? 4 : 0));
   *synced_needed = true;
   if (n <= BOUNCE_POINTS) {
@@ -261,7 +261,7 @@ int stage(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const fl
     const int bs = M->bounce_next;
     M->bounce_next ^= 1;
     if (!M->h_bounce[bs]) {
-      CUDA_TRY(cudaHostAlloc((void**)&M->h_bounce[bs], (size_t)BOUNCE_POINTS * 5 * sizeof(float), cudaHostAllocDefault));
+      if (int rc = M->h_bounce[bs].allocate(h, (size_t)BOUNCE_POINTS * 5)) return rc;
       CUDA_TRY(cudaEventCreateWithFlags(&M->ev_bounce[bs], cudaEventDisableTiming));
     }
     if (M->bounce_busy[bs]) { CUDA_TRY(cudaEventSynchronize(M->ev_bounce[bs])); M->bounce_busy[bs] = false; }   // its previous batch has left it
@@ -271,16 +271,16 @@ int stage(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const fl
     std::memcpy(hb + 3 * (size_t)n, ny, (size_t)n * 4);
     if (ids) std::memcpy(hb + 4 * (size_t)n, ids, (size_t)n * 4);
     CUDA_TRY(cudaMemcpyAsync(base, hb, (size_t)n * 12, cudaMemcpyHostToDevice, D->stream));
-    CUDA_TRY(cudaMemcpyAsync(base + 3 * (size_t)M->cap_stage, hb + 3 * (size_t)n, (size_t)n * 4, cudaMemcpyHostToDevice, D->stream));
-    if (ids) CUDA_TRY(cudaMemcpyAsync(base + 4 * (size_t)M->cap_stage, hb + 4 * (size_t)n, (size_t)n * 4, cudaMemcpyHostToDevice, D->stream));
+    CUDA_TRY(cudaMemcpyAsync(base + 3 * stride, hb + 3 * (size_t)n, (size_t)n * 4, cudaMemcpyHostToDevice, D->stream));
+    if (ids) CUDA_TRY(cudaMemcpyAsync(base + 4 * stride, hb + 4 * (size_t)n, (size_t)n * 4, cudaMemcpyHostToDevice, D->stream));
     CUDA_TRY(cudaEventRecord(M->ev_bounce[bs], D->stream));
     M->bounce_busy[bs] = true;
     *synced_needed = false;
     return MALIO_OK;
   }
   CUDA_TRY(cudaMemcpyAsync(base, xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, D->stream));
-  CUDA_TRY(cudaMemcpyAsync(base + 3 * (size_t)M->cap_stage, ny, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, D->stream));
-  if (ids) CUDA_TRY(cudaMemcpyAsync(base + 4 * (size_t)M->cap_stage, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, D->stream));
+  CUDA_TRY(cudaMemcpyAsync(base + 3 * stride, ny, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, D->stream));
+  if (ids) CUDA_TRY(cudaMemcpyAsync(base + 4 * stride, ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, D->stream));
   return MALIO_OK;
 }
 // on_device: xyz / ny / ids are device memory the append kernel reads in place, ordered on the caller's stream `caller`
@@ -290,7 +290,7 @@ int append(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const f
   if (n == 0) return MALIO_OK;
   if ((uint64_t)M->n_slots + n > MALIO_LINK_INDEX_MASK) { h->err = "device-resident map: too many slots"; return MALIO_ERR_CAPACITY; }
   if (int rc = malio_dev::grow_slots(h, M->n_slots + n, M->n_slots)) return rc;   // (drains D->stream before it frees anything)
-  if (M->n_slots + n > D->cap_slots) { h->err = "device-resident map: slot storage smaller than its recorded use"; return MALIO_ERR_CAPACITY; }
+  if (M->n_slots + n > D->d_mpts.size()) { h->err = "device-resident map: slot storage smaller than its recorded use"; return MALIO_ERR_CAPACITY; }
   const float *d_xyz = xyz, *d_ny = ny;
   const int32_t* d_ids = ids;
   bool need_sync = false;
@@ -319,11 +319,7 @@ namespace malio_map {
 void destroy(malio_handle* h) {
   MapOps* M = (MapOps*)h->mapst;
   if (!M) return;
-  void* p[] = {M->d_stage, M->d_boxes, M->d_small, M->d_blk, M->d_blkoff, M->d_mpts2, M->d_cov2, M->d_ids2};
-  for (void* q : p) if (q) cudaFree(q);
-  if (M->h_small) cudaFreeHost(M->h_small);
-  for (int k = 0; k < 2; ++k) { if (M->h_bounce[k]) cudaFreeHost(M->h_bounce[k]); if (M->ev_bounce[k]) cudaEventDestroy(M->ev_bounce[k]); }
-  if (M->h_bounce_box) cudaFreeHost(M->h_bounce_box);
+  for (cudaEvent_t e : M->ev_bounce) if (e) cudaEventDestroy(e);
   if (M->ev_bounce_box) cudaEventDestroy(M->ev_bounce_box);
   delete M;
   h->mapst = nullptr;
@@ -356,25 +352,19 @@ int commit(malio_handle* h) {
   // ---- compaction when more than half of the slots are dead (stable: slot order = age order is kept)
   if (n > 65536 && M->n_live * 2 < n) {
     const uint32_t nblk = (n + CP_T - 1) / CP_T;
-    if (nblk + 1 > M->cap_blk) {
-      if (int rc = ensure(h, M->d_blk, nblk + 1024)) return rc;
-      if (int rc = ensure(h, M->d_blkoff, nblk + 1025)) return rc;
-      M->cap_blk = nblk + 1024;
+    if (nblk + 1 > M->d_blk.size()) {
+      if (int rc = malio_buf::allocate_group(h, st, {{M->d_blk, nblk + 1024}, {M->d_blkoff, nblk + 1025}})) return rc;
     }
-    const uint32_t cap2 = D->cap_slots;
-    if (cap2 > M->cap2) {
-      if (int rc = ensure(h, M->d_mpts2, cap2)) return rc;
-      if (int rc = ensure(h, M->d_cov2, cap2)) return rc;
-      if (int rc = ensure(h, M->d_ids2, cap2)) return rc;
-      M->cap2 = cap2;
+    const size_t cap2 = D->d_mpts.size();
+    if (cap2 > M->d_mpts2.size()) {
+      if (int rc = malio_buf::allocate_group(h, st, {{M->d_mpts2, cap2}, {M->d_cov2, cap2}, {M->d_ids2, cap2}})) return rc;
     }
     cp_count_kernel<<<nblk, CP_T, 0, st>>>(D->d_mpts, n, M->d_blk);
     cp_scan_kernel<<<1, 1024, 0, st>>>(M->d_blk, nblk, M->d_blkoff);
     cp_scatter_kernel<<<nblk, CP_T, 0, st>>>(D->d_mpts, D->d_cov, D->d_ids, n, M->d_blkoff, M->d_mpts2, M->d_cov2, M->d_ids2);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(st));
-    std::swap(D->d_mpts, M->d_mpts2); std::swap(D->d_cov, M->d_cov2); std::swap(D->d_ids, M->d_ids2);
-    std::swap(D->cap_slots, M->cap2);   // each pair of buffers takes its own capacity along
+    std::swap(D->d_mpts, M->d_mpts2); std::swap(D->d_cov, M->d_cov2); std::swap(D->d_ids, M->d_ids2);   // sizes go along
     M->n_slots = M->n_live;
     D->ctr.kernel_launches += 3;
     D->ctr.map_compactions += 1;
@@ -473,11 +463,11 @@ int sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* x
   if (M->appended || !D->tree_free) { if (int rc = commit(h)) return rc; }   // the kill below reads the index: it must know every live slot
   uint32_t killed = 0;
   if (nb && D->grid_on) {
-    if (nb > M->cap_boxes) { if (int rc = ensure(h, M->d_boxes, (size_t)(nb + nb / 4 + 1024) * 6)) return rc; M->cap_boxes = nb + nb / 4 + 1024; }
+    if (nb > M->d_boxes.size() / 6) { if (int rc = M->d_boxes.allocate(h, D->stream, (size_t)(nb + nb / 4 + 1024) * 6)) return rc; }
     const bool via_bounce = !n_deleted && nb <= BOUNCE_BOXES;
     if (via_bounce) {
       if (!M->h_bounce_box) {
-        CUDA_TRY(cudaHostAlloc((void**)&M->h_bounce_box, (size_t)BOUNCE_BOXES * 6 * sizeof(float), cudaHostAllocDefault));
+        if (int rc = M->h_bounce_box.allocate(h, (size_t)BOUNCE_BOXES * 6)) return rc;
         CUDA_TRY(cudaEventCreateWithFlags(&M->ev_bounce_box, cudaEventDisableTiming));
       }
       if (M->bounce_box_busy) { CUDA_TRY(cudaEventSynchronize(M->ev_bounce_box)); M->bounce_box_busy = false; }
@@ -527,13 +517,11 @@ int download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_
   if (live == 0 || (!xyz && !normal_y && !ids && !slots)) return MALIO_OK;
   if (cap < live) { h->err = "malio_map_download: capacity below the number of live points"; return MALIO_ERR_CAPACITY; }
   const uint32_t nblk = (n + CP_T - 1) / CP_T;
-  if (nblk + 1 > M->cap_blk) {
-    if (int rc = ensure(h, M->d_blk, nblk + 1024)) return rc;
-    if (int rc = ensure(h, M->d_blkoff, nblk + 1025)) return rc;
-    M->cap_blk = nblk + 1024;
+  if (nblk + 1 > M->d_blk.size()) {
+    if (int rc = malio_buf::allocate_group(h, D->stream, {{M->d_blk, nblk + 1024}, {M->d_blkoff, nblk + 1025}})) return rc;
   }
-  float* d_out = nullptr;
-  CUDA_TRY(cudaMalloc((void**)&d_out, (size_t)live * 6 * sizeof(float)));
+  DeviceBuffer<float> d_out;   // freed on return, after the wait below
+  if (int rc = d_out.allocate(h, D->stream, (size_t)live * 6)) return rc;
   float* o_xyz = d_out; float* o_ny = d_out + 3 * (size_t)live;
   int32_t* o_ids = reinterpret_cast<int32_t*>(d_out + 4 * (size_t)live); uint32_t* o_slots = reinterpret_cast<uint32_t*>(d_out + 5 * (size_t)live);
   cp_count_kernel<<<nblk, CP_T, 0, D->stream>>>(D->d_mpts, n, M->d_blk);
@@ -544,7 +532,6 @@ int download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_
   if (ids) cudaMemcpyAsync(ids, o_ids, (size_t)live * 4, cudaMemcpyDeviceToHost, D->stream);
   if (slots) cudaMemcpyAsync(slots, o_slots, (size_t)live * 4, cudaMemcpyDeviceToHost, D->stream);
   const cudaError_t e = cudaStreamSynchronize(D->stream);
-  cudaFree(d_out);
   if (e != cudaSuccess) { h->err = std::string("malio_map_download: ") + cudaGetErrorString(e); return MALIO_ERR_CUDA; }
   D->ctr.kernel_launches += 3;
   return MALIO_OK;

@@ -1160,7 +1160,7 @@ int pass_fused(malio_handle* h, DeviceState* D, const PassConst& pc, const Param
   a.dbg = nullptr;
   a.xwait = D->d_cand + 1;
   if (D->trace_passes > 0) {
-    if (!D->d_dbg) { CUDA_TRY(cudaMalloc((void**)&D->d_dbg, (size_t)4096 * 8 * sizeof(unsigned long long))); D->trace_left = D->trace_passes; }
+    if (!D->d_dbg) { if (int rc = D->d_dbg.allocate(h, D->stream, (size_t)4096 * 8)) return rc; D->trace_left = D->trace_passes; }
     if (D->trace_left > 0 && grid <= 4096) a.dbg = D->d_dbg;
   }
   PassConst pc_arg = pc;
@@ -1364,8 +1364,8 @@ PassConst make_pass_const(const malio_handle* h, const DeviceState* D, const mal
 
 int pass_init(malio_handle* h, DeviceState* D) {
   D->red_grid = (uint32_t)D->sm_count * (PASS_MIN_BLOCKS > 4 ? PASS_MIN_BLOCKS : 4);   // slots for the per-block partial systems
-  CUDA_TRY(cudaMalloc((void**)&D->d_block_red, (size_t)D->red_grid * MALIO_RED_DOUBLES * sizeof(double)));
-  CUDA_TRY(cudaMalloc((void**)&D->d_bar, 4 * sizeof(uint32_t)));
+  if (int rc = D->d_block_red.allocate(h, D->stream, (size_t)D->red_grid * MALIO_RED_DOUBLES)) return rc;
+  if (int rc = D->d_bar.allocate(h, D->stream, 4)) return rc;
   CUDA_TRY(cudaMemset(D->d_bar, 0, 4 * sizeof(uint32_t)));
   CUDA_TRY(cudaFuncSetAttribute(pass_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RED_SMEM_DOUBLES * (int)sizeof(double)));
   CUDA_TRY(cudaFuncSetAttribute(pass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RED_SMEM_DOUBLES * (int)sizeof(double)));
@@ -1386,6 +1386,10 @@ int pass_init(malio_handle* h, DeviceState* D) {
 
 void comm_destroy(DeviceState* D) {
   if (D->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(D->comm);
+  for (unsigned char*& p : D->mail_peer) {   // the peers' mailboxes; this rank's own is D->d_mail
+    if (p && p != D->d_mail.data()) cudaIpcCloseMemHandle(p);
+    p = nullptr;
+  }
 }
 }  // namespace malio_devstate
 
@@ -1492,15 +1496,15 @@ int comm_init(malio_handle* h, const uint8_t* id, int rank, int world) {
   const char* env = getenv("MALIO_P2P");
   int ok = (world > 1 && world <= MAIL_MAX_WORLD && D->fused && g_nccl.AllGather && !(env && atoi(env) == 0)) ? 1 : 0;
   cudaIpcMemHandle_t mine{};
-  unsigned char* d_h = nullptr;
+  DeviceBuffer<unsigned char> d_h;
   std::vector<cudaIpcMemHandle_t> all((size_t)world);
   if (ok) {
-    if (cudaMalloc((void**)&D->d_mail, MAIL_BYTES) != cudaSuccess || cudaMemset(D->d_mail, 0, MAIL_BYTES) != cudaSuccess ||
+    if (D->d_mail.allocate_empty(MAIL_BYTES) != cudaSuccess || cudaMemset(D->d_mail, 0, MAIL_BYTES) != cudaSuccess ||
         cudaIpcGetMemHandle(&mine, D->d_mail) != cudaSuccess) { ok = 0; cudaGetLastError(); }
   }
   // every rank takes part in the two collectives below whatever its own outcome
   if (world > 1 && g_nccl.AllGather) {
-    CUDA_TRY(cudaMalloc((void**)&d_h, (size_t)(world + 1) * sizeof(mine) + 2 * sizeof(int)));
+    if (int rc = d_h.allocate(h, D->stream, (size_t)(world + 1) * sizeof(mine) + 2 * sizeof(int))) return rc;
     CUDA_TRY(cudaMemcpy(d_h + (size_t)world * sizeof(mine), &mine, sizeof(mine), cudaMemcpyHostToDevice));
     if (g_nccl.AllGather(d_h + (size_t)world * sizeof(mine), d_h, sizeof(mine), ncclChar, D->comm, D->stream) != ncclSuccess) ok = 0;
     CUDA_TRY(cudaStreamSynchronize(D->stream));
@@ -1519,7 +1523,6 @@ int comm_init(malio_handle* h, const uint8_t* id, int rank, int world) {
     CUDA_TRY(cudaStreamSynchronize(D->stream));
     int all_ok = 0;
     CUDA_TRY(cudaMemcpy(&all_ok, d_ok + 1, sizeof(int), cudaMemcpyDeviceToHost));
-    cudaFree(d_h);
     D->p2p = ok && all_ok;
   }
   if (D->host_prof) fprintf(stderr, "[malio] rank %d/%d: in-kernel peer exchange %s\n", rank, world, D->p2p ? "ON" : "off (NCCL path)");

@@ -31,49 +31,49 @@ using namespace malio_devstate;
 namespace {
 
 struct PreLidar {
-  uint32_t n = 0, cap = 0;            // raw / undistorted points
-  malio_raw_pt* d_raw = nullptr;
-  float* d_ud = nullptr;              // n x 5: x, y, z, intensity (= idx as float, 0 where untouched), curvature
-  int32_t* d_need = nullptr;
-  int32_t* d_idx = nullptr;
-  uint8_t* d_ok = nullptr;
-  double* d_pose = nullptr;           // n x 7: the spline pose of every point (zeros where get_pose failed, and at point 0)
-  int32_t* d_pop = nullptr;           // MALIO_MAX_COV + 1: pop points of the last malio_undistort (last = count)
+  uint32_t n = 0;                     // raw / undistorted points; the buffers below hold d_raw's size of them
+  DeviceBuffer<malio_raw_pt> d_raw;
+  DeviceBuffer<float> d_ud;           // n x 5: x, y, z, intensity (= idx as float, 0 where untouched), curvature
+  DeviceBuffer<int32_t> d_need;
+  DeviceBuffer<int32_t> d_idx;
+  DeviceBuffer<uint8_t> d_ok;
+  DeviceBuffer<double> d_pose;        // n x 7: the spline pose of every point (zeros where get_pose failed, and at point 0)
+  DeviceBuffer<int32_t> d_pop;        // MALIO_MAX_COV + 1: pop points of the last malio_undistort (last = count)
   bool ud_valid = false;              // d_ud holds the result of a completed malio_undistort (possibly of 0 points)
   // what malio_scan_uncertainty needs of that call besides the device buffers
   uint32_t n_cov = 0, n_pops = 0;
   int32_t cov_pointer = -1;
   malio_rigid lt_imu_frame{};
   // voxel grid
-  uint32_t n_ds = 0, cap_ds = 0;
-  float* d_ds = nullptr;              // n_ds x 5
+  uint32_t n_ds = 0;
+  DeviceBuffer<float> d_ds;           // n_ds x 5
   bool ds_valid = false;
 };
 struct PreState {
   cudaStream_t stream = nullptr;
   PreLidar lid[MALIO_MAX_LIDAR];
-  double *d_ct = nullptr, *d_cT = nullptr, *d_seglog = nullptr, *d_covt = nullptr;
+  DeviceBuffer<double> d_ct, d_cT, d_seglog, d_covt;
   // malio_scan_uncertainty: imu_cov (MALIO_MAX_COV x 36) and its one output buffer (table | temporal_comp | lidar_uncertainty)
-  double* d_ucov = nullptr;
-  char* d_uout = nullptr;
+  DeviceBuffer<double> d_ucov;
+  DeviceBuffer<char> d_uout;
   // voxel scratch
-  float* d_vin = nullptr; uint32_t cap_vin = 0;       // host-provided input staged on the device
-  uint32_t *d_vidx = nullptr, *d_vtmp = nullptr, *d_vorder = nullptr; uint32_t cap_vpts = 0;
-  uint32_t *d_vcnt = nullptr, *d_voff = nullptr, *d_vocc = nullptr, *d_vcur = nullptr; uint64_t cap_cells = 0;
-  uint32_t *d_ctot = nullptr, *d_cbase = nullptr;     // chunk totals / bases of the two cell scans (2 x 65536)
-  uint32_t* d_bounds = nullptr;       // 6 order-preserving keys + out count
-  uint32_t* d_order_bad = nullptr;    // malio_undistort_device: raw_order_check_kernel's flag word
+  DeviceBuffer<float> d_vin;                          // host-provided input staged on the device
+  DeviceBuffer<uint32_t> d_vidx, d_vtmp, d_vorder;    // per point
+  DeviceBuffer<uint32_t> d_vcnt, d_voff, d_vocc, d_vcur;   // per cell
+  DeviceBuffer<uint32_t> d_ctot, d_cbase;             // chunk totals / bases of the two cell scans (2 x 65536)
+  DeviceBuffer<uint32_t> d_bounds;    // 6 order-preserving keys + out count
+  DeviceBuffer<uint32_t> d_order_bad; // malio_undistort_device: raw_order_check_kernel's flag word
   // pinned, 8 words: the voxel grid's bounds and counts in [0..5]; malio_undistort_device's order flag and pop count in [6..7]
-  uint32_t* h_small = nullptr;
+  PinnedBuffer<uint32_t> h_small;
   // the table malio_scan_uncertainty* left at the head of d_uout, for malio_upload_scan_resident: its offsets, the rigid part
   // of the temporal compensations, and whether it still describes the slots (any malio_undistort* since then clears it)
   bool table_resident = false;
   uint32_t res_table_off[MALIO_MAX_LIDAR + 1] = {0, 0, 0, 0};
   malio_rigid res_tcomp[MALIO_MAX_LIDAR] = {};
   // publish_frame_world / pcd_save (world registration): {x, y, z, intensity} per point
-  float4* d_wstage = nullptr; uint64_t cap_wstage = 0;   // malio_world_register's result before its one D2H copy
-  float4* d_acc = nullptr; uint64_t n_acc = 0, cap_acc = 0;   // pcl_wait_save (laserMapping.cpp:475), device-resident
-  float4* h_bounce = nullptr;         // pinned, malio_pcd::CHUNK points: malio_world_save_pcd's D2H staging
+  DeviceBuffer<float4> d_wstage;      // malio_world_register's result before its one D2H copy
+  DeviceBuffer<float4> d_acc; uint64_t n_acc = 0;   // pcl_wait_save (laserMapping.cpp:475), device-resident
+  PinnedBuffer<float4> h_bounce;      // pinned, malio_pcd::CHUNK points: malio_world_save_pcd's D2H staging
 };
 
 int get_state(malio_handle* h, PreState*& S) {
@@ -84,16 +84,16 @@ int get_state(malio_handle* h, PreState*& S) {
   S = new PreState;
   h->pre = S;
   S->stream = D->stream;   // same stream as the scan path: malio_upload_scan_device is ordered after the voxel grid
-  CUDA_TRY(cudaMalloc((void**)&S->d_ct, MALIO_MAX_CTRL * sizeof(double)));
-  CUDA_TRY(cudaMalloc((void**)&S->d_cT, (size_t)MALIO_MAX_CTRL * 16 * sizeof(double)));
-  CUDA_TRY(cudaMalloc((void**)&S->d_seglog, (size_t)MALIO_MAX_CTRL * 6 * sizeof(double)));
-  CUDA_TRY(cudaMalloc((void**)&S->d_covt, MALIO_MAX_COV * sizeof(double)));
-  CUDA_TRY(cudaMalloc((void**)&S->d_bounds, 8 * sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&S->d_order_bad, sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&S->d_ctot, 2 * 65536 * sizeof(uint32_t)));
-  CUDA_TRY(cudaMalloc((void**)&S->d_cbase, 2 * 65536 * sizeof(uint32_t)));
-  CUDA_TRY(cudaHostAlloc((void**)&S->h_small, 8 * sizeof(uint32_t), cudaHostAllocDefault));
-  return MALIO_OK;
+  const cudaStream_t st = S->stream;
+  if (int rc = S->d_ct.allocate(h, st, MALIO_MAX_CTRL)) return rc;
+  if (int rc = S->d_cT.allocate(h, st, (size_t)MALIO_MAX_CTRL * 16)) return rc;
+  if (int rc = S->d_seglog.allocate(h, st, (size_t)MALIO_MAX_CTRL * 6)) return rc;
+  if (int rc = S->d_covt.allocate(h, st, MALIO_MAX_COV)) return rc;
+  if (int rc = S->d_bounds.allocate(h, st, 8)) return rc;
+  if (int rc = S->d_order_bad.allocate(h, st, 1)) return rc;
+  if (int rc = S->d_ctot.allocate(h, st, 2 * 65536)) return rc;
+  if (int rc = S->d_cbase.allocate(h, st, 2 * 65536)) return rc;
+  return S->h_small.allocate(h, 8);
 }
 
 // ------------------------------------------------------------------ quat_ops.h restated for the device
@@ -587,11 +587,8 @@ constexpr uint64_t WORLD_ACC_MIN = 1u << 16;   // first capacity of the accumula
 
 // d_wstage large enough for n points
 int grow_wstage(malio_handle* h, PreState* S, uint64_t n) {
-  if (n <= S->cap_wstage) return MALIO_OK;
-  const uint64_t c = n + n / 8 + 1024;
-  if (int rc = ensure(h, S->d_wstage, c)) { S->cap_wstage = 0; return rc; }
-  S->cap_wstage = c;
-  return MALIO_OK;
+  if (n <= S->d_wstage.size()) return MALIO_OK;
+  return S->d_wstage.allocate(h, S->stream, n + n / 8 + 1024);
 }
 
 // size of the cloud `source` registers, or a state error when it is not on the device
@@ -626,7 +623,7 @@ int world_launch(malio_handle* h, PreState* S, DeviceState* D, const malio_pass_
   } else if (D->N) {
     const bool sorted = h->cfg.sort_queries && D->perm_valid;
     world_kernel<<<(D->N + 255) / 256, 256, 0, S->stream>>>(nullptr, 0, 0.f, sorted ? D->d_pts_sorted : D->d_pts,
-                                                           sorted ? D->d_perm : nullptr, D->d_normal_y, D->N, pc, dst);
+                                                           sorted ? D->d_perm.data() : nullptr, D->d_normal_y, D->N, pc, dst);
     D->ctr.kernel_launches += 1;
   }
   CUDA_TRY(cudaGetLastError());
@@ -697,17 +694,13 @@ int undistort_check_args(malio_handle* h, int lidar, const malio_undistort_args*
 int undistort_prepare_slot(malio_handle* h, PreState* S, PreLidar& L, uint32_t n, const malio_undistort_args* a) {
   L.ud_valid = false;
   S->table_resident = false;   // the table in d_uout was built from this slot's previous undistortion
-  if (n > L.cap) {
+  if (n > L.d_raw.size()) {
     const uint32_t cap = n + n / 8 + 1024;
-    if (int rc = ensure(h, L.d_raw, cap)) return rc;
-    if (int rc = ensure(h, L.d_ud, (size_t)cap * 5)) return rc;
-    if (int rc = ensure(h, L.d_need, cap)) return rc;
-    if (int rc = ensure(h, L.d_idx, cap)) return rc;
-    if (int rc = ensure(h, L.d_ok, cap)) return rc;
-    if (int rc = ensure(h, L.d_pose, (size_t)cap * 7)) return rc;
-    L.cap = cap;
+    if (int rc = malio_buf::allocate_group(h, S->stream, {{L.d_raw, cap}, {L.d_ud, (size_t)cap * 5}, {L.d_need, cap}, {L.d_idx, cap},
+                                                          {L.d_ok, cap}, {L.d_pose, (size_t)cap * 7}}))
+      return rc;
   }
-  if (!L.d_pop) { if (int rc = ensure(h, L.d_pop, MALIO_MAX_COV + 1)) return rc; }
+  if (!L.d_pop) { if (int rc = L.d_pop.allocate(h, S->stream, MALIO_MAX_COV + 1)) return rc; }
   L.n = n;
   L.ds_valid = false;
   L.n_cov = a->n_cov;
@@ -746,18 +739,7 @@ int undistort_launch(malio_handle* h, PreState* S, DeviceState* D, PreLidar& L, 
 namespace malio_pre {
 
 void destroy(malio_handle* h) {
-  PreState* S = (PreState*)h->pre;
-  if (!S) return;
-  for (auto& L : S->lid) {
-    void* p[] = {L.d_raw, L.d_ud, L.d_need, L.d_idx, L.d_ok, L.d_pose, L.d_pop, L.d_ds};
-    for (void* q : p) if (q) cudaFree(q);
-  }
-  void* p[] = {S->d_ct, S->d_cT, S->d_seglog, S->d_covt, S->d_ucov, S->d_uout, S->d_vin, S->d_vidx, S->d_vtmp, S->d_vorder, S->d_vcnt, S->d_voff,
-               S->d_vocc, S->d_vcur, S->d_ctot, S->d_cbase, S->d_bounds, S->d_order_bad, S->d_wstage, S->d_acc};
-  for (void* q : p) if (q) cudaFree(q);
-  if (S->h_small) cudaFreeHost(S->h_small);
-  if (S->h_bounce) cudaFreeHost(S->h_bounce);
-  delete S;
+  delete (PreState*)h->pre;
   h->pre = nullptr;
 }
 
@@ -848,12 +830,9 @@ static int voxel_grid_run(malio_handle* h, PreState* S, DeviceState* D, PreLidar
   L.n_ds = 0;
   if (n_out) *n_out = 0;
   if (n == 0) { L.ds_valid = true; return MALIO_OK; }
-  if (n > S->cap_vpts) {
+  if (n > S->d_vidx.size()) {
     const uint32_t cap = n + n / 8 + 1024;
-    if (int rc = ensure(h, S->d_vidx, cap)) return rc;
-    if (int rc = ensure(h, S->d_vtmp, cap)) return rc;
-    if (int rc = ensure(h, S->d_vorder, cap)) return rc;
-    S->cap_vpts = cap;
+    if (int rc = malio_buf::allocate_group(h, st, {{S->d_vidx, cap}, {S->d_vtmp, cap}, {S->d_vorder, cap}})) return rc;
   }
   // ---- bounds (getMinMax3D), then the grid geometry on the host exactly as PCL derives it
   const uint32_t init[6] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u, 0u};
@@ -888,13 +867,9 @@ static int voxel_grid_run(malio_handle* h, PreState* S, DeviceState* D, PreLidar
     return MALIO_ERR_CAPACITY;
   }
   c.dx = dx; c.dxy = dx * dy;
-  if ((uint64_t)cells > S->cap_cells) {
+  if ((uint64_t)cells > S->d_vcnt.size()) {
     const uint64_t cap = (uint64_t)cells + (uint64_t)cells / 4 + 4096;
-    if (int rc = ensure(h, S->d_vcnt, cap)) return rc;
-    if (int rc = ensure(h, S->d_voff, cap)) return rc;
-    if (int rc = ensure(h, S->d_vocc, cap)) return rc;
-    if (int rc = ensure(h, S->d_vcur, cap)) return rc;
-    S->cap_cells = cap;
+    if (int rc = malio_buf::allocate_group(h, st, {{S->d_vcnt, cap}, {S->d_voff, cap}, {S->d_vocc, cap}, {S->d_vcur, cap}})) return rc;
   }
   const uint32_t nchunk = (uint32_t)((cells + VS_CHUNK - 1) / VS_CHUNK);   // <= 65536
   CUDA_TRY(cudaMemsetAsync(S->d_vcnt, 0, (size_t)cells * sizeof(uint32_t), st));
@@ -908,7 +883,7 @@ static int voxel_grid_run(malio_handle* h, PreState* S, DeviceState* D, PreLidar
   CUDA_TRY(cudaMemcpyAsync(S->h_small, S->d_bounds + 6, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   const uint32_t m = S->h_small[1];
-  if (m > L.cap_ds) { if (int rc = ensure(h, L.d_ds, (size_t)(m + m / 8 + 1024) * 5)) return rc; L.cap_ds = m + m / 8 + 1024; }
+  if (m > L.d_ds.size() / 5) { if (int rc = L.d_ds.allocate(h, st, (size_t)(m + m / 8 + 1024) * 5)) return rc; }
   vg_centroid_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_in, S->d_vidx, n, S->d_voff, S->d_vcnt, S->d_vocc, S->d_vorder, L.d_ds, m);
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 7;
@@ -937,7 +912,7 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
   cudaStream_t st = S->stream;
   const float* d_in;
   if (in) {
-    if (n > S->cap_vin) { if (int rc = ensure(h, S->d_vin, (size_t)(n + 1024) * 5)) return rc; S->cap_vin = n + 1024; }
+    if (n > S->d_vin.size() / 5) { if (int rc = S->d_vin.allocate(h, st, (size_t)(n + 1024) * 5)) return rc; }
     if (n) CUDA_TRY(cudaMemcpyAsync(S->d_vin, in, (size_t)n * 5 * sizeof(float), cudaMemcpyHostToDevice, st));
     D->ctr.h2d_bytes += (uint64_t)n * 20;
     d_in = S->d_vin;
@@ -1024,7 +999,7 @@ int upload_scan_resident(malio_handle* h, uint32_t* n_total) {
     h->err = "upload_scan_resident: no pose table on the device (run malio_scan_uncertainty* after the last malio_undistort* of the scan)";
     return MALIO_ERR_STATE;
   }
-  return merge_scan(h, S, D, (const malio_pose_entry*)S->d_uout, true, S->res_table_off, S->res_tcomp, n_total);
+  return merge_scan(h, S, D, (const malio_pose_entry*)S->d_uout.data(), true, S->res_table_off, S->res_tcomp, n_total);
 }
 
 // the registration of `source` for world_register: *n_out = its point count n, and the first k = min(n, cap) points go to
@@ -1084,27 +1059,16 @@ int world_accumulate(malio_handle* h, const malio_pass_state* s, const float* sl
   uint64_t n = 0;
   if (int rc = world_count(h, S, D, MALIO_WORLD_DENSE, n)) return rc;
   const uint64_t need = S->n_acc + n;
-  if (need > S->cap_acc) {
+  if (need > S->d_acc.size()) {
     // geometric growth: a larger buffer, the old content copied over on the device, then the old one freed.  A failed
     // allocation leaves the accumulated cloud as it was.
-    uint64_t c = S->cap_acc * 2;
+    uint64_t c = S->d_acc.size() * 2;
     if (c < need) c = need;
     if (c < WORLD_ACC_MIN) c = WORLD_ACC_MIN;
-    float4* p = nullptr;
-    const cudaError_t e = cudaMalloc((void**)&p, c * sizeof(float4));
-    if (e != cudaSuccess) {
-      cudaGetLastError();
+    if (const cudaError_t e = malio_buf::grow_keep(S->stream, {{S->d_acc, c, S->n_acc}})) {
       h->err = std::string("world accumulate: cannot grow the cloud to ") + std::to_string(c) + " points: " + cudaGetErrorString(e);
       return MALIO_ERR_CUDA;
     }
-    if (S->n_acc) {
-      const cudaError_t ec = cudaMemcpyAsync(p, S->d_acc, S->n_acc * sizeof(float4), cudaMemcpyDeviceToDevice, S->stream);
-      const cudaError_t es = ec == cudaSuccess ? cudaStreamSynchronize(S->stream) : ec;
-      if (es != cudaSuccess) { cudaFree(p); h->err = std::string("world accumulate: copy on growth: ") + cudaGetErrorString(es); return MALIO_ERR_CUDA; }
-    }
-    if (S->d_acc) cudaFree(S->d_acc);
-    S->d_acc = p;
-    S->cap_acc = c;
   }
   if (n) {
     if (int rc = world_launch(h, S, D, s, MALIO_WORLD_DENSE, slot_tag, S->d_acc + S->n_acc)) return rc;
@@ -1133,13 +1097,13 @@ int world_save_pcd(malio_handle* h, const char* path, int clear) {
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
   if (S->n_acc == 0) { h->err = "world save: the accumulated cloud is empty (nothing is written)"; return MALIO_ERR_STATE; }
-  if (!S->h_bounce) CUDA_TRY(cudaHostAlloc((void**)&S->h_bounce, (size_t)malio_pcd::CHUNK * sizeof(float4), cudaHostAllocDefault));
+  if (!S->h_bounce) { if (int rc = S->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
   const int rc = malio_pcd::write_binary(path, S->n_acc, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
     if (cudaMemcpyAsync(S->h_bounce, S->d_acc + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
         cudaStreamSynchronize(S->stream) != cudaSuccess)
       return (int)MALIO_ERR_CUDA;
     D->ctr.d2h_bytes += cnt * sizeof(float4);
-    *xyzi = (const float*)S->h_bounce;
+    *xyzi = (const float*)S->h_bounce.data();
     return (int)MALIO_OK;
   }, h->err);
   if (rc == MALIO_OK && clear) S->n_acc = 0;   // pcl_wait_save->clear() (:485); the buffer is kept
@@ -1193,15 +1157,15 @@ int scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_e
   const size_t tab_bytes = (size_t)n_tab * sizeof(malio_pose_entry);
   const size_t out_bytes = tab_bytes + (size_t)(Ln - 1 + (lidar_unc ? n_unc : 0)) * sizeof(malio_pose);
   if (!S->d_ucov) {   // sized for the largest lists: L x MALIO_MAX_COV pops, L - 1 compensations
-    if (int rc = ensure(h, S->d_ucov, (size_t)MALIO_MAX_COV * 36)) return rc;
-    if (int rc = ensure(h, S->d_uout, (size_t)MALIO_MAX_LIDAR * MALIO_MAX_COV * (sizeof(malio_pose_entry) + sizeof(malio_pose)) +
-                                        MALIO_MAX_LIDAR * sizeof(malio_pose)))
+    if (int rc = malio_buf::allocate_group(h, st, {{S->d_ucov, (size_t)MALIO_MAX_COV * 36},
+                                                   {S->d_uout, (size_t)MALIO_MAX_LIDAR * MALIO_MAX_COV * (sizeof(malio_pose_entry) + sizeof(malio_pose)) +
+                                                                   MALIO_MAX_LIDAR * sizeof(malio_pose)}}))
       return rc;
   }
   S->table_resident = false;
   if (a->n_cov) CUDA_TRY(cudaMemcpyAsync(S->d_ucov, a->imu_cov, (size_t)a->n_cov * 36 * sizeof(double), cudaMemcpyHostToDevice, st));
-  malio_pose_entry* d_tab = (malio_pose_entry*)S->d_uout;
-  malio_pose* d_tc = (malio_pose*)(S->d_uout + tab_bytes);
+  malio_pose_entry* d_tab = (malio_pose_entry*)S->d_uout.data();
+  malio_pose* d_tc = (malio_pose*)(S->d_uout.data() + tab_bytes);
   malio_pose* d_unc = d_tc + (Ln - 1);
   scan_unc_kernel<<<(n_thr + UNC_THREADS - 1) / UNC_THREADS, UNC_THREADS, 0, st>>>(c, S->d_ucov, d_tab, d_tc, d_unc);
   CUDA_TRY(cudaGetLastError());

@@ -47,19 +47,18 @@ struct VoxState {
   bool leaf_set = false;
   float leaf = 0.f;
   uint64_t n_vox = 0;                        // entries in use (exact on the host after every call)
-  VKey* d_ekey = nullptr; float4* d_esum = nullptr; uint32_t* d_ecnt = nullptr; uint64_t cap_e = 0;   // entries
-  uint32_t* d_hash = nullptr; uint64_t cap_h = 0;                                                    // power of two
-  // sort area, cap_s rows of 32 B (one allocation): keys | alternate keys (12 B each) | values | alternate values (4 B each),
-  // sized for the points of a scan or, on download and save, for the entries.  A save writes the sorted centroids (16 B a row)
+  DeviceBuffer<VKey> d_ekey; DeviceBuffer<float4> d_esum; DeviceBuffer<uint32_t> d_ecnt;   // entries
+  DeviceBuffer<uint32_t> d_hash;                                                           // power of two
+  // sort area, rows of 32 B (one allocation): keys | alternate keys (12 B each) | values | alternate values (4 B each), sized
+  // for the points of a scan or, on download and save, for the entries.  A save writes the sorted centroids (16 B a row)
   // over the two key halves and then releases the area; a download keeps it until the next save.
-  char* d_sort = nullptr; uint64_t cap_s = 0;
-  // run scratch, cap_p rows of 16 B, sized for the points of a scan only
-  uint32_t *d_head = nullptr, *d_run = nullptr, *d_rent = nullptr, *d_new = nullptr;
-  uint64_t cap_p = 0;
-  char* d_temp = nullptr; size_t cap_temp = 0;   // CUB's temporary storage (sort histograms, scan carries)
-  uint32_t* d_small = nullptr;               // [0] fault flag, [1] run count, [2] entries in use
-  uint32_t* h_small = nullptr;               // pinned mirror of d_small
-  float4* h_bounce = nullptr;                // pinned, malio_pcd::CHUNK points
+  DeviceBuffer<char> d_sort;
+  // run scratch, 16 B a row, sized for the points of a scan only
+  DeviceBuffer<uint32_t> d_head, d_run, d_rent, d_new;
+  DeviceBuffer<char> d_temp;                 // CUB's temporary storage (sort histograms, scan carries)
+  DeviceBuffer<uint32_t> d_small;            // [0] fault flag, [1] run count, [2] entries in use
+  PinnedBuffer<uint32_t> h_small;            // pinned mirror of d_small
+  PinnedBuffer<float4> h_bounce;             // pinned, malio_pcd::CHUNK points
 };
 constexpr size_t SORT_ROW = 2 * sizeof(VKey) + 2 * sizeof(uint32_t);
 constexpr size_t RUN_ROW = 4 * sizeof(uint32_t);
@@ -69,10 +68,12 @@ struct SortBufs {
   cub::DoubleBuffer<VKey> k;
   cub::DoubleBuffer<uint32_t> v;
 };
+uint64_t sort_rows(const VoxState* V) { return V->d_sort.size() / SORT_ROW; }
 SortBufs sort_bufs(const VoxState* V) {
-  VKey* k = reinterpret_cast<VKey*>(V->d_sort);
-  uint32_t* v = reinterpret_cast<uint32_t*>(V->d_sort + 2 * sizeof(VKey) * V->cap_s);
-  return SortBufs{cub::DoubleBuffer<VKey>(k, k + V->cap_s), cub::DoubleBuffer<uint32_t>(v, v + V->cap_s)};
+  const uint64_t rows = sort_rows(V);
+  VKey* k = reinterpret_cast<VKey*>(V->d_sort.data());
+  uint32_t* v = reinterpret_cast<uint32_t*>(V->d_sort + 2 * sizeof(VKey) * rows);
+  return SortBufs{cub::DoubleBuffer<VKey>(k, k + rows), cub::DoubleBuffer<uint32_t>(v, v + rows)};
 }
 
 // the dense cloud: slot of global point p and its undistorted row
@@ -225,27 +226,19 @@ int get_state(malio_handle* h, VoxState*& V) {
   CUDA_TRY(cudaSetDevice(D->device));
   V = new VoxState;
   h->voxmap = V;
-  CUDA_TRY(cudaMalloc((void**)&V->d_small, 4 * sizeof(uint32_t)));
+  if (int rc = V->d_small.allocate(h, D->stream, 4)) return rc;
   CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 4 * sizeof(uint32_t), D->stream));
-  CUDA_TRY(cudaHostAlloc((void**)&V->h_small, 4 * sizeof(uint32_t), cudaHostAllocDefault));
-  return MALIO_OK;
+  return V->h_small.allocate(h, 4);
 }
 
 // CUB's temporary storage for at least t bytes, and the sort area for n rows
 int grow_temp(malio_handle* h, VoxState* V, DeviceState* D, size_t t) {
-  if (t <= V->cap_temp) return MALIO_OK;
-  t += t / 8 + 4096;
-  V->cap_temp = 0;
-  if (int rc = ensure(h, V->d_temp, t)) return rc;
-  V->cap_temp = t;
-  return MALIO_OK;
+  if (t <= V->d_temp.size()) return MALIO_OK;
+  return V->d_temp.allocate(h, D->stream, t + t / 8 + 4096);
 }
 int grow_sort(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
-  if (n > V->cap_s) {
-    const uint64_t c = n + n / 8 + 1024;
-    V->cap_s = 0;
-    if (int rc = ensure(h, V->d_sort, c * SORT_ROW)) return rc;
-    V->cap_s = c;
+  if (n > sort_rows(V)) {
+    if (int rc = V->d_sort.allocate(h, D->stream, (n + n / 8 + 1024) * SORT_ROW)) return rc;
   }
   SortBufs b = sort_bufs(V);
   size_t t = 0;
@@ -254,12 +247,9 @@ int grow_sort(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
 }
 // the run scratch for the n points of a scan
 int grow_runs(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
-  if (n > V->cap_p) {
+  if (n > V->d_head.size()) {
     const uint64_t c = n + n / 8 + 1024;
-    V->cap_p = 0;
-    uint32_t** u[] = {&V->d_head, &V->d_run, &V->d_rent, &V->d_new};
-    for (uint32_t** p : u) if (int rc = ensure(h, *p, c)) return rc;
-    V->cap_p = c;
+    if (int rc = malio_buf::allocate_group(h, D->stream, {{V->d_head, c}, {V->d_run, c}, {V->d_rent, c}, {V->d_new, c}})) return rc;
   }
   size_t t_incl = 0, t_excl = 0;
   uint32_t* un = nullptr;
@@ -271,50 +261,26 @@ int grow_runs(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
 // room for `need` entries and a hash at most half full.  Entries move with a device-side copy, the hash is rebuilt from the
 // entries' keys; a failed allocation leaves the map as it was.
 int grow_table(malio_handle* h, VoxState* V, DeviceState* D, uint64_t need) {
-  uint64_t hc = V->cap_h ? V->cap_h : 2 * VOX_MIN_ENTRIES;
+  uint64_t hc = V->d_hash ? V->d_hash.size() : 2 * VOX_MIN_ENTRIES;
   while (hc < 2 * need) hc *= 2;
-  if (need <= V->cap_e && hc == V->cap_h) return MALIO_OK;
+  if (need <= V->d_ekey.size() && hc == V->d_hash.size()) return MALIO_OK;
   if (need > 0x7FFFFFFFull) { h->err = "world voxel map: more than 2^31 - 1 voxels"; return MALIO_ERR_CAPACITY; }
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
   cudaStream_t st = D->stream;
-  if (need > V->cap_e) {
-    uint64_t c = V->cap_e * 2;
+  if (need > V->d_ekey.size()) {
+    uint64_t c = V->d_ekey.size() * 2;
     if (c < need) c = need;
     if (c < VOX_MIN_ENTRIES) c = VOX_MIN_ENTRIES;
-    VKey* k = nullptr; float4* s = nullptr; uint32_t* n = nullptr;
-    cudaError_t e = cudaMalloc((void**)&k, c * sizeof(VKey));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&s, c * sizeof(float4));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&n, c * sizeof(uint32_t));
-    if (e == cudaSuccess && V->n_vox) {
-      e = cudaMemcpyAsync(k, V->d_ekey, V->n_vox * sizeof(VKey), cudaMemcpyDeviceToDevice, st);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(s, V->d_esum, V->n_vox * sizeof(float4), cudaMemcpyDeviceToDevice, st);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(n, V->d_ecnt, V->n_vox * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    }
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      if (k) cudaFree(k);
-      if (s) cudaFree(s);
-      if (n) cudaFree(n);
+    const uint64_t k = V->n_vox;
+    if (const cudaError_t e = malio_buf::grow_keep(st, {{V->d_ekey, c, k}, {V->d_esum, c, k}, {V->d_ecnt, c, k}})) {
       h->err = std::string("world voxel map: cannot grow to ") + std::to_string(c) + " voxels: " + cudaGetErrorString(e);
       return MALIO_ERR_CUDA;
     }
-    if (V->d_ekey) cudaFree(V->d_ekey);
-    if (V->d_esum) cudaFree(V->d_esum);
-    if (V->d_ecnt) cudaFree(V->d_ecnt);
-    V->d_ekey = k; V->d_esum = s; V->d_ecnt = n; V->cap_e = c;
   }
-  if (hc != V->cap_h) {
-    uint32_t* hp = nullptr;
-    const cudaError_t e = cudaMalloc((void**)&hp, hc * sizeof(uint32_t));
-    if (e != cudaSuccess) {
-      cudaGetLastError();
+  if (hc != V->d_hash.size()) {   // a new table, rebuilt from the entries' keys
+    if (const cudaError_t e = malio_buf::grow_keep(st, {{V->d_hash, hc}})) {
       h->err = std::string("world voxel map: cannot grow the hash to ") + std::to_string(hc) + " slots: " + cudaGetErrorString(e);
       return MALIO_ERR_CUDA;
     }
-    if (V->d_hash) cudaFree(V->d_hash);
-    V->d_hash = hp;
-    V->cap_h = hc;
     CUDA_TRY(cudaMemsetAsync(V->d_hash, 0xFF, hc * sizeof(uint32_t), st));
     if (V->n_vox) {
       vm_rehash_kernel<<<(uint32_t)((V->n_vox + 255) / 256), 256, 0, st>>>(V->d_ekey, (uint32_t)V->n_vox, V->d_hash, hc - 1);
@@ -332,7 +298,7 @@ int enqueue_sorted(malio_handle* h, VoxState* V, DeviceState* D, float4* out, ui
   const uint32_t n = (uint32_t)V->n_vox;
   SortBufs b = sort_bufs(V);
   vm_iota_kernel<<<(n + 255) / 256, 256, 0, st>>>(V->d_ekey, n, b.k.Current(), b.v.Current());
-  size_t t = V->cap_temp;
+  size_t t = V->d_temp.size();
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)n, VKeyDecomposer{}, st));
   vm_centroid_kernel<<<(n + 255) / 256, 256, 0, st>>>(b.v.Current(), n, V->d_esum, V->d_ecnt, out, cap < n ? (uint32_t)cap : n);
   CUDA_TRY(cudaGetLastError());
@@ -354,14 +320,7 @@ int check_leaf(malio_handle* h, const VoxState* V, float leaf) {
 namespace malio_vox {
 
 void destroy(malio_handle* h) {
-  VoxState* V = (VoxState*)h->voxmap;
-  if (!V) return;
-  void* p[] = {V->d_ekey, V->d_esum, V->d_ecnt, V->d_hash, V->d_sort, V->d_head, V->d_run, V->d_rent, V->d_new, V->d_temp,
-               V->d_small};
-  for (void* q : p) if (q) cudaFree(q);
-  if (V->h_small) cudaFreeHost(V->h_small);
-  if (V->h_bounce) cudaFreeHost(V->h_bounce);
-  delete V;
+  delete (VoxState*)h->voxmap;
   h->voxmap = nullptr;
 }
 
@@ -386,21 +345,21 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
     cudaStream_t st = D->stream;
     const PassConst pc = make_pass_const(h, D, s);
     const uint32_t nn = (uint32_t)n, g = (nn + 255) / 256;
-    const uint64_t mask = V->cap_h - 1;
+    const uint64_t mask = V->d_hash.size() - 1;
     CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 2 * sizeof(uint32_t), st));   // fault flag, run count
     SortBufs b = sort_bufs(V);
     vm_key_kernel<<<g, 256, 0, st>>>(c, pc, 1.0f / leaf, nn, b.k.Current(), b.v.Current(), V->d_small);
-    size_t t = V->cap_temp;
+    size_t t = V->d_temp.size();
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)nn, VKeyDecomposer{}, st));
     const VKey* key = b.k.Current();
     const uint32_t* val = b.v.Current();
     vm_head_kernel<<<g, 256, 0, st>>>(key, nn, V->d_head);
-    t = V->cap_temp;
-    CUDA_TRY(cub::DeviceScan::InclusiveSum(V->d_temp, t, V->d_head, V->d_rent, (int)nn, st));
+    t = V->d_temp.size();
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(V->d_temp, t, V->d_head.data(), V->d_rent.data(), (int)nn, st));
     vm_run_kernel<<<g, 256, 0, st>>>(V->d_head, V->d_rent, nn, V->d_run, V->d_small);
     vm_lookup_kernel<<<g, 256, 0, st>>>(V->d_run, key, nn, V->d_small, V->d_hash, mask, V->d_ekey, V->d_rent, V->d_new);
-    t = V->cap_temp;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, V->d_new, V->d_head, (int)nn, st));
+    t = V->d_temp.size();
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, V->d_new.data(), V->d_head.data(), (int)nn, st));
     vm_fold_kernel<<<(nn + 127) / 128, 128, 0, st>>>(c, pc, V->d_run, key, val, nn, V->d_small, V->d_rent, V->d_head,
                                                     V->d_hash, mask, V->d_ekey, V->d_esum, V->d_ecnt);
     vm_count_kernel<<<1, 1, 0, st>>>(V->d_head, V->d_new, V->d_small);
@@ -449,24 +408,24 @@ int save_pcd(malio_handle* h, const char* path, int clear) {
   if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
   const uint64_t n = V->n_vox;
   if (int rc = grow_sort(h, V, D, n)) return rc;
-  if (!V->h_bounce) CUDA_TRY(cudaHostAlloc((void**)&V->h_bounce, (size_t)malio_pcd::CHUNK * sizeof(float4), cudaHostAllocDefault));
-  float4* stage = reinterpret_cast<float4*>(V->d_sort);   // the key halves: 24 B a row, the centroids take 16
+  if (!V->h_bounce) { if (int rc = V->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
+  float4* stage = reinterpret_cast<float4*>(V->d_sort.data());   // the key halves: 24 B a row, the centroids take 16
   if (int rc = enqueue_sorted(h, V, D, stage, n)) return rc;
   const int rc = malio_pcd::write_binary(path, n, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
     if (cudaMemcpyAsync(V->h_bounce, stage + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, D->stream) != cudaSuccess ||
         cudaStreamSynchronize(D->stream) != cudaSuccess)
       return (int)MALIO_ERR_CUDA;
     D->ctr.d2h_bytes += cnt * sizeof(float4);
-    *xyzi = (const float*)V->h_bounce;
+    *xyzi = (const float*)V->h_bounce.data();
     return (int)MALIO_OK;
   }, h->err);
   // the entry-sized sort area and CUB's storage go back: between saves the map holds its entries, its hash and the scan-sized
   // scratch only (the next accumulate regrows the sort area for its scan)
   CUDA_TRY(cudaStreamSynchronize(D->stream));
-  cudaFree(V->d_sort); V->d_sort = nullptr; V->cap_s = 0;
-  cudaFree(V->d_temp); V->d_temp = nullptr; V->cap_temp = 0;
+  V->d_sort.release();
+  V->d_temp.release();
   if (rc == MALIO_OK && clear) {   // an empty map with its buffers kept; the next accumulate fixes the leaf again
-    CUDA_TRY(cudaMemsetAsync(V->d_hash, 0xFF, V->cap_h * sizeof(uint32_t), D->stream));
+    CUDA_TRY(cudaMemsetAsync(V->d_hash, 0xFF, V->d_hash.size() * sizeof(uint32_t), D->stream));
     CUDA_TRY(cudaMemsetAsync(V->d_small + 2, 0, sizeof(uint32_t), D->stream));
     V->n_vox = 0;
     V->leaf_set = false;
@@ -478,10 +437,10 @@ int info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* devi
   VoxState* V;
   if (int rc = get_state(h, V)) return rc;
   if (n_voxels) *n_voxels = V->n_vox;
-  if (capacity) *capacity = V->cap_e;
+  if (capacity) *capacity = V->d_ekey.size();
   if (device_bytes)
-    *device_bytes = V->cap_e * (sizeof(VKey) + sizeof(float4) + sizeof(uint32_t)) + V->cap_h * sizeof(uint32_t) +
-                    V->cap_s * SORT_ROW + V->cap_p * RUN_ROW + V->cap_temp;
+    *device_bytes = V->d_ekey.size() * (sizeof(VKey) + sizeof(float4) + sizeof(uint32_t)) + V->d_hash.size() * sizeof(uint32_t) +
+                    V->d_sort.size() + V->d_head.size() * RUN_ROW + V->d_temp.size();
   return MALIO_OK;
 }
 
