@@ -478,6 +478,68 @@ int malio_map_info(malio_handle* h, uint32_t* n_live, uint32_t* n_slots);
 /* live points in slot order (test / debug): any of xyz (n x 3), normal_y, ids, slots may be NULL */
 int malio_map_download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_t* slots, uint32_t cap, uint32_t* n);
 
+/* ---- localization in a saved map: a prior map of any extent on the device and the local-map window over it ------------------
+ * The reference reads map_file_path and never uses it (parameters.cpp:24).  These calls give it a use: load the saved map once,
+ * then per scan slide the cube lasermap_fov_segment (laserMapping.cpp:171-224) keeps around the sensor over it, and localize
+ * against the window without growing the map.  The window IS the device-resident map above (slots + cell-list index): malio_measure,
+ * malio_ieskf_update, malio_knn*, malio_map_incremental and the device-memory calls work on it unchanged (slot indices, ties).
+ * Without inserts the map is a fixed point set and the live set a pure function of it and the cube, so the device owns it alone.
+ *
+ * malio_prior_map_load / _load_device: the prior (n x 3 xyz, n normal_y, ids NULL = 0..n-1), sorted by tile on the device (20 B
+ * per point, 12 B per occupied tile); it replaces the handle's previous prior and ends the window.  A non-finite point
+ * (MALIO_ERR_INVALID_ARG) or a tile index outside +-2^20 tiles (MALIO_ERR_CAPACITY) refuses the load and keeps the previous prior
+ * and its window.  n == 0 loads an empty prior.  _load_device follows the stream-order and pointer-check contract of the
+ * device-memory entry points (block above malio_knn_device): xyz / normal_y / ids are device memory of the handle's device
+ * (NULL where required, misaligned, host, pinned, managed or other-device -> MALIO_ERR_INVALID_ARG before anything is enqueued);
+ * the handle's stream waits on an event recorded on `stream` on entry, `stream` waits on an event recorded after the last access
+ * to the caller's arrays; n == 0 reads no pointer and enqueues nothing on `stream`.  Like malio_map_build_device the call waits
+ * for the device (the key check, the tile count) before it returns.
+ *
+ * malio_prior_map_window(pos_lid, cube_len, det_range): pos_lid = state.pos + state.rot * ext_t[0] in double (:1056).
+ *   First call after a load, or after malio_map_build* / malio_upload_map* ended the window: the cube is
+ *     vertex_min = (float)(pos - cube_len / 2.0), vertex_max = (float)(pos + cube_len / 2.0)      (:177-185, BoxPointType floats)
+ *   and the device map is rebuilt to hold exactly prior ∩ cube, replacing what it held, as malio_map_build would.
+ *   Later calls: the move test, mov_dist and the new cube are :187-219 with the reference's types (dist_to_map_edge float,
+ *   MOV_THRESHOLD = 1.5f, mov_dist a float of a double max, float vertices).  On a move, old ∖ new dies through the reference's
+ *   cub_needrm slabs (malio_map_delete_boxes, half-open), then prior ∩ (new ∖ old) is appended in slot order and the index is
+ *   committed.  Without a move nothing is enqueued and no device work is done.
+ *   Invariant: in a run that makes no other map calls, the live set after every call is exactly prior ∩ cube, min <= p < max per
+ *   axis.  It holds exactly, not up to rounding: a slab's face and the new cube's face are the same float operation
+ *   (new.max = old.max - mov_dist and the slab's min = old.max - mov_dist; likewise on the other side), and old.min - mov_dist
+ *   rounds to at most old.min, so what the slabs spare of the old cube lies in the new one.  Points added with
+ *   malio_map_add_points* stay live until a slab covers them, as in the reference.
+ *   Slot order is deterministic: prior points enter in tile-key order ((z, y, x) tiles), input order within a tile; two runs give
+ *   the same slots and so the same tie breaks (knn_tie_queries).
+ *   MALIO_ERR_STATE before a load; MALIO_ERR_INVALID_ARG for a non-finite pos_lid, cube_len not finite and > 0 or det_range not
+ *   finite and >= 0; MALIO_ERR_CAPACITY when the cell-list index cannot cover the window's live points (as malio_map_build); after
+ *   an error the next call builds the window afresh.
+ *   rep: initialized / moved on this call, the cube after it, the slabs of this call (half-open), the points they killed, the
+ *   points that entered, and the live points after the window's last commit (on a call without a move: as the previous call left
+ *   them, points added since included once committed).
+ * malio_prior_map_info: points and occupied tiles of the prior, and the device bytes the prior and the window's scratch hold (the
+ * device map's slots are the device-resident map's; any output may be NULL).
+ * malio_prior_map_clear: releases the prior; the device map keeps its points, malio_prior_map_window returns MALIO_ERR_STATE until
+ * the next load. */
+typedef struct malio_window_report {
+  int32_t initialized, moved;      /* first call on this prior / the cube moved on this call */
+  float cube[6];                   /* LocalMap_Points after the call: {min3, max3} */
+  uint32_t n_boxes;
+  float boxes[3 * 6];              /* cub_needrm of this call, {min3, max3} each */
+  uint32_t n_killed, n_entered, n_live;
+} malio_window_report;
+int malio_prior_map_load(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n);
+int malio_prior_map_load_device(malio_handle* h, const float* d_xyz, const float* d_normal_y, const int32_t* d_ids, uint32_t n,
+                                void* stream);
+int malio_prior_map_window(malio_handle* h, const double pos_lid[3], double cube_len, float det_range, malio_window_report* rep);
+int malio_prior_map_info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* device_bytes);
+int malio_prior_map_clear(malio_handle* h);
+/* Host: read a binary PCD file as this library (and pcl::PCDWriter::writeBinary) writes it into n x 4 floats {x, y, z, intensity}.
+ * x y z must be fields of TYPE F, SIZE 4, COUNT 1; intensity (F 4) is optional (0 without it); every other field of fixed size
+ * is skipped.  POINTS must equal WIDTH x HEIGHT and the file must hold POINTS records.  xyzi may be NULL with cap == 0 to ask the
+ * size; *n_out = POINTS, and MALIO_ERR_CAPACITY (nothing read) when cap is smaller.  DATA ascii / binary_compressed, a malformed
+ * or truncated file, or a file that cannot be opened -> MALIO_ERR_INVALID_ARG. */
+int malio_read_pcd(const char* path, float* xyzi, uint64_t cap, uint64_t* n_out);
+
 /* cumulative counters since malio_create: kernels launched by this library, k-NN kernel launches, queries they
  * processed and their summed device time (CUDA events) — what bench.py's roofline is computed from. */
 typedef struct malio_counters {

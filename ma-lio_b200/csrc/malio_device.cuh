@@ -7,6 +7,7 @@
 //   malio_preproc.cu  undistortion, voxel grid, world registration
 //   malio_mapops.cu   the device-resident map and its Add_Points / Delete_Point_Boxes replay
 //   malio_voxmap.cu   the saved map as a voxel map
+//   malio_prior.cu    localization in a prior map: the prior's tile store and the local-map window over it
 #ifndef MALIO_DEVICE_CUH_
 #define MALIO_DEVICE_CUH_
 

@@ -26,6 +26,9 @@ struct malio_handle {
   void* pre = nullptr;   // PreState*, owned by malio_preproc.cu (undistortion / voxel grid buffers)
   void* mapst = nullptr; // MapOpsState*, owned by malio_mapops.cu (device-resident map replay)
   void* voxmap = nullptr; // VoxState*, owned by malio_voxmap.cu (the saved map as a voxel map)
+  void* prior = nullptr;  // PriorState*, owned by malio_prior.cu (localization in a prior map)
+  // counts malio_map::build_from / leave calls: a prior-map window is the device map only while no other call rebuilt or left it
+  uint64_t map_epoch = 0;
   // set while a call that returned after enqueueing (malio_knn_device) still has device-side results to hand over: its
   // traversal fault bit and search statistics.  The next entry point on the handle runs it first (MALIO_SETTLE).
   int (*deferred)(malio_handle* h) = nullptr;
@@ -101,6 +104,11 @@ int world_dense_source(malio_handle* h, const float* ud[MALIO_MAX_LIDAR], uint32
 namespace malio_vox {
 void destroy(malio_handle* h);
 }  // namespace malio_vox
+
+// malio_prior.cu — localization in a prior map
+namespace malio_prior {
+void destroy(malio_handle* h);
+}  // namespace malio_prior
 
 // malio_pcd.cpp — pcl::PCDWriter::writeBinary for PointXYZINormal (host)
 namespace malio_pcd {

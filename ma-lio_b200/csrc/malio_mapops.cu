@@ -326,6 +326,7 @@ void destroy(malio_handle* h) {
 }
 
 void leave(malio_handle* h) {
+  ++h->map_epoch;
   MapOps* M = (MapOps*)h->mapst;
   if (!M) return;
   M->active = false;
@@ -387,6 +388,7 @@ static int build_from(malio_handle* h, const float* xyz, const float* normal_y, 
                       cudaStream_t caller) {
   MapOps* M;
   if (int rc = state(h, M)) return rc;
+  ++h->map_epoch;
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
   if (D->refit_pending) { CUDA_TRY(cudaStreamSynchronize(D->stream2)); D->refit_pending = false; }

@@ -1,8 +1,10 @@
 // malio_pcd.cpp — the saved map's file format: pcl::PCDWriter::writeBinary for pcl::PointXYZINormal, the call that writes
 // pcl_wait_save every pcd_save_interval scans and at shutdown (laserMapping.cpp:484, :1090).  Host code; the header text and
-// the 32-byte record layout live only here, for malio_write_pcd_binary and malio_world_save_pcd alike.
+// the 32-byte record layout live only here, for malio_write_pcd_binary and malio_world_save_pcd alike.  malio_read_pcd reads
+// such a file back (and the other binary layouts PCL writes) for malio_prior_map_load.
 #include <cstdio>
 #include <cstring>
+#include <sstream>
 #include <string>
 #include <vector>
 
@@ -58,4 +60,109 @@ extern "C" int malio_write_pcd_binary(const char* path, const float* xyzi, uint6
     *out = xyzi + 4 * first;
     return (int)MALIO_OK;
   }, err);
+}
+
+namespace {
+
+// the header of a binary PCD file: field offsets within a record, the record size and the point count
+struct PcdLayout {
+  long off[4] = {-1, -1, -1, -1};   // x, y, z, intensity: byte offset in the record, -1 when absent
+  uint64_t rec = 0, n = 0;
+  long data = 0;                     // byte offset of the first record
+};
+
+int parse_header(FILE* f, PcdLayout& L, std::string& err) {
+  std::vector<std::string> fields, types;
+  std::vector<uint64_t> sizes, counts;
+  uint64_t width = 0, height = 0, points = 0;
+  bool has_w = false, has_h = false, has_p = false;
+  char line[4096];
+  for (int lines = 0; lines < 64; ++lines) {
+    if (!std::fgets(line, sizeof(line), f)) { err = "pcd: header ends before its DATA line"; return MALIO_ERR_INVALID_ARG; }
+    std::istringstream ss(line);
+    std::string key;
+    if (!(ss >> key) || key[0] == '#') continue;
+    std::vector<std::string> v;
+    for (std::string w; ss >> w;) v.push_back(w);
+    auto nums = [&](std::vector<uint64_t>& out) {
+      for (const std::string& w : v) {
+        if (w.empty() || w.find_first_not_of("0123456789") != std::string::npos || w.size() > 12) return false;
+        out.push_back(std::stoull(w));
+      }
+      return true;
+    };
+    auto one = [&](uint64_t& out) { std::vector<uint64_t> t; if (v.size() != 1 || !nums(t)) return false; out = t[0]; return true; };
+    bool ok = true;
+    if (key == "FIELDS") fields = v;
+    else if (key == "SIZE") ok = nums(sizes);
+    else if (key == "TYPE") types = v;
+    else if (key == "COUNT") ok = nums(counts);
+    else if (key == "WIDTH") ok = has_w = one(width);
+    else if (key == "HEIGHT") ok = has_h = one(height);
+    else if (key == "POINTS") ok = has_p = one(points);
+    else if (key == "DATA") {
+      if (v.size() != 1 || v[0] != "binary") { err = "pcd: DATA " + (v.empty() ? std::string("?") : v[0]) + " (only binary is read)"; return MALIO_ERR_INVALID_ARG; }
+      if (fields.empty() || sizes.size() != fields.size() || types.size() != fields.size() || !has_w || !has_h || !has_p) {
+        err = "pcd: malformed header (FIELDS / SIZE / TYPE / WIDTH / HEIGHT / POINTS)"; return MALIO_ERR_INVALID_ARG;
+      }
+      if (counts.empty()) counts.assign(fields.size(), 1);
+      if (counts.size() != fields.size()) { err = "pcd: COUNT does not match FIELDS"; return MALIO_ERR_INVALID_ARG; }
+      if (width * height != points) { err = "pcd: POINTS differs from WIDTH x HEIGHT"; return MALIO_ERR_INVALID_ARG; }
+      static const char* names[4] = {"x", "y", "z", "intensity"};
+      for (size_t i = 0; i < fields.size(); ++i) {
+        if (sizes[i] == 0 || sizes[i] > 8 || counts[i] == 0 || counts[i] > 1u << 16) { err = "pcd: field " + fields[i] + " has no fixed size"; return MALIO_ERR_INVALID_ARG; }
+        for (int k = 0; k < 4; ++k)
+          if (fields[i] == names[k]) {
+            if (types[i] != "F" || sizes[i] != 4 || counts[i] != 1) { err = "pcd: field " + fields[i] + " must be TYPE F, SIZE 4, COUNT 1"; return MALIO_ERR_INVALID_ARG; }
+            L.off[k] = (long)L.rec;
+          }
+        L.rec += sizes[i] * counts[i];
+      }
+      if (L.off[0] < 0 || L.off[1] < 0 || L.off[2] < 0) { err = "pcd: fields x y z are required"; return MALIO_ERR_INVALID_ARG; }
+      L.n = points;
+      L.data = std::ftell(f);
+      return MALIO_OK;
+    } else if (key != "VERSION" && key != "VIEWPOINT") { err = "pcd: unknown header line " + key; return MALIO_ERR_INVALID_ARG; }
+    if (!ok) { err = "pcd: malformed " + key + " line"; return MALIO_ERR_INVALID_ARG; }
+  }
+  err = "pcd: no DATA line in the first 64 lines";
+  return MALIO_ERR_INVALID_ARG;
+}
+
+}  // namespace
+
+extern "C" int malio_read_pcd(const char* path, float* xyzi, uint64_t cap, uint64_t* n_out) {
+  if (!path || !n_out || (cap && !xyzi)) return MALIO_ERR_INVALID_ARG;
+  FILE* f = std::fopen(path, "rb");
+  if (!f) return MALIO_ERR_INVALID_ARG;
+  PcdLayout L;
+  std::string err;
+  int rc = parse_header(f, L, err);
+  if (rc == MALIO_OK) {
+    std::fseek(f, 0, SEEK_END);
+    const long end = std::ftell(f);
+    if (end < L.data || (uint64_t)(end - L.data) / L.rec < L.n) rc = MALIO_ERR_INVALID_ARG;   // truncated
+  }
+  if (rc == MALIO_OK) {
+    *n_out = L.n;
+    if (xyzi && cap < L.n) rc = MALIO_ERR_CAPACITY;
+  }
+  if (rc == MALIO_OK && xyzi && L.n) {
+    std::fseek(f, L.data, SEEK_SET);
+    const uint64_t chunk = 1u << 16;
+    std::vector<unsigned char> buf(chunk * L.rec);
+    for (uint64_t first = 0; first < L.n && rc == MALIO_OK; first += chunk) {
+      const uint64_t cnt = (L.n - first) < chunk ? (L.n - first) : chunk;
+      if (std::fread(buf.data(), L.rec, cnt, f) != cnt) { rc = MALIO_ERR_INVALID_ARG; break; }
+      for (uint64_t i = 0; i < cnt; ++i) {
+        float* o = xyzi + 4 * (first + i);
+        for (int k = 0; k < 4; ++k) {
+          if (L.off[k] >= 0) std::memcpy(o + k, &buf[i * L.rec + L.off[k]], 4);
+          else o[k] = 0.f;
+        }
+      }
+    }
+  }
+  std::fclose(f);
+  return rc;
 }

@@ -108,6 +108,12 @@ class Counters(C.Structure):
                 ("exchange_min_wait_ms", C.c_double), ("exchange_sum_wait_ms", C.c_double), ("exchange_passes", C.c_uint64)]
 
 
+class WindowReport(C.Structure):
+    """malio_window_report: what one malio_prior_map_window call did."""
+    _fields_ = [("initialized", C.c_int32), ("moved", C.c_int32), ("cube", C.c_float * 6), ("n_boxes", C.c_uint32),
+                ("boxes", C.c_float * 18), ("n_killed", C.c_uint32), ("n_entered", C.c_uint32), ("n_live", C.c_uint32)]
+
+
 class UpdateReport(C.Structure):
     _fields_ = [("passes", C.c_int32), ("searches", C.c_int32), ("converged_count", C.c_int32),
                 ("last_status", C.c_int32), ("n_eff_last", C.c_uint32), ("ms_device_total", C.c_float),
@@ -131,6 +137,8 @@ EXPORTS = [
     "malio_upload_scan_from_device", "malio_download_aux_device", "malio_map_incremental_device", "malio_world_register_device",
     "malio_undistort_device", "malio_voxel_grid_device", "malio_scan_uncertainty_resident", "malio_upload_scan_resident",
     "malio_world_voxel_accumulate", "malio_world_voxel_download_device", "malio_world_voxel_save_pcd", "malio_world_voxel_info",
+    "malio_prior_map_load", "malio_prior_map_load_device", "malio_prior_map_window", "malio_prior_map_info", "malio_prior_map_clear",
+    "malio_read_pcd",
 ]
 
 
@@ -196,6 +204,12 @@ def load() -> C.CDLL:
     lib.malio_world_voxel_save_pcd.argtypes = [vp, C.c_char_p, i32]
     lib.malio_world_voxel_info.argtypes = [vp, vp, vp, vp]
     lib.malio_write_pcd_binary.argtypes = [C.c_char_p, vp, C.c_uint64]
+    lib.malio_read_pcd.argtypes = [C.c_char_p, vp, C.c_uint64, vp]
+    lib.malio_prior_map_load.argtypes = [vp, vp, vp, vp, u32]
+    lib.malio_prior_map_load_device.argtypes = [vp, vp, vp, vp, u32, vp]
+    lib.malio_prior_map_window.argtypes = [vp, vp, C.c_double, C.c_float, vp]
+    lib.malio_prior_map_info.argtypes = [vp, vp, vp, vp]
+    lib.malio_prior_map_clear.argtypes = [vp]
     lib.malio_measure.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, C.POINTER(PassStats)]
     lib.malio_download_rows.argtypes = [vp, vp, vp, u32, C.POINTER(u32)]
     lib.malio_download_aux.argtypes = [vp, vp, vp, vp, vp, vp]

@@ -95,6 +95,34 @@ def write_pcd_binary(path: str, xyzi: np.ndarray):
         raise capi.MalioError(rc, f"malio_write_pcd_binary({path!r})")
 
 
+def read_pcd(path: str) -> np.ndarray:
+    """A binary PCD file as this library (and pcl::PCDWriter::writeBinary) writes it: float32 (n, 4) {x, y, z, intensity}
+    (intensity 0 when the file has none).  Host code (malio_read_pcd)."""
+    lib = capi.load()
+    n = C.c_uint64(0)
+    rc = lib.malio_read_pcd(os.fsencode(path), None, 0, C.byref(n))
+    if rc != capi.OK:
+        raise capi.MalioError(rc, f"malio_read_pcd({path!r})")
+    out = np.zeros((n.value, 4), np.float32)
+    if n.value:
+        rc = lib.malio_read_pcd(os.fsencode(path), capi.ptr(out), n.value, C.byref(n))
+        if rc != capi.OK:
+            raise capi.MalioError(rc, f"malio_read_pcd({path!r})")
+    return out
+
+
+def pos_lid(s: "capi.State") -> np.ndarray:
+    """pos_lid = state.pos + state.rot * extrinsic_trans[0] (laserMapping.cpp:1056) in float64, the quaternion applied as Eigen's
+    _transformVector: v + w uv + qv x uv, uv = 2 (qv x v)."""
+    q = np.array(s.rot[:], np.float64)
+    v = np.array(s.ext[0].t[:], np.float64)
+    qv = q[1:]
+    uv = np.cross(qv, v)
+    uv = uv + uv
+    r = v + q[0] * uv + np.cross(qv, uv)
+    return np.array(s.pos[:], np.float64) + r
+
+
 class PcdSaver:
     """The pcd_save_en branch of publish_frame_world (laserMapping.cpp:466-488) and the map save at shutdown (:1083-1091) over
     a MeasurementModel: the library keeps pcl_wait_save on the device; the scan counter and the file names live here.
@@ -404,6 +432,46 @@ class MeasurementModel:
         v, c, b = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
         self._check(self.lib.malio_world_voxel_info(self._h, C.byref(v), C.byref(c), C.byref(b)))
         return dict(n_voxels=int(v.value), capacity=int(c.value), device_bytes=int(b.value))
+
+    # ---- localization in a saved map (malio_prior_map_*): the prior on the device and lasermap_fov_segment's window over it
+    def prior_map_load(self, xyz, normal_y=0.001, ids=None):
+        """Load the prior map (replaces the previous one and ends the window).  xyz float32 (n, 3); normal_y a scalar (the map-side
+        weight build_static_snapshot uses by default) or (n,); ids int32 (n,) or None (0..n-1)."""
+        xyz = self._f32(xyz, 3)
+        n = xyz.shape[0]
+        ny = np.full(n, normal_y, np.float32) if np.isscalar(normal_y) else self._f32(normal_y)
+        if ny.shape[0] != n:
+            raise ValueError(f"normal_y: {ny.shape[0]} values for {n} points")
+        i = None if ids is None else np.ascontiguousarray(ids, np.int32)
+        if i is not None and i.shape[0] != n:
+            raise ValueError(f"ids: {i.shape[0]} values for {n} points")
+        self._check(self.lib.malio_prior_map_load(self._h, capi.ptr(xyz), capi.ptr(ny), capi.ptr(i), n))
+
+    def prior_map_load_tensor(self, xyz, normal_y, ids=None):
+        """prior_map_load from CUDA tensors (as map_build_tensor), read in place, ordered on torch.cuda.current_stream()."""
+        self._map_tensor("malio_prior_map_load_device", xyz, normal_y, ids)
+
+    def prior_map_window(self, pos_or_state, cube_len: float = 1000.0, det_range: float = 100.0) -> dict:
+        """lasermap_fov_segment (laserMapping.cpp:171-224) on the device map over the prior.  pos_or_state: pos_lid (3 floats) or a
+        capi.State (pos_lid computed as at :1056).  Returns the report as a dict: initialized, moved, cube float32 (6,), boxes
+        float32 (n_boxes, 6), n_killed, n_entered, n_live."""
+        p = pos_lid(pos_or_state) if isinstance(pos_or_state, capi.State) else np.ascontiguousarray(pos_or_state, np.float64).reshape(3)
+        p = np.ascontiguousarray(p, np.float64)
+        rep = capi.WindowReport()
+        self._check(self.lib.malio_prior_map_window(self._h, capi.ptr(p), C.c_double(cube_len), C.c_float(det_range), C.byref(rep)))
+        return dict(initialized=bool(rep.initialized), moved=bool(rep.moved), cube=np.array(rep.cube[:], np.float32),
+                    boxes=np.array(rep.boxes[:6 * rep.n_boxes], np.float32).reshape(-1, 6),
+                    n_killed=int(rep.n_killed), n_entered=int(rep.n_entered), n_live=int(rep.n_live))
+
+    def prior_map_info(self) -> dict:
+        """Points and occupied tiles of the prior, and the device bytes the prior and its window's scratch hold."""
+        n, t, b = C.c_uint64(0), C.c_uint32(0), C.c_uint64(0)
+        self._check(self.lib.malio_prior_map_info(self._h, C.byref(n), C.byref(t), C.byref(b)))
+        return dict(n_points=int(n.value), n_tiles=int(t.value), device_bytes=int(b.value))
+
+    def prior_map_clear(self):
+        """Release the prior; the device map keeps its points."""
+        self._check(self.lib.malio_prior_map_clear(self._h))
 
     def rearm_scan(self):
         """Reset the per-scan state of the scan already resident on the device (no host copy)."""
