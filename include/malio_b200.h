@@ -533,6 +533,64 @@ int malio_prior_map_load_device(malio_handle* h, const float* d_xyz, const float
 int malio_prior_map_window(malio_handle* h, const double pos_lid[3], double cube_len, float det_range, malio_window_report* rep);
 int malio_prior_map_info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* device_bytes);
 int malio_prior_map_clear(malio_handle* h);
+
+/* ---- relocalization in a loaded prior map: the first pose of a drive, from a guess good to tens of metres and no heading ------
+ * A caller that starts in a saved map knows roll and pitch (gravity), a rough position (GNSS, the last stop) and nothing of the
+ * heading; the IESKF's basin is a few degrees and a few metres.  malio_relocalize closes that gap with an exact search over
+ * n_yaw candidate yaws and a lattice of positions around the guess s, keeping its tilt, on the resident scan and the loaded prior.
+ *
+ * Definitions (tests/reloc_ref.py restates each step):
+ *   1. Candidate rotation k = 0 .. n_yaw-1: theta_k = yaw_lo + (double)k * yaw_step, c = cos(theta_k / 2), s_ = sin(theta_k / 2)
+ *      (the C library's, double, host), q_k = q_yaw(theta_k) (x) s.rot computed as
+ *        w = c*w0 - s_*z0;  x = c*x0 - s_*y0;  y = c*y0 + s_*x0;  z = c*z0 + s_*w0      (host code, no FP contraction)
+ *      a yaw about the prior's z axis applied after the guess's rotation.
+ *   2. Registered points: every point of the resident scan (caller order, its lidar field, the extrinsics of s, the temporal
+ *      compensation of the last upload) as w = body_to_world(s with rot = q_k): the float bits malio_world_register gives for that
+ *      state.  A point with a non-finite w is skipped (in neither score nor n_points).
+ *   3. Voxels: a point's base voxel is floor((double)w_i / res) per axis; a prior point's voxel floor((double)x_i / res)
+ *      (normal_y ignored); a voxel is occupied when any prior point falls in it.
+ *   4. score(k, a, b, c) = the finite points whose base voxel shifted by the integer offset (a, b, c) is occupied, a and b in
+ *      [-half_xy, half_xy], c in [-half_z, half_z].  The shift is an index shift (a translation by res * (a, b, c) in real
+ *      arithmetic) so that no lattice step re-rounds a point.
+ *   5. Result: the maximum score over the n_yaw x (2 half_xy + 1)^2 x (2 half_z + 1) candidates; ties go to the smallest k, then
+ *      c, then b, then a (signed, ascending).  When no candidate scores above 0 the result is the first candidate
+ *      (0, -half_z, -half_xy, -half_xy) with score 0.  rep: rot = q_k, pos[i] = s.pos[i] + (double)offset[i] * res, offset = (a, b, c),
+ *      n_points = the finite points under yaw k.
+ * Search: exact branch-and-bound (malio_reloc.cu).  Level d of an occupancy pyramid holds G_d[v] = OR of the occupancy over
+ * v + [0, 2^d) per axis still split at d; a node (k, d, corner u) is bounded by the sum over the points of G_d[base_k + u], which
+ * no leaf under it exceeds, and is pruned when that bound is below max(best, 1) (strict: optimal leaves and ties survive, so
+ * the tie-break above is exact).  Search memory is O(levels x chunk) nodes whatever the scene; a scene where every candidate
+ * ties (a ground-only prior) takes the exhaustive time in that memory.  rep counts n_candidates, nodes_bounded (nodes whose
+ * bound was computed, leaves included) and leaves_scored; both are deterministic.  device_bytes = the call's scratch (per-yaw
+ * voxel indices, the pyramid, the node lists), all released before it returns.
+ * Errors, each leaving everything as it was:
+ *   MALIO_ERR_INVALID_ARG  NULL h, s, a or rep; n_yaw == 0; res not finite and > 0; a non-finite yaw_lo, yaw_step, s.pos or s.rot
+ *   MALIO_ERR_STATE        before a malio_prior_map_load*; before a scan upload (or after a call that took the scan's buffers,
+ *                          as malio_measure would refuse); with a communicator attached (each rank holds only its block of the scan)
+ *   MALIO_ERR_CAPACITY     more than 2^32 candidates; n_yaw x (12 B x scan points + 36 B) above MALIO_RELOC_MAX_INDEX_BYTES; a
+ *                          registered point's voxel index with |index| >= 2^30; a pyramid box of 2^31 or more voxels along an axis
+ *                          or above MALIO_RELOC_MAX_PYRAMID_BYTES (levels x one bit per voxel of the box the lookups reach: the
+ *                          scan's voxel extent + the lattice + the top window, per axis; a +-100 m box at 0.5 m with a 100 m
+ *                          scan needs about 0.2 GB)
+ * It changes nothing else: the prior, the window and the device map's slots, the resident scan (still measurable) and
+ * malio_prior_map_info stay as they were; of malio_counters only kernel_launches, h2d_bytes and d2h_bytes grow.  Synchronous. */
+#define MALIO_RELOC_MAX_PYRAMID_BYTES (2ull << 30)
+#define MALIO_RELOC_MAX_INDEX_BYTES (4ull << 30)
+typedef struct malio_reloc_args {
+  double yaw_lo, yaw_step;  /* candidate yaws theta_k = yaw_lo + k * yaw_step (double), k = 0 .. n_yaw-1 */
+  uint32_t n_yaw;
+  double res;               /* lattice step = voxel edge, metres */
+  uint32_t half_xy, half_z; /* offsets a, b in [-half_xy, half_xy], c in [-half_z, half_z] (lattice steps) */
+} malio_reloc_args;
+typedef struct malio_reloc_report {
+  double rot[4], pos[3];    /* the best candidate's state rotation (w,x,y,z) and position */
+  int32_t yaw_index, offset[3];
+  uint32_t score, n_points; /* scan points in occupied voxels / scan points with finite registered coordinates */
+  uint64_t n_candidates, nodes_bounded, leaves_scored;
+  uint64_t device_bytes;    /* peak scratch of the call, all released before it returns */
+} malio_reloc_report;
+int malio_relocalize(malio_handle* h, const malio_pass_state* s, const malio_reloc_args* a, malio_reloc_report* rep);
+
 /* Host: read a binary PCD file as this library (and pcl::PCDWriter::writeBinary) writes it into n x 4 floats {x, y, z, intensity}.
  * x y z must be fields of TYPE F, SIZE 4, COUNT 1; intensity (F 4) is optional (0 without it); every other field of fixed size
  * is skipped.  POINTS must equal WIDTH x HEIGHT and the file must hold POINTS records.  xyzi may be NULL with cap == 0 to ask the

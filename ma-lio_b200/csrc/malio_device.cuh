@@ -8,6 +8,7 @@
 //   malio_mapops.cu   the device-resident map and its Add_Points / Delete_Point_Boxes replay
 //   malio_voxmap.cu   the saved map as a voxel map
 //   malio_prior.cu    localization in a prior map: the prior's tile store and the local-map window over it
+//   malio_reloc.cu    relocalization in a loaded prior: branch-and-bound over yaws and a position lattice
 #ifndef MALIO_DEVICE_CUH_
 #define MALIO_DEVICE_CUH_
 

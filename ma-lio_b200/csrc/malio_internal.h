@@ -108,6 +108,9 @@ void destroy(malio_handle* h);
 // malio_prior.cu — localization in a prior map
 namespace malio_prior {
 void destroy(malio_handle* h);
+// the loaded prior's n points as float4 {x, y, z, normal_y} in tile order, device memory of the handle's device, valid until the
+// next load or clear (malio_reloc.cu reads them); MALIO_ERR_STATE before a load
+int points(const malio_handle* h, const float** xyzw, uint32_t* n);
 }  // namespace malio_prior
 
 // malio_pcd.cpp — pcl::PCDWriter::writeBinary for PointXYZINormal (host)

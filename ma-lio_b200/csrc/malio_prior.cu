@@ -467,6 +467,14 @@ int window(malio_handle* h, const double pos[3], double cube_len, float det_rang
   return MALIO_OK;
 }
 
+int points(const malio_handle* h, const float** xyzw, uint32_t* n) {
+  const PriorState* P = (const PriorState*)h->prior;
+  if (!P || !P->loaded) return MALIO_ERR_STATE;
+  *xyzw = reinterpret_cast<const float*>(P->d_pts.data());
+  *n = P->n;
+  return MALIO_OK;
+}
+
 int info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* device_bytes) {
   PriorState* P;
   if (int rc = get_state(h, P)) return rc;

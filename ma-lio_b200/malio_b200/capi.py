@@ -114,6 +114,19 @@ class WindowReport(C.Structure):
                 ("boxes", C.c_float * 18), ("n_killed", C.c_uint32), ("n_entered", C.c_uint32), ("n_live", C.c_uint32)]
 
 
+class RelocArgs(C.Structure):
+    """malio_reloc_args: candidate yaws yaw_lo + k * yaw_step (k < n_yaw) and the lattice (res, half_xy, half_z)."""
+    _fields_ = [("yaw_lo", C.c_double), ("yaw_step", C.c_double), ("n_yaw", C.c_uint32), ("res", C.c_double),
+                ("half_xy", C.c_uint32), ("half_z", C.c_uint32)]
+
+
+class RelocReport(C.Structure):
+    """malio_reloc_report: the best candidate of one malio_relocalize call and what the search did."""
+    _fields_ = [("rot", C.c_double * 4), ("pos", C.c_double * 3), ("yaw_index", C.c_int32), ("offset", C.c_int32 * 3),
+                ("score", C.c_uint32), ("n_points", C.c_uint32), ("n_candidates", C.c_uint64), ("nodes_bounded", C.c_uint64),
+                ("leaves_scored", C.c_uint64), ("device_bytes", C.c_uint64)]
+
+
 class UpdateReport(C.Structure):
     _fields_ = [("passes", C.c_int32), ("searches", C.c_int32), ("converged_count", C.c_int32),
                 ("last_status", C.c_int32), ("n_eff_last", C.c_uint32), ("ms_device_total", C.c_float),
@@ -138,7 +151,7 @@ EXPORTS = [
     "malio_undistort_device", "malio_voxel_grid_device", "malio_scan_uncertainty_resident", "malio_upload_scan_resident",
     "malio_world_voxel_accumulate", "malio_world_voxel_download_device", "malio_world_voxel_save_pcd", "malio_world_voxel_info",
     "malio_prior_map_load", "malio_prior_map_load_device", "malio_prior_map_window", "malio_prior_map_info", "malio_prior_map_clear",
-    "malio_read_pcd",
+    "malio_read_pcd", "malio_relocalize",
 ]
 
 
@@ -210,6 +223,7 @@ def load() -> C.CDLL:
     lib.malio_prior_map_window.argtypes = [vp, vp, C.c_double, C.c_float, vp]
     lib.malio_prior_map_info.argtypes = [vp, vp, vp, vp]
     lib.malio_prior_map_clear.argtypes = [vp]
+    lib.malio_relocalize.argtypes = [vp, vp, vp, vp]
     lib.malio_measure.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, C.POINTER(PassStats)]
     lib.malio_download_rows.argtypes = [vp, vp, vp, u32, C.POINTER(u32)]
     lib.malio_download_aux.argtypes = [vp, vp, vp, vp, vp, vp]

@@ -9,6 +9,7 @@ Everything heavy happens inside libmalio_b200.so on the GPU; this file is marsha
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from dataclasses import dataclass
 
@@ -472,6 +473,29 @@ class MeasurementModel:
     def prior_map_clear(self):
         """Release the prior; the device map keeps its points."""
         self._check(self.lib.malio_prior_map_clear(self._h))
+
+    def relocalize(self, guess: capi.State | capi.PassState, res: float, half_xy: int, half_z: int, n_yaw: int = 360,
+                   yaw_lo: float = 0.0, yaw_step: float | None = None) -> dict:
+        """malio_relocalize: the best of n_yaw yaws (yaw_lo + k * yaw_step, default step 2 pi / n_yaw) about the prior's z axis after
+        guess.rot, and of the integer voxel offsets (a, b) in [-half_xy, half_xy]^2, c in [-half_z, half_z] (steps of res metres)
+        around guess.pos, scored against the loaded prior with the resident scan.  Returns the report's fields as a dict and
+        `state`: a copy of guess with rot and pos replaced, ready for prior_map_window and update_iterated_dyn_share_modified."""
+        ps = guess.pass_state() if isinstance(guess, capi.State) else guess
+        a = capi.RelocArgs()
+        a.n_yaw = int(n_yaw)
+        a.yaw_lo = float(yaw_lo)
+        a.yaw_step = 2.0 * math.pi / max(a.n_yaw, 1) if yaw_step is None else float(yaw_step)
+        a.res, a.half_xy, a.half_z = float(res), int(half_xy), int(half_z)
+        rep = capi.RelocReport()
+        self._check(self.lib.malio_relocalize(self._h, C.byref(ps), C.byref(a), C.byref(rep)))
+        state = type(guess)()
+        C.memmove(C.byref(state), C.byref(guess), C.sizeof(guess))
+        state.rot[:] = rep.rot[:]
+        state.pos[:] = rep.pos[:]
+        return dict(rot=np.array(rep.rot[:]), pos=np.array(rep.pos[:]), yaw_index=int(rep.yaw_index),
+                    offset=tuple(int(v) for v in rep.offset), score=int(rep.score), n_points=int(rep.n_points),
+                    n_candidates=int(rep.n_candidates), nodes_bounded=int(rep.nodes_bounded),
+                    leaves_scored=int(rep.leaves_scored), device_bytes=int(rep.device_bytes), state=state)
 
     def rearm_scan(self):
         """Reset the per-scan state of the scan already resident on the device (no host copy)."""
