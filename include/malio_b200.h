@@ -414,6 +414,59 @@ int malio_world_voxel_accumulate(malio_handle* h, const malio_pass_state* s, con
 int malio_world_voxel_download_device(malio_handle* h, float* d_out, uint64_t cap, uint64_t* n_out, void* stream);
 int malio_world_voxel_save_pcd(malio_handle* h, const char* path, int clear);
 int malio_world_voxel_info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* device_bytes);
+/* Clearing moving objects out of the voxel map: free-space evidence per voxel, counted while the scans are accumulated, and a
+ * save without the voxels that later rays passed straight through (a car's trail along its lane).  tests/carve_ref.py restates
+ * every step in numpy.
+ * malio_world_voxel_accumulate_carve does to the centroids exactly what malio_world_voxel_accumulate does (same bits, same
+ * preconditions and errors), then counts this scan, one scan per call, into two u32 counters per voxel:
+ *   hit(v)  += 1 when at least one finite point of this scan has its key in v
+ *   miss(v) += 1 when v is in the map after this scan's fold, no point of this scan has its key in v, and at least one ray of
+ *           this scan passes v
+ * Both are set semantics over the scan: thread order cannot change them.  Entries created by malio_world_voxel_accumulate
+ * start at hit = miss = 0, and those calls change no counter.
+ * A ray belongs to each finite dense point p of slot l (the points the fold takes, their world bits w):
+ *   origin o = body_to_world(s, l, (0, 0, 0)), the float bits malio_world_register gives for a point at the slot's origin
+ *   u = o * il, e = w * il per axis (float products, il = 1.0f / leaf as for the key); start cell floor(u), end cell floor(e)
+ *   len = sqrt(dx*dx + dy*dy + dz*dz) with d = (double)w - (double)o, sums left to right; lim = fmin(max_range, len - end_margin)
+ *   inv_a = 1.0 / ((double)e_a - (double)u_a); next face of axis a from cell c: ((double)c + (step_a > 0 ? 1.0 : 0.0) -
+ *   (double)u_a) * inv_a, step_a = +-1 towards the end cell.  All in double, no FP contraction.
+ *   The walk takes exactly |di| + |dj| + |dk| steps (ending on floor(e), whatever the rounding); each step moves one cell
+ *   along the axis with steps left whose next face is smallest, ties to x, then y, then z.  A cell's entry parameter t is 0
+ *   for the start cell, else the face value of the step that entered it.
+ *   A visited cell is passed when it is not floor(e) and t * len < lim (strict).
+ * malio_world_voxel_evidence_device: the (hit, miss) pairs (n x 2 u32) in the centroid order of malio_world_voxel_download_device,
+ * with its size protocol and device-memory contract (8-byte alignment).  Zeros for a map that was never carved.
+ * Keep rule: a voxel is dropped when miss >= min_miss and (double)miss > (double)max_miss_per_hit * (double)hit; every other
+ * voxel is kept.  malio_world_voxel_download_kept_device gives the kept centroids in the same order, the bits the unfiltered
+ * download gives for them, with the same size protocol (*n_out = the kept count) and device-memory contract, except that it
+ * waits for the kept count before it enqueues the copy-out.  malio_world_voxel_save_pcd_kept writes them through
+ * malio_world_voxel_save_pcd's writer; MALIO_ERR_STATE (nothing written) on an empty map or when the rule keeps no voxel;
+ * clear != 0 empties the map as that call does and resets the counters (either save's clear resets them).
+ * Refusals, each before anything changes (centroids, counters and entry count stay as they were):
+ *   MALIO_ERR_INVALID_ARG  NULL h, s, slot_tag, a or k; max_range not finite and > 0; end_margin not finite and >= 0;
+ *                          max_miss_per_hit not finite and >= 0; the leaf errors of malio_world_voxel_accumulate
+ *   MALIO_ERR_CAPACITY     (double)max_range * il above MALIO_CARVE_MAX_RANGE_CELLS (a ray visits at most about three times that
+ *                          many cells before it stops being passed); an end or an origin (of a slot with points) whose voxel
+ *                          index falls outside int
+ * With a communicator attached every rank carves what it holds, as malio_world_voxel_accumulate folds it.
+ * Device memory: 12 B per entry (hit, miss and the last scan that counted the entry), allocated by the first carve call, grown
+ * with the entries; 0 for a map that is never carved.  malio_world_voxel_info's device_bytes includes it.  The kept download
+ * and save use the sort area of a download (32 B per voxel) and no more. */
+#define MALIO_CARVE_MAX_RANGE_CELLS 65536.0
+typedef struct malio_carve_args {
+  float max_range;   /* m, finite, > 0: a ray is followed at most this far from its origin */
+  float end_margin;  /* m, finite, >= 0: voxels entered within this distance of the ray's end are not passed */
+} malio_carve_args;
+typedef struct malio_carve_keep {
+  uint32_t min_miss;       /* a voxel is dropped only when miss >= min_miss ... */
+  float max_miss_per_hit;  /* ... and (double)miss > max_miss_per_hit * (double)hit */
+} malio_carve_keep;
+int malio_world_voxel_accumulate_carve(malio_handle* h, const malio_pass_state* s, const float* slot_tag, float leaf,
+                                       const malio_carve_args* a, uint64_t* n_voxels);
+int malio_world_voxel_evidence_device(malio_handle* h, uint32_t* d_hit_miss, uint64_t cap, uint64_t* n_out, void* stream);
+int malio_world_voxel_download_kept_device(malio_handle* h, const malio_carve_keep* k, float* d_out, uint64_t cap,
+                                           uint64_t* n_out, void* stream);
+int malio_world_voxel_save_pcd_kept(malio_handle* h, const char* path, const malio_carve_keep* k, int clear);
 /* Host: the same PCD file from n > 0 host points (n x 4 floats {x, y, z, intensity}): the header of PCDWriter::writeBinary for
  * PointXYZINormal (FIELDS x y z intensity normal_x normal_y normal_z curvature, WIDTH = POINTS = n, HEIGHT 1, DATA binary) and
  * n packed 32-byte records with normal_x/y/z = curvature = 0.  MALIO_ERR_INVALID_ARG for n == 0, a NULL argument or a file

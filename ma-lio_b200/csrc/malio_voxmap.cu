@@ -14,6 +14,12 @@
 //   new entries       numbered by an exclusive scan over the runs in key order (deterministic, whatever the hash layout)
 //   vm_fold_kernel    one thread per run continues its voxel's sums in point order (the points registered again)
 // The map is sorted by key on download / save only.  Compiled with -fmad=false like the rest of the library.
+// Carving (malio_world_voxel_accumulate_carve, DESIGN.md "Clearing moving objects"): the same fold, then per scan
+//   vc_hit_kernel     one thread per run: hit += 1 on the run's entry (rent, or small[2] + rank for a new one), stamp = scan
+//   vc_carve_kernel   one thread per ray (slot origin -> dense point): a double-precision DDA over the voxel indices; every
+//                     passed cell that the hash holds gets miss += 1 once per scan (the first thread to raise its stamp)
+// and on a kept download / save a flag per voxel in key order, an exclusive scan and a compaction of the order, ahead of
+// vm_centroid_kernel's arithmetic (the kept centroids are the unfiltered ones' bits).
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -59,6 +65,11 @@ struct VoxState {
   DeviceBuffer<uint32_t> d_small;            // [0] fault flag, [1] run count, [2] entries in use
   PinnedBuffer<uint32_t> h_small;            // pinned mirror of d_small
   PinnedBuffer<float4> h_bounce;             // pinned, malio_pcd::CHUNK points
+  // carving evidence, 12 B per entry, allocated by the first carve call and grown with the entries.  Entries at or beyond
+  // n_vox hold zeros, so that an entry a later fold creates starts at hit = miss = 0.
+  DeviceBuffer<uint2> d_hm;                  // (hit, miss)
+  DeviceBuffer<uint32_t> d_stamp;            // the last carve scan that hit or passed the entry (0: none)
+  uint32_t carve_scan = 0;                   // carve calls since creation or the last clearing save
 };
 constexpr size_t SORT_ROW = 2 * sizeof(VKey) + 2 * sizeof(uint32_t);
 constexpr size_t RUN_ROW = 4 * sizeof(uint32_t);
@@ -219,6 +230,116 @@ __global__ void __launch_bounds__(256) vm_centroid_kernel(const uint32_t* __rest
   out[r] = make_float4(s.x / cf, s.y / cf, s.z / cf, s.w / cf);
 }
 
+// ------------------------------------------------------------------ carving (malio_world_voxel_accumulate_carve)
+__device__ __forceinline__ bool in_int(float f) { return f >= -2147483648.f && f < 2147483648.f; }
+
+// before the fold: the origin of every slot that has points needs a voxel index in int, like the ends (vm_key_kernel), or
+// the scan is refused through the same fault flag
+__global__ void vc_origin_kernel(VmSlots c, PassConst pc, float il, uint32_t* __restrict__ fault) {
+  const int l = threadIdx.x;
+  if (l >= c.L || c.first[l + 1] == c.first[l]) return;
+  float o[3];
+  body_to_world(pc, l, 0.f, 0.f, 0.f, o);
+  if (!(in_int(floorf(o[0] * il)) && in_int(floorf(o[1] * il)) && in_int(floorf(o[2] * il)))) atomicOr(fault, 1u);
+}
+
+// between the fold and vm_count_kernel (small[2] still counts the entries before this scan): one thread per run
+__global__ void __launch_bounds__(256) vc_hit_kernel(const uint32_t* __restrict__ small, const uint32_t* __restrict__ rent,
+                                                     const uint32_t* __restrict__ rank, uint32_t n, uint2* __restrict__ hm,
+                                                     uint32_t* __restrict__ stamp, uint32_t scan) {
+  const uint32_t r = blockIdx.x * 256u + threadIdx.x;
+  if (small[0] || r >= n || r >= small[1]) return;
+  uint32_t e = rent[r];
+  if (e == RUN_NONE) return;
+  if (e == RUN_NEW) e = small[2] + rank[r];
+  hm[e].x += 1u;
+  stamp[e] = scan;
+}
+
+// one axis of the DDA: the next face's parameter, (face - u) * inv in double (the header's order)
+__device__ __forceinline__ double vc_face(int cell, int step, float u, double inv) {
+  return ((double)cell + (step > 0 ? 1.0 : 0.0) - (double)u) * inv;
+}
+
+// one thread per ray of the scan (after the fold and vm_count_kernel: the hash holds this scan's new entries).  The walk takes
+// exactly |di| + |dj| + |dk| steps from floor(u) to floor(e), each along the eligible axis (steps left) whose next face comes
+// first, ties to x, then y, then z; it stops at the first cell that is not passed (the entry parameters never decrease).
+__global__ void __launch_bounds__(256) vc_carve_kernel(VmSlots c, PassConst pc, float il, uint32_t n, double max_range,
+                                                       double end_margin, const uint32_t* __restrict__ small,
+                                                       const uint32_t* __restrict__ hash, uint64_t mask,
+                                                       const VKey* __restrict__ ekey, uint2* __restrict__ hm,
+                                                       uint32_t* __restrict__ stamp, uint32_t scan) {
+  const uint32_t p = blockIdx.x * 256u + threadIdx.x;
+  if (p >= n || small[0]) return;
+  int l = 0;
+  while (l + 1 < c.L && p >= c.first[l + 1]) ++l;
+  const float* row = c.ud[l] + 5 * (size_t)(p - c.first[l]);
+  float w[3], o[3];
+  body_to_world(pc, l, row[0], row[1], row[2], w);
+  if (!(isfinite(w[0]) && isfinite(w[1]) && isfinite(w[2]))) return;
+  body_to_world(pc, l, 0.f, 0.f, 0.f, o);
+  const double dx = (double)w[0] - (double)o[0], dy = (double)w[1] - (double)o[1], dz = (double)w[2] - (double)o[2];
+  const double len = sqrt(dx * dx + dy * dy + dz * dz);
+  const double lim = fmin(max_range, len - end_margin);
+  const float ux = o[0] * il, uy = o[1] * il, uz = o[2] * il;
+  const float ex = w[0] * il, ey = w[1] * il, ez = w[2] * il;
+  int cx = (int)floorf(ux), cy = (int)floorf(uy), cz = (int)floorf(uz);
+  const int gx = (int)floorf(ex), gy = (int)floorf(ey), gz = (int)floorf(ez);
+  const int sx = gx > cx ? 1 : -1, sy = gy > cy ? 1 : -1, sz = gz > cz ? 1 : -1;
+  uint32_t rx = (uint32_t)(gx > cx ? (long long)gx - cx : (long long)cx - gx);
+  uint32_t ry = (uint32_t)(gy > cy ? (long long)gy - cy : (long long)cy - gy);
+  uint32_t rz = (uint32_t)(gz > cz ? (long long)gz - cz : (long long)cz - gz);
+  const double ix = 1.0 / ((double)ex - (double)ux), iy = 1.0 / ((double)ey - (double)uy), iz = 1.0 / ((double)ez - (double)uz);
+  double tx = rx ? vc_face(cx, sx, ux, ix) : 0.0, ty = ry ? vc_face(cy, sy, uy, iy) : 0.0, tz = rz ? vc_face(cz, sz, uz, iz) : 0.0;
+  double t = 0.0;   // entry parameter of the current cell
+  while ((rx | ry | rz) && t * len < lim) {
+    const VKey k{cz, cy, cx};
+    for (uint64_t s = vhash(k) & mask;; s = (s + 1) & mask) {
+      const uint32_t e = hash[s];
+      if (e == EMPTY) break;
+      if (same(ekey[e], k)) {
+        if (*(volatile const uint32_t*)(stamp + e) != scan && atomicMax(stamp + e, scan) < scan) hm[e].y += 1u;
+        break;
+      }
+    }
+    int a = rx ? 0 : (ry ? 1 : 2);
+    double ta = rx ? tx : (ry ? ty : tz);
+    if (ry && ty < ta) { a = 1; ta = ty; }
+    if (rz && tz < ta) { a = 2; ta = tz; }
+    t = ta;
+    if (a == 0) { cx += sx; --rx; tx = vc_face(cx, sx, ux, ix); }
+    else if (a == 1) { cy += sy; --ry; ty = vc_face(cy, sy, uy, iy); }
+    else { cz += sz; --rz; tz = vc_face(cz, sz, uz, iz); }
+  }
+}
+
+// (hit, miss) of the r-th voxel in key order -> out[r], r < n (zeros for a map that was never carved)
+__global__ void __launch_bounds__(256) vc_evidence_kernel(const uint32_t* __restrict__ order, uint32_t n, const uint2* __restrict__ hm,
+                                                          uint2* __restrict__ out) {
+  const uint32_t r = blockIdx.x * 256u + threadIdx.x;
+  if (r >= n) return;
+  out[r] = hm ? hm[order[r]] : make_uint2(0u, 0u);
+}
+
+// the keep rule on the r-th voxel in key order: dropped when miss >= min_miss and (double)miss > ratio * (double)hit
+__global__ void __launch_bounds__(256) vc_keep_kernel(const uint32_t* __restrict__ order, uint32_t n, const uint2* __restrict__ hm,
+                                                      uint32_t min_miss, double ratio, uint32_t* __restrict__ keep) {
+  const uint32_t r = blockIdx.x * 256u + threadIdx.x;
+  if (r >= n) return;
+  const uint2 v = hm ? hm[order[r]] : make_uint2(0u, 0u);
+  keep[r] = (v.y >= min_miss && (double)v.y > ratio * (double)v.x) ? 0u : 1u;
+}
+
+// the kept entries in key order -> kept[0 .. small[3])
+__global__ void __launch_bounds__(256) vc_compact_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__ keep,
+                                                         const uint32_t* __restrict__ pos, uint32_t n, uint32_t* __restrict__ kept,
+                                                         uint32_t* __restrict__ small) {
+  const uint32_t r = blockIdx.x * 256u + threadIdx.x;
+  if (r >= n) return;
+  if (keep[r]) kept[pos[r]] = order[r];
+  if (r == n - 1) small[3] = pos[r] + keep[r];
+}
+
 int get_state(malio_handle* h, VoxState*& V) {
   V = (VoxState*)h->voxmap;
   if (V) return MALIO_OK;
@@ -271,9 +392,16 @@ int grow_table(malio_handle* h, VoxState* V, DeviceState* D, uint64_t need) {
     if (c < need) c = need;
     if (c < VOX_MIN_ENTRIES) c = VOX_MIN_ENTRIES;
     const uint64_t k = V->n_vox;
-    if (const cudaError_t e = malio_buf::grow_keep(st, {{V->d_ekey, c, k}, {V->d_esum, c, k}, {V->d_ecnt, c, k}})) {
+    const cudaError_t e = V->d_hm ? malio_buf::grow_keep(st, {{V->d_ekey, c, k}, {V->d_esum, c, k}, {V->d_ecnt, c, k}, {V->d_hm, c, k},
+                                                               {V->d_stamp, c, k}})
+                                  : malio_buf::grow_keep(st, {{V->d_ekey, c, k}, {V->d_esum, c, k}, {V->d_ecnt, c, k}});
+    if (e) {
       h->err = std::string("world voxel map: cannot grow to ") + std::to_string(c) + " voxels: " + cudaGetErrorString(e);
       return MALIO_ERR_CUDA;
+    }
+    if (V->d_hm) {   // the evidence of the entries to come starts at zero
+      CUDA_TRY(cudaMemsetAsync(V->d_hm + k, 0, (c - k) * sizeof(uint2), st));
+      CUDA_TRY(cudaMemsetAsync(V->d_stamp + k, 0, (c - k) * sizeof(uint32_t), st));
     }
   }
   if (hc != V->d_hash.size()) {   // a new table, rebuilt from the entries' keys
@@ -291,18 +419,78 @@ int grow_table(malio_handle* h, VoxState* V, DeviceState* D, uint64_t need) {
   return MALIO_OK;
 }
 
-// enqueue the centroids in key order into out[0 .. min(n_vox, cap)) on the handle's stream (sort area already grown).  out may
-// be the sort area itself (its two key halves, 24 B a row): the keys are dead once sorted, the order is read from the values.
-int enqueue_sorted(malio_handle* h, VoxState* V, DeviceState* D, float4* out, uint64_t cap) {
+// enqueue the sort of the entries by key on the handle's stream (sort area already grown): *order = the entries in key order,
+// the values half CUB left current (the other values half and the key halves are free once it is sorted)
+int enqueue_order(malio_handle* h, VoxState* V, DeviceState* D, SortBufs& b) {
   cudaStream_t st = D->stream;
   const uint32_t n = (uint32_t)V->n_vox;
-  SortBufs b = sort_bufs(V);
   vm_iota_kernel<<<(n + 255) / 256, 256, 0, st>>>(V->d_ekey, n, b.k.Current(), b.v.Current());
   size_t t = V->d_temp.size();
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)n, VKeyDecomposer{}, st));
-  vm_centroid_kernel<<<(n + 255) / 256, 256, 0, st>>>(b.v.Current(), n, V->d_esum, V->d_ecnt, out, cap < n ? (uint32_t)cap : n);
+  D->ctr.kernel_launches += 1;
+  return MALIO_OK;
+}
+
+// enqueue the centroids in key order into out[0 .. min(n_vox, cap)) on the handle's stream (sort area already grown).  out may
+// be the sort area itself (its two key halves, 24 B a row): the keys are dead once sorted, the order is read from the values.
+int enqueue_sorted(malio_handle* h, VoxState* V, DeviceState* D, float4* out, uint64_t cap) {
+  const uint32_t n = (uint32_t)V->n_vox;
+  SortBufs b = sort_bufs(V);
+  if (int rc = enqueue_order(h, V, D, b)) return rc;
+  vm_centroid_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(b.v.Current(), n, V->d_esum, V->d_ecnt, out, cap < n ? (uint32_t)cap : n);
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += 1;
+  return MALIO_OK;
+}
+
+// the kept entries in key order (malio_carve_keep), at 20 B into each row of the sort area: behind the centroids a save stages
+// over the key halves (16 B a row), beside the flags' exclusive scan (16 B into the row)
+uint32_t* kept_order(const VoxState* V) { return reinterpret_cast<uint32_t*>(V->d_sort + 20 * sort_rows(V)); }
+
+// sort, flag, scan and compact the entries the keep rule does not drop into kept_order(V); waits for their count (*n_kept)
+int enqueue_kept(malio_handle* h, VoxState* V, DeviceState* D, const malio_carve_keep* keep, uint64_t* n_kept) {
+  cudaStream_t st = D->stream;
+  const uint32_t n = (uint32_t)V->n_vox;
+  SortBufs b = sort_bufs(V);
+  size_t t = 0;
+  uint32_t* un = nullptr;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)n, st));
+  if (int rc = grow_temp(h, V, D, t)) return rc;
+  if (int rc = enqueue_order(h, V, D, b)) return rc;
+  uint32_t* flag = b.v.Alternate();
+  uint32_t* pos = reinterpret_cast<uint32_t*>(V->d_sort + 16 * sort_rows(V));
+  const uint32_t g = (n + 255) / 256;
+  vc_keep_kernel<<<g, 256, 0, st>>>(b.v.Current(), n, V->d_hm, keep->min_miss, (double)keep->max_miss_per_hit, flag);
+  t = V->d_temp.size();
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, flag, pos, (int)n, st));
+  vc_compact_kernel<<<g, 256, 0, st>>>(b.v.Current(), flag, pos, n, kept_order(V), V->d_small);
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 2;
+  CUDA_TRY(cudaMemcpyAsync(V->h_small + 3, V->d_small + 3, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));   // the kept count sizes the caller's output and the file
+  *n_kept = V->h_small[3];
+  return MALIO_OK;
+}
+
+int check_keep(malio_handle* h, const malio_carve_keep* k) {
+  if (!std::isfinite(k->max_miss_per_hit) || k->max_miss_per_hit < 0.f) {
+    h->err = "world voxel keep rule: max_miss_per_hit must be finite and >= 0";
+    return MALIO_ERR_INVALID_ARG;
+  }
+  return MALIO_OK;
+}
+
+// an empty map with its buffers kept (a clearing save); the next accumulate fixes the leaf again
+int clear_map(malio_handle* h, VoxState* V, DeviceState* D) {
+  CUDA_TRY(cudaMemsetAsync(V->d_hash, 0xFF, V->d_hash.size() * sizeof(uint32_t), D->stream));
+  CUDA_TRY(cudaMemsetAsync(V->d_small + 2, 0, sizeof(uint32_t), D->stream));
+  if (V->d_hm) {
+    CUDA_TRY(cudaMemsetAsync(V->d_hm, 0, V->d_hm.size() * sizeof(uint2), D->stream));
+    CUDA_TRY(cudaMemsetAsync(V->d_stamp, 0, V->d_stamp.size() * sizeof(uint32_t), D->stream));
+  }
+  V->n_vox = 0;
+  V->leaf_set = false;
+  V->carve_scan = 0;
   return MALIO_OK;
 }
 
@@ -324,12 +512,22 @@ void destroy(malio_handle* h) {
   h->voxmap = nullptr;
 }
 
-int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, float leaf, uint64_t* n_voxels) {
+// carve == NULL: malio_world_voxel_accumulate; otherwise the same fold, then the scan's hits and passes (checked first)
+int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, float leaf, const malio_carve_args* carve,
+               uint64_t* n_voxels) {
   VoxState* V;
   if (int rc = get_state(h, V)) return rc;
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
+  if (carve && !(std::isfinite(carve->max_range) && carve->max_range > 0.f && std::isfinite(carve->end_margin) && carve->end_margin >= 0.f)) {
+    h->err = "world voxel carve: max_range must be finite and > 0, end_margin finite and >= 0";
+    return MALIO_ERR_INVALID_ARG;
+  }
   if (int rc = check_leaf(h, V, leaf)) return rc;
+  if (carve && (double)carve->max_range * (double)(1.0f / leaf) > MALIO_CARVE_MAX_RANGE_CELLS) {
+    h->err = "world voxel carve: max_range / leaf above MALIO_CARVE_MAX_RANGE_CELLS; the map is unchanged";
+    return MALIO_ERR_CAPACITY;
+  }
   VmSlots c{};
   uint32_t m[MALIO_MAX_LIDAR] = {0, 0, 0};
   if (int rc = malio_pre::world_dense_source(h, c.ud, m)) return rc;
@@ -338,10 +536,17 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
   for (int l = 0; l < c.L; ++l) { c.tag[l] = slot_tag[l]; c.first[l] = (uint32_t)n; n += m[l]; }
   c.first[c.L] = (uint32_t)n;
   if (n > 0x7FFFFFFFull) { h->err = "world voxel map: more than 2^31 - 1 points in one scan"; return MALIO_ERR_CAPACITY; }
+  const uint32_t scan = V->carve_scan + 1;
   if (n) {
     if (int rc = grow_table(h, V, D, V->n_vox + n)) return rc;
     if (int rc = grow_sort(h, V, D, n)) return rc;
     if (int rc = grow_runs(h, V, D, n)) return rc;
+    if (carve && !V->d_hm) {   // the first carve: every entry so far starts at hit = miss = 0
+      const size_t cap = V->d_ekey.size();
+      if (int rc = malio_buf::allocate_group(h, D->stream, {{V->d_hm, cap}, {V->d_stamp, cap}})) return rc;
+      CUDA_TRY(cudaMemsetAsync(V->d_hm, 0, cap * sizeof(uint2), D->stream));
+      CUDA_TRY(cudaMemsetAsync(V->d_stamp, 0, cap * sizeof(uint32_t), D->stream));
+    }
     cudaStream_t st = D->stream;
     const PassConst pc = make_pass_const(h, D, s);
     const uint32_t nn = (uint32_t)n, g = (nn + 255) / 256;
@@ -349,6 +554,7 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
     CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 2 * sizeof(uint32_t), st));   // fault flag, run count
     SortBufs b = sort_bufs(V);
     vm_key_kernel<<<g, 256, 0, st>>>(c, pc, 1.0f / leaf, nn, b.k.Current(), b.v.Current(), V->d_small);
+    if (carve) vc_origin_kernel<<<1, 32, 0, st>>>(c, pc, 1.0f / leaf, V->d_small);
     size_t t = V->d_temp.size();
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)nn, VKeyDecomposer{}, st));
     const VKey* key = b.k.Current();
@@ -362,17 +568,23 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, V->d_new.data(), V->d_head.data(), (int)nn, st));
     vm_fold_kernel<<<(nn + 127) / 128, 128, 0, st>>>(c, pc, V->d_run, key, val, nn, V->d_small, V->d_rent, V->d_head,
                                                     V->d_hash, mask, V->d_ekey, V->d_esum, V->d_ecnt);
+    if (carve) vc_hit_kernel<<<g, 256, 0, st>>>(V->d_small, V->d_rent, V->d_head, nn, V->d_hm, V->d_stamp, scan);
     vm_count_kernel<<<1, 1, 0, st>>>(V->d_head, V->d_new, V->d_small);
+    if (carve)
+      vc_carve_kernel<<<g, 256, 0, st>>>(c, pc, 1.0f / leaf, nn, (double)carve->max_range, (double)carve->end_margin, V->d_small,
+                                         V->d_hash, mask, V->d_ekey, V->d_hm, V->d_stamp, scan);
     CUDA_TRY(cudaGetLastError());
-    D->ctr.kernel_launches += 7;
+    D->ctr.kernel_launches += carve ? 10 : 7;
     CUDA_TRY(cudaMemcpyAsync(V->h_small, V->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));   // the call's one wait: the fault flag and the entry count
     if (V->h_small[0]) {
-      h->err = "world voxel map: leaf size too small for a point's coordinates (voxel index outside int); the map is unchanged";
+      h->err = carve ? "world voxel carve: leaf size too small for a point's or a ray origin's coordinates (voxel index outside int); the map is unchanged"
+                     : "world voxel map: leaf size too small for a point's coordinates (voxel index outside int); the map is unchanged";
       return MALIO_ERR_CAPACITY;
     }
     V->n_vox = V->h_small[2];
   }
+  if (carve) V->carve_scan = scan;
   V->leaf = leaf;
   V->leaf_set = true;
   if (n_voxels) *n_voxels = V->n_vox;
@@ -400,17 +612,89 @@ int download_device(malio_handle* h, float* out, uint64_t cap, uint64_t* n_out, 
   return caller_leave(h, D, caller);
 }
 
-int save_pcd(malio_handle* h, const char* path, int clear) {
+// the (hit, miss) pairs in the order of download_device, with its size protocol and device-memory contract
+int evidence_device(malio_handle* h, uint32_t* out, uint64_t cap, uint64_t* n_out, cudaStream_t caller) {
   VoxState* V;
   if (int rc = get_state(h, V)) return rc;
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
+  const uint64_t n = V->n_vox, k = n < cap ? n : cap;
+  if (out && k) {
+    if (int rc = check_device_ptr(h, D, out, "malio_world_voxel_evidence_device out")) return rc;
+    if (reinterpret_cast<uintptr_t>(out) & 7u) {
+      h->err = "malio_world_voxel_evidence_device out: not 8-byte aligned (the pairs are stored as uint2)";
+      return MALIO_ERR_INVALID_ARG;
+    }
+  }
+  *n_out = n;
+  if (!out || k == 0) return MALIO_OK;
+  if (int rc = grow_sort(h, V, D, n)) return rc;
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  SortBufs b = sort_bufs(V);
+  if (int rc = enqueue_order(h, V, D, b)) return rc;
+  vc_evidence_kernel<<<(uint32_t)((k + 255) / 256), 256, 0, D->stream>>>(b.v.Current(), (uint32_t)k, V->d_hm, reinterpret_cast<uint2*>(out));
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += 1;
+  return caller_leave(h, D, caller);
+}
+
+// the centroids of the kept voxels in the order of download_device; waits for their count before it enqueues the copy-out
+int download_kept_device(malio_handle* h, const malio_carve_keep* keep, float* out, uint64_t cap, uint64_t* n_out, cudaStream_t caller) {
+  VoxState* V;
+  if (int rc = get_state(h, V)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (int rc = check_keep(h, keep)) return rc;
+  if (out && cap && V->n_vox) {
+    if (int rc = check_device_ptr(h, D, out, "malio_world_voxel_download_kept_device out")) return rc;
+    if (reinterpret_cast<uintptr_t>(out) & 15u) {
+      h->err = "malio_world_voxel_download_kept_device out: not 16-byte aligned (the centroids are stored as float4)";
+      return MALIO_ERR_INVALID_ARG;
+    }
+  }
+  uint64_t n = 0;
+  if (V->n_vox) {
+    if (int rc = grow_sort(h, V, D, V->n_vox)) return rc;
+    if (int rc = enqueue_kept(h, V, D, keep, &n)) return rc;
+  }
+  *n_out = n;
+  const uint64_t k = n < cap ? n : cap;
+  if (!out || k == 0) return MALIO_OK;
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  vm_centroid_kernel<<<(uint32_t)((k + 255) / 256), 256, 0, D->stream>>>(kept_order(V), (uint32_t)k, V->d_esum, V->d_ecnt,
+                                                                          reinterpret_cast<float4*>(out), (uint32_t)k);
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += 1;
+  return caller_leave(h, D, caller);
+}
+
+// keep == NULL: every voxel (malio_world_voxel_save_pcd); otherwise the voxels the rule keeps (malio_world_voxel_save_pcd_kept)
+int save_pcd(malio_handle* h, const char* path, const malio_carve_keep* keep, int clear) {
+  VoxState* V;
+  if (int rc = get_state(h, V)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (keep) { if (int rc = check_keep(h, keep)) return rc; }
   if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
-  const uint64_t n = V->n_vox;
+  uint64_t n = V->n_vox;
   if (int rc = grow_sort(h, V, D, n)) return rc;
   if (!V->h_bounce) { if (int rc = V->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
   float4* stage = reinterpret_cast<float4*>(V->d_sort.data());   // the key halves: 24 B a row, the centroids take 16
-  if (int rc = enqueue_sorted(h, V, D, stage, n)) return rc;
+  if (keep) {
+    if (int rc = enqueue_kept(h, V, D, keep, &n)) return rc;
+    if (n == 0) {
+      V->d_sort.release();   // enqueue_kept has waited for the stream
+      V->d_temp.release();
+      h->err = "world voxel save: the keep rule drops every voxel (nothing is written)";
+      return MALIO_ERR_STATE;
+    }
+    vm_centroid_kernel<<<(uint32_t)((n + 255) / 256), 256, 0, D->stream>>>(kept_order(V), (uint32_t)n, V->d_esum, V->d_ecnt, stage,
+                                                                            (uint32_t)n);
+    CUDA_TRY(cudaGetLastError());
+    D->ctr.kernel_launches += 1;
+  } else if (int rc = enqueue_sorted(h, V, D, stage, n)) {
+    return rc;
+  }
   const int rc = malio_pcd::write_binary(path, n, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
     if (cudaMemcpyAsync(V->h_bounce, stage + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, D->stream) != cudaSuccess ||
         cudaStreamSynchronize(D->stream) != cudaSuccess)
@@ -424,11 +708,8 @@ int save_pcd(malio_handle* h, const char* path, int clear) {
   CUDA_TRY(cudaStreamSynchronize(D->stream));
   V->d_sort.release();
   V->d_temp.release();
-  if (rc == MALIO_OK && clear) {   // an empty map with its buffers kept; the next accumulate fixes the leaf again
-    CUDA_TRY(cudaMemsetAsync(V->d_hash, 0xFF, V->d_hash.size() * sizeof(uint32_t), D->stream));
-    CUDA_TRY(cudaMemsetAsync(V->d_small + 2, 0, sizeof(uint32_t), D->stream));
-    V->n_vox = 0;
-    V->leaf_set = false;
+  if (rc == MALIO_OK && clear) {
+    if (int c = clear_map(h, V, D)) return c;
   }
   return rc;
 }
@@ -440,7 +721,8 @@ int info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* devi
   if (capacity) *capacity = V->d_ekey.size();
   if (device_bytes)
     *device_bytes = V->d_ekey.size() * (sizeof(VKey) + sizeof(float4) + sizeof(uint32_t)) + V->d_hash.size() * sizeof(uint32_t) +
-                    V->d_sort.size() + V->d_head.size() * RUN_ROW + V->d_temp.size();
+                    V->d_sort.size() + V->d_head.size() * RUN_ROW + V->d_temp.size() +
+                    V->d_hm.size() * sizeof(uint2) + V->d_stamp.size() * sizeof(uint32_t);
   return MALIO_OK;
 }
 
@@ -451,7 +733,32 @@ extern "C" int malio_world_voxel_accumulate(malio_handle* h, const malio_pass_st
   if (!h || !s) return MALIO_ERR_INVALID_ARG;
   if (!slot_tag) { h->err = "world voxel accumulate: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
   MALIO_SETTLE(h);
-  return malio_vox::accumulate(h, s, slot_tag, leaf, n_voxels);
+  return malio_vox::accumulate(h, s, slot_tag, leaf, nullptr, n_voxels);
+}
+extern "C" int malio_world_voxel_accumulate_carve(malio_handle* h, const malio_pass_state* s, const float* slot_tag, float leaf,
+                                                  const malio_carve_args* a, uint64_t* n_voxels) {
+  if (!h || !s || !a) return MALIO_ERR_INVALID_ARG;
+  if (!slot_tag) { h->err = "world voxel accumulate: the dense cloud needs slot_tag"; return MALIO_ERR_INVALID_ARG; }
+  MALIO_SETTLE(h);
+  return malio_vox::accumulate(h, s, slot_tag, leaf, a, n_voxels);
+}
+extern "C" int malio_world_voxel_evidence_device(malio_handle* h, uint32_t* d_hit_miss, uint64_t cap, uint64_t* n_out, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  if (!n_out || (cap && !d_hit_miss)) return MALIO_ERR_INVALID_ARG;
+  return malio_vox::evidence_device(h, d_hit_miss, cap, n_out, (cudaStream_t)stream);
+}
+extern "C" int malio_world_voxel_download_kept_device(malio_handle* h, const malio_carve_keep* k, float* d_out, uint64_t cap,
+                                                      uint64_t* n_out, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  if (!k || !n_out || (cap && !d_out)) return MALIO_ERR_INVALID_ARG;
+  return malio_vox::download_kept_device(h, k, d_out, cap, n_out, (cudaStream_t)stream);
+}
+extern "C" int malio_world_voxel_save_pcd_kept(malio_handle* h, const char* path, const malio_carve_keep* k, int clear) {
+  if (!h || !path || !k) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_vox::save_pcd(h, path, k, clear);
 }
 extern "C" int malio_world_voxel_download_device(malio_handle* h, float* d_out, uint64_t cap, uint64_t* n_out, void* stream) {
   if (!h) return MALIO_ERR_INVALID_ARG;
@@ -462,7 +769,7 @@ extern "C" int malio_world_voxel_download_device(malio_handle* h, float* d_out, 
 extern "C" int malio_world_voxel_save_pcd(malio_handle* h, const char* path, int clear) {
   if (!h || !path) return MALIO_ERR_INVALID_ARG;
   MALIO_SETTLE(h);
-  return malio_vox::save_pcd(h, path, clear);
+  return malio_vox::save_pcd(h, path, nullptr, clear);
 }
 extern "C" int malio_world_voxel_info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* device_bytes) {
   if (!h) return MALIO_ERR_INVALID_ARG;

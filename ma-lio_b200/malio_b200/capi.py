@@ -127,6 +127,16 @@ class RelocReport(C.Structure):
                 ("leaves_scored", C.c_uint64), ("device_bytes", C.c_uint64)]
 
 
+class CarveArgs(C.Structure):
+    """malio_carve_args: how far a ray of malio_world_voxel_accumulate_carve is followed (m) and the margin before its end (m)."""
+    _fields_ = [("max_range", C.c_float), ("end_margin", C.c_float)]
+
+
+class CarveKeep(C.Structure):
+    """malio_carve_keep: a voxel is dropped when miss >= min_miss and miss > max_miss_per_hit * hit."""
+    _fields_ = [("min_miss", C.c_uint32), ("max_miss_per_hit", C.c_float)]
+
+
 class UpdateReport(C.Structure):
     _fields_ = [("passes", C.c_int32), ("searches", C.c_int32), ("converged_count", C.c_int32),
                 ("last_status", C.c_int32), ("n_eff_last", C.c_uint32), ("ms_device_total", C.c_float),
@@ -152,6 +162,8 @@ EXPORTS = [
     "malio_world_voxel_accumulate", "malio_world_voxel_download_device", "malio_world_voxel_save_pcd", "malio_world_voxel_info",
     "malio_prior_map_load", "malio_prior_map_load_device", "malio_prior_map_window", "malio_prior_map_info", "malio_prior_map_clear",
     "malio_read_pcd", "malio_relocalize",
+    "malio_world_voxel_accumulate_carve", "malio_world_voxel_evidence_device", "malio_world_voxel_download_kept_device",
+    "malio_world_voxel_save_pcd_kept",
 ]
 
 
@@ -216,6 +228,10 @@ def load() -> C.CDLL:
     lib.malio_world_voxel_download_device.argtypes = [vp, vp, C.c_uint64, vp, vp]
     lib.malio_world_voxel_save_pcd.argtypes = [vp, C.c_char_p, i32]
     lib.malio_world_voxel_info.argtypes = [vp, vp, vp, vp]
+    lib.malio_world_voxel_accumulate_carve.argtypes = [vp, vp, vp, C.c_float, vp, vp]
+    lib.malio_world_voxel_evidence_device.argtypes = [vp, vp, C.c_uint64, vp, vp]
+    lib.malio_world_voxel_download_kept_device.argtypes = [vp, vp, vp, C.c_uint64, vp, vp]
+    lib.malio_world_voxel_save_pcd_kept.argtypes = [vp, C.c_char_p, vp, i32]
     lib.malio_write_pcd_binary.argtypes = [C.c_char_p, vp, C.c_uint64]
     lib.malio_read_pcd.argtypes = [C.c_char_p, vp, C.c_uint64, vp]
     lib.malio_prior_map_load.argtypes = [vp, vp, vp, vp, u32]

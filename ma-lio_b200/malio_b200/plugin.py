@@ -124,15 +124,61 @@ def pos_lid(s: "capi.State") -> np.ndarray:
     return np.array(s.pos[:], np.float64) + r
 
 
+# Defaults of the carve and the keep rule (malio_world_voxel_accumulate_carve), chosen with tests/carve_ref.py on the street
+# scene of synth.street_scan (DESIGN.md, "Clearing moving objects"): rays followed 100 m; no voxel entered within 4 m of a ray's
+# end counts as passed (grazing rays over the ground and along façades); a voxel is dropped after at least 2 scans passed it
+# and more than twice as many scans passed it as hit it.
+CARVE_MAX_RANGE = 100.0
+CARVE_END_MARGIN = 4.0
+KEEP_MIN_MISS = 2
+KEEP_MAX_MISS_PER_HIT = 2.0
+
+
+def carve_args(max_range: float = CARVE_MAX_RANGE, end_margin: float = CARVE_END_MARGIN) -> capi.CarveArgs:
+    a = capi.CarveArgs()
+    a.max_range, a.end_margin = float(max_range), float(end_margin)
+    return a
+
+
+def carve_keep(min_miss: int = KEEP_MIN_MISS, max_miss_per_hit: float = KEEP_MAX_MISS_PER_HIT) -> capi.CarveKeep:
+    k = capi.CarveKeep()
+    k.min_miss, k.max_miss_per_hit = int(min_miss), float(max_miss_per_hit)
+    return k
+
+
+def _as_carve(carve) -> capi.CarveArgs | None:
+    """None, True (the defaults), a capi.CarveArgs, or a dict of carve_args' keywords."""
+    if carve is None or carve is False:
+        return None
+    if carve is True:
+        return carve_args()
+    return carve if isinstance(carve, capi.CarveArgs) else carve_args(**carve)
+
+
+def _as_keep(keep) -> capi.CarveKeep | None:
+    """None (every voxel), True (the defaults), a capi.CarveKeep, or a dict of carve_keep's keywords."""
+    if keep is None or keep is False:
+        return None
+    if keep is True:
+        return carve_keep()
+    return keep if isinstance(keep, capi.CarveKeep) else carve_keep(**keep)
+
+
 class PcdSaver:
     """The pcd_save_en branch of publish_frame_world (laserMapping.cpp:466-488) and the map save at shutdown (:1083-1091) over
     a MeasurementModel: the library keeps pcl_wait_save on the device; the scan counter and the file names live here.
     leaf (m, optional): keep the saved map as a voxel map of that leaf instead of the dense cloud (MeasurementModel.voxel_map_*):
-    the files hold one centroid per voxel; the names and the interval logic are the same."""
+    the files hold one centroid per voxel; the names and the interval logic are the same.
+    carve / keep (with leaf): count free-space evidence while accumulating and save only the voxels the keep rule keeps (True
+    for the defaults, or CarveArgs / CarveKeep); see MeasurementModel.voxel_map_accumulate."""
 
-    def __init__(self, model: "MeasurementModel", directory: str, pcd_save_interval: int, leaf: float | None = None):
+    def __init__(self, model: "MeasurementModel", directory: str, pcd_save_interval: int, leaf: float | None = None,
+                 carve=None, keep=None):
         self.model, self.directory, self.interval = model, directory, int(pcd_save_interval)
         self.leaf = None if leaf is None else _check_leaf(leaf)
+        self.carve, self.keep = _as_carve(carve), _as_keep(keep)
+        if self.leaf is None and (self.carve is not None or self.keep is not None):
+            raise ValueError("carve and keep need the voxel map (leaf)")
         self.scan_wait_num = 0
         self.pcd_index = 0
         self.n_wait_save = 0
@@ -140,13 +186,17 @@ class PcdSaver:
     def _accumulate(self, s, slot_tag) -> int:
         if self.leaf is None:
             return self.model.pcd_accumulate(s, slot_tag)
-        return self.model.voxel_map_accumulate(s, slot_tag, self.leaf)
+        if self.carve is None:
+            return self.model.voxel_map_accumulate(s, slot_tag, self.leaf)
+        return self.model.voxel_map_accumulate(s, slot_tag, self.leaf, carve=self.carve)
 
     def _save(self, path, clear):
         if self.leaf is None:
             self.model.pcd_save(path, clear=clear)
-        else:
+        elif self.keep is None:
             self.model.voxel_map_save(path, clear=clear)
+        else:
+            self.model.voxel_map_save(path, clear=clear, keep=self.keep)
 
     def after_update(self, s, slot_tag) -> str | None:
         """Once per scan after the update.  Returns the path written, if any."""
@@ -400,33 +450,63 @@ class MeasurementModel:
         self._check(self.lib.malio_world_save_pcd(self._h, os.fsencode(path), 1 if clear else 0))
 
     # ---- the saved map as a voxel map (malio_world_voxel_*): pcl::VoxelGrid of the accumulated dense cloud, kept per voxel
-    def voxel_map_accumulate(self, s: capi.PassState | capi.State, slot_tag, leaf: float) -> int:
+    def voxel_map_accumulate(self, s: capi.PassState | capi.State, slot_tag, leaf: float, carve=None) -> int:
         """Fold the registered dense cloud into the device's voxel map (leaf in m, fixed by the first call after creation or a
-        clearing save).  Returns the number of voxels."""
+        clearing save).  carve (None, True for the defaults, capi.CarveArgs or a dict of carve_args' keywords): also count this
+        scan's hits and the voxels its rays pass (malio_world_voxel_accumulate_carve).  Returns the number of voxels."""
         leaf = _check_leaf(leaf)
         tag = np.ascontiguousarray(slot_tag, np.float32).reshape(-1)
         if tag.shape[0] != self.n_lidar:
             raise ValueError(f"slot_tag: {tag.shape[0]} values, expected one per LiDAR slot ({self.n_lidar})")
         ps = s.pass_state() if isinstance(s, capi.State) else s
         n = C.c_uint64(0)
-        self._check(self.lib.malio_world_voxel_accumulate(self._h, C.byref(ps), capi.ptr(tag), C.c_float(leaf), C.byref(n)))
+        a = _as_carve(carve)
+        if a is None:
+            self._check(self.lib.malio_world_voxel_accumulate(self._h, C.byref(ps), capi.ptr(tag), C.c_float(leaf), C.byref(n)))
+        else:
+            self._check(self.lib.malio_world_voxel_accumulate_carve(self._h, C.byref(ps), capi.ptr(tag), C.c_float(leaf), C.byref(a),
+                                                                    C.byref(n)))
         return int(n.value)
 
-    def voxel_map_tensor(self):
+    def voxel_map_tensor(self, keep=None):
         """The voxel map's centroids as a CUDA tensor float32 (n, 4) {x, y, z, intensity} in ascending (z, y, x) voxel order,
-        allocated on the current stream.  Returns once the sort and the copy are enqueued."""
+        allocated on the current stream.  Returns once the sort and the copy are enqueued.  keep (None, True for the defaults,
+        capi.CarveKeep or a dict of carve_keep's keywords): only the voxels the keep rule keeps (the call waits for their count)."""
         import torch
         n = C.c_uint64(0)
         st = torch.cuda.current_stream(self.device)
         self._check(self.lib.malio_world_voxel_download_device(self._h, None, 0, C.byref(n), st.cuda_stream))
         out = self._empty((n.value, 4), torch.float32)
+        k = _as_keep(keep)
+        if k is not None:
+            cap = n.value
+            self._check(self.lib.malio_world_voxel_download_kept_device(self._h, C.byref(k), _dptr(out) if cap else None, cap, C.byref(n),
+                                                                        st.cuda_stream))
+            return out[: n.value]
         if n.value:
             self._check(self.lib.malio_world_voxel_download_device(self._h, _dptr(out), n.value, C.byref(n), st.cuda_stream))
         return out
 
-    def voxel_map_save(self, path: str, clear: bool):
-        """The voxel map as a binary PCD file (the writer of pcd_save); clear=True also empties it and releases its leaf."""
-        self._check(self.lib.malio_world_voxel_save_pcd(self._h, os.fsencode(path), 1 if clear else 0))
+    def voxel_map_evidence_tensor(self):
+        """The (hit, miss) counters as a CUDA tensor int32 (n, 2) (the u32 bits; a counter stays below 2^31 for 2^31 scans) in the
+        order of voxel_map_tensor(), allocated on the current stream.  Zeros for a map that was never carved."""
+        import torch
+        n = C.c_uint64(0)
+        st = torch.cuda.current_stream(self.device)
+        self._check(self.lib.malio_world_voxel_evidence_device(self._h, None, 0, C.byref(n), st.cuda_stream))
+        out = self._empty((n.value, 2), torch.int32)
+        if n.value:
+            self._check(self.lib.malio_world_voxel_evidence_device(self._h, _dptr(out), n.value, C.byref(n), st.cuda_stream))
+        return out
+
+    def voxel_map_save(self, path: str, clear: bool, keep=None):
+        """The voxel map as a binary PCD file (the writer of pcd_save); clear=True also empties it, releases its leaf and resets
+        the counters.  keep (as voxel_map_tensor): only the voxels the keep rule keeps."""
+        k = _as_keep(keep)
+        if k is None:
+            self._check(self.lib.malio_world_voxel_save_pcd(self._h, os.fsencode(path), 1 if clear else 0))
+        else:
+            self._check(self.lib.malio_world_voxel_save_pcd_kept(self._h, os.fsencode(path), C.byref(k), 1 if clear else 0))
 
     def voxel_map_info(self) -> dict:
         """Voxels in use, entry capacity and the device bytes the voxel map holds."""

@@ -614,3 +614,108 @@ def undistort_case(n: int = 60000, lidar: int = 0, seed: int = 51, scan_ms: floa
     ext = (q_normalize(EXTRINSICS[lidar][0]), np.array(EXTRINSICS[lidar][1]))
     return dict(pts=pts, beg_time=t0, end_time=end_time, ctrl_t=ctrl_t, ctrl_T=ctrl_T.reshape(-1, 16), imu_cov_t=cov_t,
                 cov_pointer=int(cp), extrinsic=ext)
+
+
+# ------------------------------------------------------------------ a street with traffic, ray-cast (clearing moving objects)
+@dataclass
+class Street:
+    """A straight street along +x: ground z = 0, façades at y = +-half_width up to facade_h, parked boxes beside the right
+    façade, and one car-sized box driving along the other lane.  The sensor drives along y = ego_y at sensor_z."""
+    half_width: float = 8.0
+    facade_h: float = 12.0
+    ego_y: float = 1.5
+    sensor_z: float = 1.8
+    ego_x0: float = 0.0
+    ego_step: float = 0.5          # m per scan
+    car_y: float = -2.5
+    car_x0: float = 20.0
+    car_step: float = -1.5         # m per scan (oncoming)
+    car_size: tuple = (4.5, 1.8, 1.4)
+    car_z0: float = 0.25
+    max_range: float = 80.0        # the sensor returns nothing beyond this
+    noise: float = 0.01            # m, range noise (1 sigma)
+
+    def parked(self) -> list:
+        return [(np.array([x, 4.6, 0.0]), np.array([x + 4.0, 6.4, 1.4])) for x in np.arange(-12.0, 48.0, 9.0)]
+
+    def car(self, k: int):
+        sx, sy, sz = self.car_size
+        x = self.car_x0 + self.car_step * k
+        return np.array([x - sx / 2, self.car_y - sy / 2, self.car_z0]), np.array([x + sx / 2, self.car_y + sy / 2, self.car_z0 + sz])
+
+    def ego(self, k: int) -> np.ndarray:
+        return np.array([self.ego_x0 + self.ego_step * k, self.ego_y, self.sensor_z])
+
+
+def _ray_box(O, D, lo, hi):
+    """Entry parameter of rays O + t D (t > 0) into an axis-aligned box, inf where they miss it."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        t1, t2 = (lo - O) / D, (hi - O) / D
+    tn = np.nanmax(np.minimum(t1, t2), axis=1)
+    tf = np.nanmin(np.maximum(t1, t2), axis=1)
+    return np.where((tf >= tn) & (tn > 1e-6), tn, np.inf)
+
+
+def street_cast(street: Street, k: int, O: np.ndarray, D: np.ndarray, rng):
+    """Cast unit rays D from O at scan k.  Returns (hit points float64 (m, 3), what float (m,): 0 ground, 1 façade, 2 parked,
+    3 the moving car), rays without a return dropped."""
+    n = D.shape[0]
+    best = np.full(n, np.inf)
+    what = np.full(n, -1)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        tg = np.where(D[:, 2] < 0, -O[:, 2] / D[:, 2], np.inf)
+        best, what = np.where(tg < best, tg, best), np.where(tg < best, 0, what)
+        for y in (street.half_width, -street.half_width):
+            tw = (y - O[:, 1]) / D[:, 1]
+            z = O[:, 2] + tw * D[:, 2]
+            tw = np.where((tw > 0) & (z >= 0) & (z <= street.facade_h), tw, np.inf)
+            best, what = np.where(tw < best, tw, best), np.where(tw < best, 1, what)
+    for lo, hi in street.parked():
+        tb = _ray_box(O, D, lo, hi)
+        best, what = np.where(tb < best, tb, best), np.where(tb < best, 2, what)
+    lo, hi = street.car(k)
+    tb = _ray_box(O, D, lo, hi)
+    best, what = np.where(tb < best, tb, best), np.where(tb < best, 3, what)
+    ok = best <= street.max_range
+    t = best[ok] + rng.normal(0.0, street.noise, int(ok.sum()))
+    return O[ok] + t[:, None] * D[ok], what[ok]
+
+
+def _spinning_dirs(n_el: int, n_az: int, az0: float) -> np.ndarray:
+    el = np.radians(np.linspace(-22.5, 22.5, n_el))
+    az = az0 + np.arange(n_az) * (2 * np.pi / n_az)
+    E, A = np.meshgrid(el, az, indexing="ij")
+    return np.stack([np.cos(E) * np.cos(A), np.cos(E) * np.sin(A), np.sin(E)], axis=-1).reshape(-1, 3)
+
+
+def _cone_dirs(n: int, yaw: float, rng) -> np.ndarray:
+    a = yaw + rng.uniform(-np.radians(35), np.radians(35), n)
+    e = rng.uniform(-np.radians(25), np.radians(10), n)
+    return np.stack([np.cos(e) * np.cos(a), np.cos(e) * np.sin(a), np.sin(e)], axis=1)
+
+
+STREET_EXT_T = [np.zeros(3), np.array([0.4, 0.3, 0.1]), np.array([-0.4, -0.3, 0.1])]   # slot origins relative to the sensor
+
+
+def street_scan(street: Street, k: int, L: int = 1, spin=(32, 128), cone: int = 0, seed: int = 0):
+    """Scan k of the drive as L slots.  Slot 0 spins (spin = (elevations, azimuths), the azimuths shifted per scan); slots 1 and 2
+    look forward and backward with `cone` random rays each.  Returns dict(state, body: L float32 (m_l, 3) clouds in their slot's
+    frame (identity rotations, the slot's translation in the state's extrinsics), what: L int arrays (street_cast's labels))."""
+    rng = np.random.default_rng((seed, k))
+    pos = street.ego(k)
+    body, what = [], []
+    for l in range(L):
+        o = pos + STREET_EXT_T[l]
+        D = _spinning_dirs(spin[0], spin[1], rng.uniform(0, 2 * np.pi / spin[1])) if l == 0 else _cone_dirs(cone, 0.0 if l == 1 else np.pi, rng)
+        p, wh = street_cast(street, k, np.broadcast_to(o, D.shape), D, rng)
+        body.append((p - o).astype(np.float32))
+        what.append(wh)
+    qid = np.array([1.0, 0.0, 0.0, 0.0])
+    state = make_state(pos, qid, [qid] * L, STREET_EXT_T[:L])
+    return dict(state=state, body=body, what=what)
+
+
+def street_scan_city(street: Street, k: int, seed: int = 0):
+    """A City-size scan: 128 x 1024 spinning rays and 2 x 24000 cone rays (slots 0, 1, 2), before the rays without a return
+    are dropped."""
+    return street_scan(street, k, L=3, spin=(128, 1024), cone=24000, seed=seed)
