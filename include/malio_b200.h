@@ -644,6 +644,114 @@ typedef struct malio_reloc_report {
 } malio_reloc_report;
 int malio_relocalize(malio_handle* h, const malio_pass_state* s, const malio_reloc_args* a, malio_reloc_report* rep);
 
+/* ---- relocalization without a position guess: place descriptors of the prior, each candidate checked by malio_relocalize -------
+ * malio_relocalize needs a position good to tens of metres.  Without one (no GNSS fix, a lost track), malio_place_db_build
+ * describes every place of the loaded prior once, and malio_relocalize_global ranks them against the resident scan in
+ * milliseconds and hands the best few, each in a small box, to malio_relocalize.  Every stage is integer once the heights are
+ * binned, so tests/place_ref.py restates each step bit for bit.  All arithmetic below is IEEE double, no FP contraction.
+ *
+ * 1. Binning table (host, once per build).  Stencil: every integer column offset (ox, oy) != (0, 0) with
+ *    x^2 + y^2 < r_max^2, x = ox * cell, y = oy * cell; the sensor's own column is not in it.  Ring: the number of k in
+ *    1 .. n_ring-1 with x^2 + y^2 >= rk^2, rk = r_max * k / n_ring (so an offset on a ring boundary goes to the outer ring).
+ *    Sector (n_sector % 4 == 0, Q = n_sector / 4): quadrant q = 0 for x > 0, y >= 0; 1 for x <= 0, y > 0; 2 for x < 0, y <= 0;
+ *    3 for x >= 0, y < 0.  (u, v) = (x, y), (y, -x), (-x, -y), (-y, x) for q = 0 .. 3 turns the offset into quadrant 0; the sector
+ *    is q * Q + the number of j in 1 .. Q-1 with bx_j * v - by_j * u >= 0, where (bx_j, by_j) = (cos phi_j, sin phi_j),
+ *    phi_j = 2 pi j / n_sector (the C library's, host), and bx_j = by_j = sqrt(0.5) when 8 j == n_sector.  So an offset on a
+ *    sector boundary goes to the counter-clockwise sector, and a quarter-turned offset (-oy, ox) lands exactly Q sectors on.
+ *    Bin = ring * n_sector + sector.
+ * 2. Level of a column height z_rel (metres above the sensor): 0 (empty) when z_rel < z_lo, else
+ *    1 + clamp(floor((z_rel - z_lo) / dz), 0, 14).  A bin's value is the maximum level of its columns, capped per ring at
+ *    cap_r = the level of rho_r * tan(fov_up) (rho_r = r_max * ring / n_ring, the ring's inner radius; host tan), never below 1;
+ *    no cap when fov_up >= pi/2.  The cap keeps near tall walls comparable between a map and a scan whose beams stop at fov_up.
+ *    Occlusion (block_level > 0): in every sector, the bins of the rings beyond the first ring whose value is >= block_level
+ *    are set to 0, so that a map, which holds what lies behind a wall and the roof over a building's footprint, compares with a
+ *    scan, which does not.  Ring key: per ring, the sum of its bin values after that (rotation-invariant exactly).
+ * 3. Database (malio_place_db_build): column (i, j) = (floor((double)x / cell), floor((double)y / cell)) of every prior point;
+ *    colmax / colmin = the largest / smallest z (float) of a column's points.  Positions: every occupied column whose i and j are
+ *    multiples of m = step / cell, ordered by (j, i) ascending; its sensor sits at ((i + 0.5) cell, (j + 0.5) cell, z_s) with
+ *    z_s = (double)colmin + sensor_height (the slot-0 origin's height above ground, from calibration).  Its descriptor takes, for
+ *    every stencil offset whose column (i + ox, j + oy) is occupied, z_rel = (double)colmax - z_s.
+ * 4. Query (malio_relocalize_global, step 1): every finite point of the resident scan registered as body_to_world with s.pos = 0
+ *    (the bits malio_world_register gives), o = the slot-0 origin registered the same way (body point 0 of LiDAR 0);
+ *    rel = (double)w - (double)o per axis; column offset floor(rel / cell + 0.5) in x and y (the sensor on a column centre, as a
+ *    database position); a column's height is the largest rel z of its points; then the table, levels and caps of the database.
+ * 5. Stage 1: d1(p) = sum over rings of |key_q[r] - key_p[r]|; keep the k1 smallest (d1, p).  Stage 2: for those,
+ *    d2(p) = min over shifts s of sum_r sum_c |Q[r][c] - D_p[r][(c + s) mod n_sector]|, ties to the smallest s; keep the k2 smallest
+ *    (d2, p).  Stage 3: for each kept p in that order, malio_relocalize from the state s with rot = q_yaw(theta) (x) s.rot
+ *    (theta = shift * 2 pi / n_sector, malio_relocalize's product and cos / sin) and pos = (x_p, y_p, z_s) - rot * ext_t[0]
+ *    (q_rot of step 4, so that the slot-0 origin sits at the position), the yaws of +-1.5 sectors:
+ *    n_yaw = 2 * ceil(1.5 * (2 pi / n_sector) / yaw_step) + 1, yaw_lo = -(double)(n_yaw / 2) * yaw_step, and the lattice res,
+ *    half_xy, half_z.  The result is the highest verified score, ties to the lower rank; rep holds its pose, score and n_points as
+ *    malio_reloc_report does.  With no position (an empty prior) the result is s itself with score 0 and n_candidates 0.
+ *
+ * malio_place_db_build: replaces any database of the handle (a failed build leaves none).  Device memory: two 4 B column grids
+ * over the prior's column bounding box during the build (MALIO_PLACE_MAX_GRID_BYTES), then per position 16 B + n_ring x n_sector
+ * / 2 B of nibbles + 2 B per ring key (MALIO_PLACE_MAX_DB_BYTES).  Any later malio_prior_map_load* (refused or not) or
+ * malio_prior_map_clear releases the database; malio_prior_map_info does not count it.  Errors: MALIO_ERR_INVALID_ARG (NULL h, a
+ * or rep; cell / step / r_max / dz not finite and > 0; step not a positive integer multiple of cell; n_ring == 0; n_sector not a
+ * positive multiple of 4; n_ring x n_sector > MALIO_PLACE_MAX_BINS; r_max / cell > MALIO_PLACE_MAX_RADIUS_CELLS; sensor_height or
+ * z_lo not finite; fov_up NaN; block_level > 15), MALIO_ERR_STATE (before a prior load), MALIO_ERR_CAPACITY (a column index outside +-2^30, or
+ * either byte limit).
+ * malio_place_db_download (test / debug): positions in order, any output may be NULL: cols n x 2 (i, j), z_s n, nibbles n x
+ * bytes_per_position (bin b in byte b / 2, low nibble for even b), ring_keys n x n_ring.  *n = the count; at most cap written.
+ * malio_relocalize_global: MALIO_ERR_INVALID_ARG (NULL h, s, a or rep; k1 == 0 or > MALIO_PLACE_MAX_K1; k2 == 0, > k1 or >
+ * MALIO_PLACE_MAX_K2; yaw_step not finite and > 0; a non-finite s.rot; malio_relocalize's argument errors), MALIO_ERR_STATE
+ * (before a prior load, before a database build, before a scan upload, a communicator attached), MALIO_ERR_CAPACITY (from
+ * malio_relocalize).  It changes nothing else (prior, window, device map, resident scan, database); of malio_counters only
+ * kernel_launches, h2d_bytes and d2h_bytes grow.  Synchronous. */
+#define MALIO_PLACE_MAX_BINS 4096
+#define MALIO_PLACE_MAX_RADIUS_CELLS 256
+#define MALIO_PLACE_MAX_K1 1024
+#define MALIO_PLACE_MAX_K2 32
+#define MALIO_PLACE_MAX_GRID_BYTES (4ull << 30)
+#define MALIO_PLACE_MAX_DB_BYTES (8ull << 30)
+typedef struct malio_place_args {
+  double cell, step, r_max;           /* column edge, lattice step (a multiple of cell), stencil radius: metres (1, 1, 60) */
+  uint32_t n_ring, n_sector;          /* 20, 72 */
+  double sensor_height;               /* the slot-0 origin's height above the ground, metres */
+  double z_lo, dz;                    /* level 1 starts at z_lo (-sensor_height + 0.5: the ground is empty), dz per level (1 m) */
+  double fov_up;                      /* the LiDARs' upward field of view, radians; >= pi/2 turns the cap off */
+  uint32_t block_level;               /* occlusion: a bin of at least this level hides the rings behind it (2); 0 = off */
+} malio_place_args;
+typedef struct malio_place_db_report {
+  uint64_t n_positions;
+  uint32_t grid_nx, grid_ny;          /* column grid over the prior's bounding box */
+  uint32_t n_stencil, bytes_per_position;
+  uint64_t device_bytes;              /* the database as it stays on the device */
+  uint64_t scratch_bytes;             /* peak scratch of the build (grids, flags, scan), released before it returns */
+} malio_place_db_report;
+typedef struct malio_global_args {
+  uint32_t k1, k2;                    /* stage-1 and stage-2 survivors (256, 8) */
+  double yaw_step;                    /* verification yaw step, radians (1 degree) */
+  double res;                         /* verification lattice step, metres (0.5) */
+  uint32_t half_xy, half_z;           /* verification box (ceil(step / (2 res)) + 2, 2) */
+} malio_global_args;
+typedef struct malio_global_candidate {
+  uint32_t position, shift;           /* database index, sector shift */
+  uint32_t d1, d2;                    /* ring-key and bin distances */
+  int32_t col[2];                     /* the position's column (i, j) */
+  double z_s;
+  double guess_rot[4], guess_pos[3];  /* the state handed to malio_relocalize */
+  double rot[4], pos[3];              /* its result */
+  uint32_t score, n_points;
+} malio_global_candidate;
+typedef struct malio_global_report {
+  double rot[4], pos[3];              /* the best verified pose (rot w,x,y,z) */
+  uint32_t score, n_points, best_rank;
+  uint32_t n_candidates;              /* candidates verified: min(k2, positions) */
+  uint32_t n_stage1;                  /* min(k1, positions) */
+  malio_reloc_args verify;            /* the malio_relocalize arguments of every candidate */
+  malio_global_candidate cand[MALIO_PLACE_MAX_K2];
+  uint32_t stage1[MALIO_PLACE_MAX_K1], stage1_d1[MALIO_PLACE_MAX_K1];   /* the stage-1 list in rank order */
+  uint8_t query[MALIO_PLACE_MAX_BINS];                                  /* the query's bin values */
+  double ms_rank, ms_verify;          /* host clock: query descriptor + stages 1-2; stage 3 */
+  uint64_t device_bytes;              /* peak scratch of the call (malio_relocalize's included), released before it returns */
+} malio_global_report;
+int malio_place_db_build(malio_handle* h, const malio_place_args* a, malio_place_db_report* rep);
+int malio_place_db_info(malio_handle* h, uint64_t* n_positions, uint64_t* device_bytes);
+int malio_place_db_download(malio_handle* h, int32_t* cols, double* z_s, uint8_t* nibbles, uint16_t* ring_keys, uint64_t cap, uint64_t* n);
+int malio_relocalize_global(malio_handle* h, const malio_pass_state* s, const malio_global_args* a, malio_global_report* rep);
+
 /* Host: read a binary PCD file as this library (and pcl::PCDWriter::writeBinary) writes it into n x 4 floats {x, y, z, intensity}.
  * x y z must be fields of TYPE F, SIZE 4, COUNT 1; intensity (F 4) is optional (0 without it); every other field of fixed size
  * is skipped.  POINTS must equal WIDTH x HEIGHT and the file must hold POINTS records.  xyzi may be NULL with cap == 0 to ask the

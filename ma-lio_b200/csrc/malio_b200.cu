@@ -220,6 +220,7 @@ void destroy(malio_handle* h) {
   h->deferred = nullptr;
   malio_pre::destroy(h);
   malio_vox::destroy(h);
+  malio_place::destroy(h);
   malio_prior::destroy(h);
   malio_map::destroy(h);
   if (D->host_prof && D->host_passes)

@@ -9,6 +9,7 @@
 //   malio_voxmap.cu   the saved map as a voxel map
 //   malio_prior.cu    localization in a prior map: the prior's tile store and the local-map window over it
 //   malio_reloc.cu    relocalization in a loaded prior: branch-and-bound over yaws and a position lattice
+//   malio_place.cu    relocalization without a position guess: place descriptors of the prior, ranked, each checked by malio_reloc
 #ifndef MALIO_DEVICE_CUH_
 #define MALIO_DEVICE_CUH_
 

@@ -27,6 +27,7 @@ struct malio_handle {
   void* mapst = nullptr; // MapOpsState*, owned by malio_mapops.cu (device-resident map replay)
   void* voxmap = nullptr; // VoxState*, owned by malio_voxmap.cu (the saved map as a voxel map)
   void* prior = nullptr;  // PriorState*, owned by malio_prior.cu (localization in a prior map)
+  void* place = nullptr;  // PlaceDb*, owned by malio_place.cu (place descriptors of the prior)
   // counts malio_map::build_from / leave calls: a prior-map window is the device map only while no other call rebuilt or left it
   uint64_t map_epoch = 0;
   // set while a call that returned after enqueueing (malio_knn_device) still has device-side results to hand over: its
@@ -112,6 +113,17 @@ void destroy(malio_handle* h);
 // next load or clear (malio_reloc.cu reads them); MALIO_ERR_STATE before a load
 int points(const malio_handle* h, const float** xyzw, uint32_t* n);
 }  // namespace malio_prior
+
+// malio_reloc.cu — relocalization in a loaded prior (malio_relocalize after its NULL checks; malio_place.cu verifies with it)
+namespace malio_reloc {
+int relocalize(malio_handle* h, const malio_pass_state* s, const malio_reloc_args* a, malio_reloc_report* rep);
+}  // namespace malio_reloc
+
+// malio_place.cu — place descriptors of the prior; destroy drains the stream and releases the database (a prior load or clear,
+// the handle's destroy)
+namespace malio_place {
+void destroy(malio_handle* h);
+}  // namespace malio_place
 
 // malio_pcd.cpp — pcl::PCDWriter::writeBinary for PointXYZINormal (host)
 namespace malio_pcd {

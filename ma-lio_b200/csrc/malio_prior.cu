@@ -363,6 +363,7 @@ void destroy(malio_handle* h) {
 int load(malio_handle* h, const float* xyz, const float* ny, const int32_t* ids, uint32_t n, bool on_device, cudaStream_t caller) {
   PriorState* P;
   if (int rc = get_state(h, P)) return rc;
+  malio_place::destroy(h);   // the place database describes the prior this load replaces
   DeviceState* D = (DeviceState*)h->dev;
   CUDA_TRY(cudaSetDevice(D->device));
   if (n == 0) return load_empty(h, P, D);
@@ -487,6 +488,7 @@ int info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* devic
 }
 
 int clear(malio_handle* h) {
+  malio_place::destroy(h);
   PriorState* P = (PriorState*)h->prior;
   if (!P) return MALIO_OK;
   DeviceState* D = (DeviceState*)h->dev;

@@ -127,6 +127,43 @@ class RelocReport(C.Structure):
                 ("leaves_scored", C.c_uint64), ("device_bytes", C.c_uint64)]
 
 
+PLACE_MAX_BINS, PLACE_MAX_K1, PLACE_MAX_K2 = 4096, 1024, 32   # MALIO_PLACE_MAX_*
+
+
+class PlaceArgs(C.Structure):
+    """malio_place_args: column edge, lattice step, stencil radius, bins, the sensor's height and the level steps."""
+    _fields_ = [("cell", C.c_double), ("step", C.c_double), ("r_max", C.c_double), ("n_ring", C.c_uint32), ("n_sector", C.c_uint32),
+                ("sensor_height", C.c_double), ("z_lo", C.c_double), ("dz", C.c_double), ("fov_up", C.c_double),
+                ("block_level", C.c_uint32)]
+
+
+class PlaceDbReport(C.Structure):
+    """malio_place_db_report: what one malio_place_db_build made."""
+    _fields_ = [("n_positions", C.c_uint64), ("grid_nx", C.c_uint32), ("grid_ny", C.c_uint32), ("n_stencil", C.c_uint32),
+                ("bytes_per_position", C.c_uint32), ("device_bytes", C.c_uint64), ("scratch_bytes", C.c_uint64)]
+
+
+class GlobalArgs(C.Structure):
+    """malio_global_args: stage-1 / stage-2 survivors and the verification's yaw step and lattice."""
+    _fields_ = [("k1", C.c_uint32), ("k2", C.c_uint32), ("yaw_step", C.c_double), ("res", C.c_double), ("half_xy", C.c_uint32),
+                ("half_z", C.c_uint32)]
+
+
+class GlobalCandidate(C.Structure):
+    """malio_global_candidate: one stage-2 survivor, its guess and its verification."""
+    _fields_ = [("position", C.c_uint32), ("shift", C.c_uint32), ("d1", C.c_uint32), ("d2", C.c_uint32), ("col", C.c_int32 * 2),
+                ("z_s", C.c_double), ("guess_rot", C.c_double * 4), ("guess_pos", C.c_double * 3), ("rot", C.c_double * 4),
+                ("pos", C.c_double * 3), ("score", C.c_uint32), ("n_points", C.c_uint32)]
+
+
+class GlobalReport(C.Structure):
+    """malio_global_report: the best verified pose of one malio_relocalize_global call and every stage's list."""
+    _fields_ = [("rot", C.c_double * 4), ("pos", C.c_double * 3), ("score", C.c_uint32), ("n_points", C.c_uint32),
+                ("best_rank", C.c_uint32), ("n_candidates", C.c_uint32), ("n_stage1", C.c_uint32), ("verify", RelocArgs),
+                ("cand", GlobalCandidate * PLACE_MAX_K2), ("stage1", C.c_uint32 * PLACE_MAX_K1), ("stage1_d1", C.c_uint32 * PLACE_MAX_K1),
+                ("query", C.c_uint8 * PLACE_MAX_BINS), ("ms_rank", C.c_double), ("ms_verify", C.c_double), ("device_bytes", C.c_uint64)]
+
+
 class CarveArgs(C.Structure):
     """malio_carve_args: how far a ray of malio_world_voxel_accumulate_carve is followed (m) and the margin before its end (m)."""
     _fields_ = [("max_range", C.c_float), ("end_margin", C.c_float)]
@@ -164,6 +201,7 @@ EXPORTS = [
     "malio_read_pcd", "malio_relocalize",
     "malio_world_voxel_accumulate_carve", "malio_world_voxel_evidence_device", "malio_world_voxel_download_kept_device",
     "malio_world_voxel_save_pcd_kept",
+    "malio_place_db_build", "malio_place_db_info", "malio_place_db_download", "malio_relocalize_global",
 ]
 
 
@@ -240,6 +278,10 @@ def load() -> C.CDLL:
     lib.malio_prior_map_info.argtypes = [vp, vp, vp, vp]
     lib.malio_prior_map_clear.argtypes = [vp]
     lib.malio_relocalize.argtypes = [vp, vp, vp, vp]
+    lib.malio_place_db_build.argtypes = [vp, vp, vp]
+    lib.malio_place_db_info.argtypes = [vp, vp, vp]
+    lib.malio_place_db_download.argtypes = [vp, vp, vp, vp, vp, C.c_uint64, vp]
+    lib.malio_relocalize_global.argtypes = [vp, vp, vp, vp]
     lib.malio_measure.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, C.POINTER(PassStats)]
     lib.malio_download_rows.argtypes = [vp, vp, vp, u32, C.POINTER(u32)]
     lib.malio_download_aux.argtypes = [vp, vp, vp, vp, vp, vp]

@@ -577,6 +577,73 @@ class MeasurementModel:
                     n_candidates=int(rep.n_candidates), nodes_bounded=int(rep.nodes_bounded),
                     leaves_scored=int(rep.leaves_scored), device_bytes=int(rep.device_bytes), state=state)
 
+    @staticmethod
+    def place_args(sensor_height: float, cell: float = 1.0, step: float = 1.0, r_max: float = 60.0, n_ring: int = 20,
+                   n_sector: int = 72, z_lo: float | None = None, dz: float = 1.0, fov_up: float = math.pi / 2,
+                   block_level: int = 2) -> capi.PlaceArgs:
+        """malio_place_args with the defaults of the header; z_lo defaults to -sensor_height + 0.5 (the ground is empty), fov_up
+        to no cap."""
+        a = capi.PlaceArgs()
+        a.cell, a.step, a.r_max, a.n_ring, a.n_sector = float(cell), float(step), float(r_max), int(n_ring), int(n_sector)
+        a.sensor_height = float(sensor_height)
+        a.z_lo = -float(sensor_height) + 0.5 if z_lo is None else float(z_lo)
+        a.dz, a.fov_up, a.block_level = float(dz), float(fov_up), int(block_level)
+        return a
+
+    def place_db_build(self, sensor_height: float | None = None, args: capi.PlaceArgs | None = None, **kw) -> dict:
+        """malio_place_db_build: describe every lattice position of the loaded prior (place_args(sensor_height, **kw), or args).
+        Returns the report's fields as a dict."""
+        a = args if args is not None else self.place_args(sensor_height, **kw)
+        rep = capi.PlaceDbReport()
+        self._check(self.lib.malio_place_db_build(self._h, C.byref(a), C.byref(rep)))
+        return {f: int(getattr(rep, f)) for f, _ in capi.PlaceDbReport._fields_}
+
+    def place_db_info(self) -> dict:
+        n, b = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.malio_place_db_info(self._h, C.byref(n), C.byref(b)))
+        return dict(n_positions=int(n.value), device_bytes=int(b.value))
+
+    def place_db_download(self, n_ring: int, n_sector: int) -> dict:
+        """The database (test / debug): cols (n, 2), z_s (n,), nibbles (n, bytes per position), ring_keys (n, n_ring)."""
+        n = C.c_uint64(0)
+        self._check(self.lib.malio_place_db_download(self._h, None, None, None, None, 0, C.byref(n)))
+        m = int(n.value)
+        cols, zs = np.zeros((m, 2), np.int32), np.zeros(m, np.float64)
+        nib, rk = np.zeros((m, (n_ring * n_sector + 1) // 2), np.uint8), np.zeros((m, n_ring), np.uint16)
+        self._check(self.lib.malio_place_db_download(self._h, capi.ptr(cols), capi.ptr(zs), capi.ptr(nib), capi.ptr(rk), m, C.byref(n)))
+        return dict(cols=cols, z_s=zs, nibbles=nib, ring_keys=rk)
+
+    def relocalize_global(self, guess: capi.State | capi.PassState, k1: int = 256, k2: int = 8, yaw_step: float = math.radians(1.0),
+                          res: float = 0.5, half_xy: int | None = None, half_z: int = 2, step: float = 1.0) -> dict:
+        """malio_relocalize_global: the resident scan against the place database, the k2 best places each checked by
+        malio_relocalize.  guess supplies the tilt and the extrinsics (its position and yaw do not matter); half_xy defaults to
+        ceil(step / (2 res)) + 2 with step the database's lattice step.  Returns the report's fields as a dict, the candidates as a
+        list of dicts, and `state`: a copy of guess with rot and pos replaced, ready for prior_map_window and the update."""
+        ps = guess.pass_state() if isinstance(guess, capi.State) else guess
+        a = capi.GlobalArgs()
+        a.k1, a.k2, a.yaw_step, a.res = int(k1), int(k2), float(yaw_step), float(res)
+        a.half_xy = int(math.ceil(step / (2 * res)) + 2) if half_xy is None else int(half_xy)
+        a.half_z = int(half_z)
+        rep = capi.GlobalReport()
+        self._check(self.lib.malio_relocalize_global(self._h, C.byref(ps), C.byref(a), C.byref(rep)))
+        state = type(guess)()
+        C.memmove(C.byref(state), C.byref(guess), C.sizeof(guess))
+        state.rot[:] = rep.rot[:]
+        state.pos[:] = rep.pos[:]
+        cand = []
+        for c in rep.cand[:rep.n_candidates]:
+            cand.append(dict(position=int(c.position), shift=int(c.shift), d1=int(c.d1), d2=int(c.d2), col=tuple(c.col[:]),
+                             z_s=float(c.z_s), guess_rot=np.array(c.guess_rot[:]), guess_pos=np.array(c.guess_pos[:]),
+                             rot=np.array(c.rot[:]), pos=np.array(c.pos[:]), score=int(c.score), n_points=int(c.n_points)))
+        v = rep.verify
+        return dict(rot=np.array(rep.rot[:]), pos=np.array(rep.pos[:]), score=int(rep.score), n_points=int(rep.n_points),
+                    best_rank=int(rep.best_rank), n_candidates=int(rep.n_candidates), n_stage1=int(rep.n_stage1),
+                    verify=dict(yaw_lo=v.yaw_lo, yaw_step=v.yaw_step, n_yaw=int(v.n_yaw), res=v.res, half_xy=int(v.half_xy),
+                                half_z=int(v.half_z)),
+                    cand=cand, stage1=np.array(rep.stage1[:rep.n_stage1], np.int64),
+                    stage1_d1=np.array(rep.stage1_d1[:rep.n_stage1], np.int64), query=np.array(rep.query[:], np.uint8),
+                    ms_rank=float(rep.ms_rank), ms_verify=float(rep.ms_verify), device_bytes=int(rep.device_bytes), state=state)
+
     def rearm_scan(self):
         """Reset the per-scan state of the scan already resident on the device (no host copy)."""
         self._check(self.lib.malio_rearm_scan(self._h))
