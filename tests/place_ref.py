@@ -180,6 +180,11 @@ def _zero_pos(s):
     return out
 
 
+def query_column(rel, cell):
+    """A scan point's column offset from the sensor: round half up, floor(rel / cell + 0.5)."""
+    return np.floor(rel / cell + 0.5)
+
+
 def query_heights(s, temporal_comp, pts, a):
     """The resident scan (capi.SCAN_PT) -> {(cx, cy): largest rel z} of the columns around the slot-0 origin."""
     a = _args_dict(a)
@@ -188,8 +193,7 @@ def query_heights(s, temporal_comp, pts, a):
     o = world_ref.register_world(s0, temporal_comp, np.zeros((1, 3), np.float32), np.zeros(1, np.int64), 0.0)[0, :3]
     w = w[np.all(np.isfinite(w), axis=1)]
     rel = w.astype(np.float64) - o.astype(np.float64)
-    cx = np.floor(rel[:, 0] / a["cell"] + 0.5)
-    cy = np.floor(rel[:, 1] / a["cell"] + 0.5)
+    cx, cy = query_column(rel[:, 0], a["cell"]), query_column(rel[:, 1], a["cell"])
     out = {}
     for x, y, z in zip(cx.tolist(), cy.tolist(), rel[:, 2].tolist()):
         out[(int(x), int(y))] = max(out.get((int(x), int(y)), -np.inf), z)
