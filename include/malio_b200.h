@@ -467,6 +467,50 @@ int malio_world_voxel_evidence_device(malio_handle* h, uint32_t* d_hit_miss, uin
 int malio_world_voxel_download_kept_device(malio_handle* h, const malio_carve_keep* k, float* d_out, uint64_t cap,
                                            uint64_t* n_out, void* stream);
 int malio_world_voxel_save_pcd_kept(malio_handle* h, const char* path, const malio_carve_keep* k, int clear);
+/* Keeping a saved map current: seed the voxel map from the saved file (session n's kept map is session n+1's prior), carve it
+ * while localizing, and report what changed.  tests/world_seed_ref.py restates every step in numpy.
+ * malio_world_voxel_seed folds n > 0 points xyzi (n x 4 floats {x, y, z, intensity}: what malio_read_pcd returns) into an empty
+ * map (just created, or after a clearing save: no accumulate since).  The result is exactly the map one
+ * malio_world_voxel_accumulate would hold if its dense cloud were these n points in input order, with world bits = the input
+ * xyz and intensity = xyzi[4p + 3]: same keys, same float sums point by point, same skipping of non-finite points; the call
+ * fixes the leaf.  The seeded voxels are the entries this call creates: entries are numbered in creation order and never
+ * renumbered, so the seeded set is the entry range [0, n_seeded), one integer per map, reset by a clearing save.  Each
+ * seeded voxel starts at hit = seed_hits, miss = 0 (and no carve scan has counted it); seed_hits > 0 allocates the carve
+ * counters of the first carve call here, and that call then leaves them as they are.  Entries a later accumulate creates
+ * start at hit = miss = 0, as before.
+ * The points are folded in chunks of at most MALIO_SEED_CHUNK, in input order, each through the accumulate pipeline (a stable
+ * sort keeps input order inside a chunk), so every voxel's sums still see its points one by one in order and the result does
+ * not depend on the chunking; the scan-sized scratch (48 B per point) is bounded by the chunk, not by n.  The entry table is
+ * sized for n voxels before the first chunk (at most one per point); the call waits once, at its end, for the voxel count
+ * and the verdict.  malio_world_voxel_seed stages the points through a pinned buffer into a chunk-sized device buffer, freed
+ * before it returns.  malio_world_voxel_seed_device reads d_xyzi in place with the device-memory contract of the other
+ * _device calls (pointer check, 16-byte alignment, ordered on `stream`); it returns after its one wait.  n_voxels may be NULL.
+ * Refusals, each before anything changes:
+ *   MALIO_ERR_INVALID_ARG  NULL h or xyzi, n == 0, a leaf that is not finite and > 0, device-memory contract (_device)
+ *   MALIO_ERR_STATE        the map is not empty (it holds voxels, or an accumulate since creation or the last clearing save
+ *                          fixed its leaf)
+ *   MALIO_ERR_CAPACITY     a finite point whose voxel index falls outside int, or more than 2^31 - 1 points: the map is empty
+ *                          again with its leaf unset, even when earlier chunks had been folded
+ * The seed is per handle: with a communicator attached each rank seeds its own map from the points it is given, and nothing
+ * is split or exchanged between ranks.
+ * malio_world_voxel_changes_device: removed = the seeded voxels the keep rule k drops, added = the voxels not seeded that k
+ * keeps, each as centroids in ascending (z, y, x) order with the bits the unfiltered download gives for them (kept = (seeded
+ * minus removed) plus added, the two disjoint).  A map that was never seeded gives removed = {} and added = kept; a map that
+ * was never carved keeps everything.  The size protocol and contract of malio_world_voxel_download_kept_device per output
+ * (NULL / 0 asks the count, *n_removed / *n_added = the full counts, at most cap written, 16-byte alignment), waiting for both
+ * counts before it enqueues the copies.  malio_world_voxel_save_changes_pcd writes each set through malio_world_voxel_save_pcd's
+ * writer; a NULL path skips its set, an empty set writes no file (not an error); the counts are reported either way (each
+ * may be NULL).  The map is not cleared.  MALIO_ERR_STATE on an empty map.  Both use the sort area of a download (32 B per
+ * voxel) and no more. */
+#define MALIO_SEED_CHUNK (1u << 22)
+int malio_world_voxel_seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t seed_hits, uint64_t* n_voxels);
+int malio_world_voxel_seed_device(malio_handle* h, const float* d_xyzi, uint64_t n, float leaf, uint32_t seed_hits,
+                                  uint64_t* n_voxels, void* stream);
+int malio_world_voxel_changes_device(malio_handle* h, const malio_carve_keep* k,
+                                     float* d_removed, uint64_t cap_removed, uint64_t* n_removed,
+                                     float* d_added, uint64_t cap_added, uint64_t* n_added, void* stream);
+int malio_world_voxel_save_changes_pcd(malio_handle* h, const malio_carve_keep* k, const char* removed_path,
+                                       const char* added_path, uint64_t* n_removed, uint64_t* n_added);
 /* Host: the same PCD file from n > 0 host points (n x 4 floats {x, y, z, intensity}): the header of PCDWriter::writeBinary for
  * PointXYZINormal (FIELDS x y z intensity normal_x normal_y normal_z curvature, WIDTH = POINTS = n, HEIGHT 1, DATA binary) and
  * n packed 32-byte records with normal_x/y/z = curvature = 0.  MALIO_ERR_INVALID_ARG for n == 0, a NULL argument or a file

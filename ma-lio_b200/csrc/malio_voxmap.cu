@@ -20,6 +20,9 @@
 //                     passed cell that the hash holds gets miss += 1 once per scan (the first thread to raise its stamp)
 // and on a kept download / save a flag per voxel in key order, an exclusive scan and a compaction of the order, ahead of
 // vm_centroid_kernel's arithmetic (the kept centroids are the unfiltered ones' bits).
+// Seeding (malio_world_voxel_seed*, DESIGN.md "Keeping a saved map current"): the same pipeline per chunk of saved points, with
+// vs_key_kernel / vs_fold_kernel reading float4 rows, then vs_hits_kernel over the seeded entries [0, n_seeded); the changes
+// are vs_change_kernel's two flags per voxel in key order, each scanned and compacted as the kept download is.
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -62,7 +65,7 @@ struct VoxState {
   // run scratch, 16 B a row, sized for the points of a scan only
   DeviceBuffer<uint32_t> d_head, d_run, d_rent, d_new;
   DeviceBuffer<char> d_temp;                 // CUB's temporary storage (sort histograms, scan carries)
-  DeviceBuffer<uint32_t> d_small;            // [0] fault flag, [1] run count, [2] entries in use
+  DeviceBuffer<uint32_t> d_small;            // [0] fault flag, [1] run count, [2] entries in use, [3] kept / removed count, [5] added
   PinnedBuffer<uint32_t> h_small;            // pinned mirror of d_small
   PinnedBuffer<float4> h_bounce;             // pinned, malio_pcd::CHUNK points
   // carving evidence, 12 B per entry, allocated by the first carve call and grown with the entries.  Entries at or beyond
@@ -70,6 +73,9 @@ struct VoxState {
   DeviceBuffer<uint2> d_hm;                  // (hit, miss)
   DeviceBuffer<uint32_t> d_stamp;            // the last carve scan that hit or passed the entry (0: none)
   uint32_t carve_scan = 0;                   // carve calls since creation or the last clearing save
+  // the seeded voxels are the entries [0, n_seeded): entries are numbered in creation order and never renumbered (growth and
+  // rehash keep them), and a seed only runs on an empty map.  0 for a map that was never seeded or since a clearing save.
+  uint64_t n_seeded = 0;
 };
 constexpr size_t SORT_ROW = 2 * sizeof(VKey) + 2 * sizeof(uint32_t);
 constexpr size_t RUN_ROW = 4 * sizeof(uint32_t);
@@ -340,6 +346,82 @@ __global__ void __launch_bounds__(256) vc_compact_kernel(const uint32_t* __restr
   if (r == n - 1) small[3] = pos[r] + keep[r];
 }
 
+// ------------------------------------------------------------------ seeding (malio_world_voxel_seed*) and the changes
+// vm_key_kernel's key on seed row p of a chunk: the row's xyz are the world bits as given
+__global__ void __launch_bounds__(256) vs_key_kernel(const float4* __restrict__ xyzi, float il, uint32_t n, VKey* __restrict__ key,
+                                                     uint32_t* __restrict__ val, uint32_t* __restrict__ fault) {
+  const uint32_t p = blockIdx.x * 256u + threadIdx.x;
+  if (p >= n) return;
+  const float4 r = xyzi[p];
+  const VKey none{SKIP_K, SKIP_K, SKIP_K};
+  val[p] = p;
+  if (!(isfinite(r.x) && isfinite(r.y) && isfinite(r.z))) { key[p] = none; return; }
+  const float fx = floorf(r.x * il), fy = floorf(r.y * il), fz = floorf(r.z * il);
+  if (!(in_int(fx) && in_int(fy) && in_int(fz))) { atomicOr(fault, 1u); key[p] = none; return; }
+  key[p] = VKey{(int)fz, (int)fy, (int)fx};
+}
+
+// vm_fold_kernel on seed rows: one thread per run continues its voxel's sums row by row, intensity = the row's fourth float.
+// Nothing is written once a chunk of this seed had a point outside int (small[0] is not reset between chunks).
+__global__ void __launch_bounds__(128) vs_fold_kernel(const float4* __restrict__ xyzi, const uint32_t* __restrict__ run,
+                                                      const VKey* __restrict__ key, const uint32_t* __restrict__ val, uint32_t n,
+                                                      const uint32_t* __restrict__ small, const uint32_t* __restrict__ rent,
+                                                      const uint32_t* __restrict__ rank, uint32_t* __restrict__ hash, uint64_t mask,
+                                                      VKey* __restrict__ ekey, float4* __restrict__ esum, uint32_t* __restrict__ ecnt) {
+  const uint32_t r = blockIdx.x * 128u + threadIdx.x;
+  if (small[0]) return;
+  const uint32_t nr = small[1];
+  if (r >= nr) return;
+  uint32_t e = rent[r];
+  if (e == RUN_NONE) return;
+  const uint32_t q0 = run[r], q1 = r + 1 < nr ? run[r + 1] : n;
+  float4 s;
+  uint32_t cnt;
+  if (e == RUN_NEW) {
+    e = small[2] + rank[r];
+    const VKey k = key[q0];
+    uint64_t slot = vhash(k) & mask;
+    while (atomicCAS(hash + slot, EMPTY, e) != EMPTY) slot = (slot + 1) & mask;
+    ekey[e] = k;
+    s = make_float4(0.f, 0.f, 0.f, 0.f);
+    cnt = 0;
+  } else {
+    s = esum[e];
+    cnt = ecnt[e];
+  }
+  for (uint32_t q = q0; q < q1; ++q) {
+    const float4 p = xyzi[val[q]];
+    s.x += p.x; s.y += p.y; s.z += p.z; s.w += p.w;
+    ++cnt;
+  }
+  esum[e] = s;
+  ecnt[e] = cnt;
+}
+
+// after the last chunk: the seeded entries [0, small[2]) start at (seed_hits, 0), stamp 0
+__global__ void __launch_bounds__(256) vs_hits_kernel(const uint32_t* __restrict__ small, uint32_t n, uint32_t seed_hits,
+                                                      uint2* __restrict__ hm, uint32_t* __restrict__ stamp) {
+  const uint32_t e = blockIdx.x * 256u + threadIdx.x;
+  if (small[0] || e >= n || e >= small[2]) return;
+  hm[e] = make_uint2(seed_hits, 0u);
+  stamp[e] = 0u;
+}
+
+// the r-th voxel in key order: removed[r] = seeded and dropped by the keep rule (vc_keep_kernel's arithmetic), added[r] = not
+// seeded and kept
+__global__ void __launch_bounds__(256) vs_change_kernel(const uint32_t* __restrict__ order, uint32_t n, const uint2* __restrict__ hm,
+                                                        uint32_t min_miss, double ratio, uint32_t n_seeded,
+                                                        uint32_t* __restrict__ removed, uint32_t* __restrict__ added) {
+  const uint32_t r = blockIdx.x * 256u + threadIdx.x;
+  if (r >= n) return;
+  const uint32_t e = order[r];
+  const uint2 v = hm ? hm[e] : make_uint2(0u, 0u);
+  const bool kept = !(v.y >= min_miss && (double)v.y > ratio * (double)v.x);
+  const bool seeded = e < n_seeded;
+  removed[r] = (seeded && !kept) ? 1u : 0u;
+  added[r] = (!seeded && kept) ? 1u : 0u;
+}
+
 int get_state(malio_handle* h, VoxState*& V) {
   V = (VoxState*)h->voxmap;
   if (V) return MALIO_OK;
@@ -347,9 +429,9 @@ int get_state(malio_handle* h, VoxState*& V) {
   CUDA_TRY(cudaSetDevice(D->device));
   V = new VoxState;
   h->voxmap = V;
-  if (int rc = V->d_small.allocate(h, D->stream, 4)) return rc;
-  CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 4 * sizeof(uint32_t), D->stream));
-  return V->h_small.allocate(h, 4);
+  if (int rc = V->d_small.allocate(h, D->stream, 6)) return rc;
+  CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 6 * sizeof(uint32_t), D->stream));
+  return V->h_small.allocate(h, 6);
 }
 
 // CUB's temporary storage for at least t bytes, and the sort area for n rows
@@ -472,6 +554,43 @@ int enqueue_kept(malio_handle* h, VoxState* V, DeviceState* D, const malio_carve
   return MALIO_OK;
 }
 
+// The changes against the seed in key order, laid out in the sort area (row offsets in bytes per row): the removed order at 20
+// (kept_order) and the added order at 16, both behind the centroids a save stages over the key halves; the added flags at 0,
+// the removed flags in the values half the sort left free, the two exclusive scans at 4 and 8.  Sorts, flags, scans and
+// compacts, then waits for the two counts.
+uint32_t* added_order(const VoxState* V) { return reinterpret_cast<uint32_t*>(V->d_sort + 16 * sort_rows(V)); }
+int enqueue_changes(malio_handle* h, VoxState* V, DeviceState* D, const malio_carve_keep* keep, uint64_t* n_removed, uint64_t* n_added) {
+  cudaStream_t st = D->stream;
+  const uint32_t n = (uint32_t)V->n_vox;
+  const uint64_t rows = sort_rows(V);
+  SortBufs b = sort_bufs(V);
+  size_t t = 0;
+  uint32_t* un = nullptr;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)n, st));
+  if (int rc = grow_temp(h, V, D, t)) return rc;
+  if (int rc = enqueue_order(h, V, D, b)) return rc;
+  uint32_t* flag_r = b.v.Alternate();
+  uint32_t* flag_a = reinterpret_cast<uint32_t*>(V->d_sort.data());
+  uint32_t* pos_r = reinterpret_cast<uint32_t*>(V->d_sort + 4 * rows);
+  uint32_t* pos_a = reinterpret_cast<uint32_t*>(V->d_sort + 8 * rows);
+  const uint32_t g = (n + 255) / 256;
+  vs_change_kernel<<<g, 256, 0, st>>>(b.v.Current(), n, V->d_hm, keep->min_miss, (double)keep->max_miss_per_hit,
+                                      (uint32_t)V->n_seeded, flag_r, flag_a);
+  t = V->d_temp.size();
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, flag_r, pos_r, (int)n, st));
+  vc_compact_kernel<<<g, 256, 0, st>>>(b.v.Current(), flag_r, pos_r, n, kept_order(V), V->d_small);        // -> small[3]
+  t = V->d_temp.size();
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, flag_a, pos_a, (int)n, st));
+  vc_compact_kernel<<<g, 256, 0, st>>>(b.v.Current(), flag_a, pos_a, n, added_order(V), V->d_small + 2);   // -> small[5]
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += 3;
+  CUDA_TRY(cudaMemcpyAsync(V->h_small + 3, V->d_small + 3, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));   // the counts size the caller's outputs and the files
+  *n_removed = V->h_small[3];
+  *n_added = V->h_small[5];
+  return MALIO_OK;
+}
+
 int check_keep(malio_handle* h, const malio_carve_keep* k) {
   if (!std::isfinite(k->max_miss_per_hit) || k->max_miss_per_hit < 0.f) {
     h->err = "world voxel keep rule: max_miss_per_hit must be finite and >= 0";
@@ -491,6 +610,7 @@ int clear_map(malio_handle* h, VoxState* V, DeviceState* D) {
   V->n_vox = 0;
   V->leaf_set = false;
   V->carve_scan = 0;
+  V->n_seeded = 0;
   return MALIO_OK;
 }
 
@@ -714,6 +834,192 @@ int save_pcd(malio_handle* h, const char* path, const malio_carve_keep* keep, in
   return rc;
 }
 
+// malio_world_voxel_seed (on_device false: xyzi in host memory, staged through the pinned bounce buffer into a chunk-sized
+// device buffer) and malio_world_voxel_seed_device (xyzi read in place, ordered on `caller`).  The points are folded chunk by
+// chunk in input order, each chunk through accumulate's pipeline with vs_key_kernel / vs_fold_kernel for the row source; the
+// table is sized for n points before the first chunk, so the chunks are enqueued back to back and the call waits once.
+int seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t seed_hits, bool on_device, cudaStream_t caller,
+         uint64_t* n_voxels) {
+  VoxState* V;
+  if (int rc = get_state(h, V)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (!(leaf > 0.f) || !std::isfinite(leaf)) { h->err = "world voxel seed: leaf must be a finite size > 0"; return MALIO_ERR_INVALID_ARG; }
+  if (V->n_vox || V->leaf_set) {
+    h->err = "world voxel seed: the voxel map is not empty (seed a new map or one after a clearing save)";
+    return MALIO_ERR_STATE;
+  }
+  if (on_device) {
+    if (int rc = check_device_ptr(h, D, xyzi, "malio_world_voxel_seed_device xyzi")) return rc;
+    if (reinterpret_cast<uintptr_t>(xyzi) & 15u) {
+      h->err = "malio_world_voxel_seed_device xyzi: not 16-byte aligned (the rows are read as float4)";
+      return MALIO_ERR_INVALID_ARG;
+    }
+  }
+  const uint64_t chunk = n < MALIO_SEED_CHUNK ? n : MALIO_SEED_CHUNK;
+  if (int rc = grow_table(h, V, D, n)) return rc;
+  if (int rc = grow_sort(h, V, D, chunk)) return rc;
+  if (int rc = grow_runs(h, V, D, chunk)) return rc;
+  const bool had_hm = (bool)V->d_hm;
+  if (seed_hits && !had_hm) {   // the counters the first carve would allocate, zero beyond the seed
+    const size_t cap = V->d_ekey.size();
+    if (int rc = malio_buf::allocate_group(h, D->stream, {{V->d_hm, cap}, {V->d_stamp, cap}})) return rc;
+    CUDA_TRY(cudaMemsetAsync(V->d_hm, 0, cap * sizeof(uint2), D->stream));
+    CUDA_TRY(cudaMemsetAsync(V->d_stamp, 0, cap * sizeof(uint32_t), D->stream));
+  }
+  DeviceBuffer<float4> stage;
+  if (!on_device) {
+    if (int rc = stage.allocate(h, D->stream, chunk)) return rc;
+    if (!V->h_bounce) { if (int rc = V->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
+  } else if (int rc = caller_enter(h, D, caller)) {
+    return rc;
+  }
+  cudaStream_t st = D->stream;
+  const uint64_t mask = V->d_hash.size() - 1;
+  const float il = 1.0f / leaf;
+  CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 2 * sizeof(uint32_t), st));   // fault flag (kept over the chunks), run count
+  const float4* rows = reinterpret_cast<const float4*>(xyzi);
+  for (uint64_t first = 0; first < n; first += chunk) {
+    const uint32_t m = (uint32_t)(n - first < chunk ? n - first : chunk), g = (m + 255) / 256;
+    const float4* src = rows + first;
+    if (!on_device) {   // the previous chunk's kernels and copies are done before the bounce buffer and the stage are reused
+      for (uint32_t p = 0; p < m; p += malio_pcd::CHUNK) {
+        const uint32_t c = m - p < malio_pcd::CHUNK ? m - p : malio_pcd::CHUNK;
+        CUDA_TRY(cudaStreamSynchronize(st));
+        std::memcpy(V->h_bounce.data(), rows + first + p, (size_t)c * sizeof(float4));
+        CUDA_TRY(cudaMemcpyAsync(stage + p, V->h_bounce, (size_t)c * sizeof(float4), cudaMemcpyHostToDevice, st));
+      }
+      D->ctr.h2d_bytes += (uint64_t)m * sizeof(float4);
+      src = stage;
+    }
+    SortBufs b = sort_bufs(V);
+    vs_key_kernel<<<g, 256, 0, st>>>(src, il, m, b.k.Current(), b.v.Current(), V->d_small);
+    size_t t = V->d_temp.size();
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)m, VKeyDecomposer{}, st));
+    const VKey* key = b.k.Current();
+    const uint32_t* val = b.v.Current();
+    vm_head_kernel<<<g, 256, 0, st>>>(key, m, V->d_head);
+    t = V->d_temp.size();
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(V->d_temp, t, V->d_head.data(), V->d_rent.data(), (int)m, st));
+    vm_run_kernel<<<g, 256, 0, st>>>(V->d_head, V->d_rent, m, V->d_run, V->d_small);
+    vm_lookup_kernel<<<g, 256, 0, st>>>(V->d_run, key, m, V->d_small, V->d_hash, mask, V->d_ekey, V->d_rent, V->d_new);
+    t = V->d_temp.size();
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, V->d_new.data(), V->d_head.data(), (int)m, st));
+    vs_fold_kernel<<<(m + 127) / 128, 128, 0, st>>>(src, V->d_run, key, val, m, V->d_small, V->d_rent, V->d_head, V->d_hash, mask,
+                                                   V->d_ekey, V->d_esum, V->d_ecnt);
+    vm_count_kernel<<<1, 1, 0, st>>>(V->d_head, V->d_new, V->d_small);
+    CUDA_TRY(cudaGetLastError());
+    D->ctr.kernel_launches += 7;
+  }
+  if (V->d_hm) {
+    const uint32_t nn = (uint32_t)n;
+    vs_hits_kernel<<<(nn + 255) / 256, 256, 0, st>>>(V->d_small, nn, seed_hits, V->d_hm, V->d_stamp);
+    CUDA_TRY(cudaGetLastError());
+    D->ctr.kernel_launches += 1;
+  }
+  CUDA_TRY(cudaMemcpyAsync(V->h_small, V->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  if (on_device) { if (int rc = caller_leave(h, D, caller)) return rc; }
+  CUDA_TRY(cudaStreamSynchronize(st));   // the call's one wait on device rows: the fault flag and the entry count
+  if (V->h_small[0]) {   // an earlier chunk may have been folded: the map is made empty again, as it was
+    if (int rc = clear_map(h, V, D)) return rc;
+    if (!had_hm) {
+      CUDA_TRY(cudaStreamSynchronize(st));
+      V->d_hm.release();
+      V->d_stamp.release();
+    }
+    h->err = "world voxel seed: leaf size too small for a point's coordinates (voxel index outside int); the map is empty";
+    return MALIO_ERR_CAPACITY;
+  }
+  V->n_vox = V->h_small[2];
+  V->n_seeded = V->n_vox;
+  V->leaf = leaf;
+  V->leaf_set = true;
+  if (n_voxels) *n_voxels = V->n_vox;
+  return MALIO_OK;
+}
+
+// removed / added centroids in the order of download_device, with download_kept_device's size protocol and contract
+int changes_device(malio_handle* h, const malio_carve_keep* keep, float* d_removed, uint64_t cap_removed, uint64_t* n_removed,
+                   float* d_added, uint64_t cap_added, uint64_t* n_added, cudaStream_t caller) {
+  VoxState* V;
+  if (int rc = get_state(h, V)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (int rc = check_keep(h, keep)) return rc;
+  if (V->n_vox) {
+    const struct { const float* out; uint64_t cap; const char* what; } outs[2] = {
+        {d_removed, cap_removed, "malio_world_voxel_changes_device removed"}, {d_added, cap_added, "malio_world_voxel_changes_device added"}};
+    for (const auto& o : outs) {
+      if (!o.out || !o.cap) continue;
+      if (int rc = check_device_ptr(h, D, o.out, o.what)) return rc;
+      if (reinterpret_cast<uintptr_t>(o.out) & 15u) {
+        h->err = std::string(o.what) + ": not 16-byte aligned (the centroids are stored as float4)";
+        return MALIO_ERR_INVALID_ARG;
+      }
+    }
+  }
+  uint64_t nr = 0, na = 0;
+  if (V->n_vox) {
+    if (int rc = grow_sort(h, V, D, V->n_vox)) return rc;
+    if (int rc = enqueue_changes(h, V, D, keep, &nr, &na)) return rc;
+  }
+  *n_removed = nr;
+  *n_added = na;
+  const uint64_t kr = d_removed ? (nr < cap_removed ? nr : cap_removed) : 0, ka = d_added ? (na < cap_added ? na : cap_added) : 0;
+  if (kr == 0 && ka == 0) return MALIO_OK;
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  if (kr)
+    vm_centroid_kernel<<<(uint32_t)((kr + 255) / 256), 256, 0, D->stream>>>(kept_order(V), (uint32_t)kr, V->d_esum, V->d_ecnt,
+                                                                             reinterpret_cast<float4*>(d_removed), (uint32_t)kr);
+  if (ka)
+    vm_centroid_kernel<<<(uint32_t)((ka + 255) / 256), 256, 0, D->stream>>>(added_order(V), (uint32_t)ka, V->d_esum, V->d_ecnt,
+                                                                             reinterpret_cast<float4*>(d_added), (uint32_t)ka);
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += (kr ? 1 : 0) + (ka ? 1 : 0);
+  return caller_leave(h, D, caller);
+}
+
+// each set through save_pcd's writer (a NULL path or an empty set writes no file); the map is not cleared
+int save_changes_pcd(malio_handle* h, const malio_carve_keep* keep, const char* removed_path, const char* added_path, uint64_t* n_removed,
+                     uint64_t* n_added) {
+  VoxState* V;
+  if (int rc = get_state(h, V)) return rc;
+  DeviceState* D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
+  if (int rc = check_keep(h, keep)) return rc;
+  if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
+  if (int rc = grow_sort(h, V, D, V->n_vox)) return rc;
+  if (!V->h_bounce) { if (int rc = V->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
+  uint64_t nr = 0, na = 0;
+  if (int rc = enqueue_changes(h, V, D, keep, &nr, &na)) return rc;
+  if (n_removed) *n_removed = nr;
+  if (n_added) *n_added = na;
+  float4* stage = reinterpret_cast<float4*>(V->d_sort.data());   // the key halves: both orders lie behind them
+  int rc = MALIO_OK;
+  const struct { const char* path; const uint32_t* order; uint64_t cnt; } sets[2] = {{removed_path, kept_order(V), nr},
+                                                                                    {added_path, added_order(V), na}};
+  for (const auto& set : sets) {
+    const uint64_t cnt = set.cnt;
+    if (rc != MALIO_OK || !set.path || cnt == 0) continue;
+    vm_centroid_kernel<<<(uint32_t)((cnt + 255) / 256), 256, 0, D->stream>>>(set.order, (uint32_t)cnt, V->d_esum, V->d_ecnt, stage,
+                                                                              (uint32_t)cnt);
+    CUDA_TRY(cudaGetLastError());
+    D->ctr.kernel_launches += 1;
+    rc = malio_pcd::write_binary(set.path, cnt, [&](uint64_t first, uint64_t c, const float** xyzi) {
+      if (cudaMemcpyAsync(V->h_bounce, stage + first, c * sizeof(float4), cudaMemcpyDeviceToHost, D->stream) != cudaSuccess ||
+          cudaStreamSynchronize(D->stream) != cudaSuccess)
+        return (int)MALIO_ERR_CUDA;
+      D->ctr.d2h_bytes += c * sizeof(float4);
+      *xyzi = (const float*)V->h_bounce.data();
+      return (int)MALIO_OK;
+    }, h->err);
+  }
+  CUDA_TRY(cudaStreamSynchronize(D->stream));   // as save_pcd: the entry-sized sort area and CUB's storage go back
+  V->d_sort.release();
+  V->d_temp.release();
+  return rc;
+}
+
 int info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* device_bytes) {
   VoxState* V;
   if (int rc = get_state(h, V)) return rc;
@@ -759,6 +1065,30 @@ extern "C" int malio_world_voxel_save_pcd_kept(malio_handle* h, const char* path
   if (!h || !path || !k) return MALIO_ERR_INVALID_ARG;
   MALIO_SETTLE(h);
   return malio_vox::save_pcd(h, path, k, clear);
+}
+extern "C" int malio_world_voxel_seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t seed_hits, uint64_t* n_voxels) {
+  if (!h || !xyzi || n == 0) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_vox::seed(h, xyzi, n, leaf, seed_hits, false, nullptr, n_voxels);
+}
+extern "C" int malio_world_voxel_seed_device(malio_handle* h, const float* d_xyzi, uint64_t n, float leaf, uint32_t seed_hits,
+                                             uint64_t* n_voxels, void* stream) {
+  if (!h || !d_xyzi || n == 0) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_vox::seed(h, d_xyzi, n, leaf, seed_hits, true, (cudaStream_t)stream, n_voxels);
+}
+extern "C" int malio_world_voxel_changes_device(malio_handle* h, const malio_carve_keep* k, float* d_removed, uint64_t cap_removed,
+                                                uint64_t* n_removed, float* d_added, uint64_t cap_added, uint64_t* n_added, void* stream) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  if (!k || !n_removed || !n_added || (cap_removed && !d_removed) || (cap_added && !d_added)) return MALIO_ERR_INVALID_ARG;
+  return malio_vox::changes_device(h, k, d_removed, cap_removed, n_removed, d_added, cap_added, n_added, (cudaStream_t)stream);
+}
+extern "C" int malio_world_voxel_save_changes_pcd(malio_handle* h, const malio_carve_keep* k, const char* removed_path,
+                                                  const char* added_path, uint64_t* n_removed, uint64_t* n_added) {
+  if (!h || !k) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_vox::save_changes_pcd(h, k, removed_path, added_path, n_removed, n_added);
 }
 extern "C" int malio_world_voxel_download_device(malio_handle* h, float* d_out, uint64_t cap, uint64_t* n_out, void* stream) {
   if (!h) return MALIO_ERR_INVALID_ARG;

@@ -202,6 +202,8 @@ EXPORTS = [
     "malio_world_voxel_accumulate_carve", "malio_world_voxel_evidence_device", "malio_world_voxel_download_kept_device",
     "malio_world_voxel_save_pcd_kept",
     "malio_place_db_build", "malio_place_db_info", "malio_place_db_download", "malio_relocalize_global",
+    "malio_world_voxel_seed", "malio_world_voxel_seed_device", "malio_world_voxel_changes_device",
+    "malio_world_voxel_save_changes_pcd",
 ]
 
 
@@ -270,6 +272,10 @@ def load() -> C.CDLL:
     lib.malio_world_voxel_evidence_device.argtypes = [vp, vp, C.c_uint64, vp, vp]
     lib.malio_world_voxel_download_kept_device.argtypes = [vp, vp, vp, C.c_uint64, vp, vp]
     lib.malio_world_voxel_save_pcd_kept.argtypes = [vp, C.c_char_p, vp, i32]
+    lib.malio_world_voxel_seed.argtypes = [vp, vp, C.c_uint64, C.c_float, u32, vp]
+    lib.malio_world_voxel_seed_device.argtypes = [vp, vp, C.c_uint64, C.c_float, u32, vp, vp]
+    lib.malio_world_voxel_changes_device.argtypes = [vp, vp, vp, C.c_uint64, vp, vp, C.c_uint64, vp, vp]
+    lib.malio_world_voxel_save_changes_pcd.argtypes = [vp, vp, C.c_char_p, C.c_char_p, vp, vp]
     lib.malio_write_pcd_binary.argtypes = [C.c_char_p, vp, C.c_uint64]
     lib.malio_read_pcd.argtypes = [C.c_char_p, vp, C.c_uint64, vp]
     lib.malio_prior_map_load.argtypes = [vp, vp, vp, vp, u32]

@@ -132,6 +132,9 @@ CARVE_MAX_RANGE = 100.0
 CARVE_END_MARGIN = 4.0
 KEEP_MIN_MISS = 2
 KEEP_MAX_MISS_PER_HIT = 2.0
+# The hits a seeded voxel starts with (malio_world_voxel_seed), chosen with tests/world_seed_ref.py on the two-session street
+# scene (DESIGN.md, "Keeping a saved map current").
+SEED_HITS = 2
 
 
 def carve_args(max_range: float = CARVE_MAX_RANGE, end_margin: float = CARVE_END_MARGIN) -> capi.CarveArgs:
@@ -507,6 +510,54 @@ class MeasurementModel:
             self._check(self.lib.malio_world_voxel_save_pcd(self._h, os.fsencode(path), 1 if clear else 0))
         else:
             self._check(self.lib.malio_world_voxel_save_pcd_kept(self._h, os.fsencode(path), C.byref(k), 1 if clear else 0))
+
+    def voxel_map_seed(self, xyzi, leaf: float, seed_hits: int = SEED_HITS) -> int:
+        """Start the empty voxel map from saved points (float32 (n, 4) {x, y, z, intensity}, e.g. read_pcd of a kept file): the map
+        one voxel_map_accumulate of these points would hold, each voxel starting at hit = seed_hits, miss = 0.  The seeded voxels
+        are what voxel_map_changes compares against.  Returns the number of voxels."""
+        leaf = _check_leaf(leaf)
+        x = self._f32(xyzi, 4)
+        n = C.c_uint64(0)
+        self._check(self.lib.malio_world_voxel_seed(self._h, capi.ptr(x), x.shape[0], C.c_float(leaf), int(seed_hits), C.byref(n)))
+        return int(n.value)
+
+    def voxel_map_seed_tensor(self, xyzi, leaf: float, seed_hits: int = SEED_HITS) -> int:
+        """voxel_map_seed from a contiguous float32 CUDA tensor (n, 4) on the handle's device, read in place, ordered on
+        torch.cuda.current_stream().  Returns once the seed is done (its voxel count)."""
+        import torch
+        leaf = _check_leaf(leaf)
+        _check_tensor(xyzi, "xyzi", torch.float32, 4, self.device)
+        n = C.c_uint64(0)
+        st = torch.cuda.current_stream(xyzi.device)
+        self._check(self.lib.malio_world_voxel_seed_device(self._h, _dptr(xyzi), xyzi.shape[0], C.c_float(leaf), int(seed_hits),
+                                                           C.byref(n), st.cuda_stream))
+        return int(n.value)
+
+    def voxel_map_changes(self, keep=True):
+        """(removed, added) as CUDA tensors float32 (n, 4) in the order of voxel_map_tensor(): the seeded voxels the keep rule
+        drops and the voxels not seeded that it keeps (keep as voxel_map_tensor's, the defaults when True), allocated on the
+        current stream.  The call waits for the two counts."""
+        import torch
+        k = _as_keep(keep) or carve_keep()
+        nr, na = C.c_uint64(0), C.c_uint64(0)
+        st = torch.cuda.current_stream(self.device)
+        self._check(self.lib.malio_world_voxel_changes_device(self._h, C.byref(k), None, 0, C.byref(nr), None, 0, C.byref(na),
+                                                              st.cuda_stream))
+        rem, add = self._empty((nr.value, 4), torch.float32), self._empty((na.value, 4), torch.float32)
+        if nr.value or na.value:
+            self._check(self.lib.malio_world_voxel_changes_device(self._h, C.byref(k), _dptr(rem), nr.value, C.byref(nr), _dptr(add),
+                                                                  na.value, C.byref(na), st.cuda_stream))
+        return rem, add
+
+    def voxel_map_save_changes(self, removed_path: str | None, added_path: str | None, keep=True) -> tuple:
+        """voxel_map_changes as two binary PCD files (None skips a file; an empty set writes none).  The map is not cleared.
+        Returns (n_removed, n_added)."""
+        k = _as_keep(keep) or carve_keep()
+        nr, na = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.malio_world_voxel_save_changes_pcd(self._h, C.byref(k), None if removed_path is None else os.fsencode(removed_path),
+                                                                None if added_path is None else os.fsencode(added_path),
+                                                                C.byref(nr), C.byref(na)))
+        return int(nr.value), int(na.value)
 
     def voxel_map_info(self) -> dict:
         """Voxels in use, entry capacity and the device bytes the voxel map holds."""

@@ -634,9 +634,12 @@ class Street:
     car_z0: float = 0.25
     max_range: float = 80.0        # the sensor returns nothing beyond this
     noise: float = 0.01            # m, range noise (1 sigma)
+    gone: tuple = ()               # indices into the default parked boxes that have left (a later session of the same street)
+    extra: tuple = ()              # boxes (lo, hi) that have appeared, after the remaining parked ones
 
     def parked(self) -> list:
-        return [(np.array([x, 4.6, 0.0]), np.array([x + 4.0, 6.4, 1.4])) for x in np.arange(-12.0, 48.0, 9.0)]
+        boxes = [(np.array([x, 4.6, 0.0]), np.array([x + 4.0, 6.4, 1.4])) for x in np.arange(-12.0, 48.0, 9.0)]
+        return [b for i, b in enumerate(boxes) if i not in self.gone] + [(np.asarray(lo, float), np.asarray(hi, float)) for lo, hi in self.extra]
 
     def car(self, k: int):
         sx, sy, sz = self.car_size
