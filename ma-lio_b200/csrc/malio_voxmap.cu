@@ -7,22 +7,23 @@
 //   centroid          float sums from 0.f in accumulation order (slot 0..L-1, point order, scan after scan), u32 count,
 //                     sum / (float)count: vg_centroid_kernel's arithmetic on the concatenated cloud
 //   output order      ascending (k, j, i) = (z, y, x) voxel index as signed ints
-// Per scan, O(points in the scan), whatever the size of the map:
-//   vm_key_kernel     body_to_world (the bits of world_kernel) and the voxel key of every dense point
-//   radix sort        stable, of (key, point index) over the 96-bit key (CUB, k most significant, double-buffered)
+// The fold (enqueue_fold), per scan or per chunk of saved points, O(rows folded), whatever the size of the map.  The rows are
+// a source type: ScanRows (the dense points, registered with body_to_world: the bits of world_kernel) or SeedRows (float4 rows):
+//   vm_key_kernel     the voxel key of every row
+//   radix sort        stable, of (key, row index) over the 96-bit key (CUB, k most significant, double-buffered)
 //   runs              one run per distinct key; each run looked up in a persistent open-addressing hash (key -> entry)
 //   new entries       numbered by an exclusive scan over the runs in key order (deterministic, whatever the hash layout)
-//   vm_fold_kernel    one thread per run continues its voxel's sums in point order (the points registered again)
+//   vm_fold_kernel    one thread per run continues its voxel's sums in row order (the rows read again)
 // The map is sorted by key on download / save only.  Compiled with -fmad=false like the rest of the library.
-// Carving (malio_world_voxel_accumulate_carve, DESIGN.md "Clearing moving objects"): the same fold, then per scan
+// Carving (malio_world_voxel_accumulate_carve, DESIGN.md "Clearing moving objects"): vc_origin_kernel, the same fold, then
 //   vc_hit_kernel     one thread per run: hit += 1 on the run's entry (rent, or small[2] + rank for a new one), stamp = scan
 //   vc_carve_kernel   one thread per ray (slot origin -> dense point): a double-precision DDA over the voxel indices; every
 //                     passed cell that the hash holds gets miss += 1 once per scan (the first thread to raise its stamp)
 // and on a kept download / save a flag per voxel in key order, an exclusive scan and a compaction of the order, ahead of
 // vm_centroid_kernel's arithmetic (the kept centroids are the unfiltered ones' bits).
-// Seeding (malio_world_voxel_seed*, DESIGN.md "Keeping a saved map current"): the same pipeline per chunk of saved points, with
-// vs_key_kernel / vs_fold_kernel reading float4 rows, then vs_hits_kernel over the seeded entries [0, n_seeded); the changes
-// are vs_change_kernel's two flags per voxel in key order, each scanned and compacted as the kept download is.
+// Seeding (malio_world_voxel_seed*, DESIGN.md "Keeping a saved map current"): the same fold per chunk of saved points, then
+// vs_hits_kernel over the seeded entries [0, n_seeded); the changes are vs_change_kernel's two flags per voxel in key order,
+// each scanned and compacted as the kept download is.
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -58,11 +59,10 @@ struct VoxState {
   uint64_t n_vox = 0;                        // entries in use (exact on the host after every call)
   DeviceBuffer<VKey> d_ekey; DeviceBuffer<float4> d_esum; DeviceBuffer<uint32_t> d_ecnt;   // entries
   DeviceBuffer<uint32_t> d_hash;                                                           // power of two
-  // sort area, rows of 32 B (one allocation): keys | alternate keys (12 B each) | values | alternate values (4 B each), sized
-  // for the points of a scan or, on download and save, for the entries.  A save writes the sorted centroids (16 B a row)
-  // over the two key halves and then releases the area; a download keeps it until the next save.
+  // sort area, rows of 32 B in one allocation (the columns below), sized for the rows of a fold or, on download and save,
+  // for the entries.  A download keeps it until the next save; a save releases it.
   DeviceBuffer<char> d_sort;
-  // run scratch, 16 B a row, sized for the points of a scan only
+  // run scratch, 16 B a row, sized for the rows of a fold only
   DeviceBuffer<uint32_t> d_head, d_run, d_rent, d_new;
   DeviceBuffer<char> d_temp;                 // CUB's temporary storage (sort histograms, scan carries)
   DeviceBuffer<uint32_t> d_small;            // [0] fault flag, [1] run count, [2] entries in use, [3] kept / removed count, [5] added
@@ -77,7 +77,24 @@ struct VoxState {
   // rehash keep them), and a seed only runs on an empty map.  0 for a map that was never seeded or since a clearing save.
   uint64_t n_seeded = 0;
 };
-constexpr size_t SORT_ROW = 2 * sizeof(VKey) + 2 * sizeof(uint32_t);
+
+// The sort area holds sort_rows(V) rows as eight columns of 4 B a row; column c starts at byte 4 * c * rows.  While points or
+// entries are sorted, the columns are CUB's double buffers: keys in 0-2, alternate keys in 3-5 (12 B a row), values in 6,
+// alternate values in 7.
+constexpr uint32_t COL_KEYS = 0;
+constexpr uint32_t COL_VALUES = 6;
+constexpr size_t SORT_ROW = 8 * sizeof(uint32_t);
+static_assert(SORT_ROW == 2 * sizeof(VKey) + 2 * sizeof(uint32_t), "a sort row holds two keys and two values");
+// Once the entries are sorted (enqueue_order), their order is in the values column CUB left current and the key columns are
+// free.  A selection (enqueue_select) writes there: a flag column beside the one in the values column the sort left free, an
+// exclusive scan, and the selected entries in key order.  A save then stages the selected centroids, float4, over bytes 0-16
+// of the rows (columns 0-3), so the orders it still reads must lie at byte 16 and above, and below the values.
+constexpr uint32_t COL_FLAGS = 0;            // the added flags (enqueue_changes)
+constexpr uint32_t COL_SCAN = 1;             // exclusive scan of a flag column
+constexpr uint32_t COL_ADDED = 4;            // the added entries in key order
+constexpr uint32_t COL_KEPT = 5;             // the kept, or the removed, entries in key order
+static_assert(4 * COL_ADDED >= sizeof(float4) && 4 * COL_KEPT >= sizeof(float4), "a save's staged centroids cover the orders");
+static_assert(COL_ADDED < COL_VALUES && COL_KEPT < COL_VALUES && COL_ADDED != COL_KEPT, "the orders overlap the values");
 constexpr size_t RUN_ROW = 4 * sizeof(uint32_t);
 
 // the four arrays of the sort area as CUB's double buffers
@@ -86,10 +103,12 @@ struct SortBufs {
   cub::DoubleBuffer<uint32_t> v;
 };
 uint64_t sort_rows(const VoxState* V) { return V->d_sort.size() / SORT_ROW; }
+uint32_t* sort_col(const VoxState* V, uint32_t c) { return reinterpret_cast<uint32_t*>(V->d_sort + 4 * c * sort_rows(V)); }
+float4* sort_stage(const VoxState* V) { return reinterpret_cast<float4*>(V->d_sort.data()); }   // a save's centroids
 SortBufs sort_bufs(const VoxState* V) {
   const uint64_t rows = sort_rows(V);
-  VKey* k = reinterpret_cast<VKey*>(V->d_sort.data());
-  uint32_t* v = reinterpret_cast<uint32_t*>(V->d_sort + 2 * sizeof(VKey) * rows);
+  VKey* k = reinterpret_cast<VKey*>(sort_col(V, COL_KEYS));
+  uint32_t* v = sort_col(V, COL_VALUES);
   return SortBufs{cub::DoubleBuffer<VKey>(k, k + rows), cub::DoubleBuffer<uint32_t>(v, v + rows)};
 }
 
@@ -101,13 +120,32 @@ struct VmSlots {
   int L;
 };
 
-__device__ __forceinline__ float world_point(const VmSlots& c, const PassConst& pc, uint32_t p, float w[3]) {
+__device__ __forceinline__ int slot_row(const VmSlots& c, uint32_t p, const float** row) {
   int l = 0;
   while (l + 1 < c.L && p >= c.first[l + 1]) ++l;
-  const float* r = c.ud[l] + 5 * (size_t)(p - c.first[l]);
-  body_to_world(pc, l, r[0], r[1], r[2], w);
-  return c.tag[l];
+  *row = c.ud[l] + 5 * (size_t)(p - c.first[l]);
+  return l;
 }
+
+// The rows a fold reads.  point(p) is row p as {x, y, z, tag} in the world frame.
+// A scan's dense cloud, registered with the pass state; tag = the slot's
+struct ScanRows {
+  VmSlots c;
+  PassConst pc;
+  __device__ __forceinline__ float4 point(uint32_t p) const {
+    const float* r;
+    const int l = slot_row(c, p, &r);
+    float w[3];
+    body_to_world(pc, l, r[0], r[1], r[2], w);
+    return make_float4(w[0], w[1], w[2], c.tag[l]);
+  }
+};
+// Saved points {x, y, z, intensity} in device memory, as given.  They do not change during the fold, so they are read through
+// the read-only path.
+struct SeedRows {
+  const float4* xyzi;
+  __device__ __forceinline__ float4 point(uint32_t p) const { return __ldg(xyzi + p); }
+};
 
 __device__ __forceinline__ uint64_t vhash(const VKey& a) {
   uint64_t h = (uint64_t)(uint32_t)a.i * 0x9E3779B97F4A7C15ull ^ (uint64_t)(uint32_t)a.j * 0xC2B2AE3D27D4EB4Full ^
@@ -116,20 +154,31 @@ __device__ __forceinline__ uint64_t vhash(const VKey& a) {
   return h;
 }
 __device__ __forceinline__ bool same(const VKey& a, const VKey& b) { return a.k == b.k && a.j == b.j && a.i == b.i; }
+// the entry of voxel k, or EMPTY when the hash does not hold it
+__device__ __forceinline__ uint32_t hash_find(const uint32_t* hash, uint64_t mask, const VKey* ekey, const VKey& k) {
+  for (uint64_t s = vhash(k) & mask;; s = (s + 1) & mask) {
+    const uint32_t e = hash[s];
+    if (e == EMPTY || same(ekey[e], k)) return e;
+  }
+}
+// entry e (voxel k) into the first free slot of k's probe sequence
+__device__ __forceinline__ void hash_insert(uint32_t* hash, uint64_t mask, const VKey& k, uint32_t e) {
+  uint64_t slot = vhash(k) & mask;
+  while (atomicCAS(hash + slot, EMPTY, e) != EMPTY) slot = (slot + 1) & mask;
+}
+__device__ __forceinline__ bool in_int(float f) { return f >= -2147483648.f && f < 2147483648.f; }
 
-__global__ void __launch_bounds__(256) vm_key_kernel(VmSlots c, PassConst pc, float il, uint32_t n, VKey* __restrict__ key,
+template <class Rows>
+__global__ void __launch_bounds__(256) vm_key_kernel(Rows src, float il, uint32_t n, VKey* __restrict__ key,
                                                      uint32_t* __restrict__ val, uint32_t* __restrict__ fault) {
   const uint32_t p = blockIdx.x * 256u + threadIdx.x;
   if (p >= n) return;
-  float w[3];
-  world_point(c, pc, p, w);
+  const float4 w = src.point(p);
   const VKey none{SKIP_K, SKIP_K, SKIP_K};
   val[p] = p;
-  if (!(isfinite(w[0]) && isfinite(w[1]) && isfinite(w[2]))) { key[p] = none; return; }
-  const float fx = floorf(w[0] * il), fy = floorf(w[1] * il), fz = floorf(w[2] * il);
-  const bool in_int = fx >= -2147483648.f && fx < 2147483648.f && fy >= -2147483648.f && fy < 2147483648.f &&
-                      fz >= -2147483648.f && fz < 2147483648.f;
-  if (!in_int) { atomicOr(fault, 1u); key[p] = none; return; }
+  if (!(isfinite(w.x) && isfinite(w.y) && isfinite(w.z))) { key[p] = none; return; }
+  const float fx = floorf(w.x * il), fy = floorf(w.y * il), fz = floorf(w.z * il);
+  if (!(in_int(fx) && in_int(fy) && in_int(fz))) { atomicOr(fault, 1u); key[p] = none; return; }
   key[p] = VKey{(int)fz, (int)fy, (int)fx};
 }
 
@@ -158,16 +207,16 @@ __global__ void __launch_bounds__(256) vm_lookup_kernel(const uint32_t* __restri
   if (r >= nr) { is_new[r] = 0; return; }
   const VKey k = key[run[r]];
   if (k.k == SKIP_K) { rent[r] = RUN_NONE; is_new[r] = 0; return; }
-  for (uint64_t s = vhash(k) & mask;; s = (s + 1) & mask) {
-    const uint32_t e = hash[s];
-    if (e == EMPTY) { rent[r] = RUN_NEW; is_new[r] = 1; return; }
-    if (same(ekey[e], k)) { rent[r] = e; is_new[r] = 0; return; }
-  }
+  const uint32_t e = hash_find(hash, mask, ekey, k);
+  rent[r] = e == EMPTY ? RUN_NEW : e;
+  is_new[r] = e == EMPTY ? 1u : 0u;
 }
 
 // one thread per run: the voxel's entry (a new one numbered in key order and entered into the hash), then its sums continued
-// point by point.  Nothing is written when the scan has a point outside int (small[0]): the map stays as it was.
-__global__ void __launch_bounds__(128) vm_fold_kernel(VmSlots c, PassConst pc, const uint32_t* __restrict__ run,
+// row by row.  Nothing is written once a row of the call was outside int (small[0], which a seed keeps over its chunks): the
+// map stays as it was.
+template <class Rows>
+__global__ void __launch_bounds__(128) vm_fold_kernel(Rows src, const uint32_t* __restrict__ run,
                                                       const VKey* __restrict__ key, const uint32_t* __restrict__ val, uint32_t n,
                                                       const uint32_t* __restrict__ small, const uint32_t* __restrict__ rent,
                                                       const uint32_t* __restrict__ rank, uint32_t* __restrict__ hash, uint64_t mask,
@@ -184,8 +233,7 @@ __global__ void __launch_bounds__(128) vm_fold_kernel(VmSlots c, PassConst pc, c
   if (e == RUN_NEW) {
     e = small[2] + rank[r];
     const VKey k = key[q0];
-    uint64_t slot = vhash(k) & mask;
-    while (atomicCAS(hash + slot, EMPTY, e) != EMPTY) slot = (slot + 1) & mask;
+    hash_insert(hash, mask, k, e);
     ekey[e] = k;
     s = make_float4(0.f, 0.f, 0.f, 0.f);
     cnt = 0;
@@ -194,10 +242,8 @@ __global__ void __launch_bounds__(128) vm_fold_kernel(VmSlots c, PassConst pc, c
     cnt = ecnt[e];
   }
   for (uint32_t q = q0; q < q1; ++q) {
-    const uint32_t p = val[q];
-    float w[3];
-    const float tag = world_point(c, pc, p, w);
-    s.x += w[0]; s.y += w[1]; s.z += w[2]; s.w += tag;
+    const float4 w = src.point(val[q]);
+    s.x += w.x; s.y += w.y; s.z += w.z; s.w += w.w;
     ++cnt;
   }
   esum[e] = s;
@@ -214,8 +260,7 @@ __global__ void vm_count_kernel(const uint32_t* __restrict__ rank, const uint32_
 __global__ void __launch_bounds__(256) vm_rehash_kernel(const VKey* __restrict__ ekey, uint32_t n, uint32_t* __restrict__ hash, uint64_t mask) {
   const uint32_t e = blockIdx.x * 256u + threadIdx.x;
   if (e >= n) return;
-  uint64_t slot = vhash(ekey[e]) & mask;
-  while (atomicCAS(hash + slot, EMPTY, e) != EMPTY) slot = (slot + 1) & mask;
+  hash_insert(hash, mask, ekey[e], e);
 }
 
 __global__ void __launch_bounds__(256) vm_iota_kernel(const VKey* __restrict__ ekey, uint32_t n, VKey* __restrict__ key, uint32_t* __restrict__ val) {
@@ -237,8 +282,6 @@ __global__ void __launch_bounds__(256) vm_centroid_kernel(const uint32_t* __rest
 }
 
 // ------------------------------------------------------------------ carving (malio_world_voxel_accumulate_carve)
-__device__ __forceinline__ bool in_int(float f) { return f >= -2147483648.f && f < 2147483648.f; }
-
 // before the fold: the origin of every slot that has points needs a voxel index in int, like the ends (vm_key_kernel), or
 // the scan is refused through the same fault flag
 __global__ void vc_origin_kernel(VmSlots c, PassConst pc, float il, uint32_t* __restrict__ fault) {
@@ -277,9 +320,8 @@ __global__ void __launch_bounds__(256) vc_carve_kernel(VmSlots c, PassConst pc, 
                                                        uint32_t* __restrict__ stamp, uint32_t scan) {
   const uint32_t p = blockIdx.x * 256u + threadIdx.x;
   if (p >= n || small[0]) return;
-  int l = 0;
-  while (l + 1 < c.L && p >= c.first[l + 1]) ++l;
-  const float* row = c.ud[l] + 5 * (size_t)(p - c.first[l]);
+  const float* row;
+  const int l = slot_row(c, p, &row);
   float w[3], o[3];
   body_to_world(pc, l, row[0], row[1], row[2], w);
   if (!(isfinite(w[0]) && isfinite(w[1]) && isfinite(w[2]))) return;
@@ -299,15 +341,8 @@ __global__ void __launch_bounds__(256) vc_carve_kernel(VmSlots c, PassConst pc, 
   double tx = rx ? vc_face(cx, sx, ux, ix) : 0.0, ty = ry ? vc_face(cy, sy, uy, iy) : 0.0, tz = rz ? vc_face(cz, sz, uz, iz) : 0.0;
   double t = 0.0;   // entry parameter of the current cell
   while ((rx | ry | rz) && t * len < lim) {
-    const VKey k{cz, cy, cx};
-    for (uint64_t s = vhash(k) & mask;; s = (s + 1) & mask) {
-      const uint32_t e = hash[s];
-      if (e == EMPTY) break;
-      if (same(ekey[e], k)) {
-        if (*(volatile const uint32_t*)(stamp + e) != scan && atomicMax(stamp + e, scan) < scan) hm[e].y += 1u;
-        break;
-      }
-    }
+    const uint32_t e = hash_find(hash, mask, ekey, VKey{cz, cy, cx});
+    if (e != EMPTY && *(volatile const uint32_t*)(stamp + e) != scan && atomicMax(stamp + e, scan) < scan) hm[e].y += 1u;
     int a = rx ? 0 : (ry ? 1 : 2);
     double ta = rx ? tx : (ry ? ty : tz);
     if (ry && ty < ta) { a = 1; ta = ty; }
@@ -319,85 +354,40 @@ __global__ void __launch_bounds__(256) vc_carve_kernel(VmSlots c, PassConst pc, 
   }
 }
 
-// (hit, miss) of the r-th voxel in key order -> out[r], r < n (zeros for a map that was never carved)
+// (hit, miss) of entry e; zeros for a map that was never carved (hm NULL)
+__device__ __forceinline__ uint2 evidence(const uint2* hm, uint32_t e) { return hm ? hm[e] : make_uint2(0u, 0u); }
+// the keep rule (malio_carve_keep): a voxel is dropped when miss >= min_miss and (double)miss > ratio * (double)hit
+__device__ __forceinline__ bool dropped(uint2 v, uint32_t min_miss, double ratio) {
+  return v.y >= min_miss && (double)v.y > ratio * (double)v.x;
+}
+
+// (hit, miss) of the r-th voxel in key order -> out[r], r < n
 __global__ void __launch_bounds__(256) vc_evidence_kernel(const uint32_t* __restrict__ order, uint32_t n, const uint2* __restrict__ hm,
                                                           uint2* __restrict__ out) {
   const uint32_t r = blockIdx.x * 256u + threadIdx.x;
   if (r >= n) return;
-  out[r] = hm ? hm[order[r]] : make_uint2(0u, 0u);
+  out[r] = evidence(hm, order[r]);
 }
 
-// the keep rule on the r-th voxel in key order: dropped when miss >= min_miss and (double)miss > ratio * (double)hit
+// the keep rule on the r-th voxel in key order
 __global__ void __launch_bounds__(256) vc_keep_kernel(const uint32_t* __restrict__ order, uint32_t n, const uint2* __restrict__ hm,
                                                       uint32_t min_miss, double ratio, uint32_t* __restrict__ keep) {
   const uint32_t r = blockIdx.x * 256u + threadIdx.x;
   if (r >= n) return;
-  const uint2 v = hm ? hm[order[r]] : make_uint2(0u, 0u);
-  keep[r] = (v.y >= min_miss && (double)v.y > ratio * (double)v.x) ? 0u : 1u;
+  keep[r] = dropped(evidence(hm, order[r]), min_miss, ratio) ? 0u : 1u;
 }
 
-// the kept entries in key order -> kept[0 .. small[3])
-__global__ void __launch_bounds__(256) vc_compact_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__ keep,
-                                                         const uint32_t* __restrict__ pos, uint32_t n, uint32_t* __restrict__ kept,
-                                                         uint32_t* __restrict__ small) {
+// the flagged entries in key order -> out[0 .. *count)
+__global__ void __launch_bounds__(256) vc_compact_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__ flag,
+                                                         const uint32_t* __restrict__ pos, uint32_t n, uint32_t* __restrict__ out,
+                                                         uint32_t* __restrict__ count) {
   const uint32_t r = blockIdx.x * 256u + threadIdx.x;
   if (r >= n) return;
-  if (keep[r]) kept[pos[r]] = order[r];
-  if (r == n - 1) small[3] = pos[r] + keep[r];
+  if (flag[r]) out[pos[r]] = order[r];
+  if (r == n - 1) *count = pos[r] + flag[r];
 }
 
 // ------------------------------------------------------------------ seeding (malio_world_voxel_seed*) and the changes
-// vm_key_kernel's key on seed row p of a chunk: the row's xyz are the world bits as given
-__global__ void __launch_bounds__(256) vs_key_kernel(const float4* __restrict__ xyzi, float il, uint32_t n, VKey* __restrict__ key,
-                                                     uint32_t* __restrict__ val, uint32_t* __restrict__ fault) {
-  const uint32_t p = blockIdx.x * 256u + threadIdx.x;
-  if (p >= n) return;
-  const float4 r = xyzi[p];
-  const VKey none{SKIP_K, SKIP_K, SKIP_K};
-  val[p] = p;
-  if (!(isfinite(r.x) && isfinite(r.y) && isfinite(r.z))) { key[p] = none; return; }
-  const float fx = floorf(r.x * il), fy = floorf(r.y * il), fz = floorf(r.z * il);
-  if (!(in_int(fx) && in_int(fy) && in_int(fz))) { atomicOr(fault, 1u); key[p] = none; return; }
-  key[p] = VKey{(int)fz, (int)fy, (int)fx};
-}
-
-// vm_fold_kernel on seed rows: one thread per run continues its voxel's sums row by row, intensity = the row's fourth float.
-// Nothing is written once a chunk of this seed had a point outside int (small[0] is not reset between chunks).
-__global__ void __launch_bounds__(128) vs_fold_kernel(const float4* __restrict__ xyzi, const uint32_t* __restrict__ run,
-                                                      const VKey* __restrict__ key, const uint32_t* __restrict__ val, uint32_t n,
-                                                      const uint32_t* __restrict__ small, const uint32_t* __restrict__ rent,
-                                                      const uint32_t* __restrict__ rank, uint32_t* __restrict__ hash, uint64_t mask,
-                                                      VKey* __restrict__ ekey, float4* __restrict__ esum, uint32_t* __restrict__ ecnt) {
-  const uint32_t r = blockIdx.x * 128u + threadIdx.x;
-  if (small[0]) return;
-  const uint32_t nr = small[1];
-  if (r >= nr) return;
-  uint32_t e = rent[r];
-  if (e == RUN_NONE) return;
-  const uint32_t q0 = run[r], q1 = r + 1 < nr ? run[r + 1] : n;
-  float4 s;
-  uint32_t cnt;
-  if (e == RUN_NEW) {
-    e = small[2] + rank[r];
-    const VKey k = key[q0];
-    uint64_t slot = vhash(k) & mask;
-    while (atomicCAS(hash + slot, EMPTY, e) != EMPTY) slot = (slot + 1) & mask;
-    ekey[e] = k;
-    s = make_float4(0.f, 0.f, 0.f, 0.f);
-    cnt = 0;
-  } else {
-    s = esum[e];
-    cnt = ecnt[e];
-  }
-  for (uint32_t q = q0; q < q1; ++q) {
-    const float4 p = xyzi[val[q]];
-    s.x += p.x; s.y += p.y; s.z += p.z; s.w += p.w;
-    ++cnt;
-  }
-  esum[e] = s;
-  ecnt[e] = cnt;
-}
-
 // after the last chunk: the seeded entries [0, small[2]) start at (seed_hits, 0), stamp 0
 __global__ void __launch_bounds__(256) vs_hits_kernel(const uint32_t* __restrict__ small, uint32_t n, uint32_t seed_hits,
                                                       uint2* __restrict__ hm, uint32_t* __restrict__ stamp) {
@@ -407,26 +397,25 @@ __global__ void __launch_bounds__(256) vs_hits_kernel(const uint32_t* __restrict
   stamp[e] = 0u;
 }
 
-// the r-th voxel in key order: removed[r] = seeded and dropped by the keep rule (vc_keep_kernel's arithmetic), added[r] = not
-// seeded and kept
+// the r-th voxel in key order: removed[r] = seeded and dropped by the keep rule, added[r] = not seeded and kept
 __global__ void __launch_bounds__(256) vs_change_kernel(const uint32_t* __restrict__ order, uint32_t n, const uint2* __restrict__ hm,
                                                         uint32_t min_miss, double ratio, uint32_t n_seeded,
                                                         uint32_t* __restrict__ removed, uint32_t* __restrict__ added) {
   const uint32_t r = blockIdx.x * 256u + threadIdx.x;
   if (r >= n) return;
   const uint32_t e = order[r];
-  const uint2 v = hm ? hm[e] : make_uint2(0u, 0u);
-  const bool kept = !(v.y >= min_miss && (double)v.y > ratio * (double)v.x);
+  const bool kept = !dropped(evidence(hm, e), min_miss, ratio);
   const bool seeded = e < n_seeded;
   removed[r] = (seeded && !kept) ? 1u : 0u;
   added[r] = (!seeded && kept) ? 1u : 0u;
 }
 
-int get_state(malio_handle* h, VoxState*& V) {
+// the handle's voxel map, created empty on first use; the handle's device is selected
+int get_state(malio_handle* h, VoxState*& V, DeviceState*& D) {
+  D = (DeviceState*)h->dev;
+  CUDA_TRY(cudaSetDevice(D->device));
   V = (VoxState*)h->voxmap;
   if (V) return MALIO_OK;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
   V = new VoxState;
   h->voxmap = V;
   if (int rc = V->d_small.allocate(h, D->stream, 6)) return rc;
@@ -448,7 +437,7 @@ int grow_sort(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t, b.k, b.v, (int)n, VKeyDecomposer{}, D->stream));
   return grow_temp(h, V, D, t);
 }
-// the run scratch for the n points of a scan
+// the run scratch for n rows
 int grow_runs(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
   if (n > V->d_head.size()) {
     const uint64_t c = n + n / 8 + 1024;
@@ -501,6 +490,44 @@ int grow_table(malio_handle* h, VoxState* V, DeviceState* D, uint64_t need) {
   return MALIO_OK;
 }
 
+// the carving evidence of every entry the table holds room for, zero: allocated by the first carve, or by a seed with hits
+int ensure_evidence(malio_handle* h, VoxState* V, DeviceState* D) {
+  if (V->d_hm) return MALIO_OK;
+  const size_t cap = V->d_ekey.size();
+  if (int rc = malio_buf::allocate_group(h, D->stream, {{V->d_hm, cap}, {V->d_stamp, cap}})) return rc;
+  CUDA_TRY(cudaMemsetAsync(V->d_hm, 0, cap * sizeof(uint2), D->stream));
+  CUDA_TRY(cudaMemsetAsync(V->d_stamp, 0, cap * sizeof(uint32_t), D->stream));
+  return MALIO_OK;
+}
+
+// enqueue the fold of rows [0, n) of src on the handle's stream, from vm_key_kernel to vm_fold_kernel (table, sort area and
+// run scratch grown for them; small[0] is the call's fault flag, cleared by the caller).  Then d_rent holds each run's entry
+// and d_head the new runs' ranks; the caller enqueues vm_count_kernel, which raises small[2] by the new entries.
+template <class Rows>
+int enqueue_fold(malio_handle* h, VoxState* V, DeviceState* D, const Rows& src, float il, uint32_t n) {
+  cudaStream_t st = D->stream;
+  const uint32_t g = (n + 255) / 256;
+  const uint64_t mask = V->d_hash.size() - 1;
+  SortBufs b = sort_bufs(V);
+  vm_key_kernel<<<g, 256, 0, st>>>(src, il, n, b.k.Current(), b.v.Current(), V->d_small);
+  size_t t = V->d_temp.size();
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)n, VKeyDecomposer{}, st));
+  const VKey* key = b.k.Current();
+  const uint32_t* val = b.v.Current();
+  vm_head_kernel<<<g, 256, 0, st>>>(key, n, V->d_head);
+  t = V->d_temp.size();
+  CUDA_TRY(cub::DeviceScan::InclusiveSum(V->d_temp, t, V->d_head.data(), V->d_rent.data(), (int)n, st));
+  vm_run_kernel<<<g, 256, 0, st>>>(V->d_head, V->d_rent, n, V->d_run, V->d_small);
+  vm_lookup_kernel<<<g, 256, 0, st>>>(V->d_run, key, n, V->d_small, V->d_hash, mask, V->d_ekey, V->d_rent, V->d_new);
+  t = V->d_temp.size();
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, V->d_new.data(), V->d_head.data(), (int)n, st));
+  vm_fold_kernel<<<(n + 127) / 128, 128, 0, st>>>(src, V->d_run, key, val, n, V->d_small, V->d_rent, V->d_head, V->d_hash, mask,
+                                                 V->d_ekey, V->d_esum, V->d_ecnt);
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += 6;   // the radix sort counted as one
+  return MALIO_OK;
+}
+
 // enqueue the sort of the entries by key on the handle's stream (sort area already grown): *order = the entries in key order,
 // the values half CUB left current (the other values half and the key halves are free once it is sorted)
 int enqueue_order(malio_handle* h, VoxState* V, DeviceState* D, SortBufs& b) {
@@ -513,81 +540,110 @@ int enqueue_order(malio_handle* h, VoxState* V, DeviceState* D, SortBufs& b) {
   return MALIO_OK;
 }
 
-// enqueue the centroids in key order into out[0 .. min(n_vox, cap)) on the handle's stream (sort area already grown).  out may
-// be the sort area itself (its two key halves, 24 B a row): the keys are dead once sorted, the order is read from the values.
-int enqueue_sorted(malio_handle* h, VoxState* V, DeviceState* D, float4* out, uint64_t cap) {
-  const uint32_t n = (uint32_t)V->n_vox;
-  SortBufs b = sort_bufs(V);
-  if (int rc = enqueue_order(h, V, D, b)) return rc;
-  vm_centroid_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(b.v.Current(), n, V->d_esum, V->d_ecnt, out, cap < n ? (uint32_t)cap : n);
+// enqueue the centroids of the entries order[0 .. min(n, cap)) into out on the handle's stream, one thread per order row
+int enqueue_centroids(malio_handle* h, VoxState* V, DeviceState* D, const uint32_t* order, uint32_t n, float4* out, uint32_t cap) {
+  vm_centroid_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(order, n, V->d_esum, V->d_ecnt, out, cap);
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 1;
   return MALIO_OK;
 }
 
-// the kept entries in key order (malio_carve_keep), at 20 B into each row of the sort area: behind the centroids a save stages
-// over the key halves (16 B a row), beside the flags' exclusive scan (16 B into the row)
-uint32_t* kept_order(const VoxState* V) { return reinterpret_cast<uint32_t*>(V->d_sort + 20 * sort_rows(V)); }
+// enqueue the centroids in key order into out[0 .. min(n_vox, cap)) on the handle's stream (sort area already grown).  out may
+// be the sort area itself (sort_stage): the keys are dead once sorted, the order is read from the values.
+int enqueue_sorted(malio_handle* h, VoxState* V, DeviceState* D, float4* out, uint64_t cap) {
+  const uint32_t n = (uint32_t)V->n_vox;
+  SortBufs b = sort_bufs(V);
+  if (int rc = enqueue_order(h, V, D, b)) return rc;
+  return enqueue_centroids(h, V, D, b.v.Current(), n, out, cap < n ? (uint32_t)cap : n);
+}
 
-// sort, flag, scan and compact the entries the keep rule does not drop into kept_order(V); waits for their count (*n_kept)
+// A selection of the entries in key order (sort area grown for the entries): enqueue_select_order, one kernel that flags
+// every entry, then enqueue_select per flag column.
+int enqueue_select_order(malio_handle* h, VoxState* V, DeviceState* D, SortBufs& b) {
+  size_t t = 0;
+  uint32_t* un = nullptr;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)V->n_vox, D->stream));
+  if (int rc = grow_temp(h, V, D, t)) return rc;
+  b = sort_bufs(V);
+  return enqueue_order(h, V, D, b);
+}
+// the exclusive scan of flag into COL_SCAN, then the flagged entries of order compacted into column `col`, their count into
+// small[word]
+int enqueue_select(malio_handle* h, VoxState* V, DeviceState* D, const uint32_t* order, const uint32_t* flag, uint32_t col, int word) {
+  const uint32_t n = (uint32_t)V->n_vox;
+  uint32_t* pos = sort_col(V, COL_SCAN);
+  size_t t = V->d_temp.size();
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, flag, pos, (int)n, D->stream));
+  vc_compact_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(order, flag, pos, n, sort_col(V, col), V->d_small + word);
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += 1;
+  return MALIO_OK;
+}
+
+// the entries the keep rule does not drop into COL_KEPT; waits for their count (*n_kept)
 int enqueue_kept(malio_handle* h, VoxState* V, DeviceState* D, const malio_carve_keep* keep, uint64_t* n_kept) {
   cudaStream_t st = D->stream;
   const uint32_t n = (uint32_t)V->n_vox;
-  SortBufs b = sort_bufs(V);
-  size_t t = 0;
-  uint32_t* un = nullptr;
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)n, st));
-  if (int rc = grow_temp(h, V, D, t)) return rc;
-  if (int rc = enqueue_order(h, V, D, b)) return rc;
-  uint32_t* flag = b.v.Alternate();
-  uint32_t* pos = reinterpret_cast<uint32_t*>(V->d_sort + 16 * sort_rows(V));
-  const uint32_t g = (n + 255) / 256;
-  vc_keep_kernel<<<g, 256, 0, st>>>(b.v.Current(), n, V->d_hm, keep->min_miss, (double)keep->max_miss_per_hit, flag);
-  t = V->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, flag, pos, (int)n, st));
-  vc_compact_kernel<<<g, 256, 0, st>>>(b.v.Current(), flag, pos, n, kept_order(V), V->d_small);
-  CUDA_TRY(cudaGetLastError());
-  D->ctr.kernel_launches += 2;
+  SortBufs b;
+  if (int rc = enqueue_select_order(h, V, D, b)) return rc;
+  vc_keep_kernel<<<(n + 255) / 256, 256, 0, st>>>(b.v.Current(), n, V->d_hm, keep->min_miss, (double)keep->max_miss_per_hit,
+                                                  b.v.Alternate());
+  D->ctr.kernel_launches += 1;
+  if (int rc = enqueue_select(h, V, D, b.v.Current(), b.v.Alternate(), COL_KEPT, 3)) return rc;
   CUDA_TRY(cudaMemcpyAsync(V->h_small + 3, V->d_small + 3, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));   // the kept count sizes the caller's output and the file
   *n_kept = V->h_small[3];
   return MALIO_OK;
 }
 
-// The changes against the seed in key order, laid out in the sort area (row offsets in bytes per row): the removed order at 20
-// (kept_order) and the added order at 16, both behind the centroids a save stages over the key halves; the added flags at 0,
-// the removed flags in the values half the sort left free, the two exclusive scans at 4 and 8.  Sorts, flags, scans and
-// compacts, then waits for the two counts.
-uint32_t* added_order(const VoxState* V) { return reinterpret_cast<uint32_t*>(V->d_sort + 16 * sort_rows(V)); }
+// the changes against the seed: the removed entries into COL_KEPT, the added ones into COL_ADDED; waits for the two counts
 int enqueue_changes(malio_handle* h, VoxState* V, DeviceState* D, const malio_carve_keep* keep, uint64_t* n_removed, uint64_t* n_added) {
   cudaStream_t st = D->stream;
   const uint32_t n = (uint32_t)V->n_vox;
-  const uint64_t rows = sort_rows(V);
-  SortBufs b = sort_bufs(V);
-  size_t t = 0;
-  uint32_t* un = nullptr;
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)n, st));
-  if (int rc = grow_temp(h, V, D, t)) return rc;
-  if (int rc = enqueue_order(h, V, D, b)) return rc;
-  uint32_t* flag_r = b.v.Alternate();
-  uint32_t* flag_a = reinterpret_cast<uint32_t*>(V->d_sort.data());
-  uint32_t* pos_r = reinterpret_cast<uint32_t*>(V->d_sort + 4 * rows);
-  uint32_t* pos_a = reinterpret_cast<uint32_t*>(V->d_sort + 8 * rows);
-  const uint32_t g = (n + 255) / 256;
-  vs_change_kernel<<<g, 256, 0, st>>>(b.v.Current(), n, V->d_hm, keep->min_miss, (double)keep->max_miss_per_hit,
-                                      (uint32_t)V->n_seeded, flag_r, flag_a);
-  t = V->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, flag_r, pos_r, (int)n, st));
-  vc_compact_kernel<<<g, 256, 0, st>>>(b.v.Current(), flag_r, pos_r, n, kept_order(V), V->d_small);        // -> small[3]
-  t = V->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, flag_a, pos_a, (int)n, st));
-  vc_compact_kernel<<<g, 256, 0, st>>>(b.v.Current(), flag_a, pos_a, n, added_order(V), V->d_small + 2);   // -> small[5]
-  CUDA_TRY(cudaGetLastError());
-  D->ctr.kernel_launches += 3;
+  SortBufs b;
+  if (int rc = enqueue_select_order(h, V, D, b)) return rc;
+  uint32_t* flag_a = sort_col(V, COL_FLAGS);
+  vs_change_kernel<<<(n + 255) / 256, 256, 0, st>>>(b.v.Current(), n, V->d_hm, keep->min_miss, (double)keep->max_miss_per_hit,
+                                                    (uint32_t)V->n_seeded, b.v.Alternate(), flag_a);
+  D->ctr.kernel_launches += 1;
+  if (int rc = enqueue_select(h, V, D, b.v.Current(), b.v.Alternate(), COL_KEPT, 3)) return rc;
+  if (int rc = enqueue_select(h, V, D, b.v.Current(), flag_a, COL_ADDED, 5)) return rc;
   CUDA_TRY(cudaMemcpyAsync(V->h_small + 3, V->d_small + 3, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));   // the counts size the caller's outputs and the files
   *n_removed = V->h_small[3];
   *n_added = V->h_small[5];
+  return MALIO_OK;
+}
+
+// the first n rows of stage (device memory) as a binary PCD at path, through the pinned bounce buffer
+int write_staged(malio_handle* h, VoxState* V, DeviceState* D, const char* path, const float4* stage, uint64_t n) {
+  return malio_pcd::write_binary(path, n, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
+    if (cudaMemcpyAsync(V->h_bounce, stage + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, D->stream) != cudaSuccess ||
+        cudaStreamSynchronize(D->stream) != cudaSuccess)
+      return (int)MALIO_ERR_CUDA;
+    D->ctr.d2h_bytes += cnt * sizeof(float4);
+    *xyzi = (const float*)V->h_bounce.data();
+    return (int)MALIO_OK;
+  }, h->err);
+}
+
+// after a save: the entry-sized sort area and CUB's storage go back once the stream is drained.  Between saves the map holds
+// its entries, its hash and the scan-sized scratch only (the next accumulate regrows the sort area for its scan).
+int release_scratch(malio_handle* h, VoxState* V, DeviceState* D) {
+  CUDA_TRY(cudaStreamSynchronize(D->stream));
+  V->d_sort.release();
+  V->d_temp.release();
+  return MALIO_OK;
+}
+
+// p, rows of the caller in device memory: check_device_ptr, then p aligned to `align` bytes (h->err names `what` and `rows`)
+constexpr const char* CENTROID_ROWS = "the centroids are stored as float4";
+int check_rows(malio_handle* h, const DeviceState* D, const void* p, const char* what, uintptr_t align, const char* rows) {
+  if (int rc = check_device_ptr(h, D, p, what)) return rc;
+  if (reinterpret_cast<uintptr_t>(p) & (align - 1)) {
+    h->err = std::string(what) + ": not " + std::to_string(align) + "-byte aligned (" + rows + ")";
+    return MALIO_ERR_INVALID_ARG;
+  }
   return MALIO_OK;
 }
 
@@ -636,9 +692,8 @@ void destroy(malio_handle* h) {
 int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, float leaf, const malio_carve_args* carve,
                uint64_t* n_voxels) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   if (carve && !(std::isfinite(carve->max_range) && carve->max_range > 0.f && std::isfinite(carve->end_margin) && carve->end_margin >= 0.f)) {
     h->err = "world voxel carve: max_range must be finite and > 0, end_margin finite and >= 0";
     return MALIO_ERR_INVALID_ARG;
@@ -661,40 +716,21 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
     if (int rc = grow_table(h, V, D, V->n_vox + n)) return rc;
     if (int rc = grow_sort(h, V, D, n)) return rc;
     if (int rc = grow_runs(h, V, D, n)) return rc;
-    if (carve && !V->d_hm) {   // the first carve: every entry so far starts at hit = miss = 0
-      const size_t cap = V->d_ekey.size();
-      if (int rc = malio_buf::allocate_group(h, D->stream, {{V->d_hm, cap}, {V->d_stamp, cap}})) return rc;
-      CUDA_TRY(cudaMemsetAsync(V->d_hm, 0, cap * sizeof(uint2), D->stream));
-      CUDA_TRY(cudaMemsetAsync(V->d_stamp, 0, cap * sizeof(uint32_t), D->stream));
-    }
+    if (carve) { if (int rc = ensure_evidence(h, V, D)) return rc; }   // the first carve: every entry so far at hit = miss = 0
     cudaStream_t st = D->stream;
-    const PassConst pc = make_pass_const(h, D, s);
+    const ScanRows src{c, make_pass_const(h, D, s)};
+    const float il = 1.0f / leaf;
     const uint32_t nn = (uint32_t)n, g = (nn + 255) / 256;
-    const uint64_t mask = V->d_hash.size() - 1;
     CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 2 * sizeof(uint32_t), st));   // fault flag, run count
-    SortBufs b = sort_bufs(V);
-    vm_key_kernel<<<g, 256, 0, st>>>(c, pc, 1.0f / leaf, nn, b.k.Current(), b.v.Current(), V->d_small);
-    if (carve) vc_origin_kernel<<<1, 32, 0, st>>>(c, pc, 1.0f / leaf, V->d_small);
-    size_t t = V->d_temp.size();
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)nn, VKeyDecomposer{}, st));
-    const VKey* key = b.k.Current();
-    const uint32_t* val = b.v.Current();
-    vm_head_kernel<<<g, 256, 0, st>>>(key, nn, V->d_head);
-    t = V->d_temp.size();
-    CUDA_TRY(cub::DeviceScan::InclusiveSum(V->d_temp, t, V->d_head.data(), V->d_rent.data(), (int)nn, st));
-    vm_run_kernel<<<g, 256, 0, st>>>(V->d_head, V->d_rent, nn, V->d_run, V->d_small);
-    vm_lookup_kernel<<<g, 256, 0, st>>>(V->d_run, key, nn, V->d_small, V->d_hash, mask, V->d_ekey, V->d_rent, V->d_new);
-    t = V->d_temp.size();
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, V->d_new.data(), V->d_head.data(), (int)nn, st));
-    vm_fold_kernel<<<(nn + 127) / 128, 128, 0, st>>>(c, pc, V->d_run, key, val, nn, V->d_small, V->d_rent, V->d_head,
-                                                    V->d_hash, mask, V->d_ekey, V->d_esum, V->d_ecnt);
+    if (carve) vc_origin_kernel<<<1, 32, 0, st>>>(c, src.pc, il, V->d_small);
+    if (int rc = enqueue_fold(h, V, D, src, il, nn)) return rc;
     if (carve) vc_hit_kernel<<<g, 256, 0, st>>>(V->d_small, V->d_rent, V->d_head, nn, V->d_hm, V->d_stamp, scan);
     vm_count_kernel<<<1, 1, 0, st>>>(V->d_head, V->d_new, V->d_small);
     if (carve)
-      vc_carve_kernel<<<g, 256, 0, st>>>(c, pc, 1.0f / leaf, nn, (double)carve->max_range, (double)carve->end_margin, V->d_small,
-                                         V->d_hash, mask, V->d_ekey, V->d_hm, V->d_stamp, scan);
+      vc_carve_kernel<<<g, 256, 0, st>>>(c, src.pc, il, nn, (double)carve->max_range, (double)carve->end_margin, V->d_small,
+                                         V->d_hash, V->d_hash.size() - 1, V->d_ekey, V->d_hm, V->d_stamp, scan);
     CUDA_TRY(cudaGetLastError());
-    D->ctr.kernel_launches += carve ? 10 : 7;
+    D->ctr.kernel_launches += carve ? 4 : 1;
     CUDA_TRY(cudaMemcpyAsync(V->h_small, V->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));   // the call's one wait: the fault flag and the entry count
     if (V->h_small[0]) {
@@ -713,16 +749,11 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
 
 int download_device(malio_handle* h, float* out, uint64_t cap, uint64_t* n_out, cudaStream_t caller) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   const uint64_t n = V->n_vox, k = n < cap ? n : cap;
   if (out && k) {
-    if (int rc = check_device_ptr(h, D, out, "malio_world_voxel_download_device out")) return rc;
-    if (reinterpret_cast<uintptr_t>(out) & 15u) {
-      h->err = "malio_world_voxel_download_device out: not 16-byte aligned (the centroids are stored as float4)";
-      return MALIO_ERR_INVALID_ARG;
-    }
+    if (int rc = check_rows(h, D, out, "malio_world_voxel_download_device out", 16, CENTROID_ROWS)) return rc;
   }
   *n_out = n;
   if (!out || k == 0) return MALIO_OK;
@@ -735,16 +766,11 @@ int download_device(malio_handle* h, float* out, uint64_t cap, uint64_t* n_out, 
 // the (hit, miss) pairs in the order of download_device, with its size protocol and device-memory contract
 int evidence_device(malio_handle* h, uint32_t* out, uint64_t cap, uint64_t* n_out, cudaStream_t caller) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   const uint64_t n = V->n_vox, k = n < cap ? n : cap;
   if (out && k) {
-    if (int rc = check_device_ptr(h, D, out, "malio_world_voxel_evidence_device out")) return rc;
-    if (reinterpret_cast<uintptr_t>(out) & 7u) {
-      h->err = "malio_world_voxel_evidence_device out: not 8-byte aligned (the pairs are stored as uint2)";
-      return MALIO_ERR_INVALID_ARG;
-    }
+    if (int rc = check_rows(h, D, out, "malio_world_voxel_evidence_device out", 8, "the pairs are stored as uint2")) return rc;
   }
   *n_out = n;
   if (!out || k == 0) return MALIO_OK;
@@ -761,16 +787,11 @@ int evidence_device(malio_handle* h, uint32_t* out, uint64_t cap, uint64_t* n_ou
 // the centroids of the kept voxels in the order of download_device; waits for their count before it enqueues the copy-out
 int download_kept_device(malio_handle* h, const malio_carve_keep* keep, float* out, uint64_t cap, uint64_t* n_out, cudaStream_t caller) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   if (int rc = check_keep(h, keep)) return rc;
   if (out && cap && V->n_vox) {
-    if (int rc = check_device_ptr(h, D, out, "malio_world_voxel_download_kept_device out")) return rc;
-    if (reinterpret_cast<uintptr_t>(out) & 15u) {
-      h->err = "malio_world_voxel_download_kept_device out: not 16-byte aligned (the centroids are stored as float4)";
-      return MALIO_ERR_INVALID_ARG;
-    }
+    if (int rc = check_rows(h, D, out, "malio_world_voxel_download_kept_device out", 16, CENTROID_ROWS)) return rc;
   }
   uint64_t n = 0;
   if (V->n_vox) {
@@ -781,53 +802,34 @@ int download_kept_device(malio_handle* h, const malio_carve_keep* keep, float* o
   const uint64_t k = n < cap ? n : cap;
   if (!out || k == 0) return MALIO_OK;
   if (int rc = caller_enter(h, D, caller)) return rc;
-  vm_centroid_kernel<<<(uint32_t)((k + 255) / 256), 256, 0, D->stream>>>(kept_order(V), (uint32_t)k, V->d_esum, V->d_ecnt,
-                                                                          reinterpret_cast<float4*>(out), (uint32_t)k);
-  CUDA_TRY(cudaGetLastError());
-  D->ctr.kernel_launches += 1;
+  if (int rc = enqueue_centroids(h, V, D, sort_col(V, COL_KEPT), (uint32_t)k, reinterpret_cast<float4*>(out), (uint32_t)k)) return rc;
   return caller_leave(h, D, caller);
 }
 
 // keep == NULL: every voxel (malio_world_voxel_save_pcd); otherwise the voxels the rule keeps (malio_world_voxel_save_pcd_kept)
 int save_pcd(malio_handle* h, const char* path, const malio_carve_keep* keep, int clear) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   if (keep) { if (int rc = check_keep(h, keep)) return rc; }
   if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
   uint64_t n = V->n_vox;
   if (int rc = grow_sort(h, V, D, n)) return rc;
   if (!V->h_bounce) { if (int rc = V->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
-  float4* stage = reinterpret_cast<float4*>(V->d_sort.data());   // the key halves: 24 B a row, the centroids take 16
+  float4* stage = sort_stage(V);
   if (keep) {
     if (int rc = enqueue_kept(h, V, D, keep, &n)) return rc;
     if (n == 0) {
-      V->d_sort.release();   // enqueue_kept has waited for the stream
-      V->d_temp.release();
+      if (int rc = release_scratch(h, V, D)) return rc;
       h->err = "world voxel save: the keep rule drops every voxel (nothing is written)";
       return MALIO_ERR_STATE;
     }
-    vm_centroid_kernel<<<(uint32_t)((n + 255) / 256), 256, 0, D->stream>>>(kept_order(V), (uint32_t)n, V->d_esum, V->d_ecnt, stage,
-                                                                            (uint32_t)n);
-    CUDA_TRY(cudaGetLastError());
-    D->ctr.kernel_launches += 1;
+    if (int rc = enqueue_centroids(h, V, D, sort_col(V, COL_KEPT), (uint32_t)n, stage, (uint32_t)n)) return rc;
   } else if (int rc = enqueue_sorted(h, V, D, stage, n)) {
     return rc;
   }
-  const int rc = malio_pcd::write_binary(path, n, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
-    if (cudaMemcpyAsync(V->h_bounce, stage + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, D->stream) != cudaSuccess ||
-        cudaStreamSynchronize(D->stream) != cudaSuccess)
-      return (int)MALIO_ERR_CUDA;
-    D->ctr.d2h_bytes += cnt * sizeof(float4);
-    *xyzi = (const float*)V->h_bounce.data();
-    return (int)MALIO_OK;
-  }, h->err);
-  // the entry-sized sort area and CUB's storage go back: between saves the map holds its entries, its hash and the scan-sized
-  // scratch only (the next accumulate regrows the sort area for its scan)
-  CUDA_TRY(cudaStreamSynchronize(D->stream));
-  V->d_sort.release();
-  V->d_temp.release();
+  const int rc = write_staged(h, V, D, path, stage, n);
+  if (int e = release_scratch(h, V, D)) return e;
   if (rc == MALIO_OK && clear) {
     if (int c = clear_map(h, V, D)) return c;
   }
@@ -836,37 +838,27 @@ int save_pcd(malio_handle* h, const char* path, const malio_carve_keep* keep, in
 
 // malio_world_voxel_seed (on_device false: xyzi in host memory, staged through the pinned bounce buffer into a chunk-sized
 // device buffer) and malio_world_voxel_seed_device (xyzi read in place, ordered on `caller`).  The points are folded chunk by
-// chunk in input order, each chunk through accumulate's pipeline with vs_key_kernel / vs_fold_kernel for the row source; the
-// table is sized for n points before the first chunk, so the chunks are enqueued back to back and the call waits once.
+// chunk in input order, each chunk through enqueue_fold with SeedRows; the table is sized for n points before the first chunk,
+// so the chunks are enqueued back to back and the call waits once.
 int seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t seed_hits, bool on_device, cudaStream_t caller,
          uint64_t* n_voxels) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   if (!(leaf > 0.f) || !std::isfinite(leaf)) { h->err = "world voxel seed: leaf must be a finite size > 0"; return MALIO_ERR_INVALID_ARG; }
   if (V->n_vox || V->leaf_set) {
     h->err = "world voxel seed: the voxel map is not empty (seed a new map or one after a clearing save)";
     return MALIO_ERR_STATE;
   }
   if (on_device) {
-    if (int rc = check_device_ptr(h, D, xyzi, "malio_world_voxel_seed_device xyzi")) return rc;
-    if (reinterpret_cast<uintptr_t>(xyzi) & 15u) {
-      h->err = "malio_world_voxel_seed_device xyzi: not 16-byte aligned (the rows are read as float4)";
-      return MALIO_ERR_INVALID_ARG;
-    }
+    if (int rc = check_rows(h, D, xyzi, "malio_world_voxel_seed_device xyzi", 16, "the rows are read as float4")) return rc;
   }
   const uint64_t chunk = n < MALIO_SEED_CHUNK ? n : MALIO_SEED_CHUNK;
   if (int rc = grow_table(h, V, D, n)) return rc;
   if (int rc = grow_sort(h, V, D, chunk)) return rc;
   if (int rc = grow_runs(h, V, D, chunk)) return rc;
   const bool had_hm = (bool)V->d_hm;
-  if (seed_hits && !had_hm) {   // the counters the first carve would allocate, zero beyond the seed
-    const size_t cap = V->d_ekey.size();
-    if (int rc = malio_buf::allocate_group(h, D->stream, {{V->d_hm, cap}, {V->d_stamp, cap}})) return rc;
-    CUDA_TRY(cudaMemsetAsync(V->d_hm, 0, cap * sizeof(uint2), D->stream));
-    CUDA_TRY(cudaMemsetAsync(V->d_stamp, 0, cap * sizeof(uint32_t), D->stream));
-  }
+  if (seed_hits) { if (int rc = ensure_evidence(h, V, D)) return rc; }   // zero beyond the seed, as the first carve leaves them
   DeviceBuffer<float4> stage;
   if (!on_device) {
     if (int rc = stage.allocate(h, D->stream, chunk)) return rc;
@@ -875,12 +867,10 @@ int seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t se
     return rc;
   }
   cudaStream_t st = D->stream;
-  const uint64_t mask = V->d_hash.size() - 1;
-  const float il = 1.0f / leaf;
   CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 2 * sizeof(uint32_t), st));   // fault flag (kept over the chunks), run count
   const float4* rows = reinterpret_cast<const float4*>(xyzi);
   for (uint64_t first = 0; first < n; first += chunk) {
-    const uint32_t m = (uint32_t)(n - first < chunk ? n - first : chunk), g = (m + 255) / 256;
+    const uint32_t m = (uint32_t)(n - first < chunk ? n - first : chunk);
     const float4* src = rows + first;
     if (!on_device) {   // the previous chunk's kernels and copies are done before the bounce buffer and the stage are reused
       for (uint32_t p = 0; p < m; p += malio_pcd::CHUNK) {
@@ -892,24 +882,10 @@ int seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t se
       D->ctr.h2d_bytes += (uint64_t)m * sizeof(float4);
       src = stage;
     }
-    SortBufs b = sort_bufs(V);
-    vs_key_kernel<<<g, 256, 0, st>>>(src, il, m, b.k.Current(), b.v.Current(), V->d_small);
-    size_t t = V->d_temp.size();
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)m, VKeyDecomposer{}, st));
-    const VKey* key = b.k.Current();
-    const uint32_t* val = b.v.Current();
-    vm_head_kernel<<<g, 256, 0, st>>>(key, m, V->d_head);
-    t = V->d_temp.size();
-    CUDA_TRY(cub::DeviceScan::InclusiveSum(V->d_temp, t, V->d_head.data(), V->d_rent.data(), (int)m, st));
-    vm_run_kernel<<<g, 256, 0, st>>>(V->d_head, V->d_rent, m, V->d_run, V->d_small);
-    vm_lookup_kernel<<<g, 256, 0, st>>>(V->d_run, key, m, V->d_small, V->d_hash, mask, V->d_ekey, V->d_rent, V->d_new);
-    t = V->d_temp.size();
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, V->d_new.data(), V->d_head.data(), (int)m, st));
-    vs_fold_kernel<<<(m + 127) / 128, 128, 0, st>>>(src, V->d_run, key, val, m, V->d_small, V->d_rent, V->d_head, V->d_hash, mask,
-                                                   V->d_ekey, V->d_esum, V->d_ecnt);
+    if (int rc = enqueue_fold(h, V, D, SeedRows{src}, 1.0f / leaf, m)) return rc;
     vm_count_kernel<<<1, 1, 0, st>>>(V->d_head, V->d_new, V->d_small);
     CUDA_TRY(cudaGetLastError());
-    D->ctr.kernel_launches += 7;
+    D->ctr.kernel_launches += 1;
   }
   if (V->d_hm) {
     const uint32_t nn = (uint32_t)n;
@@ -942,20 +918,15 @@ int seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t se
 int changes_device(malio_handle* h, const malio_carve_keep* keep, float* d_removed, uint64_t cap_removed, uint64_t* n_removed,
                    float* d_added, uint64_t cap_added, uint64_t* n_added, cudaStream_t caller) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   if (int rc = check_keep(h, keep)) return rc;
   if (V->n_vox) {
-    const struct { const float* out; uint64_t cap; const char* what; } outs[2] = {
-        {d_removed, cap_removed, "malio_world_voxel_changes_device removed"}, {d_added, cap_added, "malio_world_voxel_changes_device added"}};
-    for (const auto& o : outs) {
-      if (!o.out || !o.cap) continue;
-      if (int rc = check_device_ptr(h, D, o.out, o.what)) return rc;
-      if (reinterpret_cast<uintptr_t>(o.out) & 15u) {
-        h->err = std::string(o.what) + ": not 16-byte aligned (the centroids are stored as float4)";
-        return MALIO_ERR_INVALID_ARG;
-      }
+    if (d_removed && cap_removed) {
+      if (int rc = check_rows(h, D, d_removed, "malio_world_voxel_changes_device removed", 16, CENTROID_ROWS)) return rc;
+    }
+    if (d_added && cap_added) {
+      if (int rc = check_rows(h, D, d_added, "malio_world_voxel_changes_device added", 16, CENTROID_ROWS)) return rc;
     }
   }
   uint64_t nr = 0, na = 0;
@@ -968,14 +939,12 @@ int changes_device(malio_handle* h, const malio_carve_keep* keep, float* d_remov
   const uint64_t kr = d_removed ? (nr < cap_removed ? nr : cap_removed) : 0, ka = d_added ? (na < cap_added ? na : cap_added) : 0;
   if (kr == 0 && ka == 0) return MALIO_OK;
   if (int rc = caller_enter(h, D, caller)) return rc;
-  if (kr)
-    vm_centroid_kernel<<<(uint32_t)((kr + 255) / 256), 256, 0, D->stream>>>(kept_order(V), (uint32_t)kr, V->d_esum, V->d_ecnt,
-                                                                             reinterpret_cast<float4*>(d_removed), (uint32_t)kr);
-  if (ka)
-    vm_centroid_kernel<<<(uint32_t)((ka + 255) / 256), 256, 0, D->stream>>>(added_order(V), (uint32_t)ka, V->d_esum, V->d_ecnt,
-                                                                             reinterpret_cast<float4*>(d_added), (uint32_t)ka);
-  CUDA_TRY(cudaGetLastError());
-  D->ctr.kernel_launches += (kr ? 1 : 0) + (ka ? 1 : 0);
+  if (kr) {
+    if (int rc = enqueue_centroids(h, V, D, sort_col(V, COL_KEPT), (uint32_t)kr, reinterpret_cast<float4*>(d_removed), (uint32_t)kr)) return rc;
+  }
+  if (ka) {
+    if (int rc = enqueue_centroids(h, V, D, sort_col(V, COL_ADDED), (uint32_t)ka, reinterpret_cast<float4*>(d_added), (uint32_t)ka)) return rc;
+  }
   return caller_leave(h, D, caller);
 }
 
@@ -983,9 +952,8 @@ int changes_device(malio_handle* h, const malio_carve_keep* keep, float* d_remov
 int save_changes_pcd(malio_handle* h, const malio_carve_keep* keep, const char* removed_path, const char* added_path, uint64_t* n_removed,
                      uint64_t* n_added) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   if (int rc = check_keep(h, keep)) return rc;
   if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
   if (int rc = grow_sort(h, V, D, V->n_vox)) return rc;
@@ -994,35 +962,22 @@ int save_changes_pcd(malio_handle* h, const malio_carve_keep* keep, const char* 
   if (int rc = enqueue_changes(h, V, D, keep, &nr, &na)) return rc;
   if (n_removed) *n_removed = nr;
   if (n_added) *n_added = na;
-  float4* stage = reinterpret_cast<float4*>(V->d_sort.data());   // the key halves: both orders lie behind them
+  float4* stage = sort_stage(V);
   int rc = MALIO_OK;
-  const struct { const char* path; const uint32_t* order; uint64_t cnt; } sets[2] = {{removed_path, kept_order(V), nr},
-                                                                                    {added_path, added_order(V), na}};
+  const struct { const char* path; uint32_t col; uint64_t cnt; } sets[2] = {{removed_path, COL_KEPT, nr}, {added_path, COL_ADDED, na}};
   for (const auto& set : sets) {
-    const uint64_t cnt = set.cnt;
-    if (rc != MALIO_OK || !set.path || cnt == 0) continue;
-    vm_centroid_kernel<<<(uint32_t)((cnt + 255) / 256), 256, 0, D->stream>>>(set.order, (uint32_t)cnt, V->d_esum, V->d_ecnt, stage,
-                                                                              (uint32_t)cnt);
-    CUDA_TRY(cudaGetLastError());
-    D->ctr.kernel_launches += 1;
-    rc = malio_pcd::write_binary(set.path, cnt, [&](uint64_t first, uint64_t c, const float** xyzi) {
-      if (cudaMemcpyAsync(V->h_bounce, stage + first, c * sizeof(float4), cudaMemcpyDeviceToHost, D->stream) != cudaSuccess ||
-          cudaStreamSynchronize(D->stream) != cudaSuccess)
-        return (int)MALIO_ERR_CUDA;
-      D->ctr.d2h_bytes += c * sizeof(float4);
-      *xyzi = (const float*)V->h_bounce.data();
-      return (int)MALIO_OK;
-    }, h->err);
+    if (rc != MALIO_OK || !set.path || set.cnt == 0) continue;
+    if (int e = enqueue_centroids(h, V, D, sort_col(V, set.col), (uint32_t)set.cnt, stage, (uint32_t)set.cnt)) return e;
+    rc = write_staged(h, V, D, set.path, stage, set.cnt);
   }
-  CUDA_TRY(cudaStreamSynchronize(D->stream));   // as save_pcd: the entry-sized sort area and CUB's storage go back
-  V->d_sort.release();
-  V->d_temp.release();
+  if (int e = release_scratch(h, V, D)) return e;
   return rc;
 }
 
 int info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* device_bytes) {
   VoxState* V;
-  if (int rc = get_state(h, V)) return rc;
+  DeviceState* D;
+  if (int rc = get_state(h, V, D)) return rc;
   if (n_voxels) *n_voxels = V->n_vox;
   if (capacity) *capacity = V->d_ekey.size();
   if (device_bytes)

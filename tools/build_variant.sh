@@ -16,6 +16,7 @@ for cu in *.cu; do
 done
 /usr/bin/g++ -O3 -std=c++17 -fPIC -fopenmp -Wall -I../../include -I. -c malio_host.cpp -o $out/malio_host.o
 /usr/bin/g++ -O3 -std=c++17 -fPIC -fopenmp -Wall -ffp-contract=off -I../../include -I. -c malio_dataset.cpp -o $out/malio_dataset.o
+/usr/bin/g++ -O3 -std=c++17 -fPIC -fopenmp -Wall -I../../include -I. -c malio_pcd.cpp -o $out/malio_pcd.o
 wait
 $NVCC -gencode arch=compute_90a,code=sm_90a -shared -ccbin /usr/bin/g++ -Xcompiler -fPIC $out/*.o -o $out/libmalio_b200.so -lgomp -ldl
 grep -A2 "pass_kernel" $out/ptxas_malio_pass.log | grep -E "registers|spill" | head -8
