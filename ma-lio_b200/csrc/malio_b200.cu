@@ -146,7 +146,7 @@ int caller_leave(malio_handle* h, DeviceState* D, cudaStream_t caller) {
 namespace {
 // h->deferred of malio_knn_device: wait for its statistics, fold the fast-path counters in, report a traversal fault
 int settle_knn_device(malio_handle* h) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   h->deferred = nullptr;
   CUDA_TRY(cudaSetDevice(D->device));
   CUDA_TRY(cudaEventSynchronize(D->ev_deferred));
@@ -158,8 +158,8 @@ int settle_knn_device(malio_handle* h) {
 namespace malio_dev {
 
 int create(malio_handle* h) {
-  DeviceState* D = new DeviceState;
-  h->dev = D;
+  h->dev = malio_owner<DeviceState>(new DeviceState);   // a state left half-built by a failure below goes through destroy()
+  DeviceState* D = h->dev.get();
   D->device = h->cfg.device;
   int ndev = 0;
   CUDA_TRY(cudaGetDeviceCount(&ndev));
@@ -213,33 +213,21 @@ int create(malio_handle* h) {
 }
 
 void destroy(malio_handle* h) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (!D) return;
   cudaSetDevice(D->device);
   if (D->stream) cudaStreamSynchronize(D->stream);   // an enqueued call (malio_knn_device) may still use the buffers below
   h->deferred = nullptr;
-  malio_pre::destroy(h);
-  malio_vox::destroy(h);
-  malio_place::destroy(h);
-  malio_prior::destroy(h);
-  malio_map::destroy(h);
+  release(h->pre, D->stream);
+  release(h->voxmap, D->stream);
+  release(h->place, D->stream);
+  release(h->prior, D->stream);
+  release(h->mapst, D->stream);
   if (D->host_prof && D->host_passes)
     fprintf(stderr, "[malio] passes %llu: host launch %.1f us/pass, host wait-for-device %.1f us/pass\n",
             (unsigned long long)D->host_passes, D->host_launch_us / D->host_passes, D->host_wait_us / D->host_passes);
-  cudaSetDevice(D->device);
   comm_destroy(D);
-  for (auto& e : D->ev) if (e) cudaEventDestroy(e);
-  if (D->stream2) { cudaStreamSynchronize(D->stream2); cudaStreamDestroy(D->stream2); }
-  if (D->stream3) { cudaStreamSynchronize(D->stream3); cudaStreamDestroy(D->stream3); }
-  if (D->ev_h2d) cudaEventDestroy(D->ev_h2d);
-  if (D->ev_refit) cudaEventDestroy(D->ev_refit);
-  if (D->ev_cov) cudaEventDestroy(D->ev_cov);
-  if (D->ev_sorted) cudaEventDestroy(D->ev_sorted);
-  if (D->ev_tau) cudaEventDestroy(D->ev_tau);
-  for (cudaEvent_t e : {D->ev_caller_in, D->ev_caller_out, D->ev_deferred}) if (e) cudaEventDestroy(e);
-  if (D->stream) cudaStreamDestroy(D->stream);
-  delete D;   // the buffers go back with it
-  h->dev = nullptr;
+  release(h->dev, D->stream);
 }
 
 static int ensure_point_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
@@ -257,7 +245,7 @@ static int ensure_point_buffers(malio_handle* h, DeviceState* D, uint32_t n) {
 
 int upload_scan_from(malio_handle* h, ScanSource from, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
                      cudaMemcpyKind table_kind, const uint32_t* table_off, const malio_rigid* tcomp, cudaStream_t caller) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   const int L = h->cfg.params.n_lidar;
   for (int l = 0; l < L; ++l)
@@ -310,7 +298,7 @@ int upload_scan(malio_handle* h, const malio_scan_pt* pts, uint32_t n, const mal
 }
 
 int rearm_scan(malio_handle* h) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (!D->scan_ready) { h->err = "rearm_scan before upload_scan"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
   const uint32_t cap = (uint32_t)D->d_pts.size();
@@ -321,12 +309,12 @@ int rearm_scan(malio_handle* h) {
 }
 
 int set_timing(malio_handle* h, int enable) {
-  ((DeviceState*)h->dev)->timing = enable != 0;
+  h->dev->timing = enable != 0;
   return MALIO_OK;
 }
 
 int get_counters(malio_handle* h, malio_counters* out) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   unsigned long long c[4] = {0, 0, 0, 0};
   CUDA_TRY(cudaMemcpy(c, D->d_cand, sizeof(c), cudaMemcpyDeviceToHost));
@@ -344,7 +332,7 @@ int get_counters(malio_handle* h, malio_counters* out) {
 // arrays, ordered on `caller`
 static int scatter_aux_to(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world, bool on_device,
                           cudaStream_t caller) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (!D->pass_done) { h->err = "download_aux before measure"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
   const uint32_t N = D->N;
@@ -370,7 +358,7 @@ static int scatter_aux_to(malio_handle* h, float* normal_y, uint32_t* nn_idx, fl
 
 int download_aux(malio_handle* h, float* normal_y, uint32_t* nn_idx, float* nn_d2, uint8_t* sel, float* world) {
   if (int rc = scatter_aux_to(h, normal_y, nn_idx, nn_d2, sel, world, false, nullptr)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   const uint32_t N = D->N;
   if (N == 0) return MALIO_OK;
   if (normal_y) CUDA_TRY(cudaMemcpyAsync(normal_y, D->d_o_ny, (size_t)N * sizeof(float), cudaMemcpyDeviceToHost, D->stream));
@@ -422,7 +410,7 @@ static int knn_search(malio_handle* h, DeviceState* D, const float* q, uint32_t 
 }
 
 int knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, float* ms_out) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (h->mapst) { if (int rc = malio_map::commit(h)) return rc; }
   if (!D->map_ready) { h->err = "knn before upload_map"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
@@ -448,7 +436,7 @@ int knn(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, 
 // malio_knn on device memory, ordered on the caller's stream.  Returns after enqueueing; the statistics malio_knn waits for are
 // copied behind the search and folded in by the next call on the handle (settle_knn_device).
 int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, float* d2, cudaStream_t caller) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   if (nq) {
     if (int rc = check_device_ptr(h, D, q, "malio_knn_device queries")) return rc;
@@ -474,7 +462,7 @@ int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, floa
 // copies out when D->N > 0, or the caller's device arrays, ordered on `caller`
 static int map_incr_to(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world, bool on_device,
                        cudaStream_t caller) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (!D->pass_done) { h->err = "map_incremental before measure"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
   const uint32_t N = D->N;
@@ -500,7 +488,7 @@ static int map_incr_to(malio_handle* h, const malio_pass_state* s, double fs, in
 
 int map_incremental(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world) {
   if (int rc = map_incr_to(h, s, fs, ekf_inited, cls, world, false, nullptr)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   const uint32_t N = D->N;
   if (N == 0) return MALIO_OK;
   CUDA_TRY(cudaMemcpyAsync(cls, D->d_o_sel, (size_t)N, cudaMemcpyDeviceToHost, D->stream));

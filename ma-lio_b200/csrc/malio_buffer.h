@@ -9,6 +9,10 @@
 //   grow_keep()  grow keeping the first elements: allocate every new buffer of the group, copy device to device, drain,
 //                then free the old ones.  A failed allocation or copy leaves every buffer of the group as it was.
 // Destruction frees without a drain (the stream may be gone already): the owner drains first when work may be in flight.
+//
+// States.  The buffers belong to the handle's states (malio_handle's owners, malio_internal.h): the device state and one
+// state per feature.  A feature state is created whole on first use by acquire() and freed by release(), which drains the
+// handle's stream first; teardown that is not a buffer is the state type's destructor.
 #ifndef MALIO_BUFFER_H_
 #define MALIO_BUFFER_H_
 
@@ -142,6 +146,35 @@ class PinnedBuffer {
   T* p_ = nullptr;
   size_t n_ = 0;
 };
+
+// Frees the state in `slot`, if any, after one drain of `st` (work enqueued on its buffers may be in flight; NULL: nothing
+// was ever enqueued).  The state is freed whatever the drain returns, and the drain's error is returned.
+template <class S>
+cudaError_t release(malio_owner<S>& slot, cudaStream_t st) {
+  if (!slot) return cudaSuccess;
+  const cudaError_t e = st ? cudaStreamSynchronize(st) : cudaSuccess;
+  slot.reset();
+  return e;
+}
+
+// Selects the handle's device and hands back its device state D and the feature state in `slot`, creating it on first use:
+// s.init(h, D, args...) allocates the state's fixed buffers.  The state goes into the slot only once init has succeeded;
+// after a failure (init's status and h->err are returned) the partial state is released, so the next call starts afresh.
+template <class S, class Dev, class... Args>
+int acquire(malio_handle* h, malio_owner<S>& slot, S*& s, Dev*& D, Args&&... args) {
+  D = h->dev.get();
+  if (cudaError_t e = cudaSetDevice(D->device)) return cuda_fail(h, "cudaSetDevice(D->device)", e);
+  if (!slot) {
+    malio_owner<S> fresh(new S);
+    if (int rc = fresh->init(h, D, std::forward<Args>(args)...)) {
+      release(fresh, D->stream);
+      return rc;
+    }
+    slot = std::move(fresh);
+  }
+  s = slot.get();
+  return MALIO_OK;
+}
 
 }  // namespace malio_buf
 

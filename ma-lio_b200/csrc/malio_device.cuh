@@ -26,8 +26,10 @@
 
 namespace malio_devstate {
 
+using malio_buf::acquire;
 using malio_buf::DeviceBuffer;
 using malio_buf::PinnedBuffer;
+using malio_buf::release;
 
 #define CUDA_TRY(expr)                                                                     \
   do {                                                                                     \
@@ -239,6 +241,15 @@ struct DeviceState {
   ncclComm_t comm = nullptr; int rank = 0, world = 1;
   // d_mail: this rank's mailbox; mail_peer: every rank's, the peers' opened with cudaIpcOpenMemHandle (closed by comm_destroy)
   bool p2p = false; DeviceBuffer<unsigned char> d_mail; unsigned char* mail_peer[MAIL_MAX_WORLD] = {nullptr};
+
+  // the streams and events of a state create() made, whole or in part; the owner has drained `stream` (the buffers go back
+  // after this body)
+  ~DeviceState() {
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    for (cudaStream_t s : {stream2, stream3}) if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+    for (cudaEvent_t e : {ev_h2d, ev_refit, ev_cov, ev_sorted, ev_tau, ev_caller_in, ev_caller_out, ev_deferred}) if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
+  }
 };
 
 // ---- host functions one unit calls in another

@@ -4,6 +4,7 @@
 
 #include <cstdint>
 #include <functional>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -19,15 +20,32 @@
 #define MALIO_RED_BLOCKS 27
 #define MALIO_RED_DOUBLES (MALIO_RED_BLOCKS * 16 + 2)   // + n_eff + spare
 
+// The states of a handle, each defined by the CUDA unit named beside it
+namespace malio_devstate { struct DeviceState; }   // malio_device.cuh
+namespace malio_pre { struct PreState; }           // malio_preproc.cu
+namespace malio_map { struct MapOps; }             // malio_mapops.cu
+namespace malio_vox { struct VoxState; }           // malio_voxmap.cu
+namespace malio_prior { struct PriorState; }       // malio_prior.cu
+namespace malio_place { struct PlaceDb; }          // malio_place.cu
+
+// The owner of one state of a handle.  malio_host.cpp deletes the handle without seeing the state types, so the owner keeps
+// the deleter of the unit that created the state.  Feature states are created by malio_buf::acquire and freed by
+// malio_buf::release (malio_buffer.h).
+template <class S>
+struct malio_owner : std::unique_ptr<S, void (*)(S*)> {
+  malio_owner() : std::unique_ptr<S, void (*)(S*)>(nullptr, nullptr) {}
+  explicit malio_owner(S* s) : std::unique_ptr<S, void (*)(S*)>(s, [](S* p) { delete p; }) {}
+};
+
 struct malio_handle {
   malio_config cfg{};
   std::string err;
-  void* dev = nullptr;   // DeviceState*, owned by the CUDA TU
-  void* pre = nullptr;   // PreState*, owned by malio_preproc.cu (undistortion / voxel grid buffers)
-  void* mapst = nullptr; // MapOpsState*, owned by malio_mapops.cu (device-resident map replay)
-  void* voxmap = nullptr; // VoxState*, owned by malio_voxmap.cu (the saved map as a voxel map)
-  void* prior = nullptr;  // PriorState*, owned by malio_prior.cu (localization in a prior map)
-  void* place = nullptr;  // PlaceDb*, owned by malio_place.cu (place descriptors of the prior)
+  malio_owner<malio_devstate::DeviceState> dev;
+  malio_owner<malio_pre::PreState> pre;      // undistortion, voxel grid, world registration
+  malio_owner<malio_map::MapOps> mapst;      // the device-resident map
+  malio_owner<malio_vox::VoxState> voxmap;   // the saved map as a voxel map
+  malio_owner<malio_prior::PriorState> prior;   // localization in a prior map
+  malio_owner<malio_place::PlaceDb> place;   // place descriptors of the prior
   // counts malio_map::build_from / leave calls: a prior-map window is the device map only while no other call rebuilt or left it
   uint64_t map_epoch = 0;
   // set while a call that returned after enqueueing (malio_knn_device) still has device-side results to hand over: its
@@ -73,7 +91,6 @@ int get_unique_id(uint8_t* id);
 
 // malio_mapops.cu — the device-resident map (SURVEY.md §8f N1)
 namespace malio_map {
-void destroy(malio_handle* h);
 int commit(malio_handle* h);   // pending deltas -> compaction (when worth it) + cell-list index; no-op when clean
 void leave(malio_handle* h);   // a snapshot upload took the handle: back to snapshot mode, the map_* calls refuse until the next build
 int build(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n);
@@ -90,7 +107,6 @@ int download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_
 
 // malio_preproc.cu
 namespace malio_pre {
-void destroy(malio_handle* h);
 int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, const malio_undistort_args* a, float* xyz,
               int32_t* idx, uint8_t* ok, int32_t* pop_point, uint32_t* n_pops, double* pose);
 int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap, uint32_t* n_out);
@@ -101,14 +117,8 @@ int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uin
 int world_dense_source(malio_handle* h, const float* ud[MALIO_MAX_LIDAR], uint32_t n[MALIO_MAX_LIDAR]);
 }  // namespace malio_pre
 
-// malio_voxmap.cu — the saved map as a voxel map
-namespace malio_vox {
-void destroy(malio_handle* h);
-}  // namespace malio_vox
-
 // malio_prior.cu — localization in a prior map
 namespace malio_prior {
-void destroy(malio_handle* h);
 // the loaded prior's n points as float4 {x, y, z, normal_y} in tile order, device memory of the handle's device, valid until the
 // next load or clear (malio_reloc.cu reads them); MALIO_ERR_STATE before a load
 int points(const malio_handle* h, const float** xyzw, uint32_t* n);
@@ -118,12 +128,6 @@ int points(const malio_handle* h, const float** xyzw, uint32_t* n);
 namespace malio_reloc {
 int relocalize(malio_handle* h, const malio_pass_state* s, const malio_reloc_args* a, malio_reloc_report* rep);
 }  // namespace malio_reloc
-
-// malio_place.cu — place descriptors of the prior; destroy drains the stream and releases the database (a prior load or clear,
-// the handle's destroy)
-namespace malio_place {
-void destroy(malio_handle* h);
-}  // namespace malio_place
 
 // malio_pcd.cpp — pcl::PCDWriter::writeBinary for PointXYZINormal (host)
 namespace malio_pcd {

@@ -1422,7 +1422,7 @@ static int finish_map_upload(malio_handle* h, DeviceState* D, const malio_map_no
 }
 
 int upload_map(malio_handle* h, const malio_map_node* nodes, const float* cov, uint32_t n, uint32_t depth) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   if (depth > MALIO_MAX_TREE_DEPTH) { h->err = "snapshot deeper than MALIO_MAX_TREE_DEPTH"; return MALIO_ERR_TREE_TOO_DEEP; }
   if (D->refit_pending) { CUDA_TRY(cudaStreamSynchronize(D->stream2)); D->refit_pending = false; }
@@ -1441,7 +1441,7 @@ int upload_map(malio_handle* h, const malio_map_node* nodes, const float* cov, u
 
 int upload_map_compact(malio_handle* h, const malio_map_point* pts, const float* cov, uint32_t n, uint32_t depth,
                        const float* root_box) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   if (depth > MALIO_MAX_TREE_DEPTH) { h->err = "snapshot deeper than MALIO_MAX_TREE_DEPTH"; return MALIO_ERR_TREE_TOO_DEEP; }
   if (D->refit_pending) { CUDA_TRY(cudaStreamSynchronize(D->stream2)); D->refit_pending = false; }
@@ -1489,7 +1489,7 @@ int upload_map_compact(malio_handle* h, const malio_map_point* pts, const float*
 // ---- device-resident map (malio_mapops.cu): slot storage and the index over it
 // grow d_mpts / d_cov / d_ids to hold n slots, keeping the first `keep` of them
 int grow_slots(malio_handle* h, uint32_t n, uint32_t keep) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   if (D->slot_store && n <= D->d_ids.size()) return MALIO_OK;
   uint32_t cap = n + n / 2 + 4096;
@@ -1503,7 +1503,7 @@ int grow_slots(malio_handle* h, uint32_t n, uint32_t keep) {
 }
 // (re)build the cell-list index over the n_slots slots; box = {x_min,x_max,y_min,y_max,z_min,z_max} of the live points
 int index_from_slots(malio_handle* h, uint32_t n_slots, const float box[6]) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   if (D->refit_pending) { CUDA_TRY(cudaStreamSynchronize(D->stream2)); D->refit_pending = false; }
   D->tree_free = true;
@@ -1517,7 +1517,7 @@ int index_from_slots(malio_handle* h, uint32_t n_slots, const float box[6]) {
 }
 
 int download_map_nodes(malio_handle* h, malio_map_node* out, uint32_t cap) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (!D->map_ready || D->tree_free) { h->err = "download_map_nodes needs a snapshot uploaded with malio_upload_map*"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
   const uint32_t n = D->n_nodes < cap ? D->n_nodes : cap;

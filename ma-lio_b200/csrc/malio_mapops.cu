@@ -23,7 +23,7 @@
 
 using namespace malio_devstate;
 
-namespace {
+namespace malio_map {
 
 struct MapOps {
   uint32_t n_slots = 0, n_live = 0;
@@ -40,20 +40,25 @@ struct MapOps {
   // without waiting for the device — the caller's arrays are consumed, the bounce buffer is protected by ev_bounce
   PinnedBuffer<float> h_bounce[2]; cudaEvent_t ev_bounce[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false}; int bounce_next = 0;
   PinnedBuffer<float> h_bounce_box; cudaEvent_t ev_bounce_box = nullptr; bool bounce_box_busy = false;   // same for the voxel boxes
+
+  int init(malio_handle* h, DeviceState* D) {
+    if (int rc = d_small.allocate(h, D->stream, 8)) return rc;
+    return h_small.allocate(h, 8);
+  }
+  ~MapOps() {
+    for (cudaEvent_t e : ev_bounce) if (e) cudaEventDestroy(e);
+    if (ev_bounce_box) cudaEventDestroy(ev_bounce_box);
+  }
 };
+
+}  // namespace malio_map
+
+namespace {
+
+using malio_map::MapOps;
+
 constexpr uint32_t BOUNCE_POINTS = 65536;      // 5 floats per point: 1.3 MB of pinned memory
 constexpr uint32_t BOUNCE_BOXES = 16384;       // 6 floats per box
-
-int state(malio_handle* h, MapOps*& M) {
-  M = (MapOps*)h->mapst;
-  if (M) return MALIO_OK;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
-  M = new MapOps;
-  h->mapst = M;
-  if (int rc = M->d_small.allocate(h, D->stream, 8)) return rc;
-  return M->h_small.allocate(h, 8);
-}
 
 __device__ __forceinline__ uint32_t fkey(float f) {
   const uint32_t b = __float_as_uint(f);
@@ -316,18 +321,9 @@ int append(malio_handle* h, DeviceState* D, MapOps* M, const float* xyz, const f
 
 namespace malio_map {
 
-void destroy(malio_handle* h) {
-  MapOps* M = (MapOps*)h->mapst;
-  if (!M) return;
-  for (cudaEvent_t e : M->ev_bounce) if (e) cudaEventDestroy(e);
-  if (M->ev_bounce_box) cudaEventDestroy(M->ev_bounce_box);
-  delete M;
-  h->mapst = nullptr;
-}
-
 void leave(malio_handle* h) {
   ++h->map_epoch;
-  MapOps* M = (MapOps*)h->mapst;
+  MapOps* M = h->mapst.get();
   if (!M) return;
   M->active = false;
   M->n_slots = 0; M->n_live = 0;
@@ -335,9 +331,9 @@ void leave(malio_handle* h) {
 }
 
 int commit(malio_handle* h) {
-  MapOps* M = (MapOps*)h->mapst;
+  MapOps* M = h->mapst.get();
   if (!M || !M->active) return MALIO_OK;
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (!M->dirty && D->tree_free) return MALIO_OK;
   CUDA_TRY(cudaSetDevice(D->device));
   cudaStream_t st = D->stream;
@@ -387,10 +383,9 @@ int commit(malio_handle* h) {
 static int build_from(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, bool on_device,
                       cudaStream_t caller) {
   MapOps* M;
-  if (int rc = state(h, M)) return rc;
+  DeviceState* D;
+  if (int rc = acquire(h, h->mapst, M, D)) return rc;
   ++h->map_epoch;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
   if (D->refit_pending) { CUDA_TRY(cudaStreamSynchronize(D->stream2)); D->refit_pending = false; }
   M->n_slots = 0; M->n_live = 0;
   M->active = true;
@@ -403,9 +398,9 @@ static int build_from(malio_handle* h, const float* xyz, const float* normal_y, 
 
 static int add_points_from(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n, bool on_device,
                            cudaStream_t caller) {
-  MapOps* M = (MapOps*)h->mapst;
+  MapOps* M = h->mapst.get();
   if (!M || !M->active) { h->err = "malio_map_add_points before malio_map_build"; return MALIO_ERR_STATE; }
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   return append(h, D, M, xyz, normal_y, ids, n, on_device, caller);
 }
@@ -418,7 +413,7 @@ int add_points(malio_handle* h, const float* xyz, const float* normal_y, const i
 
 // the device-memory variants: every argument the host can check is checked before anything is launched
 static int check_device_points(malio_handle* h, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t n) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   if (n == 0) return MALIO_OK;
   if (int rc = check_device_ptr(h, D, xyz, "xyz")) return rc;
@@ -435,9 +430,9 @@ int add_points_device(malio_handle* h, const float* xyz, const float* normal_y, 
 }
 
 int delete_boxes(malio_handle* h, const float* boxes, uint32_t nb, uint32_t* n_deleted) {
-  MapOps* M = (MapOps*)h->mapst;
+  MapOps* M = h->mapst.get();
   if (!M || !M->active) { h->err = "malio_map_delete_boxes before malio_map_build"; return MALIO_ERR_STATE; }
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   uint32_t total = 0;
   for (uint32_t at = 0; at < nb; at += MAX_BIG_BOXES) {
@@ -458,9 +453,9 @@ int delete_boxes(malio_handle* h, const float* boxes, uint32_t nb, uint32_t* n_d
 
 int sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t m,
                 uint32_t* n_deleted) {
-  MapOps* M = (MapOps*)h->mapst;
+  MapOps* M = h->mapst.get();
   if (!M || !M->active) { h->err = "malio_map_sync_voxels before malio_map_build"; return MALIO_ERR_STATE; }
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   if (M->appended || !D->tree_free) { if (int rc = commit(h)) return rc; }   // the kill below reads the index: it must know every live slot
   uint32_t killed = 0;
@@ -500,7 +495,7 @@ int sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* x
 }
 
 int info(malio_handle* h, uint32_t* n_live, uint32_t* n_slots) {
-  MapOps* M = (MapOps*)h->mapst;
+  MapOps* M = h->mapst.get();
   if (!M || !M->active) { h->err = "malio_map_info before malio_map_build"; return MALIO_ERR_STATE; }
   if (int rc = commit(h)) return rc;
   if (n_live) *n_live = M->n_live;
@@ -509,10 +504,10 @@ int info(malio_handle* h, uint32_t* n_live, uint32_t* n_slots) {
 }
 
 int download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_t* slots, uint32_t cap, uint32_t* n_out) {
-  MapOps* M = (MapOps*)h->mapst;
+  MapOps* M = h->mapst.get();
   if (!M || !M->active) { h->err = "malio_map_download before malio_map_build"; return MALIO_ERR_STATE; }
   if (int rc = commit(h)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   const uint32_t n = M->n_slots, live = M->n_live;
   if (n_out) *n_out = live;

@@ -1397,7 +1397,7 @@ namespace malio_dev {
 
 int measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* HtRinvH, double* HtRinvh,
             malio_pass_stats* st) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (h->mapst) { if (int rc = malio_map::commit(h)) return rc; }   // device-resident map: pending deltas -> index
   if (!D->map_ready || !D->scan_ready) { h->err = "measure before upload_map/upload_scan"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
@@ -1424,7 +1424,7 @@ int measure(malio_handle* h, const malio_pass_state* s, int redo_knn, double* Ht
 }
 
 int download_rows(malio_handle* h, double* h_x, double* hvec, uint32_t cap, uint32_t* n_rows) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   if (!D->pass_done) { h->err = "download_rows before measure"; return MALIO_ERR_STATE; }
   CUDA_TRY(cudaSetDevice(D->device));
   const malio_params& P = h->cfg.params;
@@ -1478,7 +1478,7 @@ int get_unique_id(uint8_t* id) {
 }
 
 int comm_init(malio_handle* h, const uint8_t* id, int rank, int world) {
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   if (!g_nccl.load(h->err)) return MALIO_ERR_NCCL;
   ncclUniqueId uid;

@@ -272,6 +272,10 @@ __global__ void __launch_bounds__(ST2_T) pl_stage2_kernel(const unsigned long lo
   }
 }
 
+}  // namespace
+
+namespace malio_place {
+
 // ---------------------------------------------------------------------------------------------------- host
 struct PlaceDb {
   malio_place_args args{};
@@ -283,7 +287,15 @@ struct PlaceDb {
   DeviceBuffer<uint8_t> d_nib;
   DeviceBuffer<uint16_t> d_rk;
   size_t bytes() const { return d_st.bytes() + d_cols.bytes() + d_zs.bytes() + d_nib.bytes() + d_rk.bytes(); }
+  // the database of the loaded prior (n_prior points), built whole
+  int init(malio_handle* h, DeviceState* D, const malio_place_args* a, const float4* prior, uint32_t n_prior, malio_place_db_report* rep);
 };
+
+}  // namespace malio_place
+
+namespace {
+
+using malio_place::PlaceDb;
 
 int64_t floor_div(int64_t a, int64_t b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 
@@ -529,46 +541,36 @@ void q_rot_host(const double q[4], const double v[3], double o[3]) {
 
 namespace malio_place {
 
-void destroy(malio_handle* h) {
-  PlaceDb* P = (PlaceDb*)h->place;
-  if (!P) return;
-  DeviceState* D = (DeviceState*)h->dev;
-  if (D) { cudaSetDevice(D->device); cudaStreamSynchronize(D->stream); }
-  delete P;
-  h->place = nullptr;
+int PlaceDb::init(malio_handle* h, DeviceState* D, const malio_place_args* a, const float4* prior, uint32_t n_prior,
+                  malio_place_db_report* rep) {
+  BuildScratch S;
+  const int rc = build(h, D, a, prior, n_prior, *this, S, rep);
+  CUDA_TRY(cudaStreamSynchronize(D->stream));   // before the scratch goes back
+  return rc;
 }
 
 int db_build(malio_handle* h, const malio_place_args* a, malio_place_db_report* rep) {
-  destroy(h);
+  release(h->place, h->dev->stream);
   if (int rc = check_args(h, a)) return rc;
   const float* prior = nullptr;
   uint32_t n_prior = 0;
   if (malio_prior::points(h, &prior, &n_prior) != MALIO_OK) { h->err = "malio_place_db_build before malio_prior_map_load"; return MALIO_ERR_STATE; }
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
-  PlaceDb* P = new PlaceDb;
-  int rc;
-  {
-    BuildScratch S;
-    rc = build(h, D, a, reinterpret_cast<const float4*>(prior), n_prior, *P, S, rep);
-    CUDA_TRY(cudaStreamSynchronize(D->stream));   // before the scratch goes back
-  }
-  if (rc) { delete P; return rc; }
-  h->place = P;
-  return MALIO_OK;
+  PlaceDb* P;
+  DeviceState* D;
+  return acquire(h, h->place, P, D, a, reinterpret_cast<const float4*>(prior), n_prior, rep);
 }
 
 int db_info(malio_handle* h, uint64_t* n_positions, uint64_t* device_bytes) {
-  const PlaceDb* P = (const PlaceDb*)h->place;
+  const PlaceDb* P = h->place.get();
   if (n_positions) *n_positions = P ? P->n : 0;
   if (device_bytes) *device_bytes = P ? P->bytes() : 0;
   return MALIO_OK;
 }
 
 int db_download(malio_handle* h, int32_t* cols, double* z_s, uint8_t* nib, uint16_t* rk, uint64_t cap, uint64_t* n) {
-  const PlaceDb* P = (const PlaceDb*)h->place;
+  const PlaceDb* P = h->place.get();
   if (!P) { h->err = "malio_place_db_download before malio_place_db_build"; return MALIO_ERR_STATE; }
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   *n = P->n;
   const uint64_t m = cap < P->n ? cap : P->n;
@@ -591,11 +593,11 @@ int relocalize_global(malio_handle* h, const malio_pass_state* s, const malio_gl
              "s.rot finite";
     return MALIO_ERR_INVALID_ARG;
   }
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   const float* prior = nullptr;
   uint32_t n_prior = 0;
   if (malio_prior::points(h, &prior, &n_prior) != MALIO_OK) { h->err = "malio_relocalize_global before malio_prior_map_load"; return MALIO_ERR_STATE; }
-  const PlaceDb* P = (const PlaceDb*)h->place;
+  const PlaceDb* P = h->place.get();
   if (!P) { h->err = "malio_relocalize_global before malio_place_db_build"; return MALIO_ERR_STATE; }
   if (!D->scan_ready) { h->err = "malio_relocalize_global before a scan upload"; return MALIO_ERR_STATE; }
   if (D->comm) { h->err = "malio_relocalize_global: a communicator is attached (each rank holds only its block of the scan)"; return MALIO_ERR_STATE; }

@@ -28,7 +28,7 @@
 
 using namespace malio_devstate;
 
-namespace {
+namespace malio_pre {
 
 struct PreLidar {
   uint32_t n = 0;                     // raw / undistorted points; the buffers below hold d_raw's size of them
@@ -74,27 +74,27 @@ struct PreState {
   DeviceBuffer<float4> d_wstage;      // malio_world_register's result before its one D2H copy
   DeviceBuffer<float4> d_acc; uint64_t n_acc = 0;   // pcl_wait_save (laserMapping.cpp:475), device-resident
   PinnedBuffer<float4> h_bounce;      // pinned, malio_pcd::CHUNK points: malio_world_save_pcd's D2H staging
+
+  int init(malio_handle* h, DeviceState* D) {
+    stream = D->stream;   // same stream as the scan path: malio_upload_scan_device is ordered after the voxel grid
+    if (int rc = d_ct.allocate(h, stream, MALIO_MAX_CTRL)) return rc;
+    if (int rc = d_cT.allocate(h, stream, (size_t)MALIO_MAX_CTRL * 16)) return rc;
+    if (int rc = d_seglog.allocate(h, stream, (size_t)MALIO_MAX_CTRL * 6)) return rc;
+    if (int rc = d_covt.allocate(h, stream, MALIO_MAX_COV)) return rc;
+    if (int rc = d_bounds.allocate(h, stream, 8)) return rc;
+    if (int rc = d_order_bad.allocate(h, stream, 1)) return rc;
+    if (int rc = d_ctot.allocate(h, stream, 2 * 65536)) return rc;
+    if (int rc = d_cbase.allocate(h, stream, 2 * 65536)) return rc;
+    return h_small.allocate(h, 8);
+  }
 };
 
-int get_state(malio_handle* h, PreState*& S) {
-  S = (PreState*)h->pre;
-  if (S) return MALIO_OK;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
-  S = new PreState;
-  h->pre = S;
-  S->stream = D->stream;   // same stream as the scan path: malio_upload_scan_device is ordered after the voxel grid
-  const cudaStream_t st = S->stream;
-  if (int rc = S->d_ct.allocate(h, st, MALIO_MAX_CTRL)) return rc;
-  if (int rc = S->d_cT.allocate(h, st, (size_t)MALIO_MAX_CTRL * 16)) return rc;
-  if (int rc = S->d_seglog.allocate(h, st, (size_t)MALIO_MAX_CTRL * 6)) return rc;
-  if (int rc = S->d_covt.allocate(h, st, MALIO_MAX_COV)) return rc;
-  if (int rc = S->d_bounds.allocate(h, st, 8)) return rc;
-  if (int rc = S->d_order_bad.allocate(h, st, 1)) return rc;
-  if (int rc = S->d_ctot.allocate(h, st, 2 * 65536)) return rc;
-  if (int rc = S->d_cbase.allocate(h, st, 2 * 65536)) return rc;
-  return S->h_small.allocate(h, 8);
-}
+}  // namespace malio_pre
+
+namespace {
+
+using malio_pre::PreLidar;
+using malio_pre::PreState;
 
 // ------------------------------------------------------------------ quat_ops.h restated for the device
 __host__ __device__ inline void mul3(const double* A, const double* B, double* C) {
@@ -738,17 +738,11 @@ int undistort_launch(malio_handle* h, PreState* S, DeviceState* D, PreLidar& L, 
 
 namespace malio_pre {
 
-void destroy(malio_handle* h) {
-  delete (PreState*)h->pre;
-  h->pre = nullptr;
-}
-
 int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, const malio_undistort_args* a, float* xyz,
               int32_t* idx, uint8_t* ok, int32_t* pop_point, uint32_t* n_pops, double* pose) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   if (int rc = undistort_check_args(h, lidar, a)) return rc;
   PreLidar& L = S->lid[lidar];
   cudaStream_t st = S->stream;
@@ -784,9 +778,8 @@ int undistort(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, c
 int undistort_device(malio_handle* h, int lidar, const malio_raw_pt* pts, uint32_t n, const malio_undistort_args* a, float* cloud,
                      int32_t* idx, uint8_t* ok, int32_t* pop_point, double* pose, uint32_t* n_pops, cudaStream_t caller) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   if (int rc = undistort_check_args(h, lidar, a)) return rc;
   if (n) {
     if (int rc = check_device_ptr(h, D, pts, "malio_undistort_device pts")) return rc;
@@ -904,9 +897,8 @@ static int voxel_slot_input(malio_handle* h, const PreLidar& L, const float*& d_
 
 int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap, uint32_t* n_out) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   if (lidar < 0 || lidar >= MALIO_MAX_LIDAR || !(leaf > 0.f)) { h->err = "voxel_grid: bad lidar slot or leaf size"; return MALIO_ERR_INVALID_ARG; }
   PreLidar& L = S->lid[lidar];
   cudaStream_t st = S->stream;
@@ -934,9 +926,8 @@ int voxel_grid(malio_handle* h, int lidar, const float* in, uint32_t n, float le
 int voxel_grid_device(malio_handle* h, int lidar, const float* in, uint32_t n, float leaf, float* out, uint32_t out_cap, uint32_t* n_out,
                       cudaStream_t caller) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   if (lidar < 0 || lidar >= MALIO_MAX_LIDAR || !(leaf > 0.f)) { h->err = "voxel_grid: bad lidar slot or leaf size"; return MALIO_ERR_INVALID_ARG; }
   PreLidar& L = S->lid[lidar];
   const float* d_in = in;
@@ -983,18 +974,16 @@ static int merge_scan(malio_handle* h, PreState* S, DeviceState* D, const malio_
 int upload_scan_device(malio_handle* h, const malio_pose_entry* table, const uint32_t* table_off, const malio_rigid* tcomp,
                        uint32_t* n_total) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   return merge_scan(h, S, D, table, false, table_off, tcomp, n_total);
 }
 
 // malio_upload_scan_device with the table, its offsets and the temporal compensations of the last malio_scan_uncertainty*
 int upload_scan_resident(malio_handle* h, uint32_t* n_total) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   if (!S->table_resident) {
     h->err = "upload_scan_resident: no pose table on the device (run malio_scan_uncertainty* after the last malio_undistort* of the scan)";
     return MALIO_ERR_STATE;
@@ -1010,9 +999,8 @@ static int world_register_to(malio_handle* h, const malio_pass_state* s, int sou
                              uint32_t* n_out, bool on_device, cudaStream_t caller, uint64_t* k_out) {
   *k_out = 0;
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   uint64_t n = 0;
   if (int rc = world_count(h, S, D, source, n)) return rc;
   if (n > 0xFFFFFFFFull) { h->err = "world registration: more than 2^32-1 points"; return MALIO_ERR_CAPACITY; }
@@ -1043,8 +1031,8 @@ int world_register(malio_handle* h, const malio_pass_state* s, int source, const
   uint64_t k = 0;
   if (int rc = world_register_to(h, s, source, slot_tag, out, cap, n_out, false, nullptr, &k)) return rc;
   if (k == 0) return MALIO_OK;
-  PreState* S = (PreState*)h->pre;
-  DeviceState* D = (DeviceState*)h->dev;
+  PreState* S = h->pre.get();
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaMemcpyAsync(out, S->d_wstage, (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, S->stream));
   CUDA_TRY(cudaStreamSynchronize(S->stream));
   D->ctr.d2h_bytes += k * sizeof(float4);
@@ -1053,9 +1041,8 @@ int world_register(malio_handle* h, const malio_pass_state* s, int source, const
 
 int world_accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, uint64_t* n_total) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   uint64_t n = 0;
   if (int rc = world_count(h, S, D, MALIO_WORLD_DENSE, n)) return rc;
   const uint64_t need = S->n_acc + n;
@@ -1083,8 +1070,8 @@ int world_accumulate(malio_handle* h, const malio_pass_state* s, const float* sl
 // their sizes, with world_count's state error
 int world_dense_source(malio_handle* h, const float* ud[MALIO_MAX_LIDAR], uint32_t n[MALIO_MAX_LIDAR]) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   uint64_t total = 0;
   if (int rc = world_count(h, S, D, MALIO_WORLD_DENSE, total)) return rc;
   for (int l = 0; l < h->cfg.params.n_lidar; ++l) { ud[l] = S->lid[l].d_ud; n[l] = S->lid[l].n; }
@@ -1093,9 +1080,8 @@ int world_dense_source(malio_handle* h, const float* ud[MALIO_MAX_LIDAR], uint32
 
 int world_save_pcd(malio_handle* h, const char* path, int clear) {
   PreState* S;
-  if (int rc = get_state(h, S)) return rc;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->pre, S, D)) return rc;
   if (S->n_acc == 0) { h->err = "world save: the accumulated cloud is empty (nothing is written)"; return MALIO_ERR_STATE; }
   if (!S->h_bounce) { if (int rc = S->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
   const int rc = malio_pcd::write_binary(path, S->n_acc, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
@@ -1116,7 +1102,7 @@ int world_save_pcd(malio_handle* h, const char* path, int clear) {
 // and table_off, temporal_comp may be NULL
 int scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_entry* table, uint32_t table_cap, uint32_t* table_off,
                      malio_pose* temporal_comp, malio_pose* lidar_unc, uint32_t* lidar_unc_counts) {
-  PreState* S = (PreState*)h->pre;
+  PreState* S = h->pre.get();
   uint32_t off_local[MALIO_MAX_LIDAR + 1];
   if (!table_off) table_off = off_local;
   const int Ln = h->cfg.params.n_lidar;
@@ -1151,7 +1137,7 @@ int scan_uncertainty(malio_handle* h, const malio_scan_unc_args* a, malio_pose_e
     const double* cov = l == 0 ? a->uncertainty : a->imu_cov + 36 * (size_t)P.cov_pointer;   // :450 / :471
     malio_compound::pose_initial(&c.ltl[l], P.lt_imu_frame.t, P.lt_imu_frame.q, cov);
   }
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   cudaStream_t st = S->stream;
   const size_t tab_bytes = (size_t)n_tab * sizeof(malio_pose_entry);

@@ -45,6 +45,10 @@ constexpr int TILE_BIAS = 1 << (TILE_BITS - 1);             // tile index range 
 constexpr uint32_t FLAG_NONFINITE = 1u, FLAG_RANGE = 2u;
 constexpr int CP_T = 1024;                                  // candidates per compaction block
 
+}  // namespace
+
+namespace malio_prior {
+
 struct PriorState {
   bool loaded = false;
   uint32_t n = 0, n_tiles = 0;
@@ -65,18 +69,18 @@ struct PriorState {
   DeviceBuffer<char> d_temp;                                // CUB's temporary storage of the window's scans
   DeviceBuffer<uint32_t> d_small;                           // [0] flags, [1..6] biased tile min/max, [7] tile count
   PinnedBuffer<uint32_t> h_small;
+
+  int init(malio_handle* h, DeviceState* D) {
+    if (int rc = d_small.allocate(h, D->stream, 8)) return rc;
+    return h_small.allocate(h, 8);
+  }
 };
 
-int get_state(malio_handle* h, PriorState*& P) {
-  P = (PriorState*)h->prior;
-  if (P) return MALIO_OK;
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
-  P = new PriorState;
-  h->prior = P;
-  if (int rc = P->d_small.allocate(h, D->stream, 8)) return rc;
-  return P->h_small.allocate(h, 8);
-}
+}  // namespace malio_prior
+
+namespace {
+
+using malio_prior::PriorState;
 
 __host__ __device__ __forceinline__ unsigned long long tile_key(int tx, int ty, int tz) {
   return ((unsigned long long)(uint32_t)(tz + TILE_BIAS) << (2 * TILE_BITS)) |
@@ -355,17 +359,11 @@ int feed(malio_handle* h, PriorState* P, DeviceState* D, uint32_t m, bool build)
 
 namespace malio_prior {
 
-void destroy(malio_handle* h) {
-  delete (PriorState*)h->prior;
-  h->prior = nullptr;
-}
-
 int load(malio_handle* h, const float* xyz, const float* ny, const int32_t* ids, uint32_t n, bool on_device, cudaStream_t caller) {
   PriorState* P;
-  if (int rc = get_state(h, P)) return rc;
-  malio_place::destroy(h);   // the place database describes the prior this load replaces
-  DeviceState* D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
+  DeviceState* D;
+  if (int rc = acquire(h, h->prior, P, D)) return rc;
+  release(h->place, D->stream);   // the place database describes the prior this load replaces
   if (n == 0) return load_empty(h, P, D);
   if (on_device) {
     if (int rc = check_device_ptr(h, D, xyz, "xyz")) return rc;
@@ -390,7 +388,7 @@ int load(malio_handle* h, const float* xyz, const float* ny, const int32_t* ids,
 }
 
 int window(malio_handle* h, const double pos[3], double cube_len, float det_range, malio_window_report* rep) {
-  PriorState* P = (PriorState*)h->prior;
+  PriorState* P = h->prior.get();
   if (!P || !P->loaded) { h->err = "malio_prior_map_window before malio_prior_map_load"; return MALIO_ERR_STATE; }
   for (int a = 0; a < 3; ++a)
     if (!std::isfinite(pos[a])) { h->err = "malio_prior_map_window: non-finite position"; return MALIO_ERR_INVALID_ARG; }
@@ -398,7 +396,7 @@ int window(malio_handle* h, const double pos[3], double cube_len, float det_rang
     h->err = "malio_prior_map_window: cube_len must be finite and > 0, det_range finite and >= 0";
     return MALIO_ERR_INVALID_ARG;
   }
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
   std::memset(rep, 0, sizeof(*rep));
   const bool first = !P->win || P->win_epoch != h->map_epoch;
@@ -469,7 +467,7 @@ int window(malio_handle* h, const double pos[3], double cube_len, float det_rang
 }
 
 int points(const malio_handle* h, const float** xyzw, uint32_t* n) {
-  const PriorState* P = (const PriorState*)h->prior;
+  const PriorState* P = h->prior.get();
   if (!P || !P->loaded) return MALIO_ERR_STATE;
   *xyzw = reinterpret_cast<const float*>(P->d_pts.data());
   *n = P->n;
@@ -478,7 +476,8 @@ int points(const malio_handle* h, const float** xyzw, uint32_t* n) {
 
 int info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* device_bytes) {
   PriorState* P;
-  if (int rc = get_state(h, P)) return rc;
+  DeviceState* D;
+  if (int rc = acquire(h, h->prior, P, D)) return rc;
   if (n_points) *n_points = P->n;
   if (n_tiles) *n_tiles = P->n_tiles;
   if (device_bytes)
@@ -488,14 +487,12 @@ int info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* devic
 }
 
 int clear(malio_handle* h) {
-  malio_place::destroy(h);
-  PriorState* P = (PriorState*)h->prior;
-  if (!P) return MALIO_OK;
-  DeviceState* D = (DeviceState*)h->dev;
+  if (!h->prior) return MALIO_OK;   // (nor a place database: one is built from a loaded prior)
+  DeviceState* D = h->dev.get();
   CUDA_TRY(cudaSetDevice(D->device));
-  CUDA_TRY(cudaStreamSynchronize(D->stream));   // an enqueued append may still read the scratch
-  delete P;
-  h->prior = nullptr;
+  release(h->place, D->stream);
+  // an enqueued append may still read the scratch
+  if (cudaError_t e = release(h->prior, D->stream)) return malio_buf::cuda_fail(h, "cudaStreamSynchronize(D->stream)", e);
   return MALIO_OK;
 }
 

@@ -412,7 +412,7 @@ int relocalize(malio_handle* h, const malio_pass_state* s, const malio_reloc_arg
     h->err = "malio_relocalize: n_yaw must be > 0, res finite and > 0, yaw_lo / yaw_step / s.pos / s.rot finite";
     return MALIO_ERR_INVALID_ARG;
   }
-  DeviceState* D = (DeviceState*)h->dev;
+  DeviceState* D = h->dev.get();
   const float* prior = nullptr;
   uint32_t n_prior = 0;
   if (malio_prior::points(h, &prior, &n_prior) != MALIO_OK) { h->err = "malio_relocalize before malio_prior_map_load"; return MALIO_ERR_STATE; }

@@ -53,6 +53,10 @@ constexpr uint32_t RUN_NONE = 0xFFFFFFFFu;   // the run of the skipped points
 constexpr uint32_t RUN_NEW = 0xFFFFFFFEu;    // run whose voxel the map does not hold yet
 constexpr uint64_t VOX_MIN_ENTRIES = 1u << 16;
 
+}  // namespace
+
+namespace malio_vox {
+
 struct VoxState {
   bool leaf_set = false;
   float leaf = 0.f;
@@ -76,7 +80,19 @@ struct VoxState {
   // the seeded voxels are the entries [0, n_seeded): entries are numbered in creation order and never renumbered (growth and
   // rehash keep them), and a seed only runs on an empty map.  0 for a map that was never seeded or since a clearing save.
   uint64_t n_seeded = 0;
+
+  int init(malio_handle* h, DeviceState* D) {
+    if (int rc = d_small.allocate(h, D->stream, 6)) return rc;
+    CUDA_TRY(cudaMemsetAsync(d_small, 0, 6 * sizeof(uint32_t), D->stream));
+    return h_small.allocate(h, 6);
+  }
 };
+
+}  // namespace malio_vox
+
+namespace {
+
+using malio_vox::VoxState;
 
 // The sort area holds sort_rows(V) rows as eight columns of 4 B a row; column c starts at byte 4 * c * rows.  While points or
 // entries are sorted, the columns are CUB's double buffers: keys in 0-2, alternate keys in 3-5 (12 B a row), values in 6,
@@ -410,19 +426,6 @@ __global__ void __launch_bounds__(256) vs_change_kernel(const uint32_t* __restri
   added[r] = (!seeded && kept) ? 1u : 0u;
 }
 
-// the handle's voxel map, created empty on first use; the handle's device is selected
-int get_state(malio_handle* h, VoxState*& V, DeviceState*& D) {
-  D = (DeviceState*)h->dev;
-  CUDA_TRY(cudaSetDevice(D->device));
-  V = (VoxState*)h->voxmap;
-  if (V) return MALIO_OK;
-  V = new VoxState;
-  h->voxmap = V;
-  if (int rc = V->d_small.allocate(h, D->stream, 6)) return rc;
-  CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 6 * sizeof(uint32_t), D->stream));
-  return V->h_small.allocate(h, 6);
-}
-
 // CUB's temporary storage for at least t bytes, and the sort area for n rows
 int grow_temp(malio_handle* h, VoxState* V, DeviceState* D, size_t t) {
   if (t <= V->d_temp.size()) return MALIO_OK;
@@ -683,17 +686,12 @@ int check_leaf(malio_handle* h, const VoxState* V, float leaf) {
 
 namespace malio_vox {
 
-void destroy(malio_handle* h) {
-  delete (VoxState*)h->voxmap;
-  h->voxmap = nullptr;
-}
-
 // carve == NULL: malio_world_voxel_accumulate; otherwise the same fold, then the scan's hits and passes (checked first)
 int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag, float leaf, const malio_carve_args* carve,
                uint64_t* n_voxels) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   if (carve && !(std::isfinite(carve->max_range) && carve->max_range > 0.f && std::isfinite(carve->end_margin) && carve->end_margin >= 0.f)) {
     h->err = "world voxel carve: max_range must be finite and > 0, end_margin finite and >= 0";
     return MALIO_ERR_INVALID_ARG;
@@ -750,7 +748,7 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
 int download_device(malio_handle* h, float* out, uint64_t cap, uint64_t* n_out, cudaStream_t caller) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   const uint64_t n = V->n_vox, k = n < cap ? n : cap;
   if (out && k) {
     if (int rc = check_rows(h, D, out, "malio_world_voxel_download_device out", 16, CENTROID_ROWS)) return rc;
@@ -767,7 +765,7 @@ int download_device(malio_handle* h, float* out, uint64_t cap, uint64_t* n_out, 
 int evidence_device(malio_handle* h, uint32_t* out, uint64_t cap, uint64_t* n_out, cudaStream_t caller) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   const uint64_t n = V->n_vox, k = n < cap ? n : cap;
   if (out && k) {
     if (int rc = check_rows(h, D, out, "malio_world_voxel_evidence_device out", 8, "the pairs are stored as uint2")) return rc;
@@ -788,7 +786,7 @@ int evidence_device(malio_handle* h, uint32_t* out, uint64_t cap, uint64_t* n_ou
 int download_kept_device(malio_handle* h, const malio_carve_keep* keep, float* out, uint64_t cap, uint64_t* n_out, cudaStream_t caller) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   if (int rc = check_keep(h, keep)) return rc;
   if (out && cap && V->n_vox) {
     if (int rc = check_rows(h, D, out, "malio_world_voxel_download_kept_device out", 16, CENTROID_ROWS)) return rc;
@@ -810,7 +808,7 @@ int download_kept_device(malio_handle* h, const malio_carve_keep* keep, float* o
 int save_pcd(malio_handle* h, const char* path, const malio_carve_keep* keep, int clear) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   if (keep) { if (int rc = check_keep(h, keep)) return rc; }
   if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
   uint64_t n = V->n_vox;
@@ -844,7 +842,7 @@ int seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t se
          uint64_t* n_voxels) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   if (!(leaf > 0.f) || !std::isfinite(leaf)) { h->err = "world voxel seed: leaf must be a finite size > 0"; return MALIO_ERR_INVALID_ARG; }
   if (V->n_vox || V->leaf_set) {
     h->err = "world voxel seed: the voxel map is not empty (seed a new map or one after a clearing save)";
@@ -919,7 +917,7 @@ int changes_device(malio_handle* h, const malio_carve_keep* keep, float* d_remov
                    float* d_added, uint64_t cap_added, uint64_t* n_added, cudaStream_t caller) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   if (int rc = check_keep(h, keep)) return rc;
   if (V->n_vox) {
     if (d_removed && cap_removed) {
@@ -953,7 +951,7 @@ int save_changes_pcd(malio_handle* h, const malio_carve_keep* keep, const char* 
                      uint64_t* n_added) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   if (int rc = check_keep(h, keep)) return rc;
   if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
   if (int rc = grow_sort(h, V, D, V->n_vox)) return rc;
@@ -977,7 +975,7 @@ int save_changes_pcd(malio_handle* h, const malio_carve_keep* keep, const char* 
 int info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* device_bytes) {
   VoxState* V;
   DeviceState* D;
-  if (int rc = get_state(h, V, D)) return rc;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   if (n_voxels) *n_voxels = V->n_vox;
   if (capacity) *capacity = V->d_ekey.size();
   if (device_bytes)

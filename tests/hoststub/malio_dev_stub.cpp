@@ -40,7 +40,6 @@ int get_unique_id(uint8_t*) { return MALIO_ERR_NCCL; }
 }  // namespace malio_dev
 
 namespace malio_map {
-void destroy(malio_handle*) {}
 int commit(malio_handle*) { return MALIO_OK; }
 int build(malio_handle*, const float*, const float*, const int32_t*, uint32_t) { return MALIO_ERR_STATE; }
 int add_points(malio_handle*, const float*, const float*, const int32_t*, uint32_t) { return MALIO_ERR_STATE; }
@@ -51,7 +50,6 @@ int download(malio_handle*, float*, float*, int32_t*, uint32_t*, uint32_t, uint3
 }  // namespace malio_map
 
 namespace malio_pre {
-void destroy(malio_handle*) {}
 int undistort(malio_handle*, int, const malio_raw_pt*, uint32_t, const malio_undistort_args*, float*, int32_t*, uint8_t*, int32_t*, uint32_t*, double*) { return MALIO_ERR_STATE; }
 int voxel_grid(malio_handle*, int, const float*, uint32_t, float, float*, uint32_t, uint32_t*) { return MALIO_ERR_STATE; }
 int upload_scan_device(malio_handle*, const malio_pose_entry*, const uint32_t*, const malio_rigid*, uint32_t*) { return MALIO_ERR_STATE; }
