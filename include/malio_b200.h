@@ -631,6 +631,50 @@ int malio_prior_map_window(malio_handle* h, const double pos_lid[3], double cube
 int malio_prior_map_info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* device_bytes);
 int malio_prior_map_clear(malio_handle* h);
 
+/* ---- localization past the prior's edge: the session layer ------------------------------------------------------------------
+ * Where the prior has no data a localizing drive would find no planes and lose track.  malio_prior_map_extend takes the place of
+ * map_incremental (laserMapping.cpp:398-446) in localization: run it after the IESKF update of a scan, with the state after the
+ * update and before any other map call, and it adds the scan's points where the window holds nothing.  What it adds is the
+ * session: an append-only store on the device, owned by the prior, that survives window slides.
+ *   1. Decision: the classes and world points of malio_map_incremental(s, filter_size_map, ekf_inited = 1), on the device.
+ *   2. Admission: each candidate (MALIO_MAP_ADD or MALIO_MAP_ADD_NO_DOWNSAMPLE) has Add_Points(.., true)'s voxel box
+ *      (ikd_Tree.cpp:491-497): per axis lo = floor(x / ds) * ds, hi = lo + ds in float, ds = (float)filter_size_map, half-open.
+ *      It is admitted when that box holds no live point of the window at the call's start (prior, session or caller-added
+ *      points alike; every admission of one call sees the same live set) and the point lies in its own box and in neither
+ *      neighbour's along any axis (at sizes that are not powers of two the faces round; such a point could meet another box's
+ *      fold).  The prior is never changed: where it has data it is the authority.
+ *   3. Fold: the admitted MALIO_MAP_ADD candidates of one box, in caller order, by Add_Points' down-sample rule
+ *      (ikd_Tree.cpp:498-534: downsample_size/8, strict <, same_point).  The box was empty and no other box's point lies in it,
+ *      so this is Add_Points(admitted ADD, true) on the real tree, exactly.
+ *   4. The admitted MALIO_MAP_ADD_NO_DOWNSAMPLE points are added unfolded, as Add_Points(.., false) (laserMapping.cpp:444).
+ *   5. Inserted points carry normal_y = 0.001 (feats_down_world's) and id -1 - k, k their session index.  Session order: the
+ *      fold winners by ascending caller index, then the admitted no-downsample points by caller index.
+ *   6. Every inserted point enters the session; those inside the current cube (min <= p < max) are also appended to the window,
+ *      which is then committed.
+ * The window's invariant becomes (prior ∪ session) ∩ cube, exactly, after every window and extend call of a run that makes no
+ * other map calls.  A window call that builds the window enqueues prior ∩ cube as before, then session ∩ cube in session order;
+ * a move appends prior ∩ (new ∖ old), then session ∩ (new ∖ old) in session order.  With an empty session the window does
+ * exactly what it did before.  malio_prior_map_load* starts an empty session (a refused load keeps the previous prior and its
+ * session), malio_prior_map_clear releases it; malio_map_build* and malio_upload_map* end the window, not the session.
+ * Memory: 16 B per session point ({x, y, z, normal_y}; the ids are implied), up to 20 B with the store's growth slack, plus the
+ * window's slots of the ones inside the cube.  A slide tests every session point but sizes its scratch by the points that enter.
+ * Errors: MALIO_ERR_INVALID_ARG for NULL h or s, filter_size_map not finite and > 0; MALIO_ERR_STATE without a current window
+ * (before malio_prior_map_window, or after a map build or upload ended it) or before a pass; MALIO_ERR_CAPACITY when a
+ * candidate's voxel index lies outside +-2^20 per axis or is not finite (nothing is added), or past 2^31 - 1 session points.
+ * The call always waits for the device once for its counts (and again in the commit when points entered the window); rep may
+ * be NULL.  rep: candidates, admitted candidates, inserted points, session points after the call.
+ * malio_prior_map_session_download: the session's points, n x {x, y, z, normal_y} in session order (xyzi NULL: only the count);
+ * MALIO_ERR_CAPACITY when cap < n, MALIO_ERR_STATE before a load.  Writing prior ∪ session as the next session's prior: load
+ * the concatenation of the two (the session ids are -1 - k). */
+typedef struct malio_extend_report {
+  uint32_t n_candidates;   /* points map_incremental classed MALIO_MAP_ADD or MALIO_MAP_ADD_NO_DOWNSAMPLE */
+  uint32_t n_admitted;     /* candidates whose voxel box held no live point at the call's start */
+  uint32_t n_inserted;     /* points appended to the session (fold winners + admitted no-downsample points) */
+  uint64_t n_session;      /* session points after the call */
+} malio_extend_report;
+int malio_prior_map_extend(malio_handle* h, const malio_pass_state* s, double filter_size_map, malio_extend_report* rep);
+int malio_prior_map_session_download(malio_handle* h, float* xyzi, uint64_t cap, uint64_t* n_out);
+
 /* ---- relocalization in a loaded prior map: the first pose of a drive, from a guess good to tens of metres and no heading ------
  * A caller that starts in a saved map knows roll and pitch (gravity), a rough position (GNSS, the last stop) and nothing of the
  * heading; the IESKF's basin is a few degrees and a few metres.  malio_relocalize closes that gap with an exact search over

@@ -460,7 +460,7 @@ int knn_device(malio_handle* h, const float* q, uint32_t nq, uint32_t* idx, floa
 // map_incremental's decision per point of the last pass, in caller order, into cls (N bytes) and world (N x 3 floats, may be
 // NULL): host arrays (on_device false) through the d_o_sel / d_o_world staging buffers of download_aux, which map_incremental
 // copies out when D->N > 0, or the caller's device arrays, ordered on `caller`
-static int map_incr_to(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world, bool on_device,
+int map_incr_to(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world, bool on_device,
                        cudaStream_t caller) {
   DeviceState* D = h->dev.get();
   if (!D->pass_done) { h->err = "map_incremental before measure"; return MALIO_ERR_STATE; }

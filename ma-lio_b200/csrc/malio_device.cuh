@@ -294,6 +294,10 @@ namespace malio_dev {
 enum ScanSource { SCAN_HOST, SCAN_DEVICE, SCAN_ROOM };
 int upload_scan_from(malio_handle* h, ScanSource from, const malio_scan_pt* pts, uint32_t n, const malio_pose_entry* table,
                      cudaMemcpyKind table_kind, const uint32_t* table_off, const malio_rigid* tcomp, cudaStream_t caller);
+// map_incremental's decision for the last pass (malio_b200.cu): on_device false writes the handle's staging buffers D->d_o_sel
+// and, when `world` is not NULL, D->d_o_world (`cls` unused), enqueued on the handle's stream
+int map_incr_to(malio_handle* h, const malio_pass_state* s, double fs, int ekf_inited, uint8_t* cls, float* world, bool on_device,
+                cudaStream_t caller);
 }
 
 #endif  // MALIO_DEVICE_CUH_

@@ -101,6 +101,9 @@ int add_points_device(malio_handle* h, const float* xyz, const float* normal_y, 
 int delete_boxes(malio_handle* h, const float* boxes, uint32_t nb, uint32_t* n_deleted);
 int sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* xyz, const float* normal_y, const int32_t* ids, uint32_t m,
                 uint32_t* n_deleted);
+// the live points of each of nb half-open boxes (device memory, nb x {min3, max3}) into d_counts, enqueued on the handle's
+// stream; the index must be committed (MALIO_ERR_STATE otherwise).  Changes nothing.
+int count_boxes(malio_handle* h, const float* d_boxes, uint32_t nb, uint32_t* d_counts);
 int info(malio_handle* h, uint32_t* n_live, uint32_t* n_slots);
 int download(malio_handle* h, float* xyz, float* normal_y, int32_t* ids, uint32_t* slots, uint32_t cap, uint32_t* n);
 }  // namespace malio_map

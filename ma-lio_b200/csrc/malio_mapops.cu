@@ -101,10 +101,13 @@ __global__ void kill_big_boxes_kernel(float4* __restrict__ mpts, uint32_t n_slot
 // live point that existed at the last commit) and kill what lies inside (Search_by_range's test, ikd_Tree.cpp:1270).  A thread
 // per box was 95 us for 2000 boxes (16 blocks of dependent cell_start -> point -> slot loads); boxes are disjoint voxels, so a
 // slot is written by one lane only.
+// COUNT: the same walk counts the live points of each box into out[k] and changes nothing (malio_prior_map_extend's admission);
+// otherwise out is the kill counter.
 constexpr int KV_T = 128;
+template <bool COUNT>
 __global__ void __launch_bounds__(KV_T) kill_voxel_boxes_kernel(const float* __restrict__ boxes, uint32_t nb, GridConst G,
                                                                 const uint32_t* __restrict__ cell_start, const float4* __restrict__ cell_pts,
-                                                                float4* __restrict__ mpts, uint32_t* __restrict__ killed) {
+                                                                float4* __restrict__ mpts, uint32_t* __restrict__ out) {
   const uint32_t k = (blockIdx.x * KV_T + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
   if (k >= nb) return;                         // warp-uniform
   const float* b = boxes + 6 * (size_t)k;
@@ -114,16 +117,17 @@ __global__ void __launch_bounds__(KV_T) kill_voxel_boxes_kernel(const float* __r
   const float o[3] = {G.ox, G.oy, G.oz};
   const int nn[3] = {G.nx, G.ny, G.nz};
   const float bl[3] = {b0, b1, b2}, bh[3] = {b3, b4, b5};
+  bool outside = false;
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
     const float lo = floorf((bl[a] - o[a]) * G.inv_h) - 1.f, hi = floorf((bh[a] - o[a]) * G.inv_h) + 1.f;
     c0[a] = (int)fminf(fmaxf(lo, 0.f), (float)(nn[a] - 1));
     c1[a] = (int)fminf(fmaxf(hi, 0.f), (float)(nn[a] - 1));
-    if (hi < 0.f || lo > (float)(nn[a] - 1)) return;   // the box lies outside the grid: nothing indexed there
+    outside |= hi < 0.f || lo > (float)(nn[a] - 1);   // the box lies outside the grid: nothing indexed there
   }
   const int ny = c1[1] - c0[1] + 1, nz = c1[2] - c0[2] + 1;
   uint32_t n = 0;
-  for (int row = (int)lane; row < ny * nz; row += 32) {
+  for (int row = (int)lane; !outside && row < ny * nz; row += 32) {
     const int y = c0[1] + row % ny, z = c0[2] + row / ny;
     const uint32_t rs = cell_start[grid_cell_index(G, c0[0], y, z)], re = cell_start[grid_cell_index(G, c1[0], y, z) + 1];
     for (uint32_t j = rs; j < re; ++j) {
@@ -131,13 +135,17 @@ __global__ void __launch_bounds__(KV_T) kill_voxel_boxes_kernel(const float* __r
       if (b0 <= c.x && b3 > c.x && b1 <= c.y && b4 > c.y && b2 <= c.z && b5 > c.z) {
         const uint32_t slot = __float_as_uint(c.w);
         const uint32_t w = __float_as_uint(mpts[slot].w);
-        if (!(w & MALIO_LINK_POINT_DELETED)) { mpts[slot].w = __uint_as_float(w | MALIO_LINK_POINT_DELETED); ++n; }
+        if (!(w & MALIO_LINK_POINT_DELETED)) {
+          if (!COUNT) mpts[slot].w = __uint_as_float(w | MALIO_LINK_POINT_DELETED);
+          ++n;
+        }
       }
     }
   }
 #pragma unroll
   for (int o2 = 16; o2 > 0; o2 >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o2);
-  if (lane == 0 && n) atomicAdd(killed, n);
+  if (COUNT) { if (lane == 0) out[k] = n; }
+  else if (lane == 0 && n) atomicAdd(out, n);
 }
 // bounding box + count of the live slots: grid-stride, warp shuffle + one shared-memory stage per block, ONE set of atomics
 // per block (a few hundred blocks: the atomics on the 8 result words stay uncontended)
@@ -476,7 +484,7 @@ int sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* x
       CUDA_TRY(cudaMemcpyAsync(M->d_boxes, boxes, (size_t)nb * 6 * sizeof(float), cudaMemcpyHostToDevice, D->stream));
     }
     CUDA_TRY(cudaMemsetAsync(M->d_small + 6, 0, sizeof(uint32_t), D->stream));
-    kill_voxel_boxes_kernel<<<(nb + KV_T / 32 - 1) / (KV_T / 32), KV_T, 0, D->stream>>>(M->d_boxes, nb, D->grid, D->d_cell_start, D->d_cell_pts, D->d_mpts, M->d_small + 6);
+    kill_voxel_boxes_kernel<false><<<(nb + KV_T / 32 - 1) / (KV_T / 32), KV_T, 0, D->stream>>>(M->d_boxes, nb, D->grid, D->d_cell_start, D->d_cell_pts, D->d_mpts, M->d_small + 6);
     CUDA_TRY(cudaGetLastError());
     if (n_deleted) {   // the count is only fetched (and waited for) when the caller asks for it
       CUDA_TRY(cudaMemcpyAsync(M->h_small + 6, M->d_small + 6, sizeof(uint32_t), cudaMemcpyDeviceToHost, D->stream));
@@ -492,6 +500,23 @@ int sync_voxels(malio_handle* h, const float* boxes, uint32_t nb, const float* x
   if (killed) M->dirty = true;
   if (n_deleted) *n_deleted = killed;
   return append(h, D, M, xyz, normal_y, ids, m);
+}
+
+int count_boxes(malio_handle* h, const float* d_boxes, uint32_t nb, uint32_t* d_counts) {
+  MapOps* M = h->mapst.get();
+  if (!M || !M->active) { h->err = "device-resident map: box count before malio_map_build"; return MALIO_ERR_STATE; }
+  DeviceState* D = h->dev.get();
+  if (M->dirty || !D->tree_free) { h->err = "device-resident map: box count on an uncommitted index"; return MALIO_ERR_STATE; }
+  if (nb == 0) return MALIO_OK;
+  if (!D->grid_on) {   // no live point (a committed map with live points always has its index)
+    CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nb * sizeof(uint32_t), D->stream));
+    return MALIO_OK;
+  }
+  kill_voxel_boxes_kernel<true><<<(nb + KV_T / 32 - 1) / (KV_T / 32), KV_T, 0, D->stream>>>(d_boxes, nb, D->grid, D->d_cell_start, D->d_cell_pts,
+                                                                                            D->d_mpts, d_counts);
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += 1;
+  return MALIO_OK;
 }
 
 int info(malio_handle* h, uint32_t* n_live, uint32_t* n_slots) {

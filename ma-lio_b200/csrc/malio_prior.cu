@@ -18,6 +18,19 @@
 //   pm_range_kernel   one binary search per row range in the directory -> a contiguous run of points
 //   pm_count / pm_scatter_kernel   the exact test in(new) && !in(old) per candidate, compacted stably into a scratch area
 //   malio_mapops      delete_boxes (the reference's cub_needrm slabs), add_points_device (the append), commit
+//   then the same count / scatter pair over the session store (below) for session ∩ (new ∖ old), appended after the prior's
+// Session layer (malio_prior_map_extend, per scan in localization mode): the points a session adds past the prior's edge, an
+// append-only float4 store.  A map_incremental candidate is admitted when its Add_Points(.., true) voxel box holds no live
+// point of the window at the call's start; the admitted ADD candidates of one box then meet only each other inside it, so
+// folding them in caller order replays Add_Points(admitted, true) on the real tree exactly:
+//   map_incr_to       the decision into the handle's staging buffers (malio_b200.cu)
+//   ext_box_kernel    each candidate's voxel box (floor(x / ds) * ds, + ds, float)
+//   count_boxes       live points per box through the committed cell-list index (malio_mapops.cu, the kill walk's count mode)
+//   ext_key_kernel    admission; box key of the admitted ADD candidates, flags of the admitted no-downsample points
+//   radix sort        stable CUB sort of (box key, caller index)
+//   ext_fold_kernel   one thread per box: the down-sample rule of ikd_Tree.cpp:498-534 over the box's candidates
+//   exclusive sum     over the winner / no-downsample / in-cube flags -> session order and the window's share of it
+//   ext_scatter_kernel  session rows and the window's rows; one wait, then add_points_device + commit
 // Compiled with -fmad=false like the rest of the library.
 #include <cuda_runtime.h>
 
@@ -44,6 +57,7 @@ constexpr int TILE_BITS = 21;                               // per axis; the key
 constexpr int TILE_BIAS = 1 << (TILE_BITS - 1);             // tile index range [-2^20, 2^20)
 constexpr uint32_t FLAG_NONFINITE = 1u, FLAG_RANGE = 2u;
 constexpr int CP_T = 1024;                                  // candidates per compaction block
+constexpr float SESSION_NY = 0.001f;                        // normal_y of feats_down_world, what map_incremental inserts
 
 }  // namespace
 
@@ -69,6 +83,17 @@ struct PriorState {
   DeviceBuffer<char> d_temp;                                // CUB's temporary storage of the window's scans
   DeviceBuffer<uint32_t> d_small;                           // [0] flags, [1..6] biased tile min/max, [7] tile count
   PinnedBuffer<uint32_t> h_small;
+  // the session layer: n_sess points {x, y, z, normal_y} in session order; the id of point k is -1 - k
+  uint32_t n_sess = 0;
+  DeviceBuffer<float4> d_sess;
+  // extend scratch (grow-only, sized by the scan): boxes, live counts, sort keys / values (two halves each), the four flag
+  // rows (winner | no-downsample | winner in cube | no-downsample in cube, + 1) and CUB's temporary storage
+  DeviceBuffer<float> d_ebox;
+  DeviceBuffer<uint32_t> d_ecnt, d_eval, d_eflag;
+  DeviceBuffer<unsigned long long> d_ekey;
+  DeviceBuffer<char> d_etemp;
+
+  void end_session() { n_sess = 0; d_sess.release(); }
 
   int init(malio_handle* h, DeviceState* D) {
     if (int rc = d_small.allocate(h, D->stream, 8)) return rc;
@@ -140,12 +165,17 @@ struct Cubes { float nw[6], od[6]; int has_old; };
 __device__ __forceinline__ bool in_box(const float b[6], const float4& p) {
   return b[0] <= p.x && p.x < b[3] && b[1] <= p.y && p.y < b[4] && b[2] <= p.z && p.z < b[5];
 }
-// candidate j -> its point (range found by a binary search over the exclusive offsets roff[0..nr]) and the verdict
+// candidate j -> its point (range found by a binary search over the exclusive offsets roff[0..nr]; rbeg NULL: the whole store,
+// point j, as for the session) and the verdict
 __device__ __forceinline__ bool candidate(const Cubes& c, const uint32_t* __restrict__ rbeg, const uint32_t* __restrict__ roff,
                                           uint32_t nr, const float4* __restrict__ pts, uint32_t j, uint32_t& p) {
-  uint32_t a = 0, b = nr;                       // last range with roff <= j
-  while (b - a > 1) { const uint32_t m = (a + b) >> 1; if (roff[m] <= j) a = m; else b = m; }
-  p = rbeg[a] + (j - roff[a]);
+  if (rbeg) {
+    uint32_t a = 0, b = nr;                     // last range with roff <= j
+    while (b - a > 1) { const uint32_t m = (a + b) >> 1; if (roff[m] <= j) a = m; else b = m; }
+    p = rbeg[a] + (j - roff[a]);
+  } else {
+    p = j;
+  }
   const float4 q = pts[p];
   return in_box(c.nw, q) && !(c.has_old && in_box(c.od, q));
 }
@@ -177,7 +207,131 @@ __global__ void __launch_bounds__(CP_T) pm_scatter_kernel(Cubes c, const uint32_
     const float4 q = pts[p];
     out[3 * (size_t)pos] = q.x; out[3 * (size_t)pos + 1] = q.y; out[3 * (size_t)pos + 2] = q.z;
     out[3 * (size_t)cap + pos] = q.w;
-    reinterpret_cast<int32_t*>(out + 4 * (size_t)cap)[pos] = ids[p];
+    reinterpret_cast<int32_t*>(out + 4 * (size_t)cap)[pos] = ids ? ids[p] : -1 - (int32_t)p;   // ids NULL: session ids
+  }
+}
+
+// ---- session layer (malio_prior_map_extend)
+// Add_Points(.., true)'s box along one axis (ikd_Tree.cpp:491-496, float): lo = floor(v / ds) * ds, hi = lo + ds; f the floor.
+// True when v lies in its own box and in neither neighbour's: at sizes that are not powers of two the faces round, and a point
+// outside its box or inside a neighbour's could meet another box's fold in the real tree
+__host__ __device__ __forceinline__ bool vox_axis(float v, float ds, float& f, float& lo, float& hi) {
+  f = floorf(v / ds);
+  lo = f * ds;
+  hi = lo + ds;
+  const float lm = (f - 1.f) * ds, lp = (f + 1.f) * ds;
+  return lo <= v && v < hi && !(lm <= v && v < lm + ds) && !(lp <= v && v < lp + ds);
+}
+__device__ __forceinline__ bool is_candidate(uint8_t c) { return c == MALIO_MAP_ADD || c == MALIO_MAP_ADD_NO_DOWNSAMPLE; }
+// a candidate's box (6 floats) and whether it may be admitted; f: the box's floor indices.  Sets FLAG_RANGE in *flags for a
+// candidate whose index lies outside the 21-bit key range (a non-finite point included)
+__device__ __forceinline__ bool vox_box(const float* __restrict__ w, float ds, float b[6], float f[3], uint32_t* flags) {
+  bool ok = true, range = true;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    ok &= vox_axis(w[a], ds, f[a], b[a], b[3 + a]);
+    range &= f[a] >= -(float)TILE_BIAS && f[a] < (float)TILE_BIAS;
+  }
+  if (!range && flags) atomicOr(flags, FLAG_RANGE);
+  return ok && range;
+}
+__device__ __forceinline__ bool in_cube(const float cube[6], const float* __restrict__ w) {
+  return in_box(cube, make_float4(w[0], w[1], w[2], 0.f));
+}
+struct Cube { float b[6]; };
+
+// boxes of the eligible candidates; an empty box (+inf min, -inf max: outside every grid, count 0) for every other point.
+// small[1] += candidates
+__global__ void __launch_bounds__(256) ext_box_kernel(const uint8_t* __restrict__ cls, const float* __restrict__ world, uint32_t n, float ds,
+                                                      float* __restrict__ boxes, uint32_t* __restrict__ small) {
+  const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+  const bool cand = i < n && is_candidate(cls[i]);
+  float b[6] = {INFINITY, INFINITY, INFINITY, -INFINITY, -INFINITY, -INFINITY}, f[3];
+  if (cand && !vox_box(world + 3 * (size_t)i, ds, b, f, small)) {
+    b[0] = b[1] = b[2] = INFINITY; b[3] = b[4] = b[5] = -INFINITY;
+  }
+  if (i < n) {
+#pragma unroll
+    for (int k = 0; k < 6; ++k) boxes[6 * (size_t)i + k] = b[k];
+  }
+  const int c = __syncthreads_count(cand);
+  if (threadIdx.x == 0 && c) atomicAdd(small + 1, (uint32_t)c);
+}
+// admission (eligible, box empty at the call's start): sort key of the admitted ADD candidates (~0: none), the flag rows of the
+// admitted no-downsample points, the winner rows cleared.  small[2] += admitted
+__global__ void __launch_bounds__(256) ext_key_kernel(const uint8_t* __restrict__ cls, const float* __restrict__ world, uint32_t n, float ds,
+                                                      const uint32_t* __restrict__ cnt, Cube cube, unsigned long long* __restrict__ key,
+                                                      uint32_t* __restrict__ val, uint32_t* __restrict__ flag, uint32_t* __restrict__ small) {
+  const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+  bool adm = false;
+  if (i < n) {
+    const uint8_t c = cls[i];
+    const float* w = world + 3 * (size_t)i;
+    float b[6], f[3];
+    adm = is_candidate(c) && vox_box(w, ds, b, f, nullptr) && cnt[i] == 0;
+    key[i] = adm && c == MALIO_MAP_ADD ? tile_key((int)f[0], (int)f[1], (int)f[2]) : ~0ull;
+    val[i] = i;
+    const bool nods = adm && c == MALIO_MAP_ADD_NO_DOWNSAMPLE;
+    flag[i] = 0;
+    flag[n + i] = nods;
+    flag[2 * (size_t)n + i] = 0;
+    flag[3 * (size_t)n + i] = nods && in_cube(cube.b, w);
+    if (i == 0) flag[4 * (size_t)n] = 0;
+  }
+  const int c = __syncthreads_count(adm);
+  if (threadIdx.x == 0 && c) atomicAdd(small + 2, (uint32_t)c);
+}
+// one thread per run of equal keys: Add_Points(.., true) (ikd_Tree.cpp:498-534) over the run's candidates in caller order.  The
+// box was empty at the call's start and no other box's point lies in it, so when a candidate p comes the box holds the winner so
+// far, w, alone: p's min_dist / min_cov start at p's own; w replaces p when both lie within downsample_size/8 of the centre and
+// w's normal_y is smaller (never: every candidate carries SESSION_NY), or otherwise when w lies strictly closer.  Whichever
+// wins is what the box holds after the step (a kept w is deleted and re-added when same_point(p, w): the same point).
+__global__ void __launch_bounds__(256) ext_fold_kernel(const unsigned long long* __restrict__ key, const uint32_t* __restrict__ val, uint32_t n,
+                                                       const float* __restrict__ world, float ds, Cube cube, uint32_t* __restrict__ flag) {
+  const uint32_t j = blockIdx.x * 256u + threadIdx.x;
+  if (j >= n) return;
+  const unsigned long long k = key[j];
+  if (k == ~0ull || (j > 0 && key[j - 1] == k)) return;
+  uint32_t win = val[j];
+  float mid[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    float f, lo, hi;
+    vox_axis(world[3 * (size_t)win + a], ds, f, lo, hi);
+    mid[a] = (float)((double)lo + (double)(hi - lo) / 2.0);                                  // :497-499
+  }
+  const float ds8 = ds / 8;
+  auto dist = [&](uint32_t q) {                                                              // calc_dist (:1694-1698)
+    const float* p = world + 3 * (size_t)q;
+    return (p[0] - mid[0]) * (p[0] - mid[0]) + (p[1] - mid[1]) * (p[1] - mid[1]) + (p[2] - mid[2]) * (p[2] - mid[2]);
+  };
+  float dw = dist(win);
+  for (uint32_t r = j + 1; r < n && key[r] == k; ++r) {
+    const uint32_t p = val[r];
+    const float dp = dist(p);                                                                // min_dist, :503
+    bool keep_w;
+    if (dw < ds8 && dp < ds8) keep_w = false;                                                // :510-516, equal normal_y
+    else keep_w = dw < dp;                                                                   // :517-522
+    if (!keep_w) { win = p; dw = dp; }
+  }
+  flag[win] = 1;
+  flag[2 * (size_t)n + win] = in_cube(cube.b, world + 3 * (size_t)win);
+}
+// exclusive offsets o[0 .. 4n] of the flag rows -> session rows at n_sess + o[j] (winners, then no-downsample points), and the
+// rows of the window's append (those inside the cube, in session order) at o[2n + j] - o[2n]
+__global__ void __launch_bounds__(256) ext_scatter_kernel(const uint32_t* __restrict__ o, uint32_t n, const float* __restrict__ world,
+                                                          uint32_t n_sess, float4* __restrict__ sess, float* __restrict__ out, uint32_t cap) {
+  const uint32_t j = blockIdx.x * 256u + threadIdx.x;
+  if (j >= 2 * n) return;
+  const uint32_t i = j < n ? j : j - n;
+  const float* w = world + 3 * (size_t)i;
+  if (o[j + 1] != o[j]) sess[n_sess + o[j]] = make_float4(w[0], w[1], w[2], SESSION_NY);
+  const size_t jc = 2 * (size_t)n + j;
+  if (o[jc + 1] != o[jc]) {
+    const uint32_t pos = o[jc] - o[2 * (size_t)n];
+    out[3 * (size_t)pos] = w[0]; out[3 * (size_t)pos + 1] = w[1]; out[3 * (size_t)pos + 2] = w[2];
+    out[3 * (size_t)cap + pos] = SESSION_NY;
+    reinterpret_cast<int32_t*>(out + 4 * (size_t)cap)[pos] = -1 - (int32_t)(n_sess + o[j]);
   }
 }
 
@@ -226,6 +380,7 @@ int load_core(malio_handle* h, PriorState* P, DeviceState* D, const float* xyz, 
   CUDA_TRY(cudaStreamSynchronize(st));
   P->d_pts.release(); P->d_ids.release(); P->d_tkey.release(); P->d_toff.release();
   P->loaded = false; P->win = false; P->n = 0; P->n_tiles = 0;
+  P->end_session();
   if (int rc = malio_buf::allocate_group(h, st, {{P->d_pts, n}, {P->d_ids, n}})) return rc;
   pm_gather_kernel<<<(n + 255) / 256, 256, 0, st>>>(v.Current(), n, xyz, ny, ids, P->d_pts, P->d_ids);
   // tile directory: unique keys into the free key half, counts into the free value half, offsets (exclusive sum) into the other
@@ -258,6 +413,7 @@ int load_empty(malio_handle* h, PriorState* P, DeviceState* D) {
   P->d_pts.release(); P->d_ids.release(); P->d_tkey.release(); P->d_toff.release();
   P->n = 0; P->n_tiles = 0;
   for (int a = 0; a < 3; ++a) { P->tlo[a] = 0; P->thi[a] = -1; }
+  P->end_session();
   P->win = false;
   P->loaded = true;
   return MALIO_OK;
@@ -269,6 +425,42 @@ int tile_of(float v, int lo, int hi) {
   if (!(f >= (float)lo)) return lo - 1;
   if (!(f <= (float)hi)) return hi + 1;
   return (int)f;
+}
+
+// the candidates j < n_cand (range rbeg / roff over nr ranges, or the store itself when rbeg is NULL) that lie in nw ∖ od ->
+// d_out rows, stably compacted and enqueued on the handle's stream (the host waits once, for the count); *m = count
+int compact(malio_handle* h, PriorState* P, DeviceState* D, const Cubes& c, const uint32_t* rbeg, const uint32_t* roff, uint32_t nr,
+            uint32_t n_cand, const float4* pts, const int32_t* ids, uint32_t* m) {
+  *m = 0;
+  if (n_cand == 0) return MALIO_OK;
+  cudaStream_t st = D->stream;
+  uint32_t* un = nullptr;
+  size_t t = 0;
+  const uint32_t nblk = (n_cand + CP_T - 1) / CP_T;
+  if ((size_t)nblk + 1 > P->d_blk.size()) {
+    const size_t c2 = nblk + nblk / 4 + 256;
+    if (int rc = malio_buf::allocate_group(h, st, {{P->d_blk, c2}, {P->d_blkoff, c2}})) return rc;
+  }
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)nblk + 1, st));
+  if (int rc = grow_temp(h, P->d_temp, st, t)) return rc;
+  CUDA_TRY(cudaMemsetAsync(P->d_blk + nblk, 0, sizeof(uint32_t), st));
+  pm_count_kernel<<<nblk, CP_T, 0, st>>>(c, rbeg, roff, nr, n_cand, pts, P->d_blk);
+  t = P->d_temp.size();
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(P->d_temp, t, P->d_blk.data(), P->d_blkoff.data(), (int)nblk + 1, st));
+  CUDA_TRY(cudaMemcpyAsync(P->h_small, P->d_blkoff + nblk, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  // the output is sized by the survivors, not the candidates: every session point is a candidate of a slide (the session has
+  // no tile index), and a scratch sized by them would cost more per session point than the session store itself
+  const uint32_t n_out = P->h_small[0];
+  if ((size_t)n_out * 5 > P->d_out.size()) {
+    if (int rc = P->d_out.allocate(h, st, ((size_t)n_out + n_out / 4 + 1024) * 5)) return rc;
+  }
+  const uint32_t cap = (uint32_t)(P->d_out.size() / 5);
+  pm_scatter_kernel<<<nblk, CP_T, 0, st>>>(c, rbeg, roff, nr, n_cand, pts, ids, P->d_blkoff, P->d_out, cap);
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += 3;
+  *m = n_out;
+  return MALIO_OK;
 }
 
 // prior ∩ nw ∖ od (od ignored when has_old == 0) -> d_out rows, in tile-key order and input order within a tile; *m = count
@@ -319,30 +511,12 @@ int gather(malio_handle* h, PriorState* P, DeviceState* D, const Cubes& c, uint3
   CUDA_TRY(cudaStreamSynchronize(st));
   D->ctr.kernel_launches += 2;
   const uint32_t n_cand = P->h_small[0];
-  if (n_cand == 0) return MALIO_OK;
-  const uint32_t nblk = (n_cand + CP_T - 1) / CP_T;
-  if ((size_t)nblk + 1 > P->d_blk.size()) {
-    const size_t c2 = nblk + nblk / 4 + 256;
-    if (int rc = malio_buf::allocate_group(h, st, {{P->d_blk, c2}, {P->d_blkoff, c2}})) return rc;
-  }
-  if ((size_t)n_cand * 5 > P->d_out.size()) {
-    if (int rc = P->d_out.allocate(h, st, ((size_t)n_cand + n_cand / 4 + 1024) * 5)) return rc;
-  }
-  t = 0;
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)nblk + 1, st));
-  if (int rc = grow_temp(h, P->d_temp, st, t)) return rc;
-  const uint32_t cap = (uint32_t)(P->d_out.size() / 5);
-  CUDA_TRY(cudaMemsetAsync(P->d_blk + nblk, 0, sizeof(uint32_t), st));
-  pm_count_kernel<<<nblk, CP_T, 0, st>>>(c, P->d_rbeg, P->d_roff, nr, n_cand, P->d_pts, P->d_blk);
-  t = P->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(P->d_temp, t, P->d_blk.data(), P->d_blkoff.data(), (int)nblk + 1, st));
-  pm_scatter_kernel<<<nblk, CP_T, 0, st>>>(c, P->d_rbeg, P->d_roff, nr, n_cand, P->d_pts, P->d_ids, P->d_blkoff, P->d_out, cap);
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(P->h_small, P->d_blkoff + nblk, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  D->ctr.kernel_launches += 3;
-  *m = P->h_small[0];
-  return MALIO_OK;
+  return compact(h, P, D, c, P->d_rbeg, P->d_roff, nr, n_cand, P->d_pts, P->d_ids, m);
+}
+
+// session ∩ nw ∖ od -> d_out rows in session order, ids -1 - k; *m = count
+int gather_session(malio_handle* h, PriorState* P, DeviceState* D, const Cubes& c, uint32_t* m) {
+  return compact(h, P, D, c, nullptr, nullptr, 0, P->n_sess, P->d_sess, nullptr, m);
 }
 
 // the entering points d_out[0 .. m) -> a new device map (first call) or the slots' tail
@@ -353,6 +527,16 @@ int feed(malio_handle* h, PriorState* P, DeviceState* D, uint32_t m, bool build)
   const int32_t* ids = m ? reinterpret_cast<const int32_t*>(P->d_out + 4 * cap) : nullptr;
   if (build) return malio_map::build_device(h, xyz, ny, ids, m, D->stream);
   return malio_map::add_points_device(h, xyz, ny, ids, m, D->stream);
+}
+
+// session ∩ nw ∖ od appended behind the prior's share (nothing at all with an empty session); *m += count
+int feed_session(malio_handle* h, PriorState* P, DeviceState* D, const Cubes& c, uint32_t* m) {
+  if (P->n_sess == 0) return MALIO_OK;
+  uint32_t ms = 0;
+  if (int rc = gather_session(h, P, D, c, &ms)) return rc;
+  if (int rc = feed(h, P, D, ms, false)) return rc;
+  *m += ms;
+  return MALIO_OK;
 }
 
 }  // namespace
@@ -411,6 +595,10 @@ int window(malio_handle* h, const double pos[3], double cube_len, float det_rang
     P->win = false;
     if (int rc = gather(h, P, D, c, &m)) return rc;
     if (int rc = feed(h, P, D, m, true)) return rc;   // malio_map_build: replaces the device map, commits
+    if (P->n_sess) {
+      if (int rc = feed_session(h, P, D, c, &m)) return rc;
+      if (int rc = malio_map::commit(h)) return rc;
+    }
     std::memcpy(P->cube, c.nw, sizeof(c.nw));
     P->win = true;
     P->win_epoch = h->map_epoch;
@@ -451,6 +639,7 @@ int window(malio_handle* h, const double pos[3], double cube_len, float det_rang
       if (int rc = malio_map::delete_boxes(h, &boxes[0][0], nb, &killed)) return rc;
       if (int rc = gather(h, P, D, c, &m)) return rc;
       if (int rc = feed(h, P, D, m, false)) return rc;
+      if (int rc = feed_session(h, P, D, c, &m)) return rc;
       std::memcpy(P->cube, c.nw, sizeof(c.nw));
       if (int rc = malio_map::commit(h)) return rc;
       P->win = true;
@@ -463,6 +652,102 @@ int window(malio_handle* h, const double pos[3], double cube_len, float det_rang
   }
   std::memcpy(rep->cube, P->cube, sizeof(P->cube));
   rep->n_live = (uint32_t)D->ctr.map_live;
+  return MALIO_OK;
+}
+
+int extend(malio_handle* h, const malio_pass_state* s, double fs, malio_extend_report* rep) {
+  PriorState* P = h->prior.get();
+  if (!P || !P->loaded || !P->win || P->win_epoch != h->map_epoch) {
+    h->err = "malio_prior_map_extend without a current window (malio_prior_map_window after the load or the last map build)";
+    return MALIO_ERR_STATE;
+  }
+  DeviceState* D = h->dev.get();
+  CUDA_TRY(cudaSetDevice(D->device));
+  cudaStream_t st = D->stream;
+  // the decision first: its neighbour lists are slot indices of the last pass, which a compacting commit would renumber
+  if (int rc = malio_dev::map_incr_to(h, s, fs, 1, nullptr, D->d_o_world, false, nullptr)) return rc;
+  if (int rc = malio_map::commit(h)) return rc;   // the admission counts through the index: it must know every live slot
+  const uint32_t n = D->N;
+  malio_extend_report r{0, 0, 0, P->n_sess};
+  if (n == 0) { if (rep) *rep = r; return MALIO_OK; }
+  if ((uint64_t)P->n_sess + n > 0x7FFFFFFFull) { h->err = "malio_prior_map_extend: the session would exceed 2^31 - 1 points"; return MALIO_ERR_CAPACITY; }
+  const float ds = (float)fs;
+  // scratch for n points: 6 floats of box, a count, two halves of keys and values, 4n + 1 flags; the session's room for n more
+  if ((size_t)n * 6 > P->d_ebox.size()) {
+    const size_t c = (size_t)n + n / 4 + 1024;
+    if (int rc = malio_buf::allocate_group(h, st, {{P->d_ebox, 6 * c}, {P->d_ecnt, c}, {P->d_eval, 2 * c}, {P->d_ekey, 2 * c}, {P->d_eflag, 4 * c + 1}}))
+      return rc;
+  }
+  if ((size_t)P->n_sess + n > P->d_sess.size()) {
+    const size_t c = (size_t)P->n_sess + n + (P->n_sess + n) / 4 + 1024;
+    if (const cudaError_t e = malio_buf::grow_keep(st, {{P->d_sess, c, P->n_sess}})) {
+      h->err = std::string("malio_prior_map_extend: growing the session store: ") + cudaGetErrorString(e);
+      return MALIO_ERR_CUDA;
+    }
+  }
+  if ((size_t)n * 5 > P->d_out.size()) {
+    if (int rc = P->d_out.allocate(h, st, ((size_t)n + n / 4 + 1024) * 5)) return rc;
+  }
+  const size_t c = P->d_ecnt.size();
+  cub::DoubleBuffer<unsigned long long> k(P->d_ekey.data(), P->d_ekey.data() + c);
+  cub::DoubleBuffer<uint32_t> v(P->d_eval.data(), P->d_eval.data() + c);
+  size_t t = 0, t2 = 0;
+  uint32_t* un = nullptr;
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t, k, v, (int)n, 0, 64, st));
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t2, un, un, (int)(4 * n + 1), st));
+  if (int rc = grow_temp(h, P->d_etemp, st, t > t2 ? t : t2)) return rc;
+  Cube cube;
+  std::memcpy(cube.b, P->cube, sizeof(cube.b));
+  const uint8_t* cls = D->d_o_sel;
+  const float* world = D->d_o_world;
+  const uint32_t g = (n + 255) / 256;
+  CUDA_TRY(cudaMemsetAsync(P->d_small, 0, 3 * sizeof(uint32_t), st));   // flags, candidates, admitted
+  ext_box_kernel<<<g, 256, 0, st>>>(cls, world, n, ds, P->d_ebox, P->d_small);
+  CUDA_TRY(cudaGetLastError());
+  if (int rc = malio_map::count_boxes(h, P->d_ebox, n, P->d_ecnt)) return rc;
+  ext_key_kernel<<<g, 256, 0, st>>>(cls, world, n, ds, P->d_ecnt, cube, k.Current(), v.Current(), P->d_eflag, P->d_small);
+  t = P->d_etemp.size();
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(P->d_etemp, t, k, v, (int)n, 0, 64, st));
+  ext_fold_kernel<<<g, 256, 0, st>>>(k.Current(), v.Current(), n, world, ds, cube, P->d_eflag);
+  t = P->d_etemp.size();
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(P->d_etemp, t, P->d_eflag.data(), P->d_eflag.data(), (int)(4 * n + 1), st));
+  const uint32_t cap = (uint32_t)(P->d_out.size() / 5);
+  ext_scatter_kernel<<<(2 * n + 255) / 256, 256, 0, st>>>(P->d_eflag, n, world, P->n_sess, P->d_sess, P->d_out, cap);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(P->h_small, P->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(P->h_small + 3, P->d_eflag + 2 * (size_t)n, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(P->h_small + 4, P->d_eflag + 4 * (size_t)n, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  D->ctr.kernel_launches += 7;   // box, key, fold, scatter, and the sort / scan passes counted as three (count_boxes counts its own)
+  if (P->h_small[0] & FLAG_RANGE) {
+    h->err = "malio_prior_map_extend: a candidate's voxel index lies outside +-2^20 per axis (or the point is not finite); nothing was added";
+    return MALIO_ERR_CAPACITY;
+  }
+  const uint32_t ins = P->h_small[3], in_cube_n = P->h_small[4] - P->h_small[3];
+  r.n_candidates = P->h_small[1];
+  r.n_admitted = P->h_small[2];
+  r.n_inserted = ins;
+  P->n_sess += ins;
+  r.n_session = P->n_sess;
+  if (in_cube_n) {
+    if (int rc = feed(h, P, D, in_cube_n, false)) return rc;
+    if (int rc = malio_map::commit(h)) return rc;
+  }
+  if (rep) *rep = r;
+  return MALIO_OK;
+}
+
+int session_download(malio_handle* h, float* xyzi, uint64_t cap, uint64_t* n_out) {
+  PriorState* P = h->prior.get();
+  if (!P || !P->loaded) { h->err = "malio_prior_map_session_download before malio_prior_map_load"; return MALIO_ERR_STATE; }
+  if (n_out) *n_out = P->n_sess;
+  if (!xyzi || P->n_sess == 0) return MALIO_OK;
+  if (cap < P->n_sess) { h->err = "malio_prior_map_session_download: capacity below the session's points"; return MALIO_ERR_CAPACITY; }
+  DeviceState* D = h->dev.get();
+  CUDA_TRY(cudaSetDevice(D->device));
+  CUDA_TRY(cudaMemcpyAsync(xyzi, P->d_sess, (size_t)P->n_sess * sizeof(float4), cudaMemcpyDeviceToHost, D->stream));
+  CUDA_TRY(cudaStreamSynchronize(D->stream));
+  D->ctr.d2h_bytes += (uint64_t)P->n_sess * sizeof(float4);
   return MALIO_OK;
 }
 
@@ -482,7 +767,9 @@ int info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* devic
   if (n_tiles) *n_tiles = P->n_tiles;
   if (device_bytes)
     *device_bytes = P->d_pts.bytes() + P->d_ids.bytes() + P->d_tkey.bytes() + P->d_toff.bytes() + P->d_rq.bytes() + P->d_rbeg.bytes() +
-                    P->d_roff.bytes() + P->d_blk.bytes() + P->d_blkoff.bytes() + P->d_out.bytes() + P->d_temp.bytes();
+                    P->d_roff.bytes() + P->d_blk.bytes() + P->d_blkoff.bytes() + P->d_out.bytes() + P->d_temp.bytes() +
+                    P->d_sess.bytes() + P->d_ebox.bytes() + P->d_ecnt.bytes() + P->d_eval.bytes() + P->d_ekey.bytes() + P->d_eflag.bytes() +
+                    P->d_etemp.bytes();
   return MALIO_OK;
 }
 
@@ -524,4 +811,14 @@ extern "C" int malio_prior_map_clear(malio_handle* h) {
   if (!h) return MALIO_ERR_INVALID_ARG;
   MALIO_SETTLE(h);
   return malio_prior::clear(h);
+}
+extern "C" int malio_prior_map_extend(malio_handle* h, const malio_pass_state* s, double filter_size_map, malio_extend_report* rep) {
+  if (!h || !s || !(filter_size_map > 0.0) || !std::isfinite(filter_size_map)) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_prior::extend(h, s, filter_size_map, rep);
+}
+extern "C" int malio_prior_map_session_download(malio_handle* h, float* xyzi, uint64_t cap, uint64_t* n_out) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_prior::session_download(h, xyzi, cap, n_out);
 }

@@ -114,6 +114,11 @@ class WindowReport(C.Structure):
                 ("boxes", C.c_float * 18), ("n_killed", C.c_uint32), ("n_entered", C.c_uint32), ("n_live", C.c_uint32)]
 
 
+class ExtendReport(C.Structure):
+    """malio_extend_report: what one malio_prior_map_extend call added to the session."""
+    _fields_ = [("n_candidates", C.c_uint32), ("n_admitted", C.c_uint32), ("n_inserted", C.c_uint32), ("n_session", C.c_uint64)]
+
+
 class RelocArgs(C.Structure):
     """malio_reloc_args: candidate yaws yaw_lo + k * yaw_step (k < n_yaw) and the lattice (res, half_xy, half_z)."""
     _fields_ = [("yaw_lo", C.c_double), ("yaw_step", C.c_double), ("n_yaw", C.c_uint32), ("res", C.c_double),
@@ -204,6 +209,7 @@ EXPORTS = [
     "malio_place_db_build", "malio_place_db_info", "malio_place_db_download", "malio_relocalize_global",
     "malio_world_voxel_seed", "malio_world_voxel_seed_device", "malio_world_voxel_changes_device",
     "malio_world_voxel_save_changes_pcd",
+    "malio_prior_map_extend", "malio_prior_map_session_download",
 ]
 
 
@@ -283,6 +289,8 @@ def load() -> C.CDLL:
     lib.malio_prior_map_window.argtypes = [vp, vp, C.c_double, C.c_float, vp]
     lib.malio_prior_map_info.argtypes = [vp, vp, vp, vp]
     lib.malio_prior_map_clear.argtypes = [vp]
+    lib.malio_prior_map_extend.argtypes = [vp, vp, C.c_double, vp]
+    lib.malio_prior_map_session_download.argtypes = [vp, vp, C.c_uint64, vp]
     lib.malio_relocalize.argtypes = [vp, vp, vp, vp]
     lib.malio_place_db_build.argtypes = [vp, vp, vp]
     lib.malio_place_db_info.argtypes = [vp, vp, vp]

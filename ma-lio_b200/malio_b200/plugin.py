@@ -605,6 +605,25 @@ class MeasurementModel:
         """Release the prior; the device map keeps its points."""
         self._check(self.lib.malio_prior_map_clear(self._h))
 
+    def prior_map_extend(self, state: capi.PassState | capi.State, filter_size_map: float = 0.5) -> dict:
+        """malio_prior_map_extend: map_incremental in localization mode, with the state after the update.  The scan's candidates
+        whose voxel box holds no live point of the window are folded and added to the session (and to the window where they lie
+        inside the cube).  Returns the report as a dict: n_candidates, n_admitted, n_inserted, n_session."""
+        ps = state.pass_state() if isinstance(state, capi.State) else state
+        rep = capi.ExtendReport()
+        self._check(self.lib.malio_prior_map_extend(self._h, C.byref(ps), C.c_double(filter_size_map), C.byref(rep)))
+        return dict(n_candidates=int(rep.n_candidates), n_admitted=int(rep.n_admitted), n_inserted=int(rep.n_inserted),
+                    n_session=int(rep.n_session))
+
+    def prior_map_session(self) -> np.ndarray:
+        """The session's points as float32 (n, 4) {x, y, z, normal_y} in session order (point k has id -1 - k)."""
+        n = C.c_uint64(0)
+        self._check(self.lib.malio_prior_map_session_download(self._h, None, 0, C.byref(n)))
+        out = np.zeros((n.value, 4), np.float32)
+        if n.value:
+            self._check(self.lib.malio_prior_map_session_download(self._h, capi.ptr(out), n.value, C.byref(n)))
+        return out
+
     def relocalize(self, guess: capi.State | capi.PassState, res: float, half_xy: int, half_z: int, n_yaw: int = 360,
                    yaw_lo: float = 0.0, yaw_step: float | None = None) -> dict:
         """malio_relocalize: the best of n_yaw yaws (yaw_lo + k * yaw_step, default step 2 pi / n_yaw) about the prior's z axis after
