@@ -111,7 +111,7 @@ __global__ void scan_lidar_check_kernel(const uint32_t* __restrict__ words, uint
 
 // ------------------------------------------------------------------ device-memory entry points
 namespace malio_devstate {
-int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const char* what) {
+int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const char* what, unsigned align, const char* rows) {
   if (!p) { h->err = std::string(what) + ": NULL"; return MALIO_ERR_INVALID_ARG; }
   if (reinterpret_cast<uintptr_t>(p) & 3u) { h->err = std::string(what) + ": not 4-byte aligned"; return MALIO_ERR_INVALID_ARG; }
   cudaPointerAttributes a{};
@@ -123,12 +123,28 @@ int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const
   if (a.type == cudaMemoryTypeManaged) { h->err = std::string(what) + ": managed memory is not accepted (use cudaMalloc'ed memory)"; return MALIO_ERR_INVALID_ARG; }
   if (a.type != cudaMemoryTypeDevice) { h->err = std::string(what) + ": host memory (the *_device calls take device memory)"; return MALIO_ERR_INVALID_ARG; }
   if (a.device != D->device) { h->err = std::string(what) + ": memory of another device than the handle's"; return MALIO_ERR_INVALID_ARG; }
+  if (align > 4 && (reinterpret_cast<uintptr_t>(p) & (align - 1))) {
+    h->err = std::string(what) + ": not " + std::to_string(align) + "-byte aligned (" + rows + ")";
+    return MALIO_ERR_INVALID_ARG;
+  }
   return MALIO_OK;
 }
 int check_device_ptrs(malio_handle* h, const DeviceState* D, std::initializer_list<DevicePtrArg> args) {
   for (const DevicePtrArg& a : args)
     if (a.p) { if (int rc = check_device_ptr(h, D, a.p, a.what)) return rc; }
   return MALIO_OK;
+}
+
+int write_pcd_from_device(malio_handle* h, DeviceState* D, const char* path, const float4* rows, uint64_t n, PinnedBuffer<float4>& bounce) {
+  if (!bounce) { if (int rc = bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
+  return malio_pcd::write_binary(path, n, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
+    if (cudaMemcpyAsync(bounce, rows + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, D->stream) != cudaSuccess ||
+        cudaStreamSynchronize(D->stream) != cudaSuccess)
+      return (int)MALIO_ERR_CUDA;
+    D->ctr.d2h_bytes += cnt * sizeof(float4);
+    *xyzi = (const float*)bounce.data();
+    return (int)MALIO_OK;
+  }, h->err);
 }
 
 int caller_enter(malio_handle* h, DeviceState* D, cudaStream_t caller) {

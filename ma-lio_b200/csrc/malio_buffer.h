@@ -117,6 +117,39 @@ inline cudaError_t grow_keep(cudaStream_t st, std::initializer_list<Resize> grou
   return cudaSuccess;
 }
 
+// The temporary storage of CUB's device-wide algorithms, grow-only.  A call (void* temp, size_t& bytes) -> cudaError_t names
+// one cub::Device* algorithm with its arguments; with temp NULL, CUB only reports the bytes it needs.  reserve() grows the
+// storage by replacement to t + t/8 + 4096 when it holds fewer than the largest t its calls ask for; it goes ahead of the
+// launches it serves, since a replacement drains the stream.  run() hands the storage and its size to one call.
+class CubTemp {
+ public:
+  size_t bytes() const { return buf_.bytes(); }
+  void release() { buf_.release(); }
+  template <class... Calls>
+  int reserve(malio_handle* h, cudaStream_t st, const Calls&... calls) {
+    size_t t = 0;
+    cudaError_t e = cudaSuccess;
+    auto ask = [&](const auto& call) {
+      size_t b = 0;
+      if (e == cudaSuccess) e = call(nullptr, b);
+      if (b > t) t = b;
+    };
+    (ask(calls), ...);
+    if (e != cudaSuccess) return cuda_fail(h, "CUB temporary storage query", e);
+    if (t <= buf_.size()) return MALIO_OK;
+    return buf_.allocate(h, st, t + t / 8 + 4096);
+  }
+  template <class Call>
+  int run(malio_handle* h, const Call& call) {
+    size_t b = buf_.size();
+    if (cudaError_t e = call(buf_.data(), b)) return cuda_fail(h, "CUB device-wide algorithm", e);
+    return MALIO_OK;
+  }
+
+ private:
+  DeviceBuffer<char> buf_;
+};
+
 // cudaHostAlloc'ed host memory, move-only (flags: cudaHostAllocMapped for a buffer the device writes into).  Pinned buffers
 // are allocated once, on first use, and never grow.
 template <class T>

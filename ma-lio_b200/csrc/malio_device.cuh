@@ -27,6 +27,7 @@
 namespace malio_devstate {
 
 using malio_buf::acquire;
+using malio_buf::CubTemp;
 using malio_buf::DeviceBuffer;
 using malio_buf::PinnedBuffer;
 using malio_buf::release;
@@ -267,11 +268,15 @@ int fetch_knn_stats(malio_handle* h, DeviceState* D, cudaStream_t st);
 int knn_fault(malio_handle* h, const DeviceState* D);
 // malio_b200.cu: the device-memory entry points.
 // MALIO_OK when p is 4-byte aligned device memory of D's device (cudaMalloc / a memory pool: what torch allocates); NULL, host,
-// pinned, managed or another device's memory -> MALIO_ERR_INVALID_ARG with h->err naming `what`
-int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const char* what);
+// pinned, managed or another device's memory -> MALIO_ERR_INVALID_ARG with h->err naming `what`; align > 4: p aligned to
+// `align` bytes as well, else h->err names `rows`, how the kernels store or read them
+int check_device_ptr(malio_handle* h, const DeviceState* D, const void* p, const char* what, unsigned align = 4, const char* rows = nullptr);
 // check_device_ptr on each pointer of the list that is not NULL (NULL: that output is not asked for), in list order
 struct DevicePtrArg { const void* p; const char* what; };
 int check_device_ptrs(malio_handle* h, const DeviceState* D, std::initializer_list<DevicePtrArg> args);
+// the first n of `rows` (device memory, read on D->stream) as a binary PCD at path, copied out chunk by chunk through the pinned
+// buffer `bounce` (malio_pcd::CHUNK points, allocated on first use); the copies count in D->ctr.d2h_bytes
+int write_pcd_from_device(malio_handle* h, DeviceState* D, const char* path, const float4* rows, uint64_t n, PinnedBuffer<float4>& bounce);
 // D->stream waits for everything enqueued on the caller's stream so far / the caller's stream waits for D->stream
 int caller_enter(malio_handle* h, DeviceState* D, cudaStream_t caller);
 int caller_leave(malio_handle* h, DeviceState* D, cudaStream_t caller);

@@ -374,7 +374,7 @@ int check_args(malio_handle* h, const malio_place_args* a) {
 struct BuildScratch {
   DeviceBuffer<int> d_small;
   DeviceBuffer<uint32_t> d_gmax, d_gmin, d_flag, d_off;
-  DeviceBuffer<char> d_temp;
+  CubTemp d_temp;
   size_t bytes() const { return d_small.bytes() + d_gmax.bytes() + d_gmin.bytes() + d_flag.bytes() + d_off.bytes() + d_temp.bytes(); }
 };
 
@@ -432,13 +432,11 @@ int build(malio_handle* h, DeviceState* D, const malio_place_args* a, const floa
     if (nl) {
       const uint32_t gi0 = (uint32_t)(ia * m - ilo), gj0 = (uint32_t)(ja * m - jlo);
       if (int rc = malio_buf::allocate_group(h, st, {{S.d_flag, nl + 1}, {S.d_off, nl + 1}})) return rc;
-      size_t t = 0;
-      uint32_t* un = nullptr;
-      CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)(nl + 1), st));
-      if (int rc = S.d_temp.allocate(h, st, t)) return rc;
+      auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, S.d_flag.data(), S.d_off.data(), (int)(nl + 1), st); };
+      if (int rc = S.d_temp.reserve(h, st, scan)) return rc;
       pl_flag_kernel<<<(unsigned)((nl + 1 + 255) / 256), 256, 0, st>>>(S.d_gmax, (uint32_t)nx, gi0, gj0, (uint32_t)m, (uint32_t)lx,
                                                                         (uint32_t)nl, S.d_flag);
-      CUDA_TRY(cub::DeviceScan::ExclusiveSum(S.d_temp.data(), t, S.d_flag.data(), S.d_off.data(), (int)(nl + 1), st));
+      if (int rc = S.d_temp.run(h, scan)) return rc;
       uint32_t npos = 0;
       CUDA_TRY(cudaMemcpyAsync(&npos, S.d_off + nl, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
       CUDA_TRY(cudaStreamSynchronize(st));
@@ -478,7 +476,7 @@ struct QueryScratch {
   DeviceBuffer<uint8_t> d_q;
   DeviceBuffer<uint16_t> d_qk;
   DeviceBuffer<Stage2Out> d_out;
-  DeviceBuffer<char> d_temp;
+  CubTemp d_temp;
   size_t bytes() const {
     return d_qg.bytes() + d_key.bytes() + d_sorted.bytes() + d_q.bytes() + d_qk.bytes() + d_out.bytes() + d_temp.bytes();
   }
@@ -510,11 +508,10 @@ int rank(malio_handle* h, DeviceState* D, const PlaceDb& P, const malio_pass_sta
     const uint32_t np = (uint32_t)P.n;
     if (int rc = malio_buf::allocate_group(h, st, {{S.d_key, np}, {S.d_sorted, np}})) return rc;
     if (int rc = S.d_out.allocate(h, st, n1)) return rc;
-    size_t t = 0;
-    CUDA_TRY(cub::DeviceRadixSort::SortKeys(nullptr, t, S.d_key.data(), S.d_sorted.data(), (int)np, 0, 64, st));
-    if (int rc = S.d_temp.allocate(h, st, t)) return rc;
+    auto sort = [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, S.d_key.data(), S.d_sorted.data(), (int)np, 0, 64, st); };
+    if (int rc = S.d_temp.reserve(h, st, sort)) return rc;
     pl_stage1_kernel<<<(np + 255) / 256, 256, 0, st>>>(P.d_rk, np, a.n_ring, S.d_qk, S.d_key);
-    CUDA_TRY(cub::DeviceRadixSort::SortKeys(S.d_temp.data(), t, S.d_key.data(), S.d_sorted.data(), (int)np, 0, 64, st));
+    if (int rc = S.d_temp.run(h, sort)) return rc;
     pl_stage2_kernel<<<n1, ST2_T, 0, st>>>(S.d_sorted, a.n_ring, a.n_sector, S.d_q, P.d_nib, P.bpp, P.d_cols, P.d_zs, S.d_out);
     CUDA_TRY(cudaGetLastError());
     D->ctr.kernel_launches += 3;   // stage 1, the sort (counted as one), stage 2

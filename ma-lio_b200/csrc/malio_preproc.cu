@@ -1006,11 +1006,7 @@ static int world_register_to(malio_handle* h, const malio_pass_state* s, int sou
   if (n > 0xFFFFFFFFull) { h->err = "world registration: more than 2^32-1 points"; return MALIO_ERR_CAPACITY; }
   const uint64_t k = n < cap ? n : cap;
   if (on_device && out && k) {
-    if (int rc = check_device_ptr(h, D, out, "malio_world_register_device out")) return rc;
-    if (reinterpret_cast<uintptr_t>(out) & 15u) {
-      h->err = "malio_world_register_device out: not 16-byte aligned (the points are stored as float4)";
-      return MALIO_ERR_INVALID_ARG;
-    }
+    if (int rc = check_device_ptr(h, D, out, "malio_world_register_device out", 16, "the points are stored as float4")) return rc;
   }
   *n_out = (uint32_t)n;
   if (!out || k == 0) return MALIO_OK;
@@ -1083,15 +1079,7 @@ int world_save_pcd(malio_handle* h, const char* path, int clear) {
   DeviceState* D;
   if (int rc = acquire(h, h->pre, S, D)) return rc;
   if (S->n_acc == 0) { h->err = "world save: the accumulated cloud is empty (nothing is written)"; return MALIO_ERR_STATE; }
-  if (!S->h_bounce) { if (int rc = S->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
-  const int rc = malio_pcd::write_binary(path, S->n_acc, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
-    if (cudaMemcpyAsync(S->h_bounce, S->d_acc + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, S->stream) != cudaSuccess ||
-        cudaStreamSynchronize(S->stream) != cudaSuccess)
-      return (int)MALIO_ERR_CUDA;
-    D->ctr.d2h_bytes += cnt * sizeof(float4);
-    *xyzi = (const float*)S->h_bounce.data();
-    return (int)MALIO_OK;
-  }, h->err);
+  const int rc = write_pcd_from_device(h, D, path, S->d_acc, S->n_acc, S->h_bounce);
   if (rc == MALIO_OK && clear) S->n_acc = 0;   // pcl_wait_save->clear() (:485); the buffer is kept
   return rc;
 }

@@ -80,7 +80,7 @@ struct PriorState {
   DeviceBuffer<unsigned long long> d_rq;
   DeviceBuffer<uint32_t> d_rbeg, d_roff, d_blk, d_blkoff;
   DeviceBuffer<float> d_out;
-  DeviceBuffer<char> d_temp;                                // CUB's temporary storage of the window's scans
+  CubTemp d_temp;                                           // CUB's temporary storage of the window's scans
   DeviceBuffer<uint32_t> d_small;                           // [0] flags, [1..6] biased tile min/max, [7] tile count
   PinnedBuffer<uint32_t> h_small;
   // the session layer: n_sess points {x, y, z, normal_y} in session order; the id of point k is -1 - k
@@ -91,7 +91,7 @@ struct PriorState {
   DeviceBuffer<float> d_ebox;
   DeviceBuffer<uint32_t> d_ecnt, d_eval, d_eflag;
   DeviceBuffer<unsigned long long> d_ekey;
-  DeviceBuffer<char> d_etemp;
+  CubTemp d_etemp;
 
   void end_session() { n_sess = 0; d_sess.release(); }
 
@@ -335,11 +335,6 @@ __global__ void __launch_bounds__(256) ext_scatter_kernel(const uint32_t* __rest
   }
 }
 
-int grow_temp(malio_handle* h, DeviceBuffer<char>& temp, cudaStream_t st, size_t t) {
-  if (t <= temp.size()) return MALIO_OK;
-  return temp.allocate(h, st, t + t / 8 + 4096);
-}
-
 // the prior from device arrays read on the handle's stream (the caller has ordered them there).  Refusals leave the previous
 // prior and the window as they were.
 int load_core(malio_handle* h, PriorState* P, DeviceState* D, const float* xyz, const float* ny, const int32_t* ids, uint32_t n) {
@@ -348,7 +343,7 @@ int load_core(malio_handle* h, PriorState* P, DeviceState* D, const float* xyz, 
   // sort area: keys | alternate keys | values | alternate values, released at the end of the load
   DeviceBuffer<unsigned long long> d_key;
   DeviceBuffer<uint32_t> d_val;
-  DeviceBuffer<char> d_temp;
+  CubTemp temp;
   if (int rc = malio_buf::allocate_group(h, st, {{d_key, 2 * (size_t)n}, {d_val, 2 * (size_t)n}})) return rc;
   cub::DoubleBuffer<unsigned long long> k(d_key.data(), d_key.data() + n);
   cub::DoubleBuffer<uint32_t> v(d_val.data(), d_val.data() + n);
@@ -366,16 +361,17 @@ int load_core(malio_handle* h, PriorState* P, DeviceState* D, const float* xyz, 
   }
   int tlo[3], thi[3];
   for (int a = 0; a < 3; ++a) { tlo[a] = (int)P->h_small[1 + a] - TILE_BIAS; thi[a] = (int)P->h_small[4 + a] - TILE_BIAS; }
-  size_t t = 0;
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t, k, v, (int)n, 0, 3 * TILE_BITS, st));
-  size_t t2 = 0;
-  unsigned long long* un = nullptr; uint32_t* uu = nullptr;
-  CUDA_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, t2, un, un, uu, uu, (int)n, st));
-  if (t2 > t) t = t2;
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t2, uu, uu, (int)n, st));
-  if (t2 > t) t = t2;
-  if (int rc = d_temp.allocate(h, st, t)) return rc;
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(d_temp, t, k, v, (int)n, 0, 3 * TILE_BITS, st));
+  // the sort, then the tile directory: unique keys into the free key half, counts into the free value half, offsets (exclusive
+  // sum over the m tiles) into the other; the permutation is dead once gathered (stream order)
+  auto sort = [&](void* tmp, size_t& b) { return cub::DeviceRadixSort::SortPairs(tmp, b, k, v, (int)n, 0, 3 * TILE_BITS, st); };
+  auto encode = [&](void* tmp, size_t& b) {
+    return cub::DeviceRunLengthEncode::Encode(tmp, b, k.Current(), k.Alternate(), v.Alternate(), P->d_small + 7, (int)n, st);
+  };
+  auto scan = [&](uint32_t m) {
+    return [&, m](void* tmp, size_t& b) { return cub::DeviceScan::ExclusiveSum(tmp, b, v.Alternate(), v.Current(), (int)m, st); };
+  };
+  if (int rc = temp.reserve(h, st, sort, encode, scan(n))) return rc;
+  if (int rc = temp.run(h, sort)) return rc;
   // the new store replaces the old one (the window it fed ends with it)
   CUDA_TRY(cudaStreamSynchronize(st));
   P->d_pts.release(); P->d_ids.release(); P->d_tkey.release(); P->d_toff.release();
@@ -383,20 +379,14 @@ int load_core(malio_handle* h, PriorState* P, DeviceState* D, const float* xyz, 
   P->end_session();
   if (int rc = malio_buf::allocate_group(h, st, {{P->d_pts, n}, {P->d_ids, n}})) return rc;
   pm_gather_kernel<<<(n + 255) / 256, 256, 0, st>>>(v.Current(), n, xyz, ny, ids, P->d_pts, P->d_ids);
-  // tile directory: unique keys into the free key half, counts into the free value half, offsets (exclusive sum) into the other
-  unsigned long long* uk = k.Alternate();
-  uint32_t* cnt = v.Alternate();
-  uint32_t* off = v.Current();   // the permutation is dead once gathered (stream order)
-  t2 = d_temp.size();
-  CUDA_TRY(cub::DeviceRunLengthEncode::Encode(d_temp, t2, k.Current(), uk, cnt, P->d_small + 7, (int)n, st));
+  if (int rc = temp.run(h, encode)) return rc;
   CUDA_TRY(cudaMemcpyAsync(P->h_small + 7, P->d_small + 7, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   const uint32_t nt = P->h_small[7];
-  t2 = d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(d_temp, t2, cnt, off, (int)nt, st));
+  if (int rc = temp.run(h, scan(nt))) return rc;
   if (int rc = malio_buf::allocate_group(h, st, {{P->d_tkey, nt}, {P->d_toff, (size_t)nt + 1}})) return rc;
-  CUDA_TRY(cudaMemcpyAsync(P->d_tkey, uk, (size_t)nt * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(P->d_toff, off, (size_t)nt * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(P->d_tkey, k.Alternate(), (size_t)nt * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(P->d_toff, v.Current(), (size_t)nt * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
   P->h_small[6] = n;   // (the pinned word is free again: the tile count was read above)
   CUDA_TRY(cudaMemcpyAsync(P->d_toff + nt, P->h_small + 6, sizeof(uint32_t), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaGetLastError());
@@ -434,19 +424,16 @@ int compact(malio_handle* h, PriorState* P, DeviceState* D, const Cubes& c, cons
   *m = 0;
   if (n_cand == 0) return MALIO_OK;
   cudaStream_t st = D->stream;
-  uint32_t* un = nullptr;
-  size_t t = 0;
   const uint32_t nblk = (n_cand + CP_T - 1) / CP_T;
   if ((size_t)nblk + 1 > P->d_blk.size()) {
     const size_t c2 = nblk + nblk / 4 + 256;
     if (int rc = malio_buf::allocate_group(h, st, {{P->d_blk, c2}, {P->d_blkoff, c2}})) return rc;
   }
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)nblk + 1, st));
-  if (int rc = grow_temp(h, P->d_temp, st, t)) return rc;
+  auto scan = [&](void* tmp, size_t& b) { return cub::DeviceScan::ExclusiveSum(tmp, b, P->d_blk.data(), P->d_blkoff.data(), (int)nblk + 1, st); };
+  if (int rc = P->d_temp.reserve(h, st, scan)) return rc;
   CUDA_TRY(cudaMemsetAsync(P->d_blk + nblk, 0, sizeof(uint32_t), st));
   pm_count_kernel<<<nblk, CP_T, 0, st>>>(c, rbeg, roff, nr, n_cand, pts, P->d_blk);
-  t = P->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(P->d_temp, t, P->d_blk.data(), P->d_blkoff.data(), (int)nblk + 1, st));
+  if (int rc = P->d_temp.run(h, scan)) return rc;
   CUDA_TRY(cudaMemcpyAsync(P->h_small, P->d_blkoff + nblk, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   // the output is sized by the survivors, not the candidates: every session point is a candidate of a slide (the session has
@@ -496,17 +483,14 @@ int gather(malio_handle* h, PriorState* P, DeviceState* D, const Cubes& c, uint3
     const size_t c2 = nr + nr / 4 + 256;
     if (int rc = malio_buf::allocate_group(h, st, {{P->d_rbeg, c2}, {P->d_roff, c2}})) return rc;
   }
-  size_t t = 0;
-  uint32_t* un = nullptr;
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)nr + 1, st));
-  if (int rc = grow_temp(h, P->d_temp, st, t)) return rc;
+  auto scan = [&](void* tmp, size_t& b) { return cub::DeviceScan::ExclusiveSum(tmp, b, P->d_roff.data(), P->d_roff.data(), (int)nr + 1, st); };
+  if (int rc = P->d_temp.reserve(h, st, scan)) return rc;
   CUDA_TRY(cudaMemcpyAsync(P->d_rq, rq.data(), rq.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
   D->ctr.h2d_bytes += rq.size() * sizeof(unsigned long long);
   // counts go to d_roff[0..nr) with d_roff[nr] = 0 (the "+1" row), then an exclusive sum in place: d_roff[nr] = candidates
   CUDA_TRY(cudaMemsetAsync(P->d_roff + nr, 0, sizeof(uint32_t), st));
   pm_range_kernel<<<(nr + 255) / 256, 256, 0, st>>>(P->d_rq, nr, P->d_tkey, P->n_tiles, P->d_toff, P->d_rbeg, P->d_roff);
-  t = P->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(P->d_temp, t, P->d_roff.data(), P->d_roff.data(), (int)nr + 1, st));
+  if (int rc = P->d_temp.run(h, scan)) return rc;
   CUDA_TRY(cudaMemcpyAsync(P->h_small, P->d_roff + nr, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   D->ctr.kernel_launches += 2;
@@ -691,11 +675,9 @@ int extend(malio_handle* h, const malio_pass_state* s, double fs, malio_extend_r
   const size_t c = P->d_ecnt.size();
   cub::DoubleBuffer<unsigned long long> k(P->d_ekey.data(), P->d_ekey.data() + c);
   cub::DoubleBuffer<uint32_t> v(P->d_eval.data(), P->d_eval.data() + c);
-  size_t t = 0, t2 = 0;
-  uint32_t* un = nullptr;
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t, k, v, (int)n, 0, 64, st));
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t2, un, un, (int)(4 * n + 1), st));
-  if (int rc = grow_temp(h, P->d_etemp, st, t > t2 ? t : t2)) return rc;
+  auto sort = [&](void* tmp, size_t& b) { return cub::DeviceRadixSort::SortPairs(tmp, b, k, v, (int)n, 0, 64, st); };
+  auto scan = [&](void* tmp, size_t& b) { return cub::DeviceScan::ExclusiveSum(tmp, b, P->d_eflag.data(), P->d_eflag.data(), (int)(4 * n + 1), st); };
+  if (int rc = P->d_etemp.reserve(h, st, sort, scan)) return rc;
   Cube cube;
   std::memcpy(cube.b, P->cube, sizeof(cube.b));
   const uint8_t* cls = D->d_o_sel;
@@ -706,11 +688,9 @@ int extend(malio_handle* h, const malio_pass_state* s, double fs, malio_extend_r
   CUDA_TRY(cudaGetLastError());
   if (int rc = malio_map::count_boxes(h, P->d_ebox, n, P->d_ecnt)) return rc;
   ext_key_kernel<<<g, 256, 0, st>>>(cls, world, n, ds, P->d_ecnt, cube, k.Current(), v.Current(), P->d_eflag, P->d_small);
-  t = P->d_etemp.size();
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(P->d_etemp, t, k, v, (int)n, 0, 64, st));
+  if (int rc = P->d_etemp.run(h, sort)) return rc;
   ext_fold_kernel<<<g, 256, 0, st>>>(k.Current(), v.Current(), n, world, ds, cube, P->d_eflag);
-  t = P->d_etemp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(P->d_etemp, t, P->d_eflag.data(), P->d_eflag.data(), (int)(4 * n + 1), st));
+  if (int rc = P->d_etemp.run(h, scan)) return rc;
   const uint32_t cap = (uint32_t)(P->d_out.size() / 5);
   ext_scatter_kernel<<<(2 * n + 255) / 256, 256, 0, st>>>(P->d_eflag, n, world, P->n_sess, P->d_sess, P->d_out, cap);
   CUDA_TRY(cudaGetLastError());

@@ -68,7 +68,7 @@ struct VoxState {
   DeviceBuffer<char> d_sort;
   // run scratch, 16 B a row, sized for the rows of a fold only
   DeviceBuffer<uint32_t> d_head, d_run, d_rent, d_new;
-  DeviceBuffer<char> d_temp;                 // CUB's temporary storage (sort histograms, scan carries)
+  CubTemp d_temp;                            // CUB's temporary storage (sort histograms, scan carries)
   DeviceBuffer<uint32_t> d_small;            // [0] fault flag, [1] run count, [2] entries in use, [3] kept / removed count, [5] added
   PinnedBuffer<uint32_t> h_small;            // pinned mirror of d_small
   PinnedBuffer<float4> h_bounce;             // pinned, malio_pcd::CHUNK points
@@ -426,19 +426,29 @@ __global__ void __launch_bounds__(256) vs_change_kernel(const uint32_t* __restri
   added[r] = (!seeded && kept) ? 1u : 0u;
 }
 
-// CUB's temporary storage for at least t bytes, and the sort area for n rows
-int grow_temp(malio_handle* h, VoxState* V, DeviceState* D, size_t t) {
-  if (t <= V->d_temp.size()) return MALIO_OK;
-  return V->d_temp.allocate(h, D->stream, t + t / 8 + 4096);
+// CUB's calls on d_temp, reserved by grow_sort, grow_runs and enqueue_select_order.  The stable sort of n rows of b by key:
+auto sort_call(SortBufs& b, uint64_t n, cudaStream_t st) {
+  return [&b, n, st](void* t, size_t& c) { return cub::DeviceRadixSort::SortPairs(t, c, b.k, b.v, (int)n, VKeyDecomposer{}, st); };
 }
+// the fold's scans of n rows: the head flags into the run numbers (d_rent), the new flags into the new runs' ranks (d_head)
+auto runs_call(VoxState* V, uint64_t n, cudaStream_t st) {
+  return [=](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, V->d_head.data(), V->d_rent.data(), (int)n, st); };
+}
+auto new_call(VoxState* V, uint64_t n, cudaStream_t st) {
+  return [=](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, V->d_new.data(), V->d_head.data(), (int)n, st); };
+}
+// a selection's exclusive scan of the flag column over the entries into COL_SCAN (its storage does not depend on the column)
+auto select_call(VoxState* V, const uint32_t* flag, cudaStream_t st) {
+  return [=](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, flag, sort_col(V, COL_SCAN), (int)V->n_vox, st); };
+}
+
+// the sort area for n rows and CUB's storage for their sort
 int grow_sort(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
   if (n > sort_rows(V)) {
     if (int rc = V->d_sort.allocate(h, D->stream, (n + n / 8 + 1024) * SORT_ROW)) return rc;
   }
   SortBufs b = sort_bufs(V);
-  size_t t = 0;
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t, b.k, b.v, (int)n, VKeyDecomposer{}, D->stream));
-  return grow_temp(h, V, D, t);
+  return V->d_temp.reserve(h, D->stream, sort_call(b, n, D->stream));
 }
 // the run scratch for n rows
 int grow_runs(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
@@ -446,11 +456,7 @@ int grow_runs(malio_handle* h, VoxState* V, DeviceState* D, uint64_t n) {
     const uint64_t c = n + n / 8 + 1024;
     if (int rc = malio_buf::allocate_group(h, D->stream, {{V->d_head, c}, {V->d_run, c}, {V->d_rent, c}, {V->d_new, c}})) return rc;
   }
-  size_t t_incl = 0, t_excl = 0;
-  uint32_t* un = nullptr;
-  CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, t_incl, un, un, (int)n, D->stream));
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t_excl, un, un, (int)n, D->stream));
-  return grow_temp(h, V, D, t_incl > t_excl ? t_incl : t_excl);
+  return V->d_temp.reserve(h, D->stream, runs_call(V, n, D->stream), new_call(V, n, D->stream));
 }
 
 // room for `need` entries and a hash at most half full.  Entries move with a device-side copy, the hash is rebuilt from the
@@ -513,17 +519,14 @@ int enqueue_fold(malio_handle* h, VoxState* V, DeviceState* D, const Rows& src, 
   const uint64_t mask = V->d_hash.size() - 1;
   SortBufs b = sort_bufs(V);
   vm_key_kernel<<<g, 256, 0, st>>>(src, il, n, b.k.Current(), b.v.Current(), V->d_small);
-  size_t t = V->d_temp.size();
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)n, VKeyDecomposer{}, st));
+  if (int rc = V->d_temp.run(h, sort_call(b, n, st))) return rc;
   const VKey* key = b.k.Current();
   const uint32_t* val = b.v.Current();
   vm_head_kernel<<<g, 256, 0, st>>>(key, n, V->d_head);
-  t = V->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::InclusiveSum(V->d_temp, t, V->d_head.data(), V->d_rent.data(), (int)n, st));
+  if (int rc = V->d_temp.run(h, runs_call(V, n, st))) return rc;
   vm_run_kernel<<<g, 256, 0, st>>>(V->d_head, V->d_rent, n, V->d_run, V->d_small);
   vm_lookup_kernel<<<g, 256, 0, st>>>(V->d_run, key, n, V->d_small, V->d_hash, mask, V->d_ekey, V->d_rent, V->d_new);
-  t = V->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, V->d_new.data(), V->d_head.data(), (int)n, st));
+  if (int rc = V->d_temp.run(h, new_call(V, n, st))) return rc;
   vm_fold_kernel<<<(n + 127) / 128, 128, 0, st>>>(src, V->d_run, key, val, n, V->d_small, V->d_rent, V->d_head, V->d_hash, mask,
                                                  V->d_ekey, V->d_esum, V->d_ecnt);
   CUDA_TRY(cudaGetLastError());
@@ -537,8 +540,7 @@ int enqueue_order(malio_handle* h, VoxState* V, DeviceState* D, SortBufs& b) {
   cudaStream_t st = D->stream;
   const uint32_t n = (uint32_t)V->n_vox;
   vm_iota_kernel<<<(n + 255) / 256, 256, 0, st>>>(V->d_ekey, n, b.k.Current(), b.v.Current());
-  size_t t = V->d_temp.size();
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(V->d_temp, t, b.k, b.v, (int)n, VKeyDecomposer{}, st));
+  if (int rc = V->d_temp.run(h, sort_call(b, n, st))) return rc;
   D->ctr.kernel_launches += 1;
   return MALIO_OK;
 }
@@ -563,10 +565,7 @@ int enqueue_sorted(malio_handle* h, VoxState* V, DeviceState* D, float4* out, ui
 // A selection of the entries in key order (sort area grown for the entries): enqueue_select_order, one kernel that flags
 // every entry, then enqueue_select per flag column.
 int enqueue_select_order(malio_handle* h, VoxState* V, DeviceState* D, SortBufs& b) {
-  size_t t = 0;
-  uint32_t* un = nullptr;
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t, un, un, (int)V->n_vox, D->stream));
-  if (int rc = grow_temp(h, V, D, t)) return rc;
+  if (int rc = V->d_temp.reserve(h, D->stream, select_call(V, sort_col(V, COL_FLAGS), D->stream))) return rc;
   b = sort_bufs(V);
   return enqueue_order(h, V, D, b);
 }
@@ -574,10 +573,8 @@ int enqueue_select_order(malio_handle* h, VoxState* V, DeviceState* D, SortBufs&
 // small[word]
 int enqueue_select(malio_handle* h, VoxState* V, DeviceState* D, const uint32_t* order, const uint32_t* flag, uint32_t col, int word) {
   const uint32_t n = (uint32_t)V->n_vox;
-  uint32_t* pos = sort_col(V, COL_SCAN);
-  size_t t = V->d_temp.size();
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(V->d_temp, t, flag, pos, (int)n, D->stream));
-  vc_compact_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(order, flag, pos, n, sort_col(V, col), V->d_small + word);
+  if (int rc = V->d_temp.run(h, select_call(V, flag, D->stream))) return rc;
+  vc_compact_kernel<<<(n + 255) / 256, 256, 0, D->stream>>>(order, flag, sort_col(V, COL_SCAN), n, sort_col(V, col), V->d_small + word);
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 1;
   return MALIO_OK;
@@ -618,18 +615,6 @@ int enqueue_changes(malio_handle* h, VoxState* V, DeviceState* D, const malio_ca
   return MALIO_OK;
 }
 
-// the first n rows of stage (device memory) as a binary PCD at path, through the pinned bounce buffer
-int write_staged(malio_handle* h, VoxState* V, DeviceState* D, const char* path, const float4* stage, uint64_t n) {
-  return malio_pcd::write_binary(path, n, [&](uint64_t first, uint64_t cnt, const float** xyzi) {
-    if (cudaMemcpyAsync(V->h_bounce, stage + first, cnt * sizeof(float4), cudaMemcpyDeviceToHost, D->stream) != cudaSuccess ||
-        cudaStreamSynchronize(D->stream) != cudaSuccess)
-      return (int)MALIO_ERR_CUDA;
-    D->ctr.d2h_bytes += cnt * sizeof(float4);
-    *xyzi = (const float*)V->h_bounce.data();
-    return (int)MALIO_OK;
-  }, h->err);
-}
-
 // after a save: the entry-sized sort area and CUB's storage go back once the stream is drained.  Between saves the map holds
 // its entries, its hash and the scan-sized scratch only (the next accumulate regrows the sort area for its scan).
 int release_scratch(malio_handle* h, VoxState* V, DeviceState* D) {
@@ -639,16 +624,7 @@ int release_scratch(malio_handle* h, VoxState* V, DeviceState* D) {
   return MALIO_OK;
 }
 
-// p, rows of the caller in device memory: check_device_ptr, then p aligned to `align` bytes (h->err names `what` and `rows`)
-constexpr const char* CENTROID_ROWS = "the centroids are stored as float4";
-int check_rows(malio_handle* h, const DeviceState* D, const void* p, const char* what, uintptr_t align, const char* rows) {
-  if (int rc = check_device_ptr(h, D, p, what)) return rc;
-  if (reinterpret_cast<uintptr_t>(p) & (align - 1)) {
-    h->err = std::string(what) + ": not " + std::to_string(align) + "-byte aligned (" + rows + ")";
-    return MALIO_ERR_INVALID_ARG;
-  }
-  return MALIO_OK;
-}
+constexpr const char* CENTROID_ROWS = "the centroids are stored as float4";   // check_device_ptr's reason for 16-byte rows
 
 int check_keep(malio_handle* h, const malio_carve_keep* k) {
   if (!std::isfinite(k->max_miss_per_hit) || k->max_miss_per_hit < 0.f) {
@@ -751,7 +727,7 @@ int download_device(malio_handle* h, float* out, uint64_t cap, uint64_t* n_out, 
   if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   const uint64_t n = V->n_vox, k = n < cap ? n : cap;
   if (out && k) {
-    if (int rc = check_rows(h, D, out, "malio_world_voxel_download_device out", 16, CENTROID_ROWS)) return rc;
+    if (int rc = check_device_ptr(h, D, out, "malio_world_voxel_download_device out", 16, CENTROID_ROWS)) return rc;
   }
   *n_out = n;
   if (!out || k == 0) return MALIO_OK;
@@ -768,7 +744,7 @@ int evidence_device(malio_handle* h, uint32_t* out, uint64_t cap, uint64_t* n_ou
   if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   const uint64_t n = V->n_vox, k = n < cap ? n : cap;
   if (out && k) {
-    if (int rc = check_rows(h, D, out, "malio_world_voxel_evidence_device out", 8, "the pairs are stored as uint2")) return rc;
+    if (int rc = check_device_ptr(h, D, out, "malio_world_voxel_evidence_device out", 8, "the pairs are stored as uint2")) return rc;
   }
   *n_out = n;
   if (!out || k == 0) return MALIO_OK;
@@ -789,7 +765,7 @@ int download_kept_device(malio_handle* h, const malio_carve_keep* keep, float* o
   if (int rc = acquire(h, h->voxmap, V, D)) return rc;
   if (int rc = check_keep(h, keep)) return rc;
   if (out && cap && V->n_vox) {
-    if (int rc = check_rows(h, D, out, "malio_world_voxel_download_kept_device out", 16, CENTROID_ROWS)) return rc;
+    if (int rc = check_device_ptr(h, D, out, "malio_world_voxel_download_kept_device out", 16, CENTROID_ROWS)) return rc;
   }
   uint64_t n = 0;
   if (V->n_vox) {
@@ -813,7 +789,6 @@ int save_pcd(malio_handle* h, const char* path, const malio_carve_keep* keep, in
   if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
   uint64_t n = V->n_vox;
   if (int rc = grow_sort(h, V, D, n)) return rc;
-  if (!V->h_bounce) { if (int rc = V->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
   float4* stage = sort_stage(V);
   if (keep) {
     if (int rc = enqueue_kept(h, V, D, keep, &n)) return rc;
@@ -826,7 +801,7 @@ int save_pcd(malio_handle* h, const char* path, const malio_carve_keep* keep, in
   } else if (int rc = enqueue_sorted(h, V, D, stage, n)) {
     return rc;
   }
-  const int rc = write_staged(h, V, D, path, stage, n);
+  const int rc = write_pcd_from_device(h, D, path, stage, n, V->h_bounce);
   if (int e = release_scratch(h, V, D)) return e;
   if (rc == MALIO_OK && clear) {
     if (int c = clear_map(h, V, D)) return c;
@@ -849,7 +824,7 @@ int seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t se
     return MALIO_ERR_STATE;
   }
   if (on_device) {
-    if (int rc = check_rows(h, D, xyzi, "malio_world_voxel_seed_device xyzi", 16, "the rows are read as float4")) return rc;
+    if (int rc = check_device_ptr(h, D, xyzi, "malio_world_voxel_seed_device xyzi", 16, "the rows are read as float4")) return rc;
   }
   const uint64_t chunk = n < MALIO_SEED_CHUNK ? n : MALIO_SEED_CHUNK;
   if (int rc = grow_table(h, V, D, n)) return rc;
@@ -921,10 +896,10 @@ int changes_device(malio_handle* h, const malio_carve_keep* keep, float* d_remov
   if (int rc = check_keep(h, keep)) return rc;
   if (V->n_vox) {
     if (d_removed && cap_removed) {
-      if (int rc = check_rows(h, D, d_removed, "malio_world_voxel_changes_device removed", 16, CENTROID_ROWS)) return rc;
+      if (int rc = check_device_ptr(h, D, d_removed, "malio_world_voxel_changes_device removed", 16, CENTROID_ROWS)) return rc;
     }
     if (d_added && cap_added) {
-      if (int rc = check_rows(h, D, d_added, "malio_world_voxel_changes_device added", 16, CENTROID_ROWS)) return rc;
+      if (int rc = check_device_ptr(h, D, d_added, "malio_world_voxel_changes_device added", 16, CENTROID_ROWS)) return rc;
     }
   }
   uint64_t nr = 0, na = 0;
@@ -955,7 +930,6 @@ int save_changes_pcd(malio_handle* h, const malio_carve_keep* keep, const char* 
   if (int rc = check_keep(h, keep)) return rc;
   if (V->n_vox == 0) { h->err = "world voxel save: the voxel map is empty (nothing is written)"; return MALIO_ERR_STATE; }
   if (int rc = grow_sort(h, V, D, V->n_vox)) return rc;
-  if (!V->h_bounce) { if (int rc = V->h_bounce.allocate(h, malio_pcd::CHUNK)) return rc; }
   uint64_t nr = 0, na = 0;
   if (int rc = enqueue_changes(h, V, D, keep, &nr, &na)) return rc;
   if (n_removed) *n_removed = nr;
@@ -966,7 +940,7 @@ int save_changes_pcd(malio_handle* h, const malio_carve_keep* keep, const char* 
   for (const auto& set : sets) {
     if (rc != MALIO_OK || !set.path || set.cnt == 0) continue;
     if (int e = enqueue_centroids(h, V, D, sort_col(V, set.col), (uint32_t)set.cnt, stage, (uint32_t)set.cnt)) return e;
-    rc = write_staged(h, V, D, set.path, stage, set.cnt);
+    rc = write_pcd_from_device(h, D, set.path, stage, set.cnt, V->h_bounce);
   }
   if (int e = release_scratch(h, V, D)) return e;
   return rc;
@@ -980,7 +954,7 @@ int info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* devi
   if (capacity) *capacity = V->d_ekey.size();
   if (device_bytes)
     *device_bytes = V->d_ekey.size() * (sizeof(VKey) + sizeof(float4) + sizeof(uint32_t)) + V->d_hash.size() * sizeof(uint32_t) +
-                    V->d_sort.size() + V->d_head.size() * RUN_ROW + V->d_temp.size() +
+                    V->d_sort.size() + V->d_head.size() * RUN_ROW + V->d_temp.bytes() +
                     V->d_hm.size() * sizeof(uint2) + V->d_stamp.size() * sizeof(uint32_t);
   return MALIO_OK;
 }

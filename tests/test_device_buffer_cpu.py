@@ -4,7 +4,8 @@ counts live allocations, frees, stream drains and copies, and can fail the next 
 Checked: replacement growth drains only when it replaces a live buffer, and before the free; a failed replacement leaves
 an empty buffer; keeping growth copies the first elements and leaves everything as it was when it fails, for a single buffer
 and for a group; a replacement group reads as empty after a failed member; move, swap and destruction free each allocation
-exactly once, for device and pinned buffers."""
+exactly once, for device and pinned buffers; CUB's temporary storage grows to the largest size its calls ask for plus headroom,
+only when it holds less, drains before a replacement, hands a run all its bytes, and is left as it was by a failed query."""
 import os
 import subprocess
 
@@ -189,6 +190,36 @@ static void ownership(malio_handle* h) {
   CHECK(g_live.size() == live0);
 }
 
+static void cub_temp(malio_handle* h) {
+  malio_buf::CubTemp t;
+  void* ran = nullptr;
+  size_t ran_bytes = 0;
+  // a call that asks for `need` bytes and records what a run is handed
+  auto call = [&](size_t need) {
+    return [&, need](void* p, size_t& b) {
+      if (!p) b = need; else { ran = p; ran_bytes = b; }
+      return cudaSuccess;
+    };
+  };
+  auto failing = [](void*, size_t& b) { b = 1u << 30; return cudaErrorInvalidValue; };
+  g_log.clear();
+  CHECK(t.reserve(h, ST, call(1000), call(8000), call(50)) == MALIO_OK);
+  CHECK(g_log == "m");                       // the largest size plus t/8 + 4096, without a drain for the first allocation
+  CHECK(t.bytes() == 8000 + 1000 + 4096);
+  CHECK(t.reserve(h, ST, call(13096)) == MALIO_OK && g_log == "m");   // it fits: nothing happens
+  CHECK(t.run(h, call(1)) == MALIO_OK && ran != nullptr && ran_bytes == 13096);
+  g_log.clear();
+  CHECK(t.reserve(h, ST, call(20000)) == MALIO_OK);
+  CHECK(g_log == "sfm" && t.bytes() == 20000 + 2500 + 4096);   // one drain, before the free
+  g_log.clear();
+  CHECK(t.reserve(h, ST, call(10), failing, call(1u << 20)) == MALIO_ERR_CUDA);
+  CHECK(g_log.empty() && t.bytes() == 26596);
+  CHECK(h->err == "CUB temporary storage query: error");
+  CHECK(t.run(h, failing) == MALIO_ERR_CUDA && h->err == "CUB device-wide algorithm: error");
+  t.release();
+  CHECK(t.bytes() == 0);
+}
+
 int main() {
   malio_handle h;
   replace_growth(&h);
@@ -196,6 +227,7 @@ int main() {
   keep_group(&h);
   replace_group(&h);
   ownership(&h);
+  cub_temp(&h);
   CHECK(g_live.empty());
   CHECK(g_double_free == 0);
   std::printf("%s %d\n", g_failures ? "FAILED" : "OK", g_failures);
