@@ -12,12 +12,7 @@
 #define MALIO_COMPOUND_H_
 
 #include "malio_b200.h"
-
-#ifdef __CUDACC__
-#define MALIO_CHD __host__ __device__
-#else
-#define MALIO_CHD
-#endif
+#include "malio_se3.h"
 
 namespace malio_compound {
 
@@ -39,31 +34,10 @@ MALIO_CHD inline M6 mul6(const M6& x, const M6& y) { M6 o; for (int i = 0; i < 6
 MALIO_CHD inline M6 tr6(const M6& x) { M6 o; for (int i = 0; i < 6; ++i) for (int j = 0; j < 6; ++j) o.a[i][j] = x.a[j][i]; return o; }
 MALIO_CHD inline M6 load6(const double* p) { M6 o; for (int i = 0; i < 6; ++i) for (int j = 0; j < 6; ++j) o.a[i][j] = p[6 * i + j]; return o; }
 MALIO_CHD inline void copy_n(double* dst, const double* src, int n) { for (int k = 0; k < n; ++k) dst[k] = src[k]; }
-MALIO_CHD inline void q_mul_h(const double a[4], const double b[4], double o[4]) {   // Eigen quaternion product, (w,x,y,z)
-  const double w = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
-  const double x = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
-  const double y = a[0] * b[2] + a[2] * b[0] + a[3] * b[1] - a[1] * b[3];
-  const double z = a[0] * b[3] + a[3] * b[0] + a[1] * b[2] - a[2] * b[1];
-  o[0] = w; o[1] = x; o[2] = y; o[3] = z;
-}
-MALIO_CHD inline void q_rot_h(const double q[4], const double v[3], double o[3]) {   // Eigen _transformVector
-  const double uv[3] = {2 * (q[2] * v[2] - q[3] * v[1]), 2 * (q[3] * v[0] - q[1] * v[2]), 2 * (q[1] * v[1] - q[2] * v[0])};
-  const double r[3] = {v[0] + q[0] * uv[0] + (q[2] * uv[2] - q[3] * uv[1]), v[1] + q[0] * uv[1] + (q[3] * uv[0] - q[1] * uv[2]),
-                       v[2] + q[0] * uv[2] + (q[1] * uv[1] - q[2] * uv[0])};
-  o[0] = r[0]; o[1] = r[1]; o[2] = r[2];
-}
-MALIO_CHD inline void q_to_R(const double q[4], double R[3][3]) {   // Eigen toRotationMatrix
-  const double w = q[0], x = q[1], y = q[2], z = q[3];
-  const double tx = 2 * x, ty = 2 * y, tz = 2 * z, twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x,
-               tyy = ty * y, tyz = tz * y, tzz = tz * z;
-  R[0][0] = 1 - (tyy + tzz); R[0][1] = txy - twz; R[0][2] = txz + twy;
-  R[1][0] = txy + twz; R[1][1] = 1 - (txx + tzz); R[1][2] = tyz - twx;
-  R[2][0] = txz - twy; R[2][1] = tyz + twx; R[2][2] = 1 - (txx + tyy);
-}
 MALIO_CHD inline void set_T(malio_pose* p) {   // T_ from q_, t_ (bottom row 0 0 0 1)
-  double R[3][3];
-  q_to_R(p->q, R);
-  for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) p->T[4 * i + j] = R[i][j]; p->T[4 * i + 3] = p->t[i]; }
+  double R[9];
+  malio_se3::q_to_R(p->q, R);
+  for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) p->T[4 * i + j] = R[3 * i + j]; p->T[4 * i + 3] = p->t[i]; }
   p->T[12] = 0; p->T[13] = 0; p->T[14] = 0; p->T[15] = 1;
 }
 // adjointMatrix(T.inverse()) (:8-15, :44, :99); T is a rigid transform [R t; 0 1]: inverse = [R^T, -R^T t]
@@ -111,9 +85,9 @@ MALIO_CHD inline void pose_initial(malio_pose* pose, const double t[3], const do
 MALIO_CHD inline void compound_pose_with_cov(const malio_pose* pose_1, const double* cov_1, const malio_pose* pose_2, const double* cov_2,
                                              malio_pose* pose_cp, double* cov_cp) {
   double q[4], t[3];
-  q_mul_h(pose_1->q, pose_2->q, q);
+  malio_se3::q_mul(pose_1->q, pose_2->q, q);
   for (int k = 0; k < 4; ++k) pose_cp->q[k] = q[k];                       // :93
-  q_rot_h(pose_1->q, pose_2->t, t);
+  malio_se3::q_rot(pose_1->q, pose_2->t, t);
   for (int k = 0; k < 3; ++k) pose_cp->t[k] = t[k] + pose_1->t[k];        // :94
   set_T(pose_cp);                                                         // :96-98
   const M6 Ad = adjoint_of_inverse(pose_2->T);                            // :99 (the new T_ when pose_cp aliases pose_2)
@@ -129,9 +103,9 @@ MALIO_CHD inline void compound_inv_pose_with_cov(const malio_pose* pose_1, const
                                                  malio_pose* pose_cp, double* cov_cp) {
   const double qc[4] = {pose_1->q[0], -pose_1->q[1], -pose_1->q[2], -pose_1->q[3]};
   double q[4], d[3], t[3];
-  q_mul_h(qc, pose_2->q, q);
+  malio_se3::q_mul(qc, pose_2->q, q);
   for (int k = 0; k < 3; ++k) d[k] = pose_2->t[k] - pose_1->t[k];
-  q_rot_h(qc, d, t);
+  malio_se3::q_rot(qc, d, t);
   for (int k = 0; k < 4; ++k) pose_cp->q[k] = q[k];                       // :36
   for (int k = 0; k < 3; ++k) pose_cp->t[k] = t[k];                       // :37
   set_T(pose_cp);                                                         // :41-43

@@ -23,6 +23,7 @@
 
 #include "malio_buffer.h"
 #include "malio_internal.h"
+#include "malio_se3.h"
 
 namespace malio_devstate {
 
@@ -31,6 +32,8 @@ using malio_buf::CubTemp;
 using malio_buf::DeviceBuffer;
 using malio_buf::PinnedBuffer;
 using malio_buf::release;
+using malio_se3::q_rot;
+using malio_se3::q_rot_conj;
 
 #define CUDA_TRY(expr)                                                                     \
   do {                                                                                     \
@@ -69,27 +72,6 @@ struct PassConst {
   double RcT[MALIO_MAX_LIDAR][9];      // R(temporal_comp_l)^T  (entry 0 unused)
 };
 
-// ------------------------------------------------------------------ small device algebra (mirrors Eigen's op order)
-__device__ __forceinline__ void cross3(const double a[3], const double b[3], double o[3]) {
-  o[0] = a[1] * b[2] - a[2] * b[1];
-  o[1] = a[2] * b[0] - a[0] * b[2];
-  o[2] = a[0] * b[1] - a[1] * b[0];
-}
-// Quaternion * vector as Eigen's _transformVector: v + w*uv + qv x uv, uv = 2 (qv x v); q = (w,x,y,z)
-__device__ __forceinline__ void q_rot(const double q[4], const double v[3], double o[3]) {
-  const double qv[3] = {q[1], q[2], q[3]};
-  double uv[3], c2[3];
-  cross3(qv, v, uv);
-  uv[0] += uv[0]; uv[1] += uv[1]; uv[2] += uv[2];
-  cross3(qv, uv, c2);
-  o[0] = v[0] + q[0] * uv[0] + c2[0];
-  o[1] = v[1] + q[0] * uv[1] + c2[1];
-  o[2] = v[2] + q[0] * uv[2] + c2[2];
-}
-__device__ __forceinline__ void q_rot_conj(const double q[4], const double v[3], double o[3]) {
-  const double qc[4] = {q[0], -q[1], -q[2], -q[3]};
-  q_rot(qc, v, o);
-}
 // laserMapping.cpp:569-579: point in its LiDAR frame -> LiDAR-0 body frame b, IMU frame m, world g
 __device__ __forceinline__ void transform_point(const PassConst& pc, float px, float py, float pz, int lid,
                                                 double b[3], double m[3], double g[3]) {

@@ -12,6 +12,7 @@
 #include <limits>
 
 #include "malio_b200.h"
+#include "malio_se3.h"
 
 namespace malio_manifold {
 
@@ -21,8 +22,10 @@ inline Quat qload(const double* q) { return Quat{q[0], q[1], q[2], q[3]}; }
 inline void qstore(const Quat& q, double* o) { o[0] = q.w; o[1] = q.x; o[2] = q.y; o[3] = q.z; }
 inline Quat qconj(const Quat& q) { return Quat{q.w, -q.x, -q.y, -q.z}; }
 inline Quat qmul(const Quat& a, const Quat& b) {
-  return Quat{a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
-              a.w * b.y + a.y * b.w + a.z * b.x - a.x * b.z, a.w * b.z + a.z * b.w + a.x * b.y - a.y * b.x};
+  const double qa[4] = {a.w, a.x, a.y, a.z}, qb[4] = {b.w, b.x, b.y, b.z};
+  double o[4];
+  malio_se3::q_mul(qa, qb, o);
+  return qload(o);
 }
 struct M3 { double m[3][3]; };
 inline M3 hat3(const double v[3]) { return M3{{{0, -v[2], v[1]}, {v[2], 0, -v[0]}, {-v[1], v[0], 0}}}; }
@@ -33,10 +36,10 @@ inline M3 mul3(const M3& A, const M3& B) {
   return C;
 }
 inline M3 rotmat(const Quat& q) {
-  const double tx = 2 * q.x, ty = 2 * q.y, tz = 2 * q.z;
-  const double twx = tx * q.w, twy = ty * q.w, twz = tz * q.w, txx = tx * q.x, txy = ty * q.x, txz = tz * q.x;
-  const double tyy = ty * q.y, tyz = tz * q.y, tzz = tz * q.z;
-  return M3{{{1 - (tyy + tzz), txy - twz, txz + twy}, {txy + twz, 1 - (txx + tzz), tyz - twx}, {txz - twy, tyz + twx, 1 - (txx + tyy)}}};
+  const double qa[4] = {q.w, q.x, q.y, q.z};
+  double R[9];
+  malio_se3::q_to_R(qa, R);
+  return M3{{{R[0], R[1], R[2]}, {R[3], R[4], R[5]}, {R[6], R[7], R[8]}}};
 }
 
 constexpr double kTol = 1e-11;                    // MTK::tolerance<double>() (mtkmath.hpp:122)

@@ -1347,13 +1347,9 @@ PassConst make_pass_const(const malio_handle* h, const DeviceState* D, const mal
     std::memcpy(pc.ct[l], D->tcomp[l].t, sizeof(pc.ct[l]));
   }
   for (int l = 0; l <= MALIO_MAX_LIDAR; ++l) pc.table_off[l] = D->table_off[l];
-  auto conj_R = [](const double q[4], double R[9]) {   // Eigen's toRotationMatrix of the conjugate, row-major
-    const double w = q[0], x = -q[1], y = -q[2], z = -q[3];
-    const double tx = 2 * x, ty = 2 * y, tz = 2 * z;
-    const double twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
-    R[0] = 1 - (tyy + tzz); R[1] = txy - twz;       R[2] = txz + twy;
-    R[3] = txy + twz;       R[4] = 1 - (txx + tzz); R[5] = tyz - twx;
-    R[6] = txz - twy;       R[7] = tyz + twx;       R[8] = 1 - (txx + tyy);
+  auto conj_R = [](const double q[4], double R[9]) {   // the rotation matrix of the conjugate
+    const double qc[4] = {q[0], -q[1], -q[2], -q[3]};
+    malio_se3::q_to_R(qc, R);
   };
   conj_R(pc.rot, pc.RsT);
   for (int l = 0; l < MALIO_MAX_LIDAR; ++l) { conj_R(pc.eq[l], pc.ReT[l]); conj_R(pc.cq[l], pc.RcT[l]); }

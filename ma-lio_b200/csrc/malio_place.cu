@@ -523,17 +523,6 @@ int rank(malio_handle* h, DeviceState* D, const PlaceDb& P, const malio_pass_sta
   return MALIO_OK;
 }
 
-// Eigen's _transformVector, the device's q_rot, on the host
-void q_rot_host(const double q[4], const double v[3], double o[3]) {
-  const double qv[3] = {q[1], q[2], q[3]};
-  double uv[3] = {qv[1] * v[2] - qv[2] * v[1], qv[2] * v[0] - qv[0] * v[2], qv[0] * v[1] - qv[1] * v[0]};
-  uv[0] += uv[0]; uv[1] += uv[1]; uv[2] += uv[2];
-  const double c2[3] = {qv[1] * uv[2] - qv[2] * uv[1], qv[2] * uv[0] - qv[0] * uv[2], qv[0] * uv[1] - qv[1] * uv[0]};
-  o[0] = v[0] + q[0] * uv[0] + c2[0];
-  o[1] = v[1] + q[0] * uv[1] + c2[1];
-  o[2] = v[2] + q[0] * uv[2] + c2[2];
-}
-
 }  // namespace
 
 namespace malio_place {
@@ -634,15 +623,10 @@ int relocalize_global(malio_handle* h, const malio_pass_state* s, const malio_gl
     c.position = o.p; c.shift = o.shift; c.d1 = o.d1; c.d2 = o.d2; c.col[0] = o.i; c.col[1] = o.j; c.z_s = o.z_s;
     // the guess: rot = q_yaw(theta) (x) s.rot (malio_relocalize's product), the slot-0 origin at the position's sensor
     const double theta = 2.0 * M_PI * (double)o.shift / (double)S;
-    const double cth = std::cos(theta / 2.0), sth = std::sin(theta / 2.0);
-    const double w0 = s->rot[0], x0 = s->rot[1], y0 = s->rot[2], z0 = s->rot[3];
     malio_pass_state g = *s;
-    g.rot[0] = cth * w0 - sth * z0;
-    g.rot[1] = cth * x0 - sth * y0;
-    g.rot[2] = cth * y0 + sth * x0;
-    g.rot[3] = cth * z0 + sth * w0;
+    malio_se3::q_yaw_mul(theta, s->rot, g.rot);
     double e[3];
-    q_rot_host(g.rot, s->ext[0].t, e);
+    malio_se3::q_rot(g.rot, s->ext[0].t, e);
     const double target[3] = {((double)o.i + 0.5) * P->args.cell, ((double)o.j + 0.5) * P->args.cell, o.z_s};
     for (int i = 0; i < 3; ++i) g.pos[i] = target[i] - e[i];
     std::memcpy(c.guess_rot, g.rot, sizeof(c.guess_rot));

@@ -249,17 +249,9 @@ int search(malio_handle* h, DeviceState* D, const malio_pass_state* s, const mal
   cudaStream_t st = D->stream;
   const uint32_t n = D->N, n_yaw = a->n_yaw;
   const uint64_t wxy = 2ull * a->half_xy + 1, wz = 2ull * a->half_z + 1;
-  // the candidate rotations, q_yaw(theta_k) (x) s.rot, on the host with the C library's cos / sin (malio_b200.h, step 1)
+  // the candidate rotations, q_yaw(theta_k) (x) s.rot (malio_b200.h, step 1)
   std::vector<double> q(4 * (size_t)n_yaw);
-  const double w0 = s->rot[0], x0 = s->rot[1], y0 = s->rot[2], z0 = s->rot[3];
-  for (uint32_t k = 0; k < n_yaw; ++k) {
-    const double theta = a->yaw_lo + (double)k * a->yaw_step;
-    const double c = std::cos(theta / 2.0), sn = std::sin(theta / 2.0);
-    q[4 * (size_t)k + 0] = c * w0 - sn * z0;
-    q[4 * (size_t)k + 1] = c * x0 - sn * y0;
-    q[4 * (size_t)k + 2] = c * y0 + sn * x0;
-    q[4 * (size_t)k + 3] = c * z0 + sn * w0;
-  }
+  for (uint32_t k = 0; k < n_yaw; ++k) malio_se3::q_yaw_mul(a->yaw_lo + (double)k * a->yaw_step, s->rot, &q[4 * (size_t)k]);
   malio_reloc_report r{};   // written to *rep only on success
   r.n_candidates = (uint64_t)n_yaw * wxy * wxy * wz;
   uint64_t best = 0;
