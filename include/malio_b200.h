@@ -840,6 +840,93 @@ int malio_place_db_info(malio_handle* h, uint64_t* n_positions, uint64_t* device
 int malio_place_db_download(malio_handle* h, int32_t* cols, double* z_s, uint8_t* nibbles, uint16_t* ring_keys, uint64_t cap, uint64_t* n);
 int malio_relocalize_global(malio_handle* h, const malio_pass_state* s, const malio_global_args* a, malio_global_report* rep);
 
+/* ---- a 2-D occupancy grid for navigation: ground, obstacle band and free floor per cell ------------------------------------------
+ * malio_grid_build_device turns a point set into the raster a navigation stack loads (nav_msgs/OccupancyGrid values as u8;
+ * malio_write_grid_pgm writes it in the map_server PGM + YAML format).  The grid is a pure function of the points and the
+ * arguments: no ray casting, no session state.  Every step is a min, a count or a flag per cell, so thread order cannot change
+ * the result; tests/grid_ref.py restates each step.
+ *   1. Points: rows of 4 floats {x, y, z, w}, w ignored.  A row with a non-finite x, y or z is skipped (n_nonfinite).
+ *   2. Column of a point: fi = floorf(x * ir), fj = floorf(y * ir), ir = 1.0f / res in float (the voxel map's key rule in 2-D);
+ *      the comparisons below are made on these floats.
+ *   3. Region: cells i0 <= i < i0 + nx, j0 <= j < j0 + ny, and the ground half-width w (cells).  Only points whose column lies in
+ *      the padded region [i0 - w, i0 + nx + w) x [j0 - w, j0 + ny + w) take part (n_used; the others count in n_outside).
+ *   4. zmin(c): the smallest z of column c's points, in the order of the order-preserving u32 key of the float (-0.0 < +0.0).
+ *   5. ground(c): the minimum of zmin over the (2w+1)^2 columns around c (the same key order); NaN (0x7FC00000) when none of them
+ *      holds a point.
+ *   6. A point in region cell c with d = z - ground(c) (float32) is a band point when h_lo <= d <= h_hi, a floor point when
+ *      d < h_lo, and overhead (ignored: canopies, balconies) when d > h_hi.
+ *   7. Cell class: MALIO_GRID_OCCUPIED when the cell holds at least min_obstacle_points band points, else MALIO_GRID_FREE when it
+ *      holds a floor point, else MALIO_GRID_UNKNOWN (empty cells, and cells seen only from above).
+ * Outputs: d_cls, u8 ny x nx row-major, row r at cell row j0 + r; d_ground (may be NULL), float in the same layout: ground(c)
+ * per region cell, an elevation raster.  rep (may be NULL): points used, skipped as non-finite, outside the padded region, cells
+ * per class, and device_bytes, the call's peak scratch.
+ * Tiling: the pad is exactly w, so the grid of a region equals the same cells cut from the grid of any larger region.  A map
+ * too large for one raster is exported in tiles that stitch without seams.
+ * Sources (one body):
+ *   MALIO_GRID_POINTS     n rows at d_xyzi, device memory of the handle's device, 16-byte aligned (read as float4).
+ *   MALIO_GRID_VOXEL_MAP  the handle's voxel map in place: exactly the grid of what malio_world_voxel_download_kept_device(k)
+ *                         returns, or with k NULL of what malio_world_voxel_download_device returns (the same centroid bits and
+ *                         keep rule; no sort area is used).  d_xyzi and n are ignored.
+ *   MALIO_GRID_PRIOR      the loaded prior's points followed by its session layer (malio_prior_map_session_download).
+ * malio_grid_build: MALIO_GRID_POINTS with host arrays: xyzi (n x 4), cls and ground (may be NULL) in host memory; the points are
+ * staged through a pinned chunk and a device buffer of at most MALIO_GRID_CHUNK rows (read twice), counted in device_bytes with
+ * the device copies of the outputs.
+ * malio_grid_extent_device: ext = {imin, jmin, imax, jmax}, the column indices of the source's finite points (step 2, with res);
+ * {0, 0, -1, -1} when it has none.  The region i0 = imin, nx = imax - imin + 1 (likewise j) is "the whole map".
+ * Memory: scratch of 4 (nx + 2w)(ny + 2w) + 4 nx (ny + 2w) + 4 nx ny + 64 bytes (at most 12 B per padded cell: the column minima,
+ * the filter's half-way raster, the band count and floor bit per region cell, the report's counters); the caller's outputs are
+ * extra.  All scratch is allocated by the call and released before it returns: nothing stays on the handle, and
+ * malio_world_voxel_info / malio_prior_map_info report the same bytes before and after.  With a communicator attached each
+ * rank grids what its own handle holds; nothing is exchanged.
+ * Stream order (the _device calls): the device-memory contract of the other _device calls (block above malio_knn_device); the
+ * handle's stream waits on `stream` on entry and `stream` on the handle's after the last access to the caller's arrays; the call
+ * waits once, at its end, before its scratch goes back.
+ * Errors, each before anything is written:
+ *   MALIO_ERR_INVALID_ARG  NULL h, args or d_cls (cls), d_xyzi with n > 0 for MALIO_GRID_POINTS; an unknown source; res not
+ *                          finite and > 0; nx or ny == 0; h_lo, h_hi not finite or 0 < h_lo <= h_hi not holding;
+ *                          min_obstacle_points == 0; any of i0 - w, i0 + nx + w, j0 - w, j0 + ny + w beyond +-2^24 (exact as a
+ *                          float); the device-memory contract (host, managed, other-device or misaligned pointers)
+ *   MALIO_ERR_STATE        MALIO_GRID_VOXEL_MAP with an empty voxel map; MALIO_GRID_PRIOR before a malio_prior_map_load*
+ *   MALIO_ERR_CAPACITY     scratch above MALIO_GRID_MAX_BYTES (err names the bytes needed); 2^31 or more source rows;
+ *                          (extent) a finite point's column index beyond +-2^24
+ * malio_write_grid_pgm (host, no handle): cls (ny x nx, as above) as a binary P5 PGM, top row at the largest y, occupied -> 0,
+ * free -> 254, unknown -> 205 (map_saver's trinary values), and a YAML beside it: image (the PGM's base name), mode trinary,
+ * resolution res, origin [i0 * res, j0 * res, 0.0] (double products, printed to round-trip; the nominal corner of cell (i0, j0):
+ * cells are floorf(x * ir), so a point within a rounding of a cell face may lie in the neighbour), negate 0,
+ * occupied_thresh 0.65, free_thresh 0.196 (205 decodes as unknown under p = (255 - v) / 255, the ROS 1 and nav2 loaders' rule).
+ * MALIO_ERR_INVALID_ARG for a NULL argument, nx or ny == 0, res not finite and > 0, a class value other than 0 / 100 / 255, or a
+ * file that cannot be written; neither file is left behind on an error. */
+#define MALIO_GRID_POINTS 0
+#define MALIO_GRID_VOXEL_MAP 1
+#define MALIO_GRID_PRIOR 2
+#define MALIO_GRID_FREE 0
+#define MALIO_GRID_OCCUPIED 100
+#define MALIO_GRID_UNKNOWN 255
+#define MALIO_GRID_MAX_BYTES (16ull << 30)
+#define MALIO_GRID_MAX_BOUND 16777216
+#define MALIO_GRID_CHUNK (1u << 22)
+typedef struct malio_grid_args {
+  float res;                      /* cell edge, metres */
+  int32_t i0, j0;                 /* the region's first cell */
+  uint32_t nx, ny;                /* the region's cells along x and y */
+  uint32_t ground_halfwidth;      /* w, cells */
+  float h_lo, h_hi;               /* the obstacle band above the ground, metres */
+  uint32_t min_obstacle_points;   /* band points that make a cell occupied */
+} malio_grid_args;
+typedef struct malio_grid_report {
+  uint64_t n_used, n_nonfinite, n_outside;
+  uint64_t n_occupied, n_free, n_unknown;
+  uint64_t device_bytes;          /* peak scratch of the call, released before it returns */
+} malio_grid_report;
+int malio_grid_build_device(malio_handle* h, int source, const float* d_xyzi, uint64_t n, const malio_carve_keep* k,
+                            const malio_grid_args* args, uint8_t* d_cls, float* d_ground, void* stream, malio_grid_report* rep);
+int malio_grid_build(malio_handle* h, const float* xyzi, uint64_t n, const malio_grid_args* args, uint8_t* cls, float* ground,
+                     malio_grid_report* rep);
+int malio_grid_extent_device(malio_handle* h, int source, const float* d_xyzi, uint64_t n, const malio_carve_keep* k, float res,
+                             int32_t* ext, void* stream);
+int malio_write_grid_pgm(const char* pgm_path, const char* yaml_path, const uint8_t* cls, uint32_t nx, uint32_t ny, float res,
+                         int32_t i0, int32_t j0);
+
 /* Host: read a binary PCD file as this library (and pcl::PCDWriter::writeBinary) writes it into n x 4 floats {x, y, z, intensity}.
  * x y z must be fields of TYPE F, SIZE 4, COUNT 1; intensity (F 4) is optional (0 without it); every other field of fixed size
  * is skipped.  POINTS must equal WIDTH x HEIGHT and the file must hold POINTS records.  xyzi may be NULL with cap == 0 to ask the

@@ -7,6 +7,7 @@
 //   malio_preproc.cu  undistortion, voxel grid, world registration
 //   malio_mapops.cu   the device-resident map and its Add_Points / Delete_Point_Boxes replay
 //   malio_voxmap.cu   the saved map as a voxel map
+//   malio_grid.cu     a 2-D occupancy grid of a point set, the voxel map or the prior, for navigation
 //   malio_prior.cu    localization in a prior map: the prior's tile store and the local-map window over it
 //   malio_reloc.cu    relocalization in a loaded prior: branch-and-bound over yaws and a position lattice
 //   malio_place.cu    relocalization without a position guess: place descriptors of the prior, ranked, each checked by malio_reloc

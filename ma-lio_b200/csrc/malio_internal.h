@@ -125,7 +125,18 @@ namespace malio_prior {
 // the loaded prior's n points as float4 {x, y, z, normal_y} in tile order, device memory of the handle's device, valid until the
 // next load or clear (malio_reloc.cu reads them); MALIO_ERR_STATE before a load
 int points(const malio_handle* h, const float** xyzw, uint32_t* n);
+// the session layer's n points as float4 {x, y, z, normal_y} in session order, valid until the next extend, load or clear
+// (malio_grid.cu reads them); MALIO_ERR_STATE before a load
+int session(const malio_handle* h, const float** xyzw, uint32_t* n);
 }  // namespace malio_prior
+
+// malio_voxmap.cu — the voxel map's entries for malio_grid.cu, in entry order (not key order): n entries of float4 sums and u32
+// counts, and their (hit, miss) pairs as uint2, NULL for a map that was never carved.  Device memory of the handle's device,
+// valid until the next call that changes the map.  MALIO_ERR_STATE for an empty map.
+namespace malio_vox {
+struct Entries { const float* sum; const uint32_t* cnt; const uint32_t* hit_miss; uint64_t n; };
+int entries(const malio_handle* h, Entries* e);
+}  // namespace malio_vox
 
 // malio_reloc.cu — relocalization in a loaded prior (malio_relocalize after its NULL checks; malio_place.cu verifies with it)
 namespace malio_reloc {

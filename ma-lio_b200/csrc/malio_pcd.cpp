@@ -1,7 +1,9 @@
 // malio_pcd.cpp — the saved map's file format: pcl::PCDWriter::writeBinary for pcl::PointXYZINormal, the call that writes
 // pcl_wait_save every pcd_save_interval scans and at shutdown (laserMapping.cpp:484, :1090).  Host code; the header text and
 // the 32-byte record layout live only here, for malio_write_pcd_binary and malio_world_save_pcd alike.  malio_read_pcd reads
-// such a file back (and the other binary layouts PCL writes) for malio_prior_map_load.
+// such a file back (and the other binary layouts PCL writes) for malio_prior_map_load.  malio_write_grid_pgm writes the 2-D
+// occupancy grid (malio_grid.cu) as map_server's PGM + YAML pair.
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <sstream>
@@ -130,6 +132,48 @@ int parse_header(FILE* f, PcdLayout& L, std::string& err) {
 }
 
 }  // namespace
+
+// The occupancy grid in map_server's format: a binary PGM (map_saver's trinary values, the top row at the largest y) and the
+// YAML that names it.  Every value is checked before either file is opened; on any failure both are removed.
+extern "C" int malio_write_grid_pgm(const char* pgm_path, const char* yaml_path, const uint8_t* cls, uint32_t nx, uint32_t ny,
+                                    float res, int32_t i0, int32_t j0) {
+  if (!pgm_path || !yaml_path || !cls || nx == 0 || ny == 0 || !(res > 0.f) || !std::isfinite(res)) return MALIO_ERR_INVALID_ARG;
+  const uint64_t cells = (uint64_t)nx * ny;
+  for (uint64_t c = 0; c < cells; ++c)
+    if (cls[c] != MALIO_GRID_FREE && cls[c] != MALIO_GRID_OCCUPIED && cls[c] != MALIO_GRID_UNKNOWN) return MALIO_ERR_INVALID_ARG;
+  int rc = MALIO_OK;
+  if (FILE* f = std::fopen(pgm_path, "wb")) {
+    const std::string hdr = "P5\n" + std::to_string(nx) + " " + std::to_string(ny) + "\n255\n";
+    if (std::fwrite(hdr.data(), 1, hdr.size(), f) != hdr.size()) rc = MALIO_ERR_INVALID_ARG;
+    std::vector<uint8_t> row(nx);
+    for (uint32_t r = 0; r < ny && rc == MALIO_OK; ++r) {
+      const uint8_t* src = cls + (uint64_t)(ny - 1 - r) * nx;   // file row 0 is the region's last cell row (largest y)
+      for (uint32_t i = 0; i < nx; ++i)
+        row[i] = src[i] == MALIO_GRID_OCCUPIED ? 0 : (src[i] == MALIO_GRID_FREE ? 254 : 205);
+      if (std::fwrite(row.data(), 1, nx, f) != nx) rc = MALIO_ERR_INVALID_ARG;
+    }
+    if (std::fclose(f) != 0) rc = MALIO_ERR_INVALID_ARG;
+  } else {
+    return MALIO_ERR_INVALID_ARG;
+  }
+  if (rc == MALIO_OK) {
+    const char* slash = std::strrchr(pgm_path, '/');
+    char buf[512];
+    std::snprintf(buf, sizeof(buf),
+                  "resolution: %.9g\norigin: [%.17g, %.17g, 0.0]\nnegate: 0\noccupied_thresh: 0.65\nfree_thresh: 0.196\n",
+                  (double)res, (double)i0 * (double)res, (double)j0 * (double)res);
+    const std::string yaml = std::string("image: ") + (slash ? slash + 1 : pgm_path) + "\nmode: trinary\n" + buf;
+    if (FILE* f = std::fopen(yaml_path, "wb")) {
+      if (std::fwrite(yaml.data(), 1, yaml.size(), f) != yaml.size()) rc = MALIO_ERR_INVALID_ARG;
+      if (std::fclose(f) != 0) rc = MALIO_ERR_INVALID_ARG;
+      if (rc != MALIO_OK) std::remove(yaml_path);
+    } else {
+      rc = MALIO_ERR_INVALID_ARG;
+    }
+  }
+  if (rc != MALIO_OK) std::remove(pgm_path);
+  return rc;
+}
 
 extern "C" int malio_read_pcd(const char* path, float* xyzi, uint64_t cap, uint64_t* n_out) {
   if (!path || !n_out || (cap && !xyzi)) return MALIO_ERR_INVALID_ARG;

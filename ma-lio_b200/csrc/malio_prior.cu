@@ -739,6 +739,14 @@ int points(const malio_handle* h, const float** xyzw, uint32_t* n) {
   return MALIO_OK;
 }
 
+int session(const malio_handle* h, const float** xyzw, uint32_t* n) {
+  const PriorState* P = h->prior.get();
+  if (!P || !P->loaded) return MALIO_ERR_STATE;
+  *xyzw = reinterpret_cast<const float*>(P->d_sess.data());
+  *n = P->n_sess;
+  return MALIO_OK;
+}
+
 int info(malio_handle* h, uint64_t* n_points, uint32_t* n_tiles, uint64_t* device_bytes) {
   PriorState* P;
   DeviceState* D;

@@ -35,6 +35,7 @@
 #include <cuda/std/tuple>
 
 #include "malio_device.cuh"
+#include "malio_voxrule.cuh"
 
 using namespace malio_devstate;
 
@@ -292,9 +293,7 @@ __global__ void __launch_bounds__(256) vm_centroid_kernel(const uint32_t* __rest
   const uint32_t r = blockIdx.x * 256u + threadIdx.x;
   if (r >= n || r >= cap) return;
   const uint32_t e = order[r];
-  const float4 s = esum[e];
-  const float cf = (float)ecnt[e];
-  out[r] = make_float4(s.x / cf, s.y / cf, s.z / cf, s.w / cf);
+  out[r] = malio_voxrule::centroid(esum[e], ecnt[e]);
 }
 
 // ------------------------------------------------------------------ carving (malio_world_voxel_accumulate_carve)
@@ -370,12 +369,9 @@ __global__ void __launch_bounds__(256) vc_carve_kernel(VmSlots c, PassConst pc, 
   }
 }
 
-// (hit, miss) of entry e; zeros for a map that was never carved (hm NULL)
-__device__ __forceinline__ uint2 evidence(const uint2* hm, uint32_t e) { return hm ? hm[e] : make_uint2(0u, 0u); }
-// the keep rule (malio_carve_keep): a voxel is dropped when miss >= min_miss and (double)miss > ratio * (double)hit
-__device__ __forceinline__ bool dropped(uint2 v, uint32_t min_miss, double ratio) {
-  return v.y >= min_miss && (double)v.y > ratio * (double)v.x;
-}
+// the (hit, miss) of an entry and the keep rule, shared with malio_grid.cu
+using malio_voxrule::dropped;
+using malio_voxrule::evidence;
 
 // (hit, miss) of the r-th voxel in key order -> out[r], r < n
 __global__ void __launch_bounds__(256) vc_evidence_kernel(const uint32_t* __restrict__ order, uint32_t n, const uint2* __restrict__ hm,
@@ -944,6 +940,13 @@ int save_changes_pcd(malio_handle* h, const malio_carve_keep* keep, const char* 
   }
   if (int e = release_scratch(h, V, D)) return e;
   return rc;
+}
+
+int entries(const malio_handle* h, Entries* e) {
+  const VoxState* V = h->voxmap.get();
+  if (!V || V->n_vox == 0) return MALIO_ERR_STATE;
+  *e = Entries{reinterpret_cast<const float*>(V->d_esum.data()), V->d_ecnt.data(), reinterpret_cast<const uint32_t*>(V->d_hm.data()), V->n_vox};
+  return MALIO_OK;
 }
 
 int info(malio_handle* h, uint64_t* n_voxels, uint64_t* capacity, uint64_t* device_bytes) {

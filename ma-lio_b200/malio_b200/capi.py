@@ -179,6 +179,25 @@ class CarveKeep(C.Structure):
     _fields_ = [("min_miss", C.c_uint32), ("max_miss_per_hit", C.c_float)]
 
 
+GRID_POINTS, GRID_VOXEL_MAP, GRID_PRIOR = 0, 1, 2            # MALIO_GRID_* sources
+GRID_FREE, GRID_OCCUPIED, GRID_UNKNOWN = 0, 100, 255         # nav_msgs/OccupancyGrid values
+GRID_MAX_BYTES = 16 << 30
+GRID_MAX_BOUND = 1 << 24
+
+
+class GridArgs(C.Structure):
+    """malio_grid_args: cell edge, the region (first cell, cells along x and y), the ground half-width in cells, the obstacle
+    band above the ground (m) and the band points that make a cell occupied."""
+    _fields_ = [("res", C.c_float), ("i0", C.c_int32), ("j0", C.c_int32), ("nx", C.c_uint32), ("ny", C.c_uint32),
+                ("ground_halfwidth", C.c_uint32), ("h_lo", C.c_float), ("h_hi", C.c_float), ("min_obstacle_points", C.c_uint32)]
+
+
+class GridReport(C.Structure):
+    """malio_grid_report: points used / non-finite / outside the padded region, cells per class, peak scratch bytes."""
+    _fields_ = [("n_used", C.c_uint64), ("n_nonfinite", C.c_uint64), ("n_outside", C.c_uint64), ("n_occupied", C.c_uint64),
+                ("n_free", C.c_uint64), ("n_unknown", C.c_uint64), ("device_bytes", C.c_uint64)]
+
+
 class UpdateReport(C.Structure):
     _fields_ = [("passes", C.c_int32), ("searches", C.c_int32), ("converged_count", C.c_int32),
                 ("last_status", C.c_int32), ("n_eff_last", C.c_uint32), ("ms_device_total", C.c_float),
@@ -210,6 +229,7 @@ EXPORTS = [
     "malio_world_voxel_seed", "malio_world_voxel_seed_device", "malio_world_voxel_changes_device",
     "malio_world_voxel_save_changes_pcd",
     "malio_prior_map_extend", "malio_prior_map_session_download",
+    "malio_grid_build_device", "malio_grid_build", "malio_grid_extent_device", "malio_write_grid_pgm",
 ]
 
 
@@ -296,6 +316,10 @@ def load() -> C.CDLL:
     lib.malio_place_db_info.argtypes = [vp, vp, vp]
     lib.malio_place_db_download.argtypes = [vp, vp, vp, vp, vp, C.c_uint64, vp]
     lib.malio_relocalize_global.argtypes = [vp, vp, vp, vp]
+    lib.malio_grid_build_device.argtypes = [vp, i32, vp, C.c_uint64, vp, vp, vp, vp, vp, vp]
+    lib.malio_grid_build.argtypes = [vp, vp, C.c_uint64, vp, vp, vp, vp]
+    lib.malio_grid_extent_device.argtypes = [vp, i32, vp, C.c_uint64, vp, C.c_float, vp, vp]
+    lib.malio_write_grid_pgm.argtypes = [C.c_char_p, C.c_char_p, vp, u32, u32, C.c_float, C.c_int32, C.c_int32]
     lib.malio_measure.argtypes = [vp, C.POINTER(PassState), i32, vp, vp, C.POINTER(PassStats)]
     lib.malio_download_rows.argtypes = [vp, vp, vp, u32, C.POINTER(u32)]
     lib.malio_download_aux.argtypes = [vp, vp, vp, vp, vp, vp]

@@ -135,6 +135,16 @@ KEEP_MAX_MISS_PER_HIT = 2.0
 # The hits a seeded voxel starts with (malio_world_voxel_seed), chosen with tests/world_seed_ref.py on the two-session street
 # scene (DESIGN.md, "Keeping a saved map current").
 SEED_HITS = 2
+# Defaults of the occupancy grid (malio_grid_build_device), chosen with tests/grid_ref.py on the carved street and the sloped
+# scene of tests/test_grid_cpu.py (DESIGN.md, "A 2-D occupancy grid for navigation"): 0.1 m cells, the ground taken over
+# +-1 m around a cell, an obstacle band 0.3-2.0 m above it, one band point for an obstacle (a voxel map holds one centroid per
+# voxel, so a box's roof gives one band point per column).
+GRID_RES = 0.1
+GRID_GROUND_HALFWIDTH = 10
+GRID_H_LO = 0.3
+GRID_H_HI = 2.0
+GRID_MIN_OBSTACLE_POINTS = 1
+GRID_SOURCES = {"points": capi.GRID_POINTS, "voxel_map": capi.GRID_VOXEL_MAP, "prior": capi.GRID_PRIOR}
 
 
 def carve_args(max_range: float = CARVE_MAX_RANGE, end_margin: float = CARVE_END_MARGIN) -> capi.CarveArgs:
@@ -165,6 +175,34 @@ def _as_keep(keep) -> capi.CarveKeep | None:
     if keep is True:
         return carve_keep()
     return keep if isinstance(keep, capi.CarveKeep) else carve_keep(**keep)
+
+
+def grid_args(res: float = GRID_RES, i0: int = 0, j0: int = 0, nx: int = 0, ny: int = 0, ground_halfwidth: int = GRID_GROUND_HALFWIDTH,
+              h_lo: float = GRID_H_LO, h_hi: float = GRID_H_HI, min_obstacle_points: int = GRID_MIN_OBSTACLE_POINTS) -> capi.GridArgs:
+    """malio_grid_args with the library's defaults; the region (i0, j0, nx, ny) in cells of res (nx = ny = 0: to be filled, e.g.
+    by MeasurementModel.grid from the source's extent)."""
+    a = capi.GridArgs()
+    a.res, a.i0, a.j0, a.nx, a.ny = float(res), int(i0), int(j0), int(nx), int(ny)
+    a.ground_halfwidth, a.h_lo, a.h_hi, a.min_obstacle_points = int(ground_halfwidth), float(h_lo), float(h_hi), int(min_obstacle_points)
+    return a
+
+
+def save_grid(stem: str, cls, args: capi.GridArgs):
+    """Write <stem>.pgm and <stem>.yaml, the map_server pair navigation stacks load, from a class raster (ny, nx) u8 (numpy or a
+    tensor) of the region in args (malio_write_grid_pgm, host code).  Returns the two paths."""
+    c = np.ascontiguousarray(cls.cpu().numpy() if hasattr(cls, "cpu") else cls, np.uint8)
+    if c.ndim != 2 or c.shape != (args.ny, args.nx):
+        raise ValueError(f"cls: shape {c.shape}, expected ({args.ny}, {args.nx})")
+    pgm, yaml = stem + ".pgm", stem + ".yaml"
+    rc = capi.load().malio_write_grid_pgm(os.fsencode(pgm), os.fsencode(yaml), capi.ptr(c), args.nx, args.ny, C.c_float(args.res),
+                                          args.i0, args.j0)
+    if rc != capi.OK:
+        raise capi.MalioError(rc, f"malio_write_grid_pgm({pgm!r}, {yaml!r})")
+    return pgm, yaml
+
+
+def _grid_report(r: capi.GridReport) -> dict:
+    return {f: int(getattr(r, f)) for f, _ in capi.GridReport._fields_}
 
 
 class PcdSaver:
@@ -564,6 +602,61 @@ class MeasurementModel:
         v, c, b = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
         self._check(self.lib.malio_world_voxel_info(self._h, C.byref(v), C.byref(c), C.byref(b)))
         return dict(n_voxels=int(v.value), capacity=int(c.value), device_bytes=int(b.value))
+
+    # ---- a 2-D occupancy grid for navigation (malio_grid_*)
+    def _grid_source(self, source, xyzi, keep):
+        """(source code, device pointer, rows, CarveKeep or None, the current stream) of grid / grid_extent's arguments."""
+        import torch
+        if source not in GRID_SOURCES:
+            raise ValueError(f"source: {source!r}, expected one of {sorted(GRID_SOURCES)}")
+        src = GRID_SOURCES[source]
+        if (xyzi is not None) != (src == capi.GRID_POINTS):
+            raise ValueError("xyzi is the 'points' source's input and only its")
+        if keep is not None and src != capi.GRID_VOXEL_MAP:
+            raise ValueError("keep applies to the 'voxel_map' source only")
+        if xyzi is not None:
+            _check_tensor(xyzi, "xyzi", torch.float32, 4, self.device)
+        k = _as_keep(keep)
+        return src, _dptr(xyzi), 0 if xyzi is None else xyzi.shape[0], k, torch.cuda.current_stream(self.device)
+
+    def grid_extent(self, source: str = "voxel_map", xyzi=None, keep=None, res: float = GRID_RES) -> tuple:
+        """(imin, jmin, imax, jmax): the column indices floorf(x / res) of the source's finite points ((0, 0, -1, -1) when there are
+        none).  source: "points" (xyzi a float32 CUDA tensor (n, 4)), "voxel_map" (keep as voxel_map_tensor's) or "prior"."""
+        src, p, n, k, st = self._grid_source(source, xyzi, keep)
+        ext = np.zeros(4, np.int32)
+        self._check(self.lib.malio_grid_extent_device(self._h, src, p, n, None if k is None else C.byref(k), C.c_float(res),
+                                                      capi.ptr(ext), st.cuda_stream))
+        return tuple(int(v) for v in ext)
+
+    def grid(self, source: str = "voxel_map", xyzi=None, keep=None, args: capi.GridArgs | None = None):
+        """The occupancy grid of a source on the device: (cls, ground, report).  cls uint8 (ny, nx) (GRID_FREE / GRID_OCCUPIED /
+        GRID_UNKNOWN, row r at cell row j0 + r), ground float32 (ny, nx) (NaN where no point lies within the ground window), both
+        CUDA tensors on the current stream; report a dict of malio_grid_report.  source and keep as grid_extent's; args from
+        grid_args, or None for the defaults over the whole extent of the source (with nx or ny 0 the extent fills the region)."""
+        import torch
+        src, p, n, k, st = self._grid_source(source, xyzi, keep)
+        a = grid_args() if args is None else args
+        if a.nx == 0 or a.ny == 0:
+            lo_i, lo_j, hi_i, hi_j = self.grid_extent(source, xyzi, keep, a.res)
+            if hi_i < lo_i:
+                raise ValueError("the source has no finite point: give the region in args")
+            a = grid_args(a.res, lo_i, lo_j, hi_i - lo_i + 1, hi_j - lo_j + 1, a.ground_halfwidth, a.h_lo, a.h_hi, a.min_obstacle_points)
+        cls, ground = self._empty((a.ny, a.nx), torch.uint8), self._empty((a.ny, a.nx), torch.float32)
+        rep = capi.GridReport()
+        self._check(self.lib.malio_grid_build_device(self._h, src, p, n, None if k is None else C.byref(k), C.byref(a), _dptr(cls),
+                                                     _dptr(ground), st.cuda_stream, C.byref(rep)))
+        r = _grid_report(rep)
+        r["args"] = a
+        return cls, ground, r
+
+    def grid_host(self, xyzi, args: capi.GridArgs, want_ground: bool = True):
+        """malio_grid_build: the grid of host points (float32 (n, 4)) into numpy arrays (cls, ground or None, report)."""
+        x = self._f32(xyzi, 4)
+        cls = np.empty((args.ny, args.nx), np.uint8)
+        ground = np.empty((args.ny, args.nx), np.float32) if want_ground else None
+        rep = capi.GridReport()
+        self._check(self.lib.malio_grid_build(self._h, capi.ptr(x), x.shape[0], C.byref(args), capi.ptr(cls), capi.ptr(ground), C.byref(rep)))
+        return cls, ground, _grid_report(rep)
 
     # ---- localization in a saved map (malio_prior_map_*): the prior on the device and lasermap_fov_segment's window over it
     def prior_map_load(self, xyz, normal_y=0.001, ids=None):
