@@ -511,6 +511,69 @@ int malio_world_voxel_changes_device(malio_handle* h, const malio_carve_keep* k,
                                      float* d_added, uint64_t cap_added, uint64_t* n_added, void* stream);
 int malio_world_voxel_save_changes_pcd(malio_handle* h, const malio_carve_keep* k, const char* removed_path,
                                        const char* added_path, uint64_t* n_removed, uint64_t* n_added);
+/* Rebuilding the voxel map from a corrected trajectory: keep the session's dense scans on the device, then fold them again under
+ * other states (a pose graph's, a GNSS/INS fusion's, ground truth), another leaf or other carve settings.
+ * tests/scan_store_ref.py restates the rebuild as a loop over the accumulate restatements.
+ * The scan store (per handle, independent of the voxel map: a clearing save does not touch it) holds per stored scan
+ *   points   the dense rows malio_world_accumulate registers: slots 0..L-1 in slot order, each in its buffer order (point 0 and
+ *            the untouched points included), as x, y, z in the LiDAR frame with their bits unchanged, 12 B per point.  The points
+ *            live in device blocks of MALIO_STORE_BLOCK_POINTS points; a scan never crosses a block, a larger scan gets a block
+ *            of its own.  Growing allocates a new block and copies nothing: a failed allocation returns MALIO_ERR_CUDA with the
+ *            store unchanged.
+ *   record   malio_stored_scan on the host: the caller's time stamp as given, the state, the temporal compensation of the last
+ *            malio_upload_scan* (identity before the first), slot_tag and the point count per slot (0 beyond L).
+ * malio_scan_store_add stores the current dense cloud with state s: the preconditions and errors of malio_world_accumulate
+ * (MALIO_ERR_STATE until malio_undistort* has run on every slot 0..L-1, slot_tag required), MALIO_ERR_CAPACITY above 2^31 - 1
+ * points.  The rows are copied device to device on the handle's stream; the call returns after enqueueing (it waits only
+ * when it allocates a block) and changes nothing any other call returns.  n_scans (may be NULL) = the stored scans.
+ * malio_scan_store_put appends a record and its n x 3 host points (n = the sum of rec->n_points): how a store is loaded back
+ * from a file.  MALIO_ERR_INVALID_ARG when n_points is not 0 beyond L or n is above 2^31 - 1.
+ * malio_scan_store_get: record k (rec may be NULL) and, with xyz != NULL, its points into xyz (cap points); *n_out = its
+ * point count; cap below it returns MALIO_ERR_CAPACITY with nothing read.  MALIO_ERR_INVALID_ARG for k beyond the store.
+ * malio_scan_store_register_device: stored scan k registered with s (NULL: its stored state) and its stored temporal
+ * compensation, as n x 4 floats {x, y, z, slot_tag}: the bits malio_world_register(.., MALIO_WORLD_DENSE, ..) gave for that
+ * scan (rot = identity, pos = 0 gives the scan in the body frame).  The size protocol and device-memory contract of
+ * malio_world_register_device (d_out == NULL and cap == 0 asks the size, 16-byte alignment, ordered on `stream`, returns after
+ * enqueueing).
+ * malio_scan_store_info: stored scans, stored points and the device bytes of the blocks (any may be NULL).
+ * malio_scan_store_clear releases every block and record.
+ * With a communicator attached each rank stores what it holds, as malio_world_voxel_accumulate folds it.
+ *
+ * malio_world_voxel_rebuild is the sequence malio_world_voxel_accumulate(_carve)(states[k - first] or, with states == NULL, the
+ * stored state; the stored slot_tag; leaf; carve) for k = first .. first + count - 1 in index order, each scan with its stored
+ * points and stored temporal compensation.  After it the centroids, the evidence, n_voxels, the leaf and the carve scan count
+ * are exactly what that sequence leaves; the entry capacity and device_bytes may differ (the table grows per chunk, not per
+ * scan).  It works on any map those calls accept: a cleared map gives a fresh one, a seeded map carved by the corrected
+ * session is malio_world_voxel_seed followed by a carved rebuild.  n_seeded is not touched; count == 0 changes nothing.
+ * Plain: the rows of whole scans of one block are folded in chunks of at most MALIO_SEED_CHUNK rows (a larger scan alone),
+ * one fold per chunk; the stable sort keeps (scan, slot, point) order, so each voxel's sums continue point by point as the
+ * per-scan calls continue them.  Carved: one scan at a time (hit and miss are per-scan sets), enqueued back to back.  Either
+ * way the call waits once, at its end; growing the table drains the handle's stream first.
+ * Refusals, each before anything changes (centroids, counters, entry count and leaf stay as they were):
+ *   MALIO_ERR_INVALID_ARG  NULL h; first + count beyond the store; the leaf errors of malio_world_voxel_accumulate; the argument
+ *                          errors of malio_world_voxel_accumulate_carve
+ *   MALIO_ERR_CAPACITY     the max_range cap; any row's voxel index outside int under its scan's state, or with carve any
+ *                          origin of a slot with points.  The one difference from the sequence, which would have folded the
+ *                          scans before the faulty one: every row of the range is checked in a key-only pass first.
+ * Device memory: the rebuild's scratch is that of one chunk (48 B per row) plus about 1 KB per scan of the range, released
+ * before the call returns; a carved rebuild adds 20 B per row of its largest scan. */
+#define MALIO_STORE_BLOCK_POINTS (1u << 24)
+typedef struct malio_stored_scan {
+  double time;                                      /* the caller's stamp, as given */
+  malio_pass_state state;                           /* the state it was stored with */
+  malio_rigid temporal_comp[MALIO_MAX_LIDAR - 1];   /* LiDAR l >= 1 at l - 1 */
+  float slot_tag[MALIO_MAX_LIDAR];
+  uint32_t n_points[MALIO_MAX_LIDAR];               /* 0 beyond L */
+} malio_stored_scan;
+int malio_scan_store_add(malio_handle* h, const malio_pass_state* s, const float* slot_tag, double time, uint64_t* n_scans);
+int malio_scan_store_put(malio_handle* h, const malio_stored_scan* rec, const float* xyz, uint64_t* n_scans);
+int malio_scan_store_get(malio_handle* h, uint64_t k, malio_stored_scan* rec, float* xyz, uint64_t cap, uint64_t* n_out);
+int malio_scan_store_register_device(malio_handle* h, uint64_t k, const malio_pass_state* s, float* d_out, uint64_t cap,
+                                     uint64_t* n_out, void* stream);
+int malio_scan_store_info(malio_handle* h, uint64_t* n_scans, uint64_t* n_points, uint64_t* device_bytes);
+int malio_scan_store_clear(malio_handle* h);
+int malio_world_voxel_rebuild(malio_handle* h, uint64_t first, uint64_t count, const malio_pass_state* states, float leaf,
+                              const malio_carve_args* carve, uint64_t* n_voxels);
 /* Host: the same PCD file from n > 0 host points (n x 4 floats {x, y, z, intensity}): the header of PCDWriter::writeBinary for
  * PointXYZINormal (FIELDS x y z intensity normal_x normal_y normal_z curvature, WIDTH = POINTS = n, HEIGHT 1, DATA binary) and
  * n packed 32-byte records with normal_x/y/z = curvature = 0.  MALIO_ERR_INVALID_ARG for n == 0, a NULL argument or a file

@@ -236,6 +236,7 @@ void destroy(malio_handle* h) {
   h->deferred = nullptr;
   release(h->pre, D->stream);
   release(h->voxmap, D->stream);
+  release(h->store, D->stream);
   release(h->place, D->stream);
   release(h->prior, D->stream);
   release(h->mapst, D->stream);

@@ -6,7 +6,8 @@
 //   malio_b200.cu     handle lifecycle and per-scan data movement (create / destroy, scan upload, downloads)
 //   malio_preproc.cu  undistortion, voxel grid, world registration
 //   malio_mapops.cu   the device-resident map and its Add_Points / Delete_Point_Boxes replay
-//   malio_voxmap.cu   the saved map as a voxel map
+//   malio_voxmap.cu   the saved map as a voxel map, and its rebuild from the stored scans
+//   malio_store.cu    the session's dense scans kept on the device (the rows a rebuild folds again)
 //   malio_grid.cu     a 2-D occupancy grid of a point set, the voxel map or the prior, for navigation
 //   malio_prior.cu    localization in a prior map: the prior's tile store and the local-map window over it
 //   malio_reloc.cu    relocalization in a loaded prior: branch-and-bound over yaws and a position lattice
@@ -265,6 +266,8 @@ int caller_enter(malio_handle* h, DeviceState* D, cudaStream_t caller);
 int caller_leave(malio_handle* h, DeviceState* D, cudaStream_t caller);
 // malio_pass.cu
 PassConst make_pass_const(const malio_handle* h, const DeviceState* D, const malio_pass_state* s);
+// the same with the temporal compensation given: tcomp[l] for LiDAR l (entry 0 unused), as D->tcomp holds it
+PassConst make_pass_const(const malio_handle* h, const DeviceState* D, const malio_pass_state* s, const malio_rigid* tcomp);
 int pass_init(malio_handle* h, DeviceState* D);   // part of create(): per-block result slots, pass_kernel launch limits
 void comm_destroy(DeviceState* D);
 

@@ -27,6 +27,7 @@ namespace malio_map { struct MapOps; }             // malio_mapops.cu
 namespace malio_vox { struct VoxState; }           // malio_voxmap.cu
 namespace malio_prior { struct PriorState; }       // malio_prior.cu
 namespace malio_place { struct PlaceDb; }          // malio_place.cu
+namespace malio_store { struct StoreState; }       // malio_store.cu
 
 // The owner of one state of a handle.  malio_host.cpp deletes the handle without seeing the state types, so the owner keeps
 // the deleter of the unit that created the state.  Feature states are created by malio_buf::acquire and freed by
@@ -46,6 +47,7 @@ struct malio_handle {
   malio_owner<malio_vox::VoxState> voxmap;   // the saved map as a voxel map
   malio_owner<malio_prior::PriorState> prior;   // localization in a prior map
   malio_owner<malio_place::PlaceDb> place;   // place descriptors of the prior
+  malio_owner<malio_store::StoreState> store;   // the session's dense scans, kept for a rebuild of the voxel map
   // counts malio_map::build_from / leave calls: a prior-map window is the device map only while no other call rebuilt or left it
   uint64_t map_epoch = 0;
   // set while a call that returned after enqueueing (malio_knn_device) still has device-side results to hand over: its
@@ -137,6 +139,15 @@ namespace malio_vox {
 struct Entries { const float* sum; const uint32_t* cnt; const uint32_t* hit_miss; uint64_t n; };
 int entries(const malio_handle* h, Entries* e);
 }  // namespace malio_vox
+
+// malio_store.cu — the stored scans for malio_voxmap.cu's rebuild: scan k's record and its n_points[0] + .. rows of {x, y, z}
+// floats in device memory (NULL when it has no point), valid until the next put, add or clear; `block` numbers the device
+// block that holds them.  count() is 0 for a handle that never stored a scan.
+namespace malio_store {
+struct View { const malio_stored_scan* rec; const float* xyz; uint64_t rows; uint32_t block; };
+uint64_t count(const malio_handle* h);
+View view(const malio_handle* h, uint64_t k);
+}  // namespace malio_store
 
 // malio_reloc.cu — relocalization in a loaded prior (malio_relocalize after its NULL checks; malio_place.cu verifies with it)
 namespace malio_reloc {

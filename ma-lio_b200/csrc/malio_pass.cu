@@ -1337,14 +1337,18 @@ int pass_epilogue(malio_handle* h, DeviceState* D, int redo_knn, bool sorted_now
 namespace malio_devstate {
 
 PassConst make_pass_const(const malio_handle* h, const DeviceState* D, const malio_pass_state* s) {
+  return make_pass_const(h, D, s, D->tcomp);
+}
+
+PassConst make_pass_const(const malio_handle* h, const DeviceState* D, const malio_pass_state* s, const malio_rigid* tcomp) {
   PassConst pc{};
   std::memcpy(pc.rot, s->rot, sizeof(pc.rot));
   std::memcpy(pc.pos, s->pos, sizeof(pc.pos));
   for (int l = 0; l < MALIO_MAX_LIDAR; ++l) {
     std::memcpy(pc.eq[l], s->ext[l].q, sizeof(pc.eq[l]));
     std::memcpy(pc.et[l], s->ext[l].t, sizeof(pc.et[l]));
-    std::memcpy(pc.cq[l], D->tcomp[l].q, sizeof(pc.cq[l]));
-    std::memcpy(pc.ct[l], D->tcomp[l].t, sizeof(pc.ct[l]));
+    std::memcpy(pc.cq[l], tcomp[l].q, sizeof(pc.cq[l]));
+    std::memcpy(pc.ct[l], tcomp[l].t, sizeof(pc.ct[l]));
   }
   for (int l = 0; l <= MALIO_MAX_LIDAR; ++l) pc.table_off[l] = D->table_off[l];
   auto conj_R = [](const double q[4], double R[9]) {   // the rotation matrix of the conjugate

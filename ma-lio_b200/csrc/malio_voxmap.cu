@@ -29,6 +29,7 @@
 #include <cmath>
 #include <cstring>
 #include <string>
+#include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -162,6 +163,35 @@ struct ScanRows {
 struct SeedRows {
   const float4* xyzi;
   __device__ __forceinline__ float4 point(uint32_t p) const { return __ldg(xyzi + p); }
+};
+// Stored scans (malio_world_voxel_rebuild): a chunk of whole scans of one store block, rows in (scan, slot, point) order as
+// {x, y, z} in the LiDAR frame.  Row p belongs to the last scan whose first row is <= p (a binary search; an empty scan shares
+// its first row with the next one and is never the last such scan) and is registered with that scan's PassConst through
+// body_to_world: the bits of ScanRows for the same scan.  The scan table is in device memory.
+struct StoreScan {
+  PassConst pc;                          // the scan's state and its stored temporal compensation
+  uint32_t first[MALIO_MAX_LIDAR + 1];   // its slots' first rows in the chunk; first[L] = the next scan's first row
+  float tag[MALIO_MAX_LIDAR];
+};
+struct StoreRows {
+  const float* xyz;                      // the chunk's first row
+  const StoreScan* scan;                 // the chunk's scans in index order
+  uint32_t n_scans;
+  int L;
+  __device__ __forceinline__ float4 point(uint32_t p) const {
+    uint32_t lo = 0, hi = n_scans;
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) / 2;
+      if (scan[mid].first[0] <= p) lo = mid; else hi = mid;
+    }
+    const StoreScan& s = scan[lo];
+    int l = 0;
+    while (l + 1 < L && p >= s.first[l + 1]) ++l;
+    const float* r = xyz + 3 * (size_t)p;
+    float w[3];
+    body_to_world(s.pc, l, r[0], r[1], r[2], w);
+    return make_float4(w[0], w[1], w[2], s.tag[l]);
+  }
 };
 
 __device__ __forceinline__ uint64_t vhash(const VKey& a) {
@@ -422,6 +452,17 @@ __global__ void __launch_bounds__(256) vs_change_kernel(const uint32_t* __restri
   added[r] = (!seeded && kept) ? 1u : 0u;
 }
 
+// ------------------------------------------------------------------ rebuilding from the stored scans (malio_world_voxel_rebuild)
+// a carved rebuild's scan: its 12-byte stored rows -> the 20-byte rows of an undistorted cloud (x, y, z; the other two words
+// are not read), which ScanRows and the carve kernels take as they take a live scan's
+__global__ void __launch_bounds__(256) vr_unpack_kernel(const float* __restrict__ xyz, uint32_t n, float* __restrict__ ud) {
+  const uint32_t p = blockIdx.x * 256u + threadIdx.x;
+  if (p >= n) return;
+  const float* r = xyz + 3 * (size_t)p;
+  float* o = ud + 5 * (size_t)p;
+  o[0] = r[0]; o[1] = r[1]; o[2] = r[2];
+}
+
 // CUB's calls on d_temp, reserved by grow_sort, grow_runs and enqueue_select_order.  The stable sort of n rows of b by key:
 auto sort_call(SortBufs& b, uint64_t n, cudaStream_t st) {
   return [&b, n, st](void* t, size_t& c) { return cub::DeviceRadixSort::SortPairs(t, c, b.k, b.v, (int)n, VKeyDecomposer{}, st); };
@@ -654,6 +695,44 @@ int check_leaf(malio_handle* h, const VoxState* V, float leaf) {
   return MALIO_OK;
 }
 
+// the argument refusals of an accumulate (carve NULL) or a carved accumulate, in their order: carve arguments, leaf, range cap
+int check_fold_args(malio_handle* h, const VoxState* V, float leaf, const malio_carve_args* carve) {
+  if (carve && !(std::isfinite(carve->max_range) && carve->max_range > 0.f && std::isfinite(carve->end_margin) && carve->end_margin >= 0.f)) {
+    h->err = "world voxel carve: max_range must be finite and > 0, end_margin finite and >= 0";
+    return MALIO_ERR_INVALID_ARG;
+  }
+  if (int rc = check_leaf(h, V, leaf)) return rc;
+  if (carve && (double)carve->max_range * (double)(1.0f / leaf) > MALIO_CARVE_MAX_RANGE_CELLS) {
+    h->err = "world voxel carve: max_range / leaf above MALIO_CARVE_MAX_RANGE_CELLS; the map is unchanged";
+    return MALIO_ERR_CAPACITY;
+  }
+  return MALIO_OK;
+}
+
+// enqueue the fold of one scan's nn > 0 dense rows on the handle's stream (table, sort area, run scratch and, with carve, the
+// evidence already grown; small[0] is the fault flag the caller cleared): with carve, the origins' check first and the
+// scan's hits and passes (carve scan number `scan`) after the fold
+int enqueue_scan(malio_handle* h, VoxState* V, DeviceState* D, const ScanRows& src, float il, uint32_t nn, const malio_carve_args* carve,
+                 uint32_t scan) {
+  cudaStream_t st = D->stream;
+  const uint32_t g = (nn + 255) / 256;
+  if (carve) vc_origin_kernel<<<1, 32, 0, st>>>(src.c, src.pc, il, V->d_small);
+  if (int rc = enqueue_fold(h, V, D, src, il, nn)) return rc;
+  if (carve) vc_hit_kernel<<<g, 256, 0, st>>>(V->d_small, V->d_rent, V->d_head, nn, V->d_hm, V->d_stamp, scan);
+  vm_count_kernel<<<1, 1, 0, st>>>(V->d_head, V->d_new, V->d_small);
+  if (carve)
+    vc_carve_kernel<<<g, 256, 0, st>>>(src.c, src.pc, il, nn, (double)carve->max_range, (double)carve->end_margin, V->d_small,
+                                       V->d_hash, V->d_hash.size() - 1, V->d_ekey, V->d_hm, V->d_stamp, scan);
+  CUDA_TRY(cudaGetLastError());
+  D->ctr.kernel_launches += carve ? 4 : 1;
+  return MALIO_OK;
+}
+
+// the table holds room for `need` entries with the hash at most half full (grow_table would change nothing)
+bool table_fits(const VoxState* V, uint64_t need) {
+  return V->d_hash && need <= V->d_ekey.size() && 2 * need <= V->d_hash.size();
+}
+
 }  // namespace
 
 namespace malio_vox {
@@ -664,15 +743,7 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
   VoxState* V;
   DeviceState* D;
   if (int rc = acquire(h, h->voxmap, V, D)) return rc;
-  if (carve && !(std::isfinite(carve->max_range) && carve->max_range > 0.f && std::isfinite(carve->end_margin) && carve->end_margin >= 0.f)) {
-    h->err = "world voxel carve: max_range must be finite and > 0, end_margin finite and >= 0";
-    return MALIO_ERR_INVALID_ARG;
-  }
-  if (int rc = check_leaf(h, V, leaf)) return rc;
-  if (carve && (double)carve->max_range * (double)(1.0f / leaf) > MALIO_CARVE_MAX_RANGE_CELLS) {
-    h->err = "world voxel carve: max_range / leaf above MALIO_CARVE_MAX_RANGE_CELLS; the map is unchanged";
-    return MALIO_ERR_CAPACITY;
-  }
+  if (int rc = check_fold_args(h, V, leaf, carve)) return rc;
   VmSlots c{};
   uint32_t m[MALIO_MAX_LIDAR] = {0, 0, 0};
   if (int rc = malio_pre::world_dense_source(h, c.ud, m)) return rc;
@@ -689,18 +760,8 @@ int accumulate(malio_handle* h, const malio_pass_state* s, const float* slot_tag
     if (carve) { if (int rc = ensure_evidence(h, V, D)) return rc; }   // the first carve: every entry so far at hit = miss = 0
     cudaStream_t st = D->stream;
     const ScanRows src{c, make_pass_const(h, D, s)};
-    const float il = 1.0f / leaf;
-    const uint32_t nn = (uint32_t)n, g = (nn + 255) / 256;
     CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 2 * sizeof(uint32_t), st));   // fault flag, run count
-    if (carve) vc_origin_kernel<<<1, 32, 0, st>>>(c, src.pc, il, V->d_small);
-    if (int rc = enqueue_fold(h, V, D, src, il, nn)) return rc;
-    if (carve) vc_hit_kernel<<<g, 256, 0, st>>>(V->d_small, V->d_rent, V->d_head, nn, V->d_hm, V->d_stamp, scan);
-    vm_count_kernel<<<1, 1, 0, st>>>(V->d_head, V->d_new, V->d_small);
-    if (carve)
-      vc_carve_kernel<<<g, 256, 0, st>>>(c, src.pc, il, nn, (double)carve->max_range, (double)carve->end_margin, V->d_small,
-                                         V->d_hash, V->d_hash.size() - 1, V->d_ekey, V->d_hm, V->d_stamp, scan);
-    CUDA_TRY(cudaGetLastError());
-    D->ctr.kernel_launches += carve ? 4 : 1;
+    if (int rc = enqueue_scan(h, V, D, src, 1.0f / leaf, (uint32_t)n, carve, scan)) return rc;
     CUDA_TRY(cudaMemcpyAsync(V->h_small, V->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));   // the call's one wait: the fault flag and the entry count
     if (V->h_small[0]) {
@@ -883,6 +944,131 @@ int seed(malio_handle* h, const float* xyzi, uint64_t n, float leaf, uint32_t se
   return MALIO_OK;
 }
 
+// malio_world_voxel_rebuild (malio_b200.h): the stored scans [first, first + count) through the accumulate pipeline.
+//   1. a StoreScan per scan (its PassConst from the given or stored state and its stored compensation), grouped into chunks:
+//      plain, consecutive scans of one block up to MALIO_SEED_CHUNK rows (a larger scan alone); carved, one scan per chunk
+//   2. the check: vm_key_kernel over every chunk (and vc_origin_kernel per carved scan) raises small[0] for a row or an origin
+//      outside int; every kernel after it then writes nothing, so a refused rebuild leaves the map as it was
+//   3. per chunk, enqueued back to back: plain, one enqueue_fold with StoreRows and vm_count_kernel; carved, the scan's rows
+//      unpacked to 20-byte rows and accumulate's own sequence (enqueue_scan) with carve scan number carve_scan + 1 + i
+//   The table grows per chunk for an upper bound of the entries (the rows enqueued so far); only when that bound does not fit
+//   does the call wait for the exact count first.  One wait at the end for the verdict and the count.
+int rebuild(malio_handle* h, uint64_t first, uint64_t count, const malio_pass_state* states, float leaf, const malio_carve_args* carve,
+            uint64_t* n_voxels) {
+  VoxState* V;
+  DeviceState* D;
+  if (int rc = acquire(h, h->voxmap, V, D)) return rc;
+  const uint64_t stored = malio_store::count(h);
+  if (first > stored || count > stored - first) {
+    h->err = "world voxel rebuild: scans [" + std::to_string(first) + ", " + std::to_string(first + count) + ") beyond the store (" +
+             std::to_string(stored) + " scans)";
+    return MALIO_ERR_INVALID_ARG;
+  }
+  if (count == 0) {
+    if (n_voxels) *n_voxels = V->n_vox;
+    return MALIO_OK;
+  }
+  if (int rc = check_fold_args(h, V, leaf, carve)) return rc;
+  const int L = h->cfg.params.n_lidar;
+  struct Chunk { uint64_t s0, s1; const float* xyz; uint32_t block; uint64_t rows; };
+  std::vector<StoreScan> scans(count);
+  std::vector<Chunk> chunks;
+  uint64_t max_rows = 0;
+  for (uint64_t i = 0; i < count; ++i) {
+    const malio_store::View v = malio_store::view(h, first + i);
+    malio_rigid tc[MALIO_MAX_LIDAR];
+    tc[0] = D->tcomp[0];   // (not read: slot 0 has no compensation)
+    for (int l = 1; l < MALIO_MAX_LIDAR; ++l) tc[l] = v.rec->temporal_comp[l - 1];
+    StoreScan& sc = scans[i];
+    sc.pc = make_pass_const(h, D, states ? states + i : &v.rec->state, tc);
+    Chunk* c = chunks.empty() ? nullptr : &chunks.back();
+    const bool joins = c && !carve &&
+                       (v.rows == 0 || c->rows == 0 ||
+                        (v.block == c->block && v.xyz == c->xyz + 3 * c->rows && c->rows + v.rows <= MALIO_SEED_CHUNK));
+    if (!joins) { chunks.push_back(Chunk{i, i, v.xyz, v.block, 0}); c = &chunks.back(); }
+    if (c->rows == 0 && v.rows) { c->xyz = v.xyz; c->block = v.block; }
+    uint64_t at = c->rows;
+    for (int l = 0; l < L; ++l) { sc.first[l] = (uint32_t)at; sc.tag[l] = v.rec->slot_tag[l]; at += v.rec->n_points[l]; }
+    for (int l = L; l <= MALIO_MAX_LIDAR; ++l) sc.first[l] = (uint32_t)at;
+    for (int l = L; l < MALIO_MAX_LIDAR; ++l) sc.tag[l] = 0.f;
+    c->s1 = i + 1;
+    c->rows = at;
+    if (at > max_rows) max_rows = at;
+  }
+  cudaStream_t st = D->stream;
+  const float il = 1.0f / leaf;
+  DeviceBuffer<StoreScan> d_scans;   // the chunks' scan tables; freed after the call's wait
+  DeviceBuffer<float> d_ud;          // a carved scan's unpacked rows
+  if (int rc = d_scans.allocate(h, st, count)) return rc;
+  if (carve && max_rows) { if (int rc = d_ud.allocate(h, st, 5 * max_rows)) return rc; }
+  if (max_rows) {
+    if (int rc = grow_sort(h, V, D, max_rows)) return rc;
+    if (int rc = grow_runs(h, V, D, max_rows)) return rc;
+  }
+  CUDA_TRY(cudaMemcpyAsync(d_scans, scans.data(), count * sizeof(StoreScan), cudaMemcpyHostToDevice, st));
+  D->ctr.h2d_bytes += count * sizeof(StoreScan);
+  CUDA_TRY(cudaMemsetAsync(V->d_small, 0, 2 * sizeof(uint32_t), st));   // fault flag (kept over the whole call), run count
+  auto rows_of = [&](const Chunk& c) { return StoreRows{c.xyz, d_scans + c.s0, (uint32_t)(c.s1 - c.s0), L}; };
+  for (const Chunk& c : chunks) {   // the check: nothing is folded once a row or an origin is outside int
+    if (c.rows) {
+      SortBufs b = sort_bufs(V);
+      const uint32_t m = (uint32_t)c.rows;
+      vm_key_kernel<<<(m + 255) / 256, 256, 0, st>>>(rows_of(c), il, m, b.k.Current(), b.v.Current(), V->d_small);
+      D->ctr.kernel_launches += 1;
+    }
+    if (carve && c.rows) {
+      VmSlots o{};
+      o.L = L;
+      for (int l = 0; l <= L; ++l) o.first[l] = scans[c.s0].first[l];
+      vc_origin_kernel<<<1, 32, 0, st>>>(o, scans[c.s0].pc, il, V->d_small);
+      D->ctr.kernel_launches += 1;
+    }
+  }
+  CUDA_TRY(cudaGetLastError());
+  uint64_t bound = V->n_vox;   // at least the entries after the chunks enqueued so far
+  for (const Chunk& c : chunks) {
+    if (c.rows == 0) continue;
+    const uint32_t m = (uint32_t)c.rows;
+    if (!table_fits(V, bound + m)) {   // the exact count first, then the table for it
+      CUDA_TRY(cudaMemcpyAsync(V->h_small, V->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      if (V->h_small[0]) break;   // refused: the verdict below
+      V->n_vox = bound = V->h_small[2];
+      if (int rc = grow_table(h, V, D, bound + m)) return rc;
+    }
+    if (carve) {
+      if (int rc = ensure_evidence(h, V, D)) return rc;   // the first carve: every entry so far at hit = miss = 0
+      vr_unpack_kernel<<<(m + 255) / 256, 256, 0, st>>>(c.xyz, m, d_ud);
+      D->ctr.kernel_launches += 1;
+      const StoreScan& sc = scans[c.s0];
+      VmSlots u{};
+      u.L = L;
+      for (int l = 0; l < L; ++l) { u.ud[l] = d_ud + 5 * (size_t)sc.first[l]; u.tag[l] = sc.tag[l]; u.first[l] = sc.first[l]; }
+      u.first[L] = sc.first[L];
+      if (int rc = enqueue_scan(h, V, D, ScanRows{u, sc.pc}, il, m, carve, V->carve_scan + 1 + (uint32_t)c.s0)) return rc;
+    } else {
+      if (int rc = enqueue_fold(h, V, D, rows_of(c), il, m)) return rc;
+      vm_count_kernel<<<1, 1, 0, st>>>(V->d_head, V->d_new, V->d_small);
+      CUDA_TRY(cudaGetLastError());
+      D->ctr.kernel_launches += 1;
+    }
+    bound += m;
+  }
+  CUDA_TRY(cudaMemcpyAsync(V->h_small, V->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));   // the call's one wait: the fault flag and the entry count
+  if (V->h_small[0]) {
+    h->err = carve ? "world voxel rebuild: leaf size too small for a stored point's or a ray origin's coordinates under its scan's state (voxel index outside int); the map is unchanged"
+                   : "world voxel rebuild: leaf size too small for a stored point's coordinates under its scan's state (voxel index outside int); the map is unchanged";
+    return MALIO_ERR_CAPACITY;
+  }
+  V->n_vox = V->h_small[2];
+  if (carve) V->carve_scan += (uint32_t)count;
+  V->leaf = leaf;
+  V->leaf_set = true;
+  if (n_voxels) *n_voxels = V->n_vox;
+  return MALIO_OK;
+}
+
 // removed / added centroids in the order of download_device, with download_kept_device's size protocol and contract
 int changes_device(malio_handle* h, const malio_carve_keep* keep, float* d_removed, uint64_t cap_removed, uint64_t* n_removed,
                    float* d_added, uint64_t cap_added, uint64_t* n_added, cudaStream_t caller) {
@@ -1035,4 +1221,10 @@ extern "C" int malio_world_voxel_info(malio_handle* h, uint64_t* n_voxels, uint6
   if (!h) return MALIO_ERR_INVALID_ARG;
   MALIO_SETTLE(h);
   return malio_vox::info(h, n_voxels, capacity, device_bytes);
+}
+extern "C" int malio_world_voxel_rebuild(malio_handle* h, uint64_t first, uint64_t count, const malio_pass_state* states, float leaf,
+                                         const malio_carve_args* carve, uint64_t* n_voxels) {
+  if (!h) return MALIO_ERR_INVALID_ARG;
+  MALIO_SETTLE(h);
+  return malio_vox::rebuild(h, first, count, states, leaf, carve, n_voxels);
 }

@@ -179,6 +179,16 @@ class CarveKeep(C.Structure):
     _fields_ = [("min_miss", C.c_uint32), ("max_miss_per_hit", C.c_float)]
 
 
+STORE_BLOCK_POINTS = 1 << 24   # MALIO_STORE_BLOCK_POINTS
+
+
+class StoredScan(C.Structure):
+    """malio_stored_scan: a stored scan's record: the caller's time stamp, the state it was stored with, the temporal compensation
+    of LiDAR l >= 1 at l - 1, the slot tags and the points per slot (0 beyond L)."""
+    _fields_ = [("time", C.c_double), ("state", PassState), ("temporal_comp", Rigid * (MAX_LIDAR - 1)),
+                ("slot_tag", C.c_float * MAX_LIDAR), ("n_points", C.c_uint32 * MAX_LIDAR)]
+
+
 GRID_POINTS, GRID_VOXEL_MAP, GRID_PRIOR = 0, 1, 2            # MALIO_GRID_* sources
 GRID_FREE, GRID_OCCUPIED, GRID_UNKNOWN = 0, 100, 255         # nav_msgs/OccupancyGrid values
 GRID_MAX_BYTES = 16 << 30
@@ -230,6 +240,8 @@ EXPORTS = [
     "malio_world_voxel_save_changes_pcd",
     "malio_prior_map_extend", "malio_prior_map_session_download",
     "malio_grid_build_device", "malio_grid_build", "malio_grid_extent_device", "malio_write_grid_pgm",
+    "malio_scan_store_add", "malio_scan_store_put", "malio_scan_store_get", "malio_scan_store_register_device",
+    "malio_scan_store_info", "malio_scan_store_clear", "malio_world_voxel_rebuild",
 ]
 
 
@@ -302,6 +314,13 @@ def load() -> C.CDLL:
     lib.malio_world_voxel_seed_device.argtypes = [vp, vp, C.c_uint64, C.c_float, u32, vp, vp]
     lib.malio_world_voxel_changes_device.argtypes = [vp, vp, vp, C.c_uint64, vp, vp, C.c_uint64, vp, vp]
     lib.malio_world_voxel_save_changes_pcd.argtypes = [vp, vp, C.c_char_p, C.c_char_p, vp, vp]
+    lib.malio_scan_store_add.argtypes = [vp, vp, vp, C.c_double, vp]
+    lib.malio_scan_store_put.argtypes = [vp, vp, vp, vp]
+    lib.malio_scan_store_get.argtypes = [vp, C.c_uint64, vp, vp, C.c_uint64, vp]
+    lib.malio_scan_store_register_device.argtypes = [vp, C.c_uint64, vp, vp, C.c_uint64, vp, vp]
+    lib.malio_scan_store_info.argtypes = [vp, vp, vp, vp]
+    lib.malio_scan_store_clear.argtypes = [vp]
+    lib.malio_world_voxel_rebuild.argtypes = [vp, C.c_uint64, C.c_uint64, vp, C.c_float, vp, vp]
     lib.malio_write_pcd_binary.argtypes = [C.c_char_p, vp, C.c_uint64]
     lib.malio_read_pcd.argtypes = [C.c_char_p, vp, C.c_uint64, vp]
     lib.malio_prior_map_load.argtypes = [vp, vp, vp, vp, u32]

@@ -603,6 +603,92 @@ class MeasurementModel:
         self._check(self.lib.malio_world_voxel_info(self._h, C.byref(v), C.byref(c), C.byref(b)))
         return dict(n_voxels=int(v.value), capacity=int(c.value), device_bytes=int(b.value))
 
+    # ---- the scan store and the voxel map's rebuild from it (malio_scan_store_*, malio_world_voxel_rebuild)
+    def scan_store_add(self, s: capi.PassState | capi.State, slot_tag, time: float = 0.0) -> int:
+        """Keep the current dense cloud (the rows voxel_map_accumulate folds, LiDAR frame) on the device with state s, slot_tag
+        and the caller's time stamp, so that a later voxel_map_rebuild can fold it again.  Returns the number of stored scans."""
+        tag = np.ascontiguousarray(slot_tag, np.float32).reshape(-1)
+        if tag.shape[0] != self.n_lidar:
+            raise ValueError(f"slot_tag: {tag.shape[0]} values, expected one per LiDAR slot ({self.n_lidar})")
+        ps = s.pass_state() if isinstance(s, capi.State) else s
+        n = C.c_uint64(0)
+        self._check(self.lib.malio_scan_store_add(self._h, C.byref(ps), capi.ptr(tag), C.c_double(time), C.byref(n)))
+        return int(n.value)
+
+    def scan_store_put(self, record: capi.StoredScan, xyz) -> int:
+        """Append a stored scan: its record and its points, float32 (n, 3) with n = sum(record.n_points).  Returns the number of
+        stored scans."""
+        x = self._f32(xyz, 3)
+        if x.shape[0] != sum(record.n_points):
+            raise ValueError(f"xyz: {x.shape[0]} points, the record counts {sum(record.n_points)}")
+        n = C.c_uint64(0)
+        self._check(self.lib.malio_scan_store_put(self._h, C.byref(record), capi.ptr(x) if x.shape[0] else None, C.byref(n)))
+        return int(n.value)
+
+    def scan_store_get(self, k: int) -> tuple:
+        """(record, xyz float32 (n, 3)) of stored scan k."""
+        rec, n = capi.StoredScan(), C.c_uint64(0)
+        self._check(self.lib.malio_scan_store_get(self._h, int(k), C.byref(rec), None, 0, C.byref(n)))
+        xyz = np.zeros((n.value, 3), np.float32)
+        if n.value:
+            self._check(self.lib.malio_scan_store_get(self._h, int(k), None, capi.ptr(xyz), n.value, C.byref(n)))
+        return rec, xyz
+
+    def scan_store_records(self) -> list:
+        """Every stored scan's record (copies: edit their states and pass them, or theirs, to voxel_map_rebuild)."""
+        out = []
+        for k in range(self.scan_store_info()["n_scans"]):
+            rec, n = capi.StoredScan(), C.c_uint64(0)
+            self._check(self.lib.malio_scan_store_get(self._h, k, C.byref(rec), None, 0, C.byref(n)))
+            out.append(rec)
+        return out
+
+    def scan_store_register_tensor(self, k: int, state: capi.PassState | capi.State | None = None):
+        """Stored scan k registered with `state` (None: its stored state) as a CUDA tensor float32 (n, 4) {x, y, z, slot_tag},
+        the bits publish_frame_world(dense=True) gave for it; allocated and ordered on the current stream."""
+        import torch
+        ps = None if state is None else (state.pass_state() if isinstance(state, capi.State) else state)
+        sp = None if ps is None else C.byref(ps)
+        n = C.c_uint64(0)
+        st = torch.cuda.current_stream(self.device)
+        self._check(self.lib.malio_scan_store_register_device(self._h, int(k), sp, None, 0, C.byref(n), st.cuda_stream))
+        out = self._empty((n.value, 4), torch.float32)
+        if n.value:
+            self._check(self.lib.malio_scan_store_register_device(self._h, int(k), sp, _dptr(out), n.value, C.byref(n), st.cuda_stream))
+        return out
+
+    def scan_store_info(self) -> dict:
+        """Stored scans, stored points and the device bytes of the store's blocks."""
+        s, p, b = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.malio_scan_store_info(self._h, C.byref(s), C.byref(p), C.byref(b)))
+        return dict(n_scans=int(s.value), n_points=int(p.value), device_bytes=int(b.value))
+
+    def scan_store_clear(self):
+        """Release every stored scan."""
+        self._check(self.lib.malio_scan_store_clear(self._h))
+
+    def voxel_map_rebuild(self, leaf: float, states=None, first: int = 0, count: int | None = None, carve=None) -> int:
+        """Fold stored scans [first, first + count) into the voxel map again, as voxel_map_accumulate of each in index order
+        would, each under states[k - first] (capi.PassState or capi.State; None: the stored states) with its stored slot tags
+        and temporal compensation.  count None: every scan from first on.  carve as voxel_map_accumulate's.  Clear the map
+        first (voxel_map_save(.., clear=True)) for a fresh map.  Returns the number of voxels."""
+        leaf = _check_leaf(leaf)
+        if count is None:
+            count = max(self.scan_store_info()["n_scans"] - int(first), 0)
+        arr = None
+        if states is not None:
+            states = list(states)
+            if len(states) != count:
+                raise ValueError(f"states: {len(states)} states for {count} scans")
+            arr = (capi.PassState * max(count, 1))()
+            for i, s in enumerate(states):
+                arr[i] = s.pass_state() if isinstance(s, capi.State) else s
+        a = _as_carve(carve)
+        n = C.c_uint64(0)
+        self._check(self.lib.malio_world_voxel_rebuild(self._h, int(first), int(count), arr, C.c_float(leaf),
+                                                       None if a is None else C.byref(a), C.byref(n)))
+        return int(n.value)
+
     # ---- a 2-D occupancy grid for navigation (malio_grid_*)
     def _grid_source(self, source, xyzi, keep):
         """(source code, device pointer, rows, CarveKeep or None, the current stream) of grid / grid_extent's arguments."""
@@ -1057,6 +1143,59 @@ class MeasurementModel:
         self._check(self.lib.malio_upload_scan_resident(self._h, C.addressof(n)))
         self.n_points = int(n.value)
         return self.n_points
+
+
+STORED_SCAN = np.dtype([("time", "<f8"), ("rot", "<f8", 4), ("pos", "<f8", 3), ("ext", capi.RIGID, capi.MAX_LIDAR),
+                        ("temporal_comp", capi.RIGID, capi.MAX_LIDAR - 1), ("slot_tag", "<f4", capi.MAX_LIDAR),
+                        ("n_points", "<u4", capi.MAX_LIDAR)])   # malio_stored_scan as a numpy record
+assert STORED_SCAN.itemsize == C.sizeof(capi.StoredScan)
+SCAN_STORE_FORMAT = 1
+
+
+def write_scan_store_npz(path: str, records: np.ndarray, xyz: np.ndarray):
+    """A scan store as one .npz: records (STORED_SCAN, one per scan) and every scan's points concatenated in index order
+    (float32 (sum of n_points, 3)).  ValueError when the counts do not add up."""
+    records = np.ascontiguousarray(records, STORED_SCAN)
+    xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+    if int(records["n_points"].astype(np.int64).sum()) != xyz.shape[0]:
+        raise ValueError(f"xyz: {xyz.shape[0]} points, the records count {int(records['n_points'].astype(np.int64).sum())}")
+    with open(path, "wb") as f:
+        np.savez(f, format=np.int64(SCAN_STORE_FORMAT), records=records, xyz=xyz)
+
+
+def read_scan_store_npz(path: str) -> tuple:
+    """(records, list of each scan's float32 (n, 3) points) of a file write_scan_store_npz wrote."""
+    with np.load(path, allow_pickle=False) as z:
+        if int(z["format"]) != SCAN_STORE_FORMAT:
+            raise ValueError(f"{path}: scan store format {int(z['format'])}, expected {SCAN_STORE_FORMAT}")
+        records = np.ascontiguousarray(z["records"], STORED_SCAN)
+        xyz = np.ascontiguousarray(z["xyz"], np.float32).reshape(-1, 3)
+    ends = np.cumsum(records["n_points"].astype(np.int64).sum(axis=1))
+    if (ends[-1] if ends.shape[0] else 0) != xyz.shape[0]:
+        raise ValueError(f"{path}: {xyz.shape[0]} points, the records count {int(ends[-1]) if ends.shape[0] else 0}")
+    starts = np.concatenate([[0], ends[:-1]]).astype(np.int64)
+    return records, [xyz[a:b] for a, b in zip(starts, ends)]
+
+
+def save_scan_store(model: MeasurementModel, path: str):
+    """Every scan model stores, records and points, into one .npz (write_scan_store_npz), so that a later process can correct
+    the states and rebuild the map (load_scan_store, then MeasurementModel.voxel_map_rebuild)."""
+    recs, pts = [], []
+    for k in range(model.scan_store_info()["n_scans"]):
+        rec, xyz = model.scan_store_get(k)
+        recs.append(np.frombuffer(bytes(rec), STORED_SCAN)[0])
+        pts.append(xyz)
+    records = np.array(recs, STORED_SCAN) if recs else np.zeros(0, STORED_SCAN)
+    write_scan_store_npz(path, records, np.concatenate(pts) if pts else np.zeros((0, 3), np.float32))
+
+
+def load_scan_store(model: MeasurementModel, path: str) -> int:
+    """Append the scans of a save_scan_store file to model's store.  Returns the number of stored scans."""
+    records, pts = read_scan_store_npz(path)
+    n = model.scan_store_info()["n_scans"]
+    for r, xyz in zip(records, pts):
+        n = model.scan_store_put(capi.StoredScan.from_buffer_copy(r.tobytes()), xyz)
+    return n
 
 
 def _undistort_args(beg_time, extrinsic, lt_imu_frame, ctrl_t, ctrl_T, imu_cov_t, cov_pointer):
