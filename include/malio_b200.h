@@ -574,6 +574,100 @@ int malio_scan_store_info(malio_handle* h, uint64_t* n_scans, uint64_t* n_points
 int malio_scan_store_clear(malio_handle* h);
 int malio_world_voxel_rebuild(malio_handle* h, uint64_t first, uint64_t count, const malio_pass_state* states, float leaf,
                               const malio_carve_args* carve, uint64_t* n_voxels);
+/* Closing loops over the scan store: register a stored scan against a submap of stored scans on the device
+ * (malio_scan_store_match), then optimize the odometry chain with the loop edges on the host (malio_pose_graph_optimize); the
+ * corrected states go to malio_world_voxel_rebuild.  tests/loop_ref.py restates the match bit for bit.
+ * malio_scan_store_match, the contract (every device expression uses only +, -, *, / and sqrt on doubles, plus floor, each sum
+ * in the order given; the transcendental functions run on the host):
+ *   target rows  for each stored scan k in [target_first, target_first + target_count), in (scan, slot, point) order, the float4
+ *                rows malio_scan_store_register_device(k, NULL) gives; a row with a non-finite coordinate is left out.
+ *   source rows  stored scan `source` registered with its stored extrinsics and temporal compensation under rot = identity,
+ *                pos = 0 (the body frame), as floats b; non-finite rows are left out, n_points counts the others.
+ *   model        per level l, leaf = (double)leaf[l]: a target row's key is floor((double)x / leaf) per axis; a key outside
+ *                [-2^20, 2^20) refuses the call (MALIO_ERR_CAPACITY).  Per voxel, in row order: n, the sums (one addition at a
+ *                time from 0.0), mu = sum / n, then C_ij = sum of d_i * d_j (d = x - mu) in row order, / n.  Cyclic Jacobi with
+ *                MALIO_MATCH_JACOBI_SWEEPS sweeps over the pairs (0,1), (0,2), (1,2): a pair with A_pq == 0 is skipped, else
+ *                theta = (A_qq - A_pp) / (2 A_pq), t = 1 / (|theta| + sqrt(theta^2 + 1)) negated for theta < 0,
+ *                c = 1 / sqrt(t^2 + 1), s = t c; columns p, q of A and V become (c a_p - s a_q, s a_p + c a_q), then rows p, q of
+ *                A the same.  The eigenvalues are A's diagonal ordered by (value, index); the normal n is V's column of the
+ *                smallest.  The voxel has a plane when n >= min_points and lambda0 <= planarity * lambda1.
+ *   pose         (q, p), starting at the guess's rot / pos (NULL: the source's stored state); R = q_to_R(q) on the host.
+ *   correspond   w_i = ((R_i0 b0 + R_i1 b1) + R_i2 b2) + p_i; base key floor(w_i / leaf); among the plane voxels of the base
+ *                voxel and its 26 neighbours (offsets in (dz, dy, dx) ascending order, keys outside the range skipped) the one
+ *                with the smallest e = (d0 d0 + d1 d1) + d2 d2, d = w - mu, the first on ties.  Inlier when e <= leaf * leaf and
+ *                |r| <= gate[l], r = (n0 d0 + n1 d1) + n2 d2.
+ *   step         per inlier m_i = (R_0i n0 + R_1i n1) + R_2i n2 (R^T n), J = [b x m, m]; the 29 doubles J_i J_j (i <= j,
+ *                row-major), J_i r, r r and 1, zero for the other rows, are summed as a perfect binary tree (pairs of adjacent
+ *                entries, level by level) over the source index padded with zeros to the smallest power of two >= the source
+ *                rows.  The host solves (J^T J) delta = -J^T r by LL^T Cholesky (in index order; a pivot <= 0, or fewer than 6
+ *                inliers, ends the level as failed), then q <- normalize(q (x) quat_from_R(R(exp_se3(delta)))),
+ *                p <- p + q_rot(q_old, t(exp_se3(delta))).  A level ends after the step whose every |delta_i| is below eps_rot
+ *                (i < 3) / eps_pos (i >= 3), after max_iter steps, or on a failure; iterations[l] counts the steps taken.
+ *   report       at the final pose, one more evaluation at the finest level: info = J^T J / sigma^2 (symmetric 6 x 6),
+ *                rms = sqrt(sum r^2 / inliers) (0 without inliers), fitness = inliers / n_points, eig_min the smallest
+ *                eigenvalue of info (host Jacobi, to a tolerance).  rot / pos: the estimate T_est; rel = T_anchor^-1 T_est as
+ *                rel_rot = conj(q_anchor) * q_est, rel_pos = q_rot_conj(q_anchor, p_est - p_anchor) with the anchor's stored
+ *                state: the loop edge (anchor, source) of malio_pose_graph_optimize, its info the edge's.  converged: the finest
+ *                level ended on eps (the coarser levels only bring the pose into its basin and may end on max_iter).
+ *                target_voxels[l]: the voxels of level l with a plane.
+ * Errors, each leaving the handle as it was:
+ *   MALIO_ERR_INVALID_ARG  NULL h, a or rep; source or anchor beyond the store; an empty range or one beyond the store; the
+ *                          anchor outside the range; n_levels 0 or above MALIO_MATCH_MAX_LEVELS; a leaf, gate, sigma or
+ *                          planarity that is not finite and > 0; max_iter 0; a guess rot / pos that is not finite
+ *   MALIO_ERR_STATE        a communicator is attached (each rank stores only its block of a scan)
+ *   MALIO_ERR_CAPACITY     a key outside [-2^20, 2^20); 2^31 or more target rows; scratch above MALIO_MATCH_MAX_BYTES
+ * The call changes no store record or block, voxel map, device map or prior; of the counters only launches and copies grow.
+ * It is synchronous.  Device memory: about 105 B per target row plus 16 B per source row, local to the call and released
+ * before it returns; device_bytes reports it. */
+#define MALIO_MATCH_MAX_LEVELS 4
+#define MALIO_MATCH_JACOBI_SWEEPS 8
+#define MALIO_MATCH_KEY_RANGE (1 << 20)
+#define MALIO_MATCH_MAX_BYTES (16ull << 30)
+typedef struct malio_match_args {
+  uint64_t target_first, target_count;   /* the submap: stored scans [first, first + count) under their stored states */
+  uint32_t n_levels;                     /* coarse to fine */
+  float leaf[MALIO_MATCH_MAX_LEVELS];    /* voxel edge of the plane model per level, metres */
+  float gate[MALIO_MATCH_MAX_LEVELS];    /* inlier gate on |residual| per level, metres */
+  uint32_t max_iter;                     /* Gauss-Newton steps per level */
+  double eps_rot, eps_pos;               /* a level ends when every |dtheta_i| < eps_rot and every |dt_i| < eps_pos */
+  uint32_t min_points;                   /* a voxel with fewer target points has no plane */
+  double planarity;                      /* plane when lambda0 <= planarity * lambda1 */
+  double sigma;                          /* residual standard deviation for the information matrix, metres */
+} malio_match_args;
+typedef struct malio_match_report {
+  double rot[4], pos[3];                 /* the source scan's state in the submap's frame */
+  double rel_rot[4], rel_pos[3];         /* the loop edge: T_anchor^-1 * T_source, with T_anchor = the anchor's stored state */
+  double info[36];                       /* 6 x 6 information of the edge, order [dtheta, dt] (log_se3's order) */
+  double rms, fitness, eig_min;          /* over the inliers; inliers / finite source points; smallest eigenvalue of info */
+  uint32_t n_points, n_inliers, iterations[MALIO_MATCH_MAX_LEVELS];
+  int32_t converged;                     /* the finest level ended on eps, not on max_iter or a failed step */
+  uint64_t target_points, target_voxels[MALIO_MATCH_MAX_LEVELS], device_bytes;
+} malio_match_report;
+int malio_scan_store_match(malio_handle* h, uint64_t source, uint64_t anchor, const malio_pass_state* guess,
+                           const malio_match_args* a, malio_match_report* rep);
+/* malio_pose_graph_optimize (host, no handle): node k is (rot, pos) of odo[k], node 0 fixed.  Edges: odometry k -> k + 1 with
+ * Z = odo[k]^-1 odo[k + 1] and Omega = diag(sigma_rot^-2 x 3, sigma_pos^-2 x 3); loops[i] with Z = (rot, pos) and Omega = info.
+ * Residual e = log_se3(Z^-1 T_a^-1 T_b), the nodes perturbed on the right as malio_scan_store_match's pose
+ * (T <- T exp_se3(delta)), Jacobians J_b = I and J_a = -Ad(T_b^-1 T_a) (first order in e).  Gauss-Newton: the exact solve of
+ * the normal equations (block-tridiagonal Cholesky of the chain, the loop edges through Woodbury with Omega = S S^T from its
+ * eigen-decomposition: the capacitance I + V^T T^-1 V is SPD for a rank-deficient Omega too); the step is halved (at most 20
+ * times) while the total chi^2 grows.  The solve ends with converged = 1 when every |delta| is below eps_rot / eps_pos, or when
+ * no halving of a later step lowers chi^2 (the Jacobians are first order, so at the minimum their step may point past it).  It
+ * ends with converged = 0 after max_iter steps, when a factor is not positive definite, or when no halving of the first step
+ * lowers chi^2 (out is then odo's states).  out[k] is odo[k] with rot and pos replaced (the extrinsics copied);
+ * with no loop edge out is odo byte for byte.  loop_chi2 (may be NULL): each loop edge's final e^T Omega e.
+ *   MALIO_ERR_INVALID_ARG  NULL odo, a, out or rep, n == 0, NULL loops with n_loops > 0, n_loops above the cap; a loop index
+ *                          >= n or a == b; a loop info that is not finite or not symmetric; a sigma or eps that is not > 0
+ *                          (or not finite); max_iter 0 */
+#define MALIO_POSE_GRAPH_MAX_LOOPS 256
+typedef struct malio_pose_edge { uint64_t a, b; double rot[4], pos[3]; double info[36]; } malio_pose_edge;
+typedef struct malio_pose_graph_args { double sigma_rot, sigma_pos; uint32_t max_iter; double eps_rot, eps_pos; } malio_pose_graph_args;
+typedef struct malio_pose_graph_report {
+  uint32_t iterations; int32_t converged; double chi2_odo, chi2_loop, chi2_loop_before; double ms;
+} malio_pose_graph_report;
+int malio_pose_graph_optimize(const malio_pass_state* odo, uint64_t n, const malio_pose_edge* loops, uint32_t n_loops,
+                              const malio_pose_graph_args* a, malio_pass_state* out, double* loop_chi2,
+                              malio_pose_graph_report* rep);
 /* Host: the same PCD file from n > 0 host points (n x 4 floats {x, y, z, intensity}): the header of PCDWriter::writeBinary for
  * PointXYZINormal (FIELDS x y z intensity normal_x normal_y normal_z curvature, WIDTH = POINTS = n, HEIGHT 1, DATA binary) and
  * n packed 32-byte records with normal_x/y/z = curvature = 0.  MALIO_ERR_INVALID_ARG for n == 0, a NULL argument or a file

@@ -147,6 +147,10 @@ namespace malio_store {
 struct View { const malio_stored_scan* rec; const float* xyz; uint64_t rows; uint32_t block; };
 uint64_t count(const malio_handle* h);
 View view(const malio_handle* h, uint64_t k);
+// the first n rows of stored scan k registered with s (NULL: its stored state) as malio_scan_store_register_device registers
+// them, n x 4 floats {x, y, z, slot_tag} into out (16-byte aligned device memory of the handle's device), enqueued on the
+// handle's stream
+int enqueue_register(malio_handle* h, uint64_t k, const malio_pass_state* s, uint64_t n, float* out);
 }  // namespace malio_store
 
 // malio_reloc.cu — relocalization in a loaded prior (malio_relocalize after its NULL checks; malio_place.cu verifies with it)

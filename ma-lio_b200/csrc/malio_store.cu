@@ -230,17 +230,25 @@ int register_device(malio_handle* h, uint64_t k, const malio_pass_state* s, floa
   }
   *n_out = v.rows;
   if (!out || kk == 0) return MALIO_OK;
+  if (int rc = caller_enter(h, D, caller)) return rc;
+  if (int rc = enqueue_register(h, k, s, kk, out)) return rc;
+  return caller_leave(h, D, caller);
+}
+
+int enqueue_register(malio_handle* h, uint64_t k, const malio_pass_state* s, uint64_t n, float* out) {
+  DeviceState* D = h->dev.get();
+  const View v = view(h, k);
+  if (n == 0) return MALIO_OK;
   malio_rigid tc[MALIO_MAX_LIDAR];
   tc[0] = D->tcomp[0];
   for (int l = 1; l < MALIO_MAX_LIDAR; ++l) tc[l] = v.rec->temporal_comp[l - 1];
   const PassConst pc = make_pass_const(h, D, s ? s : &v.rec->state, tc);
-  if (int rc = caller_enter(h, D, caller)) return rc;
-  const uint32_t nn = (uint32_t)kk;
+  const uint32_t nn = (uint32_t)n;
   st_register_kernel<<<(nn + 255) / 256, 256, 0, D->stream>>>(v.xyz, slots_of(*v.rec, h->cfg.params.n_lidar), pc, nn,
                                                              reinterpret_cast<float4*>(out));
   CUDA_TRY(cudaGetLastError());
   D->ctr.kernel_launches += 1;
-  return caller_leave(h, D, caller);
+  return MALIO_OK;
 }
 
 int info(malio_handle* h, uint64_t* n_scans, uint64_t* n_points, uint64_t* device_bytes) {

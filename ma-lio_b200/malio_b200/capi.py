@@ -208,6 +208,47 @@ class GridReport(C.Structure):
                 ("n_free", C.c_uint64), ("n_unknown", C.c_uint64), ("device_bytes", C.c_uint64)]
 
 
+MATCH_MAX_LEVELS = 4                 # MALIO_MATCH_MAX_LEVELS
+MATCH_JACOBI_SWEEPS = 8              # MALIO_MATCH_JACOBI_SWEEPS
+MATCH_KEY_RANGE = 1 << 20            # MALIO_MATCH_KEY_RANGE
+MATCH_MAX_BYTES = 16 << 30           # MALIO_MATCH_MAX_BYTES
+POSE_GRAPH_MAX_LOOPS = 256           # MALIO_POSE_GRAPH_MAX_LOOPS
+
+
+class MatchArgs(C.Structure):
+    """malio_match_args: the submap (stored scans [target_first, target_first + target_count)), the levels' leaves and gates
+    (coarse to fine), Gauss-Newton steps and end tests per level, the plane test and the residual sigma."""
+    _fields_ = [("target_first", C.c_uint64), ("target_count", C.c_uint64), ("n_levels", C.c_uint32),
+                ("leaf", C.c_float * MATCH_MAX_LEVELS), ("gate", C.c_float * MATCH_MAX_LEVELS), ("max_iter", C.c_uint32),
+                ("eps_rot", C.c_double), ("eps_pos", C.c_double), ("min_points", C.c_uint32), ("planarity", C.c_double),
+                ("sigma", C.c_double)]
+
+
+class MatchReport(C.Structure):
+    """malio_match_report: the estimate, the loop edge T_anchor^-1 T_est and its 6 x 6 information, the fit's quality, steps
+    per level, the submap's size and the call's peak scratch bytes."""
+    _fields_ = [("rot", C.c_double * 4), ("pos", C.c_double * 3), ("rel_rot", C.c_double * 4), ("rel_pos", C.c_double * 3),
+                ("info", C.c_double * 36), ("rms", C.c_double), ("fitness", C.c_double), ("eig_min", C.c_double),
+                ("n_points", C.c_uint32), ("n_inliers", C.c_uint32), ("iterations", C.c_uint32 * MATCH_MAX_LEVELS),
+                ("converged", C.c_int32), ("target_points", C.c_uint64), ("target_voxels", C.c_uint64 * MATCH_MAX_LEVELS),
+                ("device_bytes", C.c_uint64)]
+
+
+class PoseEdge(C.Structure):
+    """malio_pose_edge: a loop edge a -> b, Z = (rot, pos) = T_a^-1 T_b, and its information (order [dtheta, dt])."""
+    _fields_ = [("a", C.c_uint64), ("b", C.c_uint64), ("rot", C.c_double * 4), ("pos", C.c_double * 3), ("info", C.c_double * 36)]
+
+
+class PoseGraphArgs(C.Structure):
+    _fields_ = [("sigma_rot", C.c_double), ("sigma_pos", C.c_double), ("max_iter", C.c_uint32), ("eps_rot", C.c_double),
+                ("eps_pos", C.c_double)]
+
+
+class PoseGraphReport(C.Structure):
+    _fields_ = [("iterations", C.c_uint32), ("converged", C.c_int32), ("chi2_odo", C.c_double), ("chi2_loop", C.c_double),
+                ("chi2_loop_before", C.c_double), ("ms", C.c_double)]
+
+
 class UpdateReport(C.Structure):
     _fields_ = [("passes", C.c_int32), ("searches", C.c_int32), ("converged_count", C.c_int32),
                 ("last_status", C.c_int32), ("n_eff_last", C.c_uint32), ("ms_device_total", C.c_float),
@@ -242,6 +283,7 @@ EXPORTS = [
     "malio_grid_build_device", "malio_grid_build", "malio_grid_extent_device", "malio_write_grid_pgm",
     "malio_scan_store_add", "malio_scan_store_put", "malio_scan_store_get", "malio_scan_store_register_device",
     "malio_scan_store_info", "malio_scan_store_clear", "malio_world_voxel_rebuild",
+    "malio_scan_store_match", "malio_pose_graph_optimize",
 ]
 
 
@@ -321,6 +363,8 @@ def load() -> C.CDLL:
     lib.malio_scan_store_info.argtypes = [vp, vp, vp, vp]
     lib.malio_scan_store_clear.argtypes = [vp]
     lib.malio_world_voxel_rebuild.argtypes = [vp, C.c_uint64, C.c_uint64, vp, C.c_float, vp, vp]
+    lib.malio_scan_store_match.argtypes = [vp, C.c_uint64, C.c_uint64, vp, vp, vp]
+    lib.malio_pose_graph_optimize.argtypes = [vp, C.c_uint64, vp, u32, vp, vp, vp, vp]
     lib.malio_write_pcd_binary.argtypes = [C.c_char_p, vp, C.c_uint64]
     lib.malio_read_pcd.argtypes = [C.c_char_p, vp, C.c_uint64, vp]
     lib.malio_prior_map_load.argtypes = [vp, vp, vp, vp, u32]

@@ -144,7 +144,131 @@ GRID_GROUND_HALFWIDTH = 10
 GRID_H_LO = 0.3
 GRID_H_HI = 2.0
 GRID_MIN_OBSTACLE_POINTS = 1
+# Defaults of the loop closure (malio_scan_store_match, close_loops), chosen on the synthetic ray-cast drives of
+# tests/test_gpu_loop.py (DESIGN.md, "Closing loops over the scan store"): three levels from 2 m to 0.5 m voxels, a submap of the
+# anchor +- 10 stored scans, an edge accepted at fitness >= 0.3, rms <= 0.1 m and a per-inlier constraint (accept_edge) >= ACCEPT_CONSTRAINT.
+MATCH_LEAF = (2.0, 1.0, 0.5)
+MATCH_GATE = (1.0, 0.5, 0.25)
+MATCH_MAX_ITER = 30
+MATCH_EPS_ROT = 1e-6
+MATCH_EPS_POS = 1e-5
+MATCH_MIN_POINTS = 5
+MATCH_PLANARITY = 0.1
+MATCH_SIGMA = 0.05
+MATCH_HALF_WINDOW = 10
+ACCEPT_FITNESS = 0.3
+ACCEPT_RMS = 0.1
+# eig_min * sigma^2 / n_inliers: the smallest eigenvalue of the mean J^T J per inlier, independent of the scan's size and of
+# sigma (a corridor gave 0.006, the drive around a block 0.041-0.047, a street corner 0.073)
+ACCEPT_CONSTRAINT = 0.02
+POSE_GRAPH_SIGMA_ROT = 0.01
+POSE_GRAPH_SIGMA_POS = 0.1
 GRID_SOURCES = {"points": capi.GRID_POINTS, "voxel_map": capi.GRID_VOXEL_MAP, "prior": capi.GRID_PRIOR}
+
+
+def match_args(target_first: int = 0, target_count: int = 1, leaf=MATCH_LEAF, gate=MATCH_GATE, max_iter: int = MATCH_MAX_ITER,
+               eps_rot: float = MATCH_EPS_ROT, eps_pos: float = MATCH_EPS_POS, min_points: int = MATCH_MIN_POINTS,
+               planarity: float = MATCH_PLANARITY, sigma: float = MATCH_SIGMA) -> capi.MatchArgs:
+    """malio_match_args; leaf and gate: one value per level, coarse to fine (at most MATCH_MAX_LEVELS)."""
+    leaf, gate = [float(v) for v in np.atleast_1d(leaf)], [float(v) for v in np.atleast_1d(gate)]
+    if len(leaf) != len(gate) or not 0 < len(leaf) <= capi.MATCH_MAX_LEVELS:
+        raise ValueError(f"leaf and gate: one value each per level, 1..{capi.MATCH_MAX_LEVELS} levels")
+    a = capi.MatchArgs()
+    a.target_first, a.target_count, a.n_levels = int(target_first), int(target_count), len(leaf)
+    for l, (f, g) in enumerate(zip(leaf, gate)):
+        a.leaf[l], a.gate[l] = f, g
+    a.max_iter, a.eps_rot, a.eps_pos = int(max_iter), float(eps_rot), float(eps_pos)
+    a.min_points, a.planarity, a.sigma = int(min_points), float(planarity), float(sigma)
+    return a
+
+
+def pose_graph_optimize(states, edges, sigma_rot: float = POSE_GRAPH_SIGMA_ROT, sigma_pos: float = POSE_GRAPH_SIGMA_POS,
+                        max_iter: int = 50, eps_rot: float = 1e-9, eps_pos: float = 1e-8) -> tuple:
+    """The odometry chain of `states` (capi.PassState / capi.State, node 0 fixed) plus loop `edges` (capi.PoseEdge, or dicts
+    with a, b, rel_rot, rel_pos, info as close_loops accepts them) optimized on the host (malio_pose_graph_optimize).
+    Returns (corrected capi.PassState list, per-loop chi^2 array, report dict)."""
+    lib = capi.load()
+    states = [s.pass_state() if isinstance(s, capi.State) else s for s in states]
+    n, m = len(states), len(edges)
+    odo = (capi.PassState * max(n, 1))(*states)
+    loops = (capi.PoseEdge * max(m, 1))()
+    for i, e in enumerate(edges):
+        if isinstance(e, capi.PoseEdge):
+            loops[i] = e
+            continue
+        loops[i].a, loops[i].b = int(e["a"]), int(e["b"])
+        loops[i].rot[:] = [float(v) for v in e["rel_rot"]]
+        loops[i].pos[:] = [float(v) for v in e["rel_pos"]]
+        loops[i].info[:] = [float(v) for v in np.asarray(e["info"], np.float64).reshape(36)]
+    a = capi.PoseGraphArgs(float(sigma_rot), float(sigma_pos), int(max_iter), float(eps_rot), float(eps_pos))
+    out = (capi.PassState * max(n, 1))()
+    chi = np.zeros(max(m, 1))
+    rep = capi.PoseGraphReport()
+    rc = lib.malio_pose_graph_optimize(odo, n, loops if m else None, m, C.byref(a), out, capi.ptr(chi), C.byref(rep))
+    if rc != capi.OK:
+        raise capi.MalioError(rc, "malio_pose_graph_optimize: invalid argument")
+    return ([out[k] for k in range(n)], chi[:m].copy(),
+            dict(iterations=int(rep.iterations), converged=bool(rep.converged), chi2_odo=rep.chi2_odo, chi2_loop=rep.chi2_loop,
+                 chi2_loop_before=rep.chi2_loop_before, ms=rep.ms))
+
+
+def loop_candidates(records, radius: float, min_gap: int, stride: int = 1) -> list:
+    """(i, j) pairs: for every stride-th stored scan j, the scan i <= j - min_gap whose stored position is nearest to j's,
+    when it lies within radius (first index on ties).  records: capi.StoredScan (or capi.PassState) list."""
+    pos = np.array([list((r.state if hasattr(r, "state") else r).pos) for r in records], np.float64).reshape(-1, 3)
+    out = []
+    for j in range(0, len(pos), max(int(stride), 1)):
+        if j - min_gap < 0:
+            continue
+        d = np.linalg.norm(pos[:j - min_gap + 1] - pos[j], axis=1)
+        i = int(np.argmin(d))
+        if d[i] <= radius:
+            out.append((i, j))
+    return out
+
+
+def constraint(rep: dict) -> float:
+    """eig_min * sigma^2 / n_inliers of a match report: how well the weakest direction of the edge is held, per inlier (0 for
+    no inlier).  Unlike eig_min it does not grow with the scan's size or the chosen sigma."""
+    return rep["eig_min"] * rep["sigma"] ** 2 / rep["n_inliers"] if rep["n_inliers"] else 0.0
+
+
+def accept_edge(rep: dict, fitness: float = ACCEPT_FITNESS, rms: float = ACCEPT_RMS, min_constraint: float = ACCEPT_CONSTRAINT) -> bool:
+    """The acceptance rule of close_loops: a match whose finest level converged, with fitness, rms and constraint(rep) on the
+    right side of the thresholds."""
+    return bool(rep["converged"] and rep["fitness"] >= fitness and rep["rms"] <= rms and constraint(rep) >= min_constraint)
+
+
+def close_loops(model: "MeasurementModel", radius: float = 10.0, min_gap: int = 30, stride: int = 1,
+                half_window: int = MATCH_HALF_WINDOW, accept: dict | None = None, graph: dict | None = None, **match) -> dict:
+    """Loop closure over the model's scan store: loop_candidates, each candidate's source matched against its anchor
+    +- half_window (scan_store_match from the source's stored state), the edges accept_edge keeps, then pose_graph_optimize
+    of the stored states with them.  Returns dict(states = the corrected capi.PassState list (for voxel_map_rebuild),
+    edges = the accepted match reports the pose graph used (with a = anchor, b = source; more accepted edges than
+    capi.POSE_GRAPH_MAX_LOOPS are thinned evenly along the drive), reports = every match report (accepted, used), graph = the
+    pose graph's report)."""
+    recs = model.scan_store_records()
+    reports, edges = [], []
+    for i, j in loop_candidates(recs, radius, min_gap, stride):
+        first = max(i - half_window, 0)
+        count = min(i + half_window + 1, j - min_gap + 1, len(recs)) - first
+        r = model.scan_store_match(j, i, target_first=first, target_count=count, **match)
+        r["accepted"] = accept_edge(r, **(accept or {}))
+        reports.append(r)
+        if r["accepted"]:
+            edges.append(dict(r, a=i, b=j))
+    if len(edges) > capi.POSE_GRAPH_MAX_LOOPS:   # thinned evenly along the drive to what the pose graph takes
+        keep = np.unique(np.linspace(0, len(edges) - 1, capi.POSE_GRAPH_MAX_LOOPS).round().astype(int))
+        edges = [edges[k] for k in keep]
+    used = {(e["a"], e["b"]) for e in edges}
+    for r in reports:
+        r["used"] = (r["anchor"], r["source"]) in used
+    states = [r.state for r in recs]
+    if edges:
+        states, _, g = pose_graph_optimize(states, edges, **(graph or {}))
+    else:
+        g = dict(iterations=0, converged=True, chi2_odo=0.0, chi2_loop=0.0, chi2_loop_before=0.0, ms=0.0)
+    return dict(states=states, edges=edges, reports=reports, graph=g)
 
 
 def carve_args(max_range: float = CARVE_MAX_RANGE, end_margin: float = CARVE_END_MARGIN) -> capi.CarveArgs:
@@ -688,6 +812,30 @@ class MeasurementModel:
         self._check(self.lib.malio_world_voxel_rebuild(self._h, int(first), int(count), arr, C.c_float(leaf),
                                                        None if a is None else C.byref(a), C.byref(n)))
         return int(n.value)
+
+    def scan_store_match(self, source: int, anchor: int, guess: capi.PassState | capi.State | None = None, **args) -> dict:
+        """Register stored scan `source` against a submap of stored scans on the device (malio_scan_store_match), starting from
+        guess (None: the source's stored state).  args: match_args' keywords (target_first / target_count default to anchor
+        +- half_window).  Returns the report as a dict: rot, pos, rel_rot, rel_pos (the loop edge T_anchor^-1 T_est), info
+        (6 x 6), rms, fitness, eig_min, n_points, n_inliers, iterations, converged, target_points, target_voxels, device_bytes,
+        and the call's source, anchor and sigma."""
+        half = int(args.pop("half_window", MATCH_HALF_WINDOW))
+        if "target_first" not in args:
+            n = self.scan_store_info()["n_scans"]
+            args["target_first"] = max(int(anchor) - half, 0)
+            args["target_count"] = min(int(anchor) + half + 1, n) - args["target_first"]
+        a = match_args(**args)
+        ps = None if guess is None else (guess.pass_state() if isinstance(guess, capi.State) else guess)
+        rep = capi.MatchReport()
+        self._check(self.lib.malio_scan_store_match(self._h, int(source), int(anchor), None if ps is None else C.byref(ps), C.byref(a),
+                                                    C.byref(rep)))
+        L = a.n_levels
+        return dict(rot=np.array(rep.rot[:]), pos=np.array(rep.pos[:]), rel_rot=np.array(rep.rel_rot[:]), rel_pos=np.array(rep.rel_pos[:]),
+                    info=np.array(rep.info[:]).reshape(6, 6), rms=rep.rms, fitness=rep.fitness, eig_min=rep.eig_min,
+                    n_points=int(rep.n_points), n_inliers=int(rep.n_inliers), iterations=[int(v) for v in rep.iterations[:L]],
+                    converged=bool(rep.converged), target_points=int(rep.target_points),
+                    target_voxels=[int(v) for v in rep.target_voxels[:L]], device_bytes=int(rep.device_bytes),
+                    source=int(source), anchor=int(anchor), sigma=float(a.sigma))
 
     # ---- a 2-D occupancy grid for navigation (malio_grid_*)
     def _grid_source(self, source, xyzi, keep):
